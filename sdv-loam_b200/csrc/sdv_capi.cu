@@ -93,15 +93,16 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
   make_geom(c, K);
   CK(cudaMalloc(&c->tc_dev, sizeof(TrackConst)));
   CK(cudaMemcpy(c->tc_dev, &c->tc, sizeof(TrackConst), cudaMemcpyHostToDevice));
-  // frame pool: level-0 intensity plane + packed texels of levels >= 1 per frame; packed level-0 texels come from a small keyframe pool
+  // frame pool: planar intensity of every level per frame (level 0 + one allocation for levels >= 1), plus the storage of the packed-texel cache of
+  // levels >= 1; packed level-0 texels come from a small keyframe pool
   size_t texels = 0; c->lvl_off[0] = 0; for (int l=1;l<levels;l++) { c->lvl_off[l] = texels; texels += (size_t)(w>>l)*(h>>l); }
   c->frame_texels = texels;
   c->frames.resize(s.max_frames);
   for (auto& f : c->frames) {
-    f.used = false; f.adopted = false; f.lvl0_slot = -1; f.base = nullptr; f.ingest_seq = 0;
-    CK(cudaMalloc(&f.I0_own, (size_t)w*h*sizeof(float))); f.I0 = f.I0_own;
-    if (texels) CK(cudaMalloc(&f.base, texels*sizeof(float4)));
-    f.lvl[0] = nullptr; for (int l=1;l<levels;l++) f.lvl[l] = f.base + c->lvl_off[l];
+    f.used = false; f.adopted = false; f.lvl0_slot = -1; f.hi_tex = false; f.pyr = nullptr; f.base = nullptr; f.ingest_seq = 0;
+    CK(cudaMalloc(&f.I0_own, (size_t)w*h*sizeof(float))); f.I0 = f.I0_own; f.img[0] = f.I0;
+    if (texels) { CK(cudaMalloc(&f.pyr, texels*sizeof(float))); CK(cudaMalloc(&f.base, texels*sizeof(float4))); }
+    f.lvl[0] = nullptr; for (int l=1;l<levels;l++) { f.img[l] = f.pyr + c->lvl_off[l]; f.lvl[l] = f.base + c->lvl_off[l]; }
   }
   { int nkf = s.max_kf_images > 0 ? s.max_kf_images : SDV_MAX_FRAMES_WINDOW + 4; if (nkf > s.max_frames) nkf = s.max_frames;
     c->lvl0_pool.resize(nkf); for (int i=0;i<nkf;i++) { CK(cudaMalloc(&c->lvl0_pool[i], (size_t)w*h*sizeof(float4))); c->lvl0_free.push_back(nkf-1-i); } }
@@ -131,7 +132,7 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
   CK(cudaMallocHost(&c->cd_scalars_host, 8*sizeof(int)));
   c->cd_cap = 0; c->cd_pts4 = nullptr; c->cd_round = nullptr; c->cd_splats = nullptr; c->cd_done = nullptr;
   c->jobs_cap = 0; c->jobs_dev = nullptr; c->jobs_host = nullptr;
-  c->stage_cap = 0; c->last_ms = 0;
+  c->desc_cap = 0; c->last_ms = 0;
   return SDV_OK;
 }
 
@@ -139,7 +140,7 @@ void sdv_destroy(sdv_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
   if (c->st_cp) cudaStreamSynchronize(c->st_cp); if (c->st_in) cudaStreamSynchronize(c->st_in); if (c->st) cudaStreamSynchronize(c->st);
-  for (auto& f : c->frames) { cudaFree(f.base); cudaFree(f.I0_own); }
+  for (auto& f : c->frames) { cudaFree(f.base); cudaFree(f.pyr); cudaFree(f.I0_own); }
   for (auto p : c->lvl0_pool) cudaFree(p);
   for (auto& t : c->slots) for (int l=0;l<c->levels;l++) cudaFree(t.pts[l]);
   for (int l=0;l<c->levels;l++) { cudaFree(c->cd_id[l]); cudaFree(c->cd_ws[l]); cudaFree(c->cd_id2[l]); cudaFree(c->cd_ws2[l]); }
@@ -147,7 +148,7 @@ void sdv_destroy(sdv_ctx* c) {
   cudaFree(c->cd_pts4); cudaFree(c->cd_round); cudaFree(c->cd_splats); cudaFree(c->cd_done);
   for (int i=0;i<2;i++) { cudaFree(c->pyr_batch_dev[i]); cudaFreeHost(c->pyr_batch_host[i]); } cudaFree(c->partials); cudaFree(c->ticket); cudaFree(c->totals_dev); cudaFreeHost(c->totals_host);
   cudaFree(c->tc_dev); cudaFree(c->jobs_dev); cudaFreeHost(c->jobs_host);
-  for (int i=0;i<2;i++) { for (auto p : c->stage[i]) cudaFree(p); cudaFree(c->stage_u8[i]); }
+  for (int i=0;i<2;i++) cudaFree(c->stage_u8[i]);
   cudaFree(c->und_buf); cudaFree(c->trace_dev);
   for (int i=0;i<sdv_ctx::kIngRing;i++) if (c->ev_ing[i]) cudaEventDestroy(c->ev_ing[i]); for (int i=0;i<2;i++) if (c->ev_cp[i]) cudaEventDestroy(c->ev_cp[i]); if (c->st_cp) cudaStreamDestroy(c->st_cp);
   cudaFree(c->refine_dev); cudaFreeHost(c->refine_host);
@@ -170,25 +171,23 @@ float sdv_last_kernel_ms(sdv_ctx* c) { return c ? c->last_ms : 0.f; }
 // ------------------------------------------------------------------------------------------------ frames
 static FrameDev* find_frame(sdv_ctx* c, uint64_t id) { auto it = c->frame_index.find(id); return it == c->frame_index.end() ? nullptr : &c->frames[it->second]; }
 
-static int ensure_stage(sdv_ctx* c, int n, int par) {
-  size_t fl = (size_t)c->w*c->h + pyramid_scratch_floats(c->w, c->h, c->levels);
-  while ((int)c->stage[par].size() < n) { float* p = nullptr; CK(cudaMalloc(&p, fl*sizeof(float))); c->stage[par].push_back(p); }
-  if (n > c->stage_cap) {
+static int ensure_desc(sdv_ctx* c, int n) {
+  if (n > c->desc_cap) {
     CK(cudaStreamSynchronize(c->st_in));
     for (int i=0;i<2;i++) { cudaFree(c->pyr_batch_dev[i]); cudaFreeHost(c->pyr_batch_host[i]);
       CK(cudaMalloc(&c->pyr_batch_dev[i], (size_t)n*sizeof(PyrBatchHost) + 16)); CK(cudaMallocHost(&c->pyr_batch_host[i], (size_t)n*sizeof(PyrBatchHost) + 16)); }
-    c->stage_cap = n;
+    c->desc_cap = n;
   }
   return SDV_OK;
 }
 
-static void frame_drop_lvl0(sdv_ctx* c, FrameDev& f) { if (f.lvl0_slot >= 0) { c->lvl0_free.push_back(f.lvl0_slot); f.lvl0_slot = -1; } f.lvl[0] = nullptr; }
+static void frame_drop_texels(sdv_ctx* c, FrameDev& f) { if (f.lvl0_slot >= 0) { c->lvl0_free.push_back(f.lvl0_slot); f.lvl0_slot = -1; } f.lvl[0] = nullptr; f.hi_tex = false; }
 
 // kind bit0: mono8 input, bit1: input already in device memory, bit2: adopt the (device, float) buffer as the frame's level-0 plane,
 // bit3: RAW mono8 input of the camera's native size, rectified through the tables of sdv_set_undistort inside the level-0 kernel.
 // Everything is enqueued on the ingest stream; the compute stream picks it up through ev_in at the next tracker / BA call, so an
-// upload overlaps the tracking of the previous batch.  Level 0 stays a planar intensity image: a pinned-host float upload lands
-// directly in frame storage and only levels >= 1 are built (gradients of level 0 are formed on the fly by the consumers).
+// upload overlaps the tracking of the previous batch.  Every level is a planar intensity image: a pinned-host float upload lands directly in
+// frame storage, levels >= 1 are built by one fused launch, and the consumers form gradients on the fly.
 static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs, const float* exposures, int kind) {
   if (!c || n < 0 || !frames || !imgs) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK;
@@ -197,7 +196,7 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
   // staging buffers + descriptors of this parity were last used by ingest seq-2: it must have drained before the host rewrites the pinned
   // descriptors (the device-side order copy(seq) after pyramid(seq-2) is enforced on the copy stream below)
   if (seq > 2) CK(cudaEventSynchronize(c->ev_ing[(seq-2) % sdv_ctx::kIngRing]));
-  int rc = ensure_stage(c, n, par); if (rc) return rc;
+  int rc = ensure_desc(c, n); if (rc) return rc;
   const bool raw = (kind & 8), u8 = (kind & 1) || raw, dev = (kind & 2), adopt = (kind & 4) && dev && !u8;
   if (raw && !c->has_und) return ctx_fail(c, SDV_ERR_STATE, "raw upload before sdv_set_undistort");
   const size_t px = (size_t)c->w*c->h, px_in = raw ? (size_t)c->und.wOrg*c->und.hOrg : px;     // bytes of one mono8 input image
@@ -205,7 +204,7 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
     c->stage_u8_cap[par] = (size_t)n*px_in; CK(cudaMalloc(&c->stage_u8[par], c->stage_u8_cap[par])); }
   c->cp_dst.clear(); c->cp_src.clear(); c->cp_sz.clear();
   if (c->levels > 1 && ((c->w | c->h) & 1)) return ctx_fail(c, SDV_ERR_ARG, "pyramid needs even image sizes");
-  PyrBatchHost* desc = c->pyr_batch_host[par];
+  PyrBatchHost* desc = c->pyr_batch_host[par]; bool vec = true;
   for (int k=0;k<n;k++) {
     int idx = -1;
     auto it = c->frame_index.find(frames[k]);
@@ -214,15 +213,16 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
     else { for (size_t i=0;i<c->frames.size();i++) if (!c->frames[i].used) { idx = (int)i; break; } }
     if (idx < 0) return ctx_fail(c, SDV_ERR_CAPACITY, "frame pool exhausted (max_frames=%d)", (int)c->frames.size());
     FrameDev& f = c->frames[idx]; f.used = true; f.id = frames[k]; f.exposure = exposures ? exposures[k] : 1.0f; c->frame_index[frames[k]] = idx;
-    frame_drop_lvl0(c, f); f.ingest_seq = seq;
-    f.adopted = adopt; f.I0 = adopt ? const_cast<float*>(reinterpret_cast<const float*>(imgs[k])) : f.I0_own;
+    frame_drop_texels(c, f); f.ingest_seq = seq;
+    f.adopted = adopt; f.I0 = adopt ? const_cast<float*>(reinterpret_cast<const float*>(imgs[k])) : f.I0_own; f.img[0] = f.I0;
     PyrBatchHost& b = desc[k];
-    b.scratch = c->stage[par][k] + px; b.out = f.base; b.I0 = f.I0; b.flags = (f.exposure > 0.f) ? 1 : 0; b.pad = 0;
+    b.pyr = f.pyr; b.I0 = f.I0; b.flags = (f.exposure > 0.f) ? 1 : 0; b.pad = 0;
     if (dev) b.src = imgs[k];
     else if (u8) { unsigned char* d8 = c->stage_u8[par] + (size_t)k*px_in; b.src = d8;
       if (!c->cp_dst.empty() && (unsigned char*)c->cp_src.back() + c->cp_sz.back() == (const unsigned char*)imgs[k] && (unsigned char*)c->cp_dst.back() + c->cp_sz.back() == d8) c->cp_sz.back() += px_in;   // adjacent in host memory: one copy
       else { c->cp_dst.push_back(d8); c->cp_src.push_back(const_cast<void*>(imgs[k])); c->cp_sz.push_back(px_in); } }
     else { b.src = f.I0; c->cp_dst.push_back(f.I0); c->cp_src.push_back(const_cast<void*>(imgs[k])); c->cp_sz.push_back(px*sizeof(float)); }
+    vec = vec && ((uintptr_t)b.src % (u8 ? 4 : 16)) == 0 && ((uintptr_t)b.I0 % 16) == 0;   // 4-pixel vector loads / stores of the pyramid kernel
   }
   if (!c->cp_dst.empty()) {                                               // all H2D copies of the batch in ONE runtime call, on the copy stream: PCIe stays busy while the
     if (seq > 2) CK(cudaStreamWaitEvent(c->st_cp, c->ev_ing[(seq-2) % sdv_ctx::kIngRing], 0));   // previous batch's pyramid runs on st_in
@@ -240,7 +240,7 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
   launch_h2d_words(c->pyr_batch_dev[par], desc, (size_t)n*sizeof(PyrBatchHost), c->st_in);   // kernel copy: a cudaMemcpyAsync here becomes ready only after this batch's bulk copy and
   c->launches += 1;                                                                              // would queue behind the NEXT batch's bulk copy on the H2D engine
   const UndistortDev* und = raw ? &c->und : nullptr;
-  if (c->levels > 1) { launch_pyramid_batch(c->pyr_batch_dev[par], n, u8, c->lvl_off, c->w, c->h, c->levels, c->st_in, und); c->launches += 2*(c->levels - 1); }
+  if (c->levels > 1) { launch_pyramid_batch(c->pyr_batch_dev[par], n, u8, vec, c->w, c->h, c->levels, c->st_in, und); c->launches += 1; }
   else if (u8 || (dev && !adopt)) { launch_pyramid_copy0(c->pyr_batch_dev[par], n, u8, c->w, c->h, c->st_in, und); c->launches += 1; }
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev_ing[seq % sdv_ctx::kIngRing], c->st_in)); c->ingest_seq = seq; c->ingest_pending = true;
@@ -261,8 +261,18 @@ int ensure_lvl0(sdv_ctx* c, FrameDev& f) {        // FrameHessian::dI of a keyfr
   if (c->lvl0_free.empty()) return ctx_fail(c, SDV_ERR_CAPACITY, "keyframe level-0 image pool exhausted (max_kf_images=%d)", (int)c->lvl0_pool.size());
   int rc = join_ingest(c); if (rc) return rc;
   f.lvl0_slot = c->lvl0_free.back(); c->lvl0_free.pop_back(); f.lvl[0] = c->lvl0_pool[f.lvl0_slot];
-  launch_pyramid_level0_texels(f.I0, f.lvl[0], c->w, c->h, c->st); c->launches += 1;
+  launch_grad_texels(f.I0, f.lvl[0], c->w, c->h, c->st); c->launches += 1;
   CK(cudaGetLastError());
+  return SDV_OK;
+}
+int ensure_texels(sdv_ctx* c, FrameDev& f, int lvl) {   // FrameHessian::dIp / absSquaredGrad of levels >= 1 for the selector and read-back, built once per ingest
+  if (lvl == 0) return ensure_lvl0(c, f);
+  if (f.hi_tex) return SDV_OK;
+  int rc = join_ingest_upto(c, f.ingest_seq); if (rc) return rc;        // only the ingest that built this frame: a later batch keeps streaming
+  for (int l=1;l<c->levels;l++) launch_grad_texels(f.img[l], f.lvl[l], c->w>>l, c->h>>l, c->st);
+  c->launches += c->levels - 1;
+  CK(cudaGetLastError());
+  f.hi_tex = true;
   return SDV_OK;
 }
 }
@@ -312,14 +322,14 @@ int sdv_frame_release(sdv_ctx* c, uint64_t frame) { SDV_GUARD_TRK(c);
   if (!c) return SDV_ERR_ARG;
   auto it = c->frame_index.find(frame); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown frame %llu", (unsigned long long)frame);
   if (frame_pinned(c, frame)) return ctx_fail(c, SDV_ERR_STATE, "frame %llu is referenced by a resident BA window / map slot: replace or clear that window / map first", (unsigned long long)frame);
-  FrameDev& f = c->frames[it->second]; f.used = false; frame_drop_lvl0(c, f); f.adopted = false; f.I0 = f.I0_own; c->frame_index.erase(it); return SDV_OK;
+  FrameDev& f = c->frames[it->second]; f.used = false; frame_drop_texels(c, f); f.adopted = false; f.I0 = f.I0_own; f.img[0] = f.I0; c->frame_index.erase(it); return SDV_OK;
 }
 int sdv_frame_download(sdv_ctx* c, uint64_t frame, int lvl, float* dI3_out, float* abs_out) { SDV_GUARD_TRK(c);
   if (!c || lvl < 0 || lvl >= c->levels) return SDV_ERR_ARG;
   CK(cudaSetDevice(c->device));
   FrameDev* f = find_frame(c, frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown frame %llu", (unsigned long long)frame);
   { int rcj = join_ingest(c); if (rcj) return rcj; }
-  if (lvl == 0) { int rc0 = ensure_lvl0(c, *f); if (rc0) return rc0; }
+  { int rct = ensure_texels(c, *f, lvl); if (rct) return rct; }
   int n = (c->w>>lvl)*(c->h>>lvl); float *d3 = nullptr, *da = nullptr;
   if (dI3_out) CK(cudaMalloc(&d3, (size_t)3*n*sizeof(float)));
   if (abs_out) CK(cudaMalloc(&da, (size_t)n*sizeof(float)));
@@ -395,7 +405,7 @@ int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const f
   for (int l=1;l<c->levels;l++) launch_cd_pool(c->cd_id[l-1], c->cd_ws[l-1], c->cd_id[l], c->cd_ws[l], w>>l, h>>l, w>>(l-1), c->st);
   for (int l=0;l<c->levels;l++) {
     launch_cd_dilate(c->cd_id[l], c->cd_ws[l], c->cd_id2[l], c->cd_ws2[l], w>>l, h>>l, l < 2 ? 1 : 0, c->st);
-    launch_cd_compact(c->cd_id2[l], c->cd_ws2[l], l == 0 ? nullptr : f->lvl[l], l == 0 ? f->I0 : nullptr, w>>l, h>>l, c->cd_counts, c->cd_scalars + 1 + l, t.pts[l], t.cap[l], c->st);
+    launch_cd_compact(c->cd_id2[l], c->cd_ws2[l], f->img[l], w>>l, h>>l, c->cd_counts, c->cd_scalars + 1 + l, t.pts[l], t.cap[l], c->st);
   }
   CK(cudaMemcpyAsync(c->cd_scalars_host, c->cd_scalars, 8*sizeof(int), cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st));
@@ -421,7 +431,7 @@ int sdv_tracker_calc_res(sdv_ctx* c, int slot, uint64_t new_frame, int lvl, cons
   { int rcj = join_ingest(c); if (rcj) return rcj; }
   CK(cudaEventRecord(c->ev0, c->st));
   c->launches += 1;
-  launch_coarse_res_gs(t.pts[lvl], t.npts[lvl], lvl == 0 ? nullptr : f->lvl[lvl], lvl == 0 ? f->I0 : nullptr, c->tc.geom[lvl], ep, c->partials, c->ticket, c->totals_dev, c->st);
+  launch_coarse_res_gs(t.pts[lvl], t.npts[lvl], f->img[lvl], c->tc.geom[lvl], ep, c->partials, c->ticket, c->totals_dev, c->st);
   CK(cudaEventRecord(c->ev1, c->st));
   CK(cudaMemcpyAsync(c->totals_host, c->totals_dev, kNAcc*sizeof(double), cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st)); CK(cudaGetLastError());
@@ -455,8 +465,7 @@ int sdv_tracker_track_batch(sdv_ctx* c, int n, const int32_t* slots, const uint6
     if (f->ingest_seq > need_seq) need_seq = f->ingest_seq;
     if (t.ref_frame == ~0ull) return ctx_fail(c, SDV_ERR_STATE, "tracker slot %d has no reference", slots[k]);
     TrackJob& J = c->jobs_host[k]; memset(&J, 0, sizeof(J));
-    J.img0 = f->I0;
-    for (int l=0;l<c->levels;l++) { J.img[l] = (l == 0) ? nullptr : f->lvl[l]; J.pts[l] = t.pts[l]; J.npts[l] = t.npts[l]; }
+    for (int l=0;l<c->levels;l++) { J.img[l] = f->img[l]; J.pts[l] = t.pts[l]; J.npts[l] = t.npts[l]; }
     J.refExposure = t.refExposure; J.newExposure = f->exposure; J.ref_a = t.ref_a; J.ref_b = t.ref_b;
     for (int i=0;i<7;i++) J.T[i] = T_io[7*k+i];
     J.ab[0] = ab_io[2*k]; J.ab[1] = ab_io[2*k+1];

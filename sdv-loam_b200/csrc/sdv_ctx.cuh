@@ -12,8 +12,11 @@ namespace sdv {
 struct FrameDev {                         // one FrameHessian's images on the device
   uint64_t id; float exposure; bool used;
   float* I0; float* I0_own; bool adopted;  // level-0 intensity plane (own storage, or an adopted caller buffer)
-  float4* base; float4* lvl[kLevels];     // packed {I,dx,dy,|grad|^2} texels of levels >= 1 (lvl[0] = lazily built level-0 texels or nullptr)
-  int lvl0_slot;                          // index into the keyframe level-0 texel pool, -1 if not built
+  float* pyr;                             // planar intensity of levels >= 1 (level l at sdv_ctx::lvl_off[l])
+  const float* img[kLevels];              // planar intensity of every level: img[0] = I0, img[l] = pyr + lvl_off[l]
+  // packed {I,dx,dy,|grad|^2} texels: a cache built on demand from the planes (ensure_texels) for the keyframe-rate consumers, dropped by a re-ingest.
+  // lvl[0] is a slot of the keyframe level-0 pool (lvl0_slot, -1 if not built); levels >= 1 live in `base` at lvl_off[l] and are valid while hi_tex is set.
+  float4* base; float4* lvl[kLevels]; int lvl0_slot; bool hi_tex;
   long long ingest_seq;                   // ingest call that (re)built this frame's pyramid
 };
 
@@ -45,7 +48,7 @@ struct sdv_ctx {
   // A pinned frame can be neither released nor re-uploaded (SDV_ERR_STATE) — its pool storage would be handed to another frame under the reader.
   std::unordered_map<uint64_t,int> pins;
   unsigned char* stage_u8[2] = {nullptr, nullptr}; size_t stage_u8_cap[2] = {0, 0};   // contiguous mono8 staging per parity (adjacent host images coalesce into one copy)
-  std::vector<float*> stage[2]; int stage_cap; sdv::PyrBatchHost* pyr_batch_dev[2]; sdv::PyrBatchHost* pyr_batch_host[2];     // double-buffered by ingest parity
+  int desc_cap; sdv::PyrBatchHost* pyr_batch_dev[2]; sdv::PyrBatchHost* pyr_batch_host[2];     // double-buffered by ingest parity
   sdv::UndistortDev und = {}; bool has_und = false; float* und_buf = nullptr;       // sdv_set_undistort: remap tables (+ response / vignette) of the raw-image ingest
   std::vector<float4*> lvl0_pool; std::vector<int> lvl0_free;
   std::vector<void*> cp_dst, cp_src; std::vector<size_t> cp_sz; bool no_batch_copy = false;
@@ -76,6 +79,7 @@ void rp_calib_changed(sdv_ctx* c);             // the Reprojector constants (K, 
 int ctx_fail(sdv_ctx* c, int code, const char* fmt, ...);
 void ba_destroy(sdv_ctx* c);
 int  ensure_lvl0(sdv_ctx* c, FrameDev& f);     // build the packed level-0 texels of a frame on demand (keyframes / read-back)
+int  ensure_texels(sdv_ctx* c, FrameDev& f, int lvl);   // f.lvl[lvl] holds the packed texels of that level afterwards (levels >= 1 are built together)
 inline void frame_pin(sdv_ctx* c, uint64_t id) { c->pins[id]++; }
 inline void frame_unpin(sdv_ctx* c, uint64_t id) { auto it = c->pins.find(id); if (it != c->pins.end() && --it->second <= 0) c->pins.erase(it); }
 inline bool frame_pinned(const sdv_ctx* c, uint64_t id) { return c->pins.find(id) != c->pins.end(); }

@@ -1,8 +1,9 @@
 // sdv_device.cuh — device-side data layout and per-point evaluation shared by the tracker kernels.
 //
 // HBM layout (DESIGN.md §3):
-//   image pyramid level : float4 texel {I, dx, dy, absSquaredGrad}   (reference: AoS Vector3f dIp[lvl] + float absSquaredGrad[lvl],
-//                         HessianBlocks.h:190-204) -> one 16-byte LDG per bilinear tap
+//   image pyramid level : planar float intensity (reference: AoS Vector3f dIp[lvl] + float absSquaredGrad[lvl], HessianBlocks.h:190-204); the consumers
+//                         form the central differences of a bilinear footprint from its 12 planar taps, bit-identically to makeImages.  Packed float4
+//                         {I, dx, dy, absSquaredGrad} texels are a per-frame cache built only for keyframe-rate consumers (selector, BA, read-back).
 //   reference cloud     : float4 point {u, v, idepth, color}         (reference: 4 SoA arrays pc_u/pc_v/pc_idepth/pc_color,
 //                         CoarseTracker.h) -> one coalesced 16-byte LDG per point
 #pragma once
@@ -93,38 +94,13 @@ __device__ __forceinline__ void finalize_gs_warp(const double* tot, double* H /*
 #endif
 
 #if defined(__CUDACC__)
-#ifndef SDV_PREFETCH_MODE
-#define SDV_PREFETCH_MODE 0                // 0 none, 1 prefetch.global.L1, 2 prefetch.global.L2
-#endif
-// Software prefetch of the 2x2 bilinear footprint of a point that will be evaluated one iteration later: repeats the cheap
-// projection (no gather) so the real loads of eval_point hit L1/L2 instead of paying a second dependent HBM round trip.
-__device__ __forceinline__ void prefetch_taps(const float4 p, const LevelGeom& g, const EvalParams& ep, const float4* __restrict__ img) {
-#if SDV_PREFETCH_MODE != 0
-  if (img == nullptr) return;
-  const float x = p.x, y = p.y, id = p.z;
-  float pt0 = ((ep.RKi[0]*x + ep.RKi[1]*y) + ep.RKi[2]*1.0f) + ep.t[0]*id;
-  float pt1 = ((ep.RKi[3]*x + ep.RKi[4]*y) + ep.RKi[5]*1.0f) + ep.t[1]*id;
-  float pt2 = ((ep.RKi[6]*x + ep.RKi[7]*y) + ep.RKi[8]*1.0f) + ep.t[2]*id;
-  float Ku = g.fx*(pt0/pt2) + g.cx, Kv = g.fy*(pt1/pt2) + g.cy;
-  if (!(Ku > 2 && Kv > 2 && Ku < (float)(g.w-3) && Kv < (float)(g.h-3))) return;
-  const float4* bp = img + (int)Ku + (int)Kv*g.w;
-#if SDV_PREFETCH_MODE == 1
-  asm volatile("prefetch.global.L1 [%0];" :: "l"(bp));         asm volatile("prefetch.global.L1 [%0];" :: "l"(bp+1));
-  asm volatile("prefetch.global.L1 [%0];" :: "l"(bp+g.w));     asm volatile("prefetch.global.L1 [%0];" :: "l"(bp+g.w+1));
-#else
-  asm volatile("prefetch.global.L2 [%0];" :: "l"(bp));         asm volatile("prefetch.global.L2 [%0];" :: "l"(bp+1));
-  asm volatile("prefetch.global.L2 [%0];" :: "l"(bp+g.w));     asm volatile("prefetch.global.L2 [%0];" :: "l"(bp+g.w+1));
-#endif
-#endif
-}
-
 // One reference point through calcRes (CoarseTracker.cpp:525-601) and, if it lands in buf_warped_*, through the
 // Jacobian/outer-product of calcGSSSE + Accumulator9::updateSSE_eighted (CoarseTracker.cpp:442-466, MatrixAccumulators.h:1040-1115).
 // Arithmetic order follows the reference expression trees; the TU is compiled with --fmad=false so only the explicit
 // fmaf() of the accumulation contracts.
 __device__ __forceinline__ float grad_guard(float d) { return isfinite(d) ? d : 0.0f; }     // if(!std::isfinite(dx)) dx=0;
 __device__ __forceinline__ void eval_point(const float4 p, int i, const LevelGeom& g, const EvalParams& ep,
-                                           const float4* __restrict__ img, const float* __restrict__ I0, float (&acc)[kNAcc]) {
+                                           const float* __restrict__ I, float (&acc)[kNAcc]) {
   const float x = p.x, y = p.y, id = p.z, refColor = p.w;
   float pt0 = ((ep.RKi[0]*x + ep.RKi[1]*y) + ep.RKi[2]*1.0f) + ep.t[0]*id;
   float pt1 = ((ep.RKi[3]*x + ep.RKi[4]*y) + ep.RKi[5]*1.0f) + ep.t[1]*id;
@@ -154,21 +130,16 @@ __device__ __forceinline__ void eval_point(const float4 p, int i, const LevelGeo
   // getInterpolatedElement33, util/globalFuncs.h:51-65
   int ix = (int)Ku, iy = (int)Kv;
   float dx = Ku - ix, dy = Kv - iy, dxdy = dx*dy;
-  float4 p00, p10, p01, p11;
-  if (I0 != nullptr) {                                      // level 0: planar intensity, gradients formed on the fly exactly like
-    const float* b = I0 + ix + iy*g.w; const int w = g.w;   // makeImages does (HessianBlocks.cpp:147-156; taps never touch rows 0 / h-1)
-    float a_m1_0 = __ldg(b - w),     a_m1_1 = __ldg(b - w + 1);
-    float a_0_m1 = __ldg(b - 1),     a_0_0 = __ldg(b),         a_0_1 = __ldg(b + 1),         a_0_2 = __ldg(b + 2);
-    float a_1_m1 = __ldg(b + w - 1), a_1_0 = __ldg(b + w),     a_1_1 = __ldg(b + w + 1),     a_1_2 = __ldg(b + w + 2);
-    float a_2_0 = __ldg(b + 2*w),    a_2_1 = __ldg(b + 2*w + 1);
-    p00.x = a_0_0; p00.y = grad_guard(0.5f*(a_0_1 - a_0_m1)); p00.z = grad_guard(0.5f*(a_1_0 - a_m1_0));
-    p10.x = a_0_1; p10.y = grad_guard(0.5f*(a_0_2 - a_0_0));  p10.z = grad_guard(0.5f*(a_1_1 - a_m1_1));
-    p01.x = a_1_0; p01.y = grad_guard(0.5f*(a_1_1 - a_1_m1)); p01.z = grad_guard(0.5f*(a_2_0 - a_0_0));
-    p11.x = a_1_1; p11.y = grad_guard(0.5f*(a_1_2 - a_1_0));  p11.z = grad_guard(0.5f*(a_2_1 - a_0_1));
-  } else {
-    const float4* bp = img + ix + iy*g.w;
-    p00 = __ldg(bp); p10 = __ldg(bp+1); p01 = __ldg(bp+g.w); p11 = __ldg(bp+1+g.w);
-  }
+  float4 p00, p10, p01, p11;                                // planar intensity, gradients formed on the fly exactly like makeImages does
+  const float* b = I + ix + iy*g.w; const int w = g.w;      // (HessianBlocks.cpp:147-156; taps never touch rows 0 / h-1)
+  float a_m1_0 = __ldg(b - w),     a_m1_1 = __ldg(b - w + 1);
+  float a_0_m1 = __ldg(b - 1),     a_0_0 = __ldg(b),         a_0_1 = __ldg(b + 1),         a_0_2 = __ldg(b + 2);
+  float a_1_m1 = __ldg(b + w - 1), a_1_0 = __ldg(b + w),     a_1_1 = __ldg(b + w + 1),     a_1_2 = __ldg(b + w + 2);
+  float a_2_0 = __ldg(b + 2*w),    a_2_1 = __ldg(b + 2*w + 1);
+  p00.x = a_0_0; p00.y = grad_guard(0.5f*(a_0_1 - a_0_m1)); p00.z = grad_guard(0.5f*(a_1_0 - a_m1_0));
+  p10.x = a_0_1; p10.y = grad_guard(0.5f*(a_0_2 - a_0_0));  p10.z = grad_guard(0.5f*(a_1_1 - a_m1_1));
+  p01.x = a_1_0; p01.y = grad_guard(0.5f*(a_1_1 - a_1_m1)); p01.z = grad_guard(0.5f*(a_2_0 - a_0_0));
+  p11.x = a_1_1; p11.y = grad_guard(0.5f*(a_1_2 - a_1_0));  p11.z = grad_guard(0.5f*(a_2_1 - a_0_1));
   float w11 = dxdy, w01 = dy-dxdy, w10 = dx-dxdy, w00 = 1-dx-dy+dxdy;
   float hit0 = ((w11*p11.x + w01*p01.x) + w10*p10.x) + w00*p00.x;
   float hit1 = ((w11*p11.y + w01*p01.y) + w10*p10.y) + w00*p00.y;
@@ -210,8 +181,7 @@ struct TrackerRef {                       // one CoarseTracker instance's refere
 };
 
 struct TrackJob {                         // one trackNewestCoarse call
-  const float* img0;                      // newFrame level-0 intensity plane (gradients formed on the fly)
-  const float4* img[kLevels];            // newFrame->dIp[lvl], lvl >= 1 (img[0] unused)
+  const float* img[kLevels];              // newFrame planar intensity of every level (gradients formed on the fly)
   const float4* pts[kLevels]; int npts[kLevels];
   float refExposure, newExposure; double ref_a, ref_b;
   double T[7]; double ab[2];              // in: lastToNew_out / aff_g2l_out initial ; out: result (if not aborted)

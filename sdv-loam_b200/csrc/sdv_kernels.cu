@@ -1,6 +1,6 @@
 // sdv_kernels.cu — hand-written sm_90a (H100) kernels of the tracker path (compiled with --fmad=false; see DESIGN.md §4).
 //
-//   pyr_grad_kernel / pyr_down_kernel      FrameHessian::makeImages           HessianBlocks.cpp:107-167
+//   pyr_fused_kernel / grad_texel_kernel   FrameHessian::makeImages           HessianBlocks.cpp:107-167
 //   coarse_res_gs_kernel                   CoarseTracker::calcRes + calcGSSSE  CoarseTracker.cpp:486-634, 427-484 (one fused pass)
 //   track_cluster_kernel                   CoarseTracker::trackNewestCoarse    CoarseTracker.cpp:662-838 (whole coarse-to-fine LM
 //                                          device-resident: one thread-block cluster per call, DSMEM all-reduce, per-CTA redundant solve)
@@ -28,16 +28,22 @@ static int num_sms() {
 }
 
 // ================================================================================================ pyramid
-// Batched over frames (blockIdx.y = frame of the batch): one launch per level for the whole batch.
-// gradient + pack of one level from a planar intensity image (HessianBlocks.cpp:147-165).  Flat-index neighbours on
-// purpose: at x=0 / x=w-1 the reference reads across the row boundary (idx±1), and so do we.
-struct PyrBatch { const void* src; float* I0; float* scratch; float4* out; int flags; int pad; };   // per frame: level-0 input (float/u8; may equal I0), level-0 plane, planar scratch, base of levels >= 1; flags bit0: photometric response applies (exposure > 0)
+// Every level of a frame is a planar float intensity plane (level 0: the frame's I0; levels >= 1: the frame's `pyr` allocation at lvl_off[l]).
+// Packed {I,dx,dy,|grad|^2} texels are a derived cache that only keyframe-rate consumers build (grad_texel_kernel).
+struct PyrBatch { const void* src; float* I0; float* pyr; int flags; int pad; };   // per frame: level-0 input (float/u8; may equal I0), level-0 plane, planes of levels >= 1; flags bit0: photometric response applies (exposure > 0)
 static_assert(sizeof(PyrBatch) == sizeof(PyrBatchHost), "PyrBatch mirrors PyrBatchHost");
 
 template <typename T> __device__ __forceinline__ float px_load(const T* p, int i);
 template <> __device__ __forceinline__ float px_load<float>(const float* p, int i) { return __ldg(p + i); }
 template <> __device__ __forceinline__ float px_load<unsigned char>(const unsigned char* p, int i) { return (float)__ldg(p + i); }
+template <typename T> __device__ __forceinline__ float4 px_load4(const T* p, int i);         // 4 consecutive pixels, i a multiple of 4 on an aligned plane
+template <> __device__ __forceinline__ float4 px_load4<float>(const float* p, int i) { return __ldg(reinterpret_cast<const float4*>(p + i)); }
+template <> __device__ __forceinline__ float4 px_load4<unsigned char>(const unsigned char* p, int i) {
+  const uchar4 v = __ldg(reinterpret_cast<const uchar4*>(p + i)); return make_float4((float)v.x, (float)v.y, (float)v.z, (float)v.w);
+}
 
+// gradient + pack of one texel of a planar intensity image (HessianBlocks.cpp:147-165).  Flat-index neighbours on purpose: at x=0 / x=w-1 the
+// reference reads across the row boundary (idx±1), and so do we.
 __device__ __forceinline__ float4 grad_texel(const float* __restrict__ I, int idx, int w, int h) {
   float c = __ldg(I + idx); float dx = 0.f, dy = 0.f, ab = 0.f;
   if (idx >= w && idx < w*(h-1)) {
@@ -49,33 +55,10 @@ __device__ __forceinline__ float4 grad_texel(const float* __restrict__ I, int id
   }
   return make_float4(c, dx, dy, ab);
 }
-// packed {I,dx,dy,|grad|^2} texels of one level >= 1 from its planar intensity in scratch
-__global__ void __launch_bounds__(256) pyr_grad_kernel(const PyrBatch* __restrict__ batch, size_t scratch_off, size_t out_off, int w, int h) {
-  const PyrBatch b = batch[blockIdx.y];
-  const float* I = b.scratch + scratch_off; float4* out = b.out + out_off; const int n = w*h;
-  for (int idx = blockIdx.x*blockDim.x + threadIdx.x; idx < n; idx += gridDim.x*blockDim.x) out[idx] = grad_texel(I, idx, w, h);
-}
-// level-0 packed texels on demand (keyframes entering the BA window, debugging read-back)
-__global__ void __launch_bounds__(256) pyr_grad0_kernel(const float* __restrict__ I, float4* __restrict__ out, int w, int h) {
+// packed texels of one level from its planar intensity, on demand (keyframes entering the BA window or the selector, debugging read-back)
+__global__ void __launch_bounds__(256) grad_texel_kernel(const float* __restrict__ I, float4* __restrict__ out, int w, int h) {
   const int n = w*h;
   for (int idx = blockIdx.x*blockDim.x + threadIdx.x; idx < n; idx += gridDim.x*blockDim.x) out[idx] = grad_texel(I, idx, w, h);
-}
-// 2x2 box filter of intensities (HessianBlocks.cpp:137-145): 0.25f*(((a+b)+c)+d).  Level 1 reads the level-0 input (float or mono8) and,
-// when that input is not already the frame's own plane, also materialises the level-0 float plane in the same pass.
-template <typename T>
-__global__ void __launch_bounds__(256) pyr_down_kernel(const PyrBatch* __restrict__ batch, int from_src, size_t src_off, size_t dst_off, int wl, int hl, int wlm1) {
-  const PyrBatch b = batch[blockIdx.y];
-  const T* Iprev = from_src ? reinterpret_cast<const T*>(b.src) : reinterpret_cast<const T*>(b.scratch + src_off);
-  float* I = b.scratch + dst_off;
-  float* I0 = (from_src && reinterpret_cast<const void*>(b.I0) != b.src) ? b.I0 : nullptr;
-  const int n = wl*hl;
-  for (int idx = blockIdx.x*blockDim.x + threadIdx.x; idx < n; idx += gridDim.x*blockDim.x) {
-    int y = idx / wl, x = idx - y*wl;
-    int bi = 2*x + 2*y*wlm1;
-    float a0 = px_load<T>(Iprev, bi), a1 = px_load<T>(Iprev, bi+1), a2 = px_load<T>(Iprev, bi+wlm1), a3 = px_load<T>(Iprev, bi+wlm1+1);
-    I[idx] = 0.25f * (((a0 + a1) + a2) + a3);
-    if (I0) { I0[bi] = a0; I0[bi+1] = a1; I0[bi+wlm1] = a2; I0[bi+wlm1+1] = a3; }
-  }
 }
 
 // Undistort::undistort<unsigned char> (util/Undistort.cpp:341-435) fused with PhotometricUndistorter::processFrame (:177-214): one rectified level-0 pixel from the
@@ -99,45 +82,108 @@ __device__ __forceinline__ float undist_px(const unsigned char* __restrict__ raw
   const float s0 = undist_tap(raw, o, U, photo), s1 = undist_tap(raw, o+1, U, photo), sw = undist_tap(raw, o+U.wOrg, U, photo), sw1 = undist_tap(raw, o+1+U.wOrg, U, photo);
   return xxyy*sw1 + (yy-xxyy)*sw + (xx-xxyy)*s1 + (1-xx-yy+xxyy)*s0;
 }
-// raw ingest, levels > 1: level-0 plane + level 1 in one pass (one thread = one level-1 pixel = a 2x2 quad of rectified pixels)
-__global__ void __launch_bounds__(256) pyr_down_remap_kernel(const PyrBatch* __restrict__ batch, UndistortDev U, size_t dst_off, int wl, int hl, int wlm1) {
-  const PyrBatch b = batch[blockIdx.y];
-  const unsigned char* raw = reinterpret_cast<const unsigned char*>(b.src); const bool photo = (b.flags & 1) && U.G;
-  float* I = b.scratch + dst_off; float* I0 = b.I0;
-  const int n = wl*hl;
-  for (int idx = blockIdx.x*blockDim.x + threadIdx.x; idx < n; idx += gridDim.x*blockDim.x) {
-    int y = idx / wl, x = idx - y*wl;
-    int bi = 2*x + 2*y*wlm1;
-    float a0 = undist_px(raw, bi, U, photo), a1 = undist_px(raw, bi+1, U, photo), a2 = undist_px(raw, bi+wlm1, U, photo), a3 = undist_px(raw, bi+wlm1+1, U, photo);
-    I[idx] = 0.25f * (((a0 + a1) + a2) + a3);
-    *reinterpret_cast<float2*>(I0 + bi) = make_float2(a0, a1); *reinterpret_cast<float2*>(I0 + bi + wlm1) = make_float2(a2, a3);
-  }
-}
 __global__ void __launch_bounds__(256) pyr_remap0_kernel(const PyrBatch* __restrict__ batch, UndistortDev U, int n) {
   const PyrBatch b = batch[blockIdx.y]; const bool photo = (b.flags & 1) && U.G;
   for (int idx = blockIdx.x*blockDim.x + threadIdx.x; idx < n; idx += gridDim.x*blockDim.x) b.I0[idx] = undist_px(reinterpret_cast<const unsigned char*>(b.src), idx, U, photo);
 }
 
-size_t pyramid_scratch_floats(int w, int h, int levels) { size_t n = 0; for (int l = 1; l < levels; l++) n += (size_t)(w>>l)*(h>>l); return n + 4; }
-
-// batch_dev: nframes PyrBatch descriptors in device memory.  src_u8: level-0 input is mono8 (sensor_msgs/Image wire format) instead of float.
-// Requires even w,h whenever levels > 1 (pyrLevelsUsed only halves even sizes, globalCalib.cpp:24).
-void launch_pyramid_batch(const void* batch_dev_v, int nframes, bool src_u8, const size_t* lvl_off, int w, int h, int levels, cudaStream_t st, const UndistortDev* und) {
-  const PyrBatch* batch_dev = reinterpret_cast<const PyrBatch*>(batch_dev_v);
-  if (nframes <= 0) return;
-  size_t soff = 0, prev_soff = 0; int wl = w, hl = h;
-  int cap = (num_sms()*16 + nframes - 1)/nframes; if (cap < 4) cap = 4;
-  for (int l = 0; l + 1 < levels; l++) {
-    int wn = wl>>1, hn = hl>>1; int gn = (wn*hn + 255)/256; if (gn > cap) gn = cap;
-    dim3 g2(gn, nframes);
-    if (l == 0 && und) pyr_down_remap_kernel<<<g2, 256, 0, st>>>(batch_dev, *und, soff, wn, hn, wl);
-    else if (l == 0 && src_u8) pyr_down_kernel<unsigned char><<<g2, 256, 0, st>>>(batch_dev, 1, 0, soff, wn, hn, wl);
-    else pyr_down_kernel<float><<<g2, 256, 0, st>>>(batch_dev, l == 0, prev_soff, soff, wn, hn, wl);
-    pyr_grad_kernel<<<g2, 256, 0, st>>>(batch_dev, soff, lvl_off[l+1], wn, hn);
-    prev_soff = soff; soff += (size_t)wn*hn; wl = wn; hl = hn;
+// The whole pyramid of a frame in one pass (FrameHessian::makeImages, HessianBlocks.cpp:137-145): one CTA per (band of 2^(levels-1) level-0 rows, frame).
+// The CTA reads its band of the level-0 input once, keeps levels 1..levels-2 of the band in shared memory and writes every level >= 1 to the frame's planes.
+// Each pixel is 0.25f*(((a+b)+c)+d) of its 2x2 parent quad in the flat-index layout of the per-level filter (parent row 2y, columns 2x, 2x+1 of a level of
+// width wlm1 at 2x + 2y*wlm1), so odd intermediate sizes drop the last column / row exactly as that filter did; a band past the last row of a coarse level
+// simply has fewer (or no) rows there.  Level 0 comes from a float plane (resident or adopted), mono8, or RAW mono8 through the Undistort tables (RAW),
+// and is written to the frame's I0 plane whenever the input is not that plane already.
+// P = level-1 pixels per work item: 2 reads each parent row as one 16-byte (float) / 4-byte (mono8) vector, 1 reads scalars (unaligned input or w % 4 != 0).
+constexpr int kPyrThreads = 256;
+template <typename T, bool RAW, int P>
+__global__ void __launch_bounds__(kPyrThreads) pyr_fused_kernel(const PyrBatch* __restrict__ batch, UndistortDev U, int w, int h, int levels) {
+  extern __shared__ float pyr_band[];                       // levels 1..levels-2 of the band: [R1][w1] [R1/2][w2] ...
+  const PyrBatch b = batch[blockIdx.y];
+  const T* src = reinterpret_cast<const T*>(b.src);
+  float* I0 = (RAW || reinterpret_cast<const void*>(b.I0) != b.src) ? b.I0 : nullptr;
+  const bool photo = RAW && (b.flags & 1) && U.G;
+  const int R1 = 1 << (levels - 2);                         // level-1 rows per band
+  const int w1 = w >> 1, h1 = h >> 1, y1 = blockIdx.x*R1, n1 = min(R1, h1 - y1);
+  const bool keep = levels > 2;
+  {
+    const int items = w1 / P;
+    for (int k = threadIdx.x; k < n1*items; k += kPyrThreads) {
+      const int rr = k / items, x = (k - rr*items)*P, y = y1 + rr;
+      const int bi = 2*x + 2*y*w;
+      float t[2*P], u[2*P];                                 // parent rows 2y and 2y+1, columns 2x .. 2x+2P-1
+      if constexpr (RAW) {
+#pragma unroll
+        for (int j = 0; j < 2*P; j++) { t[j] = undist_px(reinterpret_cast<const unsigned char*>(src), bi + j, U, photo); u[j] = undist_px(reinterpret_cast<const unsigned char*>(src), bi + w + j, U, photo); }
+      } else if constexpr (P == 2) {
+        const float4 a = px_load4<T>(src, bi), c = px_load4<T>(src, bi + w);
+        t[0] = a.x; t[1] = a.y; t[2] = a.z; t[3] = a.w; u[0] = c.x; u[1] = c.y; u[2] = c.z; u[3] = c.w;
+      } else {
+#pragma unroll
+        for (int j = 0; j < 2*P; j++) { t[j] = px_load<T>(src, bi + j); u[j] = px_load<T>(src, bi + w + j); }
+      }
+      float v[P];
+#pragma unroll
+      for (int j = 0; j < P; j++) v[j] = 0.25f * (((t[2*j] + t[2*j+1]) + u[2*j]) + u[2*j+1]);
+      if constexpr (P == 2) {
+        *reinterpret_cast<float2*>(b.pyr + y*w1 + x) = make_float2(v[0], v[1]);
+        if (keep) *reinterpret_cast<float2*>(pyr_band + rr*w1 + x) = make_float2(v[0], v[1]);
+      } else {
+        b.pyr[y*w1 + x] = v[0];
+        if (keep) pyr_band[rr*w1 + x] = v[0];
+      }
+      if (I0) {
+        if constexpr (P == 2) { *reinterpret_cast<float4*>(I0 + bi) = make_float4(t[0], t[1], t[2], t[3]); *reinterpret_cast<float4*>(I0 + bi + w) = make_float4(u[0], u[1], u[2], u[3]); }
+        else {
+#pragma unroll
+          for (int j = 0; j < 2*P; j++) { I0[bi + j] = t[j]; I0[bi + w + j] = u[j]; }
+        }
+      }
+    }
+  }
+  const float* prev = pyr_band; float* cur = pyr_band + (size_t)R1*w1;
+  int wp = w1, hp = h1; size_t off = (size_t)w1*h1;
+  for (int l = 2; l < levels; l++) {
+    __syncthreads();
+    const int wl = wp >> 1, hl = hp >> 1, Rl = R1 >> (l - 1), yl = blockIdx.x*Rl, nl = min(Rl, hl - yl);
+    const bool keep_l = l + 1 < levels;
+    float* out = b.pyr + off;
+    for (int k = threadIdx.x; k < nl*wl; k += kPyrThreads) {
+      const int rr = k / wl, x = k - rr*wl;
+      const float* s = prev + 2*rr*wp + 2*x;                // band-local parent rows 2rr, 2rr+1
+      const float v = 0.25f * (((s[0] + s[1]) + s[wp]) + s[wp+1]);
+      out[(size_t)(yl + rr)*wl + x] = v;
+      if (keep_l) cur[rr*wl + x] = v;
+    }
+    prev = cur; cur += (size_t)Rl*wl; off += (size_t)wl*hl; wp = wl; hp = hl;
   }
 }
-// levels == 1 or odd sizes: the level-0 plane still has to be materialised from a foreign / mono8 source
+static size_t pyr_band_bytes(int w, int levels) {
+  size_t n = 0; const int R1 = 1 << (levels - 2);
+  for (int l = 1; l + 1 < levels; l++) n += (size_t)(R1 >> (l - 1))*(w >> l);
+  return n*sizeof(float);
+}
+template <typename T, bool RAW, int P>
+static void launch_pyr_fused(const PyrBatch* batch_dev, int nframes, int w, int h, int levels, const UndistortDev& U, cudaStream_t st) {
+  const size_t smem = pyr_band_bytes(w, levels);
+  if (smem > 48*1024) cudaFuncSetAttribute(pyr_fused_kernel<T, RAW, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);   // very wide images; a refusal surfaces as the launch error
+  const int R1 = 1 << (levels - 2);
+  dim3 g(((h >> 1) + R1 - 1)/R1, nframes);
+  pyr_fused_kernel<T, RAW, P><<<g, kPyrThreads, smem, st>>>(batch_dev, U, w, h, levels);
+}
+
+// batch_dev: nframes PyrBatch descriptors in device memory.  src_u8: level-0 input is mono8 (sensor_msgs/Image wire format) instead of float.
+// vec: every level-0 input (and I0 plane written) of the batch is 16-byte aligned; the 4-pixel vector path additionally needs w % 4 == 0.
+// Requires even w,h whenever levels > 1 (pyrLevelsUsed only halves even sizes, globalCalib.cpp:24).
+void launch_pyramid_batch(const void* batch_dev_v, int nframes, bool src_u8, bool vec, int w, int h, int levels, cudaStream_t st, const UndistortDev* und) {
+  const PyrBatch* batch_dev = reinterpret_cast<const PyrBatch*>(batch_dev_v);
+  if (nframes <= 0 || levels < 2) return;
+  const UndistortDev U = und ? *und : UndistortDev{};
+  vec = vec && (w % 4 == 0);
+  if (und) launch_pyr_fused<unsigned char, true, 1>(batch_dev, nframes, w, h, levels, U, st);
+  else if (src_u8) { if (vec) launch_pyr_fused<unsigned char, false, 2>(batch_dev, nframes, w, h, levels, U, st); else launch_pyr_fused<unsigned char, false, 1>(batch_dev, nframes, w, h, levels, U, st); }
+  else             { if (vec) launch_pyr_fused<float, false, 2>(batch_dev, nframes, w, h, levels, U, st);         else launch_pyr_fused<float, false, 1>(batch_dev, nframes, w, h, levels, U, st); }
+}
+// levels == 1: the level-0 plane still has to be materialised from a foreign / mono8 source
 template <typename T> __global__ void pyr_copy0_kernel(const PyrBatch* __restrict__ batch, int n) {
   const PyrBatch b = batch[blockIdx.y]; if (reinterpret_cast<const void*>(b.I0) == b.src) return;
   for (int idx = blockIdx.x*blockDim.x + threadIdx.x; idx < n; idx += gridDim.x*blockDim.x) b.I0[idx] = px_load<T>(reinterpret_cast<const T*>(b.src), idx);
@@ -148,9 +194,9 @@ void launch_pyramid_copy0(const void* batch_dev_v, int nframes, bool src_u8, int
   if (und) pyr_remap0_kernel<<<g, 256, 0, st>>>(batch_dev, *und, w*h);
   else if (src_u8) pyr_copy0_kernel<unsigned char><<<g, 256, 0, st>>>(batch_dev, w*h); else pyr_copy0_kernel<float><<<g, 256, 0, st>>>(batch_dev, w*h);
 }
-void launch_pyramid_level0_texels(const float* I0, float4* out, int w, int h, cudaStream_t st) {
+void launch_grad_texels(const float* I, float4* out, int w, int h, cudaStream_t st) {
   int n = w*h; int grid = (n + 255)/256; if (grid > num_sms()*16) grid = num_sms()*16;
-  pyr_grad0_kernel<<<grid, 256, 0, st>>>(I0, out, w, h);
+  grad_texel_kernel<<<grid, 256, 0, st>>>(I, out, w, h);
 }
 
 __global__ void unpack_level_kernel(const float4* __restrict__ in, float* dI3, float* ab, int n) {
@@ -188,7 +234,7 @@ __device__ __forceinline__ void block_reduce_acc(const float (&acc)[kNAcc], floa
 // grid-stride over the reference cloud; per-block partials -> global; the last block to finish (ticket) sums the block
 // partials in block order and writes the 51 totals.  One launch per calcRes.
 template <int THREADS>
-__global__ void __launch_bounds__(THREADS) coarse_res_gs_kernel(const float4* __restrict__ pts, int n, const float4* __restrict__ img, const float* __restrict__ I0,
+__global__ void __launch_bounds__(THREADS) coarse_res_gs_kernel(const float4* __restrict__ pts, int n, const float* __restrict__ I,
                                                                LevelGeom g, EvalParams ep, double* __restrict__ partials,
                                                                unsigned int* __restrict__ ticket, double* __restrict__ totals) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -203,11 +249,9 @@ __global__ void __launch_bounds__(THREADS) coarse_res_gs_kernel(const float4* __
     const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
     float4 pc = (i < n) ? __ldg(pts + i) : zero4;
     float4 pn = (i + stride < n) ? __ldg(pts + i + stride) : zero4;
-    if (i < n) prefetch_taps(pc, g, ep, img);
     for (; i < n; i += stride) {
       const float4 pn2 = (i + 2*stride < n) ? __ldg(pts + i + 2*stride) : zero4;
-      if (i + stride < n) prefetch_taps(pn, g, ep, img);
-      eval_point(pc, i, g, ep, img, I0, acc);
+      eval_point(pc, i, g, ep, I, acc);
       pc = pn; pn = pn2;
     }
   }
@@ -229,244 +273,27 @@ __global__ void __launch_bounds__(THREADS) coarse_res_gs_kernel(const float4* __
 
 constexpr int kStepThreads = 256;
 int step_kernel_max_grid() { return num_sms()*4; }
-void launch_coarse_res_gs(const float4* pts, int n, const float4* img, const float* I0, const LevelGeom& g, const EvalParams& ep,
+void launch_coarse_res_gs(const float4* pts, int n, const float* I, const LevelGeom& g, const EvalParams& ep,
                           double* partials, unsigned int* ticket, double* totals, cudaStream_t st) {
   size_t smem = (size_t)kNAcc*kStepThreads*sizeof(float);                // opt-in size set per device by kernels_init_device()
   int grid = (n + kStepThreads - 1)/kStepThreads; if (grid < 1) grid = 1; if (grid > step_kernel_max_grid()) grid = step_kernel_max_grid();
-  coarse_res_gs_kernel<kStepThreads><<<grid, kStepThreads, smem, st>>>(pts, n, img, I0, g, ep, partials, ticket, totals);
+  coarse_res_gs_kernel<kStepThreads><<<grid, kStepThreads, smem, st>>>(pts, n, I, g, ep, partials, ticket, totals);
 }
 
 // ================================================================================================ device-resident LM
-struct Ctl {                               // per-CTA copy of the LM state (every CTA of the cluster computes it redundantly and identically)
-  SE3d cur; double a_cur, b_cur;           // refToNew_current, aff_g2l_current
-  SE3d cand; double a_cand, b_cand;        // refToNew_new, aff_g2l_new
-  double H[64], b[8];
-  double resOld[6], resNew[6];
-  double lastRes[5], flow[3];
-  float lambda;
-  int flag;
-  EvalParams ep;
-};
-
 constexpr int kMaxCluster = 16;
 
-// THREADS x MINB chosen so that several jobs are resident per SM: one job's (single-warp, latency-bound) LM control step
-// overlaps the point sweeps of the others.  <128,4> is the batched-throughput configuration (cluster size 1);
-// <256,1> with a cluster of 8-16 CTAs is the low-latency single-sequence configuration.
-template <int THREADS, int MINB>
-__global__ void __launch_bounds__(THREADS, MINB) track_cluster_v1_kernel(TrackJob* __restrict__ jobs, const TrackConst* __restrict__ tc_g) {
-  cg::cluster_group cluster = cg::this_cluster();
-  const int C = (int)cluster.num_blocks();
-  const int rank = (int)cluster.block_rank();
-  const int tid = threadIdx.x;
-  TrackJob& J = jobs[blockIdx.x / C];
-
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  float*  red    = reinterpret_cast<float*>(smem_raw);                                   // [kNAcc][THREADS]
-  double* gather = reinterpret_cast<double*>(smem_raw + (size_t)kNAcc*THREADS*sizeof(float)); // [2][kMaxCluster][kNAcc]
-  double* bsum   = gather + 2*kMaxCluster*kNAcc;                                           // [kNAcc]
-  double* tot    = bsum + kNAcc;                                                           // [kNAcc]
-  __shared__ Ctl ctl;
-  __shared__ TrackConst tc;
-  for (int i = tid; i < (int)(sizeof(TrackConst)/4); i += THREADS) reinterpret_cast<int*>(&tc)[i] = reinterpret_cast<const int*>(tc_g)[i];
-  if (tid == 0) {
-    ctl.cur = se3_from7(J.T); ctl.a_cur = J.ab[0]; ctl.b_cur = J.ab[1];
-    for (int i = 0; i < 5; i++) ctl.lastRes[i] = nan("");
-    for (int i = 0; i < 3; i++) ctl.flow[i] = 1000.0;
-  }
-  // NOTE: keep these statistics as per-thread local arrays.  Moving them to shared memory changed ptxas' allocation under the
-  // 128-register cap (a spill in the sweep) and cost a large share of the kernel's throughput.
-  long long evals[kLevels]; int iters[kLevels], accs[kLevels];
-#pragma unroll
-  for (int i = 0; i < kLevels; i++) { evals[i] = 0; iters[i] = 0; accs[i] = 0; }
-  __syncthreads();
-  if (C > 1) cluster.sync();                                // every CTA of the cluster must be running before the first distributed-shared-memory write (racecheck)
-
-  int evalCount = 0;
-  // all threads: evaluate the residual + GN system at ctl.ep for level `lvl`; totals (identical in every CTA) land in tot[]
-  auto eval = [&](int lvl) {
-    float acc[kNAcc];
-#pragma unroll
-    for (int k = 0; k < kNAcc; k++) acc[k] = 0.f;
-    const float4* __restrict__ pts = J.pts[lvl]; const int n = J.npts[lvl];
-    const float4* __restrict__ img = (lvl == 0) ? nullptr : J.img[lvl]; const float* __restrict__ I0 = (lvl == 0) ? J.img0 : nullptr;
-    const LevelGeom& g = tc.geom[lvl];
-    {                                                      // 3-deep software pipeline: point k+2 in flight, taps of k+1 prefetched, k evaluated
-      const int stride = C*THREADS; int i = rank*THREADS + tid;
-      const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      float4 pc = (i < n) ? __ldg(pts + i) : zero4;
-      float4 pn = (i + stride < n) ? __ldg(pts + i + stride) : zero4;
-      if (i < n) prefetch_taps(pc, g, ctl.ep, img);
-      for (; i < n; i += stride) {
-        const float4 pn2 = (i + 2*stride < n) ? __ldg(pts + i + 2*stride) : zero4;
-        if (i + stride < n) prefetch_taps(pn, g, ctl.ep, img);
-        eval_point(pc, i, g, ctl.ep, img, I0, acc);
-        pc = pn; pn = pn2;
-      }
-    }
-    block_reduce_acc<THREADS>(acc, red, bsum);
-    if (C > 1) {
-      const int buf = evalCount & 1;
-      for (int k = tid; k < kNAcc*C; k += THREADS) {
-        int r = k / kNAcc, e = k - r*kNAcc;
-        double* dst = cluster.map_shared_rank(gather, r);
-        dst[(buf*kMaxCluster + rank)*kNAcc + e] = bsum[e];
-      }
-      cluster.sync();
-      if (tid < kNAcc) { double s = 0; for (int r = 0; r < C; r++) s += gather[(buf*kMaxCluster + r)*kNAcc + tid]; tot[tid] = s; }
-    } else {
-      if (tid < kNAcc) tot[tid] = bsum[tid];
-    }
-    __syncthreads();
-    evalCount++; evals[lvl] += n;
-  };
-
-  const int maxIterations[5] = {10,20,50,50,50};           // CoarseTracker.cpp:679
-  const float lambdaExtrapolationLimit = 0.001f;            // :680
-  bool haveRepeated = false, aborted = false;
-  for (int lvl = J.coarsest; lvl >= 0; lvl--) {
-    float levelCutoffRepeat = 1;
-    if (tid == 0) make_eval_params(ctl.cur, ctl.a_cur, ctl.b_cur, J.refExposure, J.newExposure, J.ref_a, J.ref_b, tc.geom[lvl], lvl,
-                                   tc.coarseCutoffTH*levelCutoffRepeat, tc.huberTH, ctl.ep);
-    __syncthreads();
-    eval(lvl);
-    if (tid == 0) { finalize_res(tot, ctl.resOld); ctl.flag = (ctl.resOld[5] > 0.6 && levelCutoffRepeat < 50); }
-    __syncthreads();
-    while (ctl.flag) {                                      // :694-701
-      levelCutoffRepeat *= 2;
-      __syncthreads();
-      if (tid == 0) make_eval_params(ctl.cur, ctl.a_cur, ctl.b_cur, J.refExposure, J.newExposure, J.ref_a, J.ref_b, tc.geom[lvl], lvl,
-                                     tc.coarseCutoffTH*levelCutoffRepeat, tc.huberTH, ctl.ep);
-      __syncthreads();
-      eval(lvl);
-      if (tid == 0) { finalize_res(tot, ctl.resOld); ctl.flag = (ctl.resOld[5] > 0.6 && levelCutoffRepeat < 50); }
-      __syncthreads();
-    }
-    if (tid == 0) { finalize_gs(tot, ctl.H, ctl.b); ctl.lambda = 0.01f; }
-
-    for (int iteration = 0; iteration < maxIterations[lvl]; iteration++) {
-      iters[lvl]++;
-      double incn = 0;
-      if (tid < 32) {                                        // warp 0: propose the LM step (CoarseTracker.cpp:722-765)
-        __syncwarp();                                        // ctl.H / ctl.b / ctl.lambda were written by lane 0 (finalize_gs) — order them before the other lanes' reads (racecheck)
-        const int r = tid & 7;
-        const float lambda = ctl.lambda;
-        const bool fixA = tc.affineOptModeA < 0, fixB = tc.affineOptModeB < 0;
-        const int nv = (!fixA && !fixB) ? 8 : ((fixA && fixB) ? 6 : 7);
-        const bool stitch = fixA && !fixB;                   // fix a only: b takes slot 6 (:736-748)
-        const int rr = (stitch && r == 6) ? 7 : r;
-        double a[8];
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-          const int cc = (stitch && j == 6) ? 7 : j;
-          double hv = ctl.H[rr*8 + cc];
-          if (rr == cc) hv *= (1 + lambda);
-          a[j] = (r < nv && j < nv) ? hv : ((r == j) ? 1.0 : 0.0);
-        }
-        double rhs = (r < nv) ? -ctl.b[rr] : 0.0;
-        const double x = warp_ldlt_solve8(a, rhs);
-        double inc[8];
-#pragma unroll
-        for (int j = 0; j < 8; j++) inc[j] = __shfl_sync(0xffffffffu, x, j, 8);
-        if (fixA && fixB) { inc[6] = 0; inc[7] = 0; }
-        else if (!fixA && fixB) { inc[7] = 0; }
-        else if (stitch) { inc[7] = inc[6]; inc[6] = 0; }
-        float extrapFac = 1;
-        if (lambda < lambdaExtrapolationLimit) extrapFac = sqrtf(sqrtf(lambdaExtrapolationLimit / lambda));
-#pragma unroll
-        for (int i = 0; i < 8; i++) inc[i] *= extrapFac;
-        double incScaled[8];
-#pragma unroll
-        for (int i = 0; i < 3; i++) incScaled[i] = inc[i]*1.0f;        // SCALE_XI_ROT   (:755)
-#pragma unroll
-        for (int i = 3; i < 6; i++) incScaled[i] = inc[i]*0.5f;        // SCALE_XI_TRANS (:756)
-        incScaled[6] = inc[6]*10.0f; incScaled[7] = inc[7]*1000.0f;    // SCALE_A, SCALE_B
-        double s = 0;
-#pragma unroll
-        for (int i = 0; i < 8; i++) s += incScaled[i];
-        if (!isfinite(s)) {
-#pragma unroll
-          for (int i = 0; i < 8; i++) incScaled[i] = 0;
-        }
-        const SE3d cand = se3_mul(se3_exp(incScaled), ctl.cur);
-        const double a_cand = ctl.a_cur + incScaled[6], b_cand = ctl.b_cur + incScaled[7];
-        EvalParams ep;
-        make_eval_params(cand, a_cand, b_cand, J.refExposure, J.newExposure, J.ref_a, J.ref_b, tc.geom[lvl], lvl,
-                         tc.coarseCutoffTH*levelCutoffRepeat, tc.huberTH, ep);
-#pragma unroll
-        for (int i = 0; i < 8; i++) incn += inc[i]*inc[i];
-        incn = sqrt(incn);
-        __syncwarp();
-        if (tid == 0) { ctl.cand = cand; ctl.a_cand = a_cand; ctl.b_cand = b_cand; ctl.ep = ep; }
-      }
-      __syncthreads();
-      eval(lvl);
-      if (tid == 0) {
-        finalize_res(tot, ctl.resNew);
-        bool accept = (ctl.resNew[0]/ctl.resNew[1]) < (ctl.resOld[0]/ctl.resOld[1]);
-        if (accept) {
-          finalize_gs(tot, ctl.H, ctl.b);
-          for (int i = 0; i < 6; i++) ctl.resOld[i] = ctl.resNew[i];
-          ctl.cur = ctl.cand; ctl.a_cur = ctl.a_cand; ctl.b_cur = ctl.b_cand;
-          ctl.lambda *= 0.5f;
-        } else {
-          ctl.lambda *= 4;
-          if (ctl.lambda < lambdaExtrapolationLimit) ctl.lambda = lambdaExtrapolationLimit;
-        }
-        ctl.flag = (accept ? 1 : 0) | ((!(incn > 1e-3)) ? 2 : 0);
-      }
-      __syncthreads();
-      const int f = ctl.flag;
-      __syncthreads();
-      if (f & 1) accs[lvl]++;
-      if (f & 2) break;
-    }
-    if (tid == 0) {
-      ctl.lastRes[lvl] = sqrtf((float)(ctl.resOld[0]/ctl.resOld[1]));
-      ctl.flow[0] = ctl.resOld[2]; ctl.flow[1] = ctl.resOld[3]; ctl.flow[2] = ctl.resOld[4];
-      ctl.flag = (ctl.lastRes[lvl] > 1.5*J.minRes[lvl]) ? 1 : 0;
-    }
-    __syncthreads();
-    const int ab = ctl.flag;
-    __syncthreads();
-    if (ab) { aborted = true; break; }
-    if (levelCutoffRepeat > 1 && !haveRepeated) { lvl++; haveRepeated = true; }
-  }
-
-  if (rank == 0 && tid == 0) {
-    int good = 0;
-    if (!aborted) {
-      se3_to7(ctl.cur, J.T);
-      double a_out = ctl.a_cur, b_out = ctl.b_cur;
-      good = 1;
-      if ((tc.affineOptModeA != 0 && (fabsf((float)a_out) > 1.2f)) || (tc.affineOptModeB != 0 && (fabsf((float)b_out) > 200))) good = 0;
-      if (good) {
-        double rel[2]; aff_from_to(J.refExposure, J.newExposure, J.ref_a, J.ref_b, a_out, b_out, rel);
-        float r0 = (float)rel[0], r1 = (float)rel[1];
-        if ((tc.affineOptModeA == 0 && (fabsf(logf(r0)) > 1.5f)) || (tc.affineOptModeB == 0 && (fabsf(r1) > 200))) good = 0;
-        if (good) { if (tc.affineOptModeA < 0) a_out = 0; if (tc.affineOptModeB < 0) b_out = 0; }
-      }
-      J.ab[0] = a_out; J.ab[1] = b_out;
-    }
-    J.good = good;
-    for (int i = 0; i < 5; i++) J.lastRes[i] = ctl.lastRes[i];
-    for (int i = 0; i < 3; i++) J.flow[i] = ctl.flow[i];
-    for (int i = 0; i < kLevels; i++) { J.point_evals[i] = evals[i]; J.iterations[i] = iters[i]; J.accepts[i] = accs[i]; }
-  }
-  if (C > 1) cluster.sync();                                // keep every CTA's shared memory alive until all remote writes/reads are done
-}
-
-
-// ================================================================================================ device-resident LM, asynchronous data path (round 2)
-// Same algorithm and the same point -> thread mapping and summation order as track_cluster_v1_kernel (results are bit-identical), but no
-// load ever stalls a warp on HBM:
+// ================================================================================================ device-resident LM
+// One trackNewestCoarse per cluster of CTAs, the whole coarse-to-fine LM on the device.  THREADS x MINB is chosen so that several jobs are resident per SM:
+// one job's (single-warp, latency-bound) LM control step overlaps the point sweeps of the others.  <128,4> is the batched-throughput configuration
+// (cluster size 1); <256,1> with a cluster of 8-16 CTAs is the low-latency single-sequence configuration.  No load ever stalls a warp on HBM:
 //   * the reference cloud streams through shared memory in chunks: one elected thread issues cp.async.bulk (TMA bulk copy, SASS UBLKCP) per
 //     2 KB block of float4 points, completion is signalled on an mbarrier (expect_tx), two chunks in flight;
-//   * the bilinear footprint of point k+1 is gathered by per-thread cp.async (SASS LDGSTS) into a private shared-memory slot while point k
-//     is accumulated — the gather needs no registers and is complete one full iteration later;
+//   * the 12-tap planar footprint of point k+1 (bilinear 2x2 plus the neighbours its central differences need) is gathered by per-thread cp.async
+//     (SASS LDGSTS) into a private shared-memory slot while point k is accumulated — the gather needs no registers and is complete one full iteration later;
 //   * the level-0 flow indicators (every 32nd point, CoarseTracker.cpp:538-566) are a dense pre-pass (all lanes busy) instead of a divergent branch
 //     that cost one lane's 6 divisions per warp iteration;
-//   * the LM control flow is a state machine around ONE instance of the sweep (a third of the code size of v1).
+//   * the LM control flow is a state machine around ONE instance of the sweep.
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_u32(bar)), "r"(count) : "memory"); }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
@@ -488,7 +315,6 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                :: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void cp_async16(uint32_t s, const void* g) { asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" :: "r"(s), "l"(g) : "memory"); }
 __device__ __forceinline__ void cp_async4(uint32_t s, const void* g)  { asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" :: "r"(s), "l"(g) : "memory"); }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait1()  { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
@@ -496,9 +322,10 @@ __device__ __forceinline__ void cp_async_wait0()  { asm volatile("cp.async.wait_
 
 struct PtState { float u, v, nid, dx, dy, col; bool ok; };     // what the accumulate stage needs of a projected point (its taps are in the thread's smem slot)
 
-// calcRes, first half (CoarseTracker.cpp:525-575): projection + bounds, then launch the gather of the 2x2 (level 0: 12-tap) footprint into `slot`.
-template <int THREADS, bool LVL0>
-__device__ __forceinline__ PtState stage_project(const float4 p, const LevelGeom& g, const EvalParams& ep, const float4* __restrict__ img, const float* __restrict__ I0, uint32_t slot) {
+// calcRes, first half (CoarseTracker.cpp:525-575): projection + bounds, then launch the gather of the 12-tap planar footprint into `slot`.
+constexpr int kTaps = 12;
+template <int THREADS>
+__device__ __forceinline__ PtState stage_project(const float4 p, const LevelGeom& g, const EvalParams& ep, const float* __restrict__ I, uint32_t slot) {
   PtState s; const float x = p.x, y = p.y, id = p.z; s.col = p.w;
   float pt0 = ((ep.RKi[0]*x + ep.RKi[1]*y) + ep.RKi[2]*1.0f) + ep.t[0]*id;
   float pt1 = ((ep.RKi[3]*x + ep.RKi[4]*y) + ep.RKi[5]*1.0f) + ep.t[1]*id;
@@ -511,38 +338,28 @@ __device__ __forceinline__ PtState stage_project(const float4 p, const LevelGeom
   if (s.ok) {
     const int ix = (int)Ku, iy = (int)Kv, w = g.w;
     s.dx = Ku - ix; s.dy = Kv - iy;
-    if (LVL0) {                                             // planar intensity: rows -1..2 (gradients are formed in stage_accumulate exactly like makeImages does)
-      const float* b = I0 + ix + iy*w;
-      cp_async4(slot + 0*THREADS*4, b - w);       cp_async4(slot + 1*THREADS*4, b - w + 1);
-      cp_async4(slot + 2*THREADS*4, b - 1);       cp_async4(slot + 3*THREADS*4, b);         cp_async4(slot + 4*THREADS*4, b + 1);     cp_async4(slot + 5*THREADS*4, b + 2);
-      cp_async4(slot + 6*THREADS*4, b + w - 1);   cp_async4(slot + 7*THREADS*4, b + w);     cp_async4(slot + 8*THREADS*4, b + w + 1); cp_async4(slot + 9*THREADS*4, b + w + 2);
-      cp_async4(slot + 10*THREADS*4, b + 2*w);    cp_async4(slot + 11*THREADS*4, b + 2*w + 1);
-    } else {
-      const float4* bp = img + ix + iy*w;
-      cp_async16(slot + 0*THREADS*16, bp); cp_async16(slot + 1*THREADS*16, bp + 1); cp_async16(slot + 2*THREADS*16, bp + w); cp_async16(slot + 3*THREADS*16, bp + w + 1);
-    }
+    const float* b = I + ix + iy*w;                         // rows -1..2 (gradients are formed in stage_accumulate exactly like makeImages does)
+    cp_async4(slot + 0*THREADS*4, b - w);       cp_async4(slot + 1*THREADS*4, b - w + 1);
+    cp_async4(slot + 2*THREADS*4, b - 1);       cp_async4(slot + 3*THREADS*4, b);         cp_async4(slot + 4*THREADS*4, b + 1);     cp_async4(slot + 5*THREADS*4, b + 2);
+    cp_async4(slot + 6*THREADS*4, b + w - 1);   cp_async4(slot + 7*THREADS*4, b + w);     cp_async4(slot + 8*THREADS*4, b + w + 1); cp_async4(slot + 9*THREADS*4, b + w + 2);
+    cp_async4(slot + 10*THREADS*4, b + 2*w);    cp_async4(slot + 11*THREADS*4, b + 2*w + 1);
   }
   return s;
 }
 // calcRes second half + calcGSSSE for one point whose taps have landed (CoarseTracker.cpp:576-601, 442-466).  Expression trees identical to eval_point.
-template <int THREADS, bool LVL0>
-__device__ __forceinline__ void stage_accumulate(const PtState s, const LevelGeom& g, const EvalParams& ep, const unsigned char* slot, float (&acc)[kNAcc]) {
+template <int THREADS>
+__device__ __forceinline__ void stage_accumulate(const PtState s, const LevelGeom& g, const EvalParams& ep, const float* slot, float (&acc)[kNAcc]) {
   if (!s.ok) return;
   float4 p00, p10, p01, p11;
-  if (LVL0) {
-    const float* t = reinterpret_cast<const float*>(slot);
-    float a_m1_0 = t[0*THREADS], a_m1_1 = t[1*THREADS];
-    float a_0_m1 = t[2*THREADS], a_0_0 = t[3*THREADS], a_0_1 = t[4*THREADS], a_0_2 = t[5*THREADS];
-    float a_1_m1 = t[6*THREADS], a_1_0 = t[7*THREADS], a_1_1 = t[8*THREADS], a_1_2 = t[9*THREADS];
-    float a_2_0 = t[10*THREADS], a_2_1 = t[11*THREADS];
-    p00.x = a_0_0; p00.y = grad_guard(0.5f*(a_0_1 - a_0_m1)); p00.z = grad_guard(0.5f*(a_1_0 - a_m1_0));
-    p10.x = a_0_1; p10.y = grad_guard(0.5f*(a_0_2 - a_0_0));  p10.z = grad_guard(0.5f*(a_1_1 - a_m1_1));
-    p01.x = a_1_0; p01.y = grad_guard(0.5f*(a_1_1 - a_1_m1)); p01.z = grad_guard(0.5f*(a_2_0 - a_0_0));
-    p11.x = a_1_1; p11.y = grad_guard(0.5f*(a_1_2 - a_1_0));  p11.z = grad_guard(0.5f*(a_2_1 - a_0_1));
-  } else {
-    const float4* t = reinterpret_cast<const float4*>(slot);
-    p00 = t[0*THREADS]; p10 = t[1*THREADS]; p01 = t[2*THREADS]; p11 = t[3*THREADS];
-  }
+  const float* t = slot;
+  float a_m1_0 = t[0*THREADS], a_m1_1 = t[1*THREADS];
+  float a_0_m1 = t[2*THREADS], a_0_0 = t[3*THREADS], a_0_1 = t[4*THREADS], a_0_2 = t[5*THREADS];
+  float a_1_m1 = t[6*THREADS], a_1_0 = t[7*THREADS], a_1_1 = t[8*THREADS], a_1_2 = t[9*THREADS];
+  float a_2_0 = t[10*THREADS], a_2_1 = t[11*THREADS];
+  p00.x = a_0_0; p00.y = grad_guard(0.5f*(a_0_1 - a_0_m1)); p00.z = grad_guard(0.5f*(a_1_0 - a_m1_0));
+  p10.x = a_0_1; p10.y = grad_guard(0.5f*(a_0_2 - a_0_0));  p10.z = grad_guard(0.5f*(a_1_1 - a_m1_1));
+  p01.x = a_1_0; p01.y = grad_guard(0.5f*(a_1_1 - a_1_m1)); p01.z = grad_guard(0.5f*(a_2_0 - a_0_0));
+  p11.x = a_1_1; p11.y = grad_guard(0.5f*(a_1_2 - a_1_0));  p11.z = grad_guard(0.5f*(a_2_1 - a_0_1));
   const float dx = s.dx, dy = s.dy, dxdy = dx*dy, u = s.u, v = s.v, new_idepth = s.nid, refColor = s.col;
   float w11 = dxdy, w01 = dy-dxdy, w10 = dx-dxdy, w00 = 1-dx-dy+dxdy;
   float hit0 = ((w11*p11.x + w01*p01.x) + w10*p10.x) + w00*p00.x;
@@ -645,10 +462,10 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
     for (unsigned k = 0; k < wave; k++) __nanosleep(stagger_ns);
   }
 
-  // dynamic smem: [ tap ring 2 x 4 x THREADS x 16 B | point chunks 2 x kPtChunk x THREADS x 16 B ] aliased by the reduction scratch [kNAcc][THREADS] floats,
+  // dynamic smem: [ tap ring 2 x kTaps x THREADS x 4 B | point chunks 2 x kPtChunk x THREADS x 16 B ] aliased by the reduction scratch [kNAcc][THREADS] floats,
   // then the DSMEM gather buffers and the reduced sums
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  constexpr size_t kRingBytes = (size_t)2*4*THREADS*16, kPtsBytes = (size_t)2*kPtChunk*THREADS*16, kRedBytes = (size_t)kNAcc*THREADS*sizeof(float);
+  constexpr size_t kRingBytes = (size_t)2*kTaps*THREADS*4, kPtsBytes = (size_t)2*kPtChunk*THREADS*16, kRedBytes = (size_t)kNAcc*THREADS*sizeof(float);
   constexpr size_t kStageBytes = (kRingBytes + kPtsBytes) > kRedBytes ? (kRingBytes + kPtsBytes) : kRedBytes;
   unsigned char* ring = smem_raw;
   float4* pbuf   = reinterpret_cast<float4*>(smem_raw + kRingBytes);
@@ -678,9 +495,8 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
   int evalCount = 0;
   uint32_t bar_phase = 0;                                   // bit b = parity the next wait on full_bar[b] expects
   const int stride = C*THREADS;
-  const uint32_t slot_base = smem_u32(ring) + tid*16;       // level >= 1: [slot][tap][tid] float4 ; level 0 reuses the bytes as [slot][tap 0..11][tid] float
-  const uint32_t slot_base0 = smem_u32(ring) + tid*4;
-  constexpr uint32_t kSlotStride = 4*THREADS*16;
+  const uint32_t slot_base = smem_u32(ring) + tid*4;        // [slot][tap 0..11][tid] float
+  constexpr uint32_t kSlotStride = kTaps*THREADS*4;
 
   while (true) {
     const int lvl = ctl.lvl; int n_eval = 0;
@@ -690,7 +506,7 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
     for (int k = 0; k < kNAcc; k++) acc[k] = 0.f;
     {
       const float4* __restrict__ pts = J.pts[lvl]; const int n = J.npts[lvl];
-      const float4* __restrict__ img = (lvl == 0) ? nullptr : J.img[lvl]; const float* __restrict__ I0 = J.img0;
+      const float* __restrict__ I = J.img[lvl];
       const LevelGeom& g = tc.geom[lvl];
       const int K = (n + stride - 1)/stride;                // sweep iterations (uniform over the CTA)
       const int NC = (K + kPtChunk - 1)/kPtChunk;           // point chunks
@@ -725,7 +541,7 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
           const float4 p = pbuf[(((m/kPtChunk) & 1)*kPtChunk + (m % kPtChunk))*THREADS + tid];
 #endif
           const uint32_t so = (uint32_t)(m & 1)*kSlotStride;
-          s = (lvl == 0) ? stage_project<THREADS, true>(p, g, ctl.ep, img, I0, slot_base0 + so) : stage_project<THREADS, false>(p, g, ctl.ep, img, I0, slot_base + so);
+          s = stage_project<THREADS>(p, g, ctl.ep, I, slot_base + so);
         }
         return s;
       };
@@ -753,9 +569,7 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
         }
         cp_async_commit();
         cp_async_wait1();                                   // the gather of iteration k (committed one iteration ago) has landed in this thread's slot
-        const unsigned char* slot = ring + (size_t)(k & 1)*kSlotStride;
-        if (lvl == 0) stage_accumulate<THREADS, true>(sC, g, ctl.ep, slot + tid*4, acc);
-        else          stage_accumulate<THREADS, false>(sC, g, ctl.ep, slot + tid*16, acc);
+        stage_accumulate<THREADS>(sC, g, ctl.ep, reinterpret_cast<const float*>(ring + (size_t)(k & 1)*kSlotStride) + tid, acc);
       }
       SDV_PROF_T(tp4); SDV_PROF_ADD(3, tp3, tp4);
       cp_async_wait0();
@@ -933,15 +747,10 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
 }
 
 template <int THREADS>
-static size_t track_kernel_smem_v2(int cluster_size = kMaxCluster) {
-  size_t stage = (size_t)2*4*THREADS*16 + (size_t)2*kPtChunk*THREADS*16, red = (size_t)kNAcc*THREADS*sizeof(float);
+static size_t track_kernel_smem(int cluster_size = kMaxCluster) {
+  size_t stage = (size_t)2*kTaps*THREADS*4 + (size_t)2*kPtChunk*THREADS*16, red = (size_t)kNAcc*THREADS*sizeof(float);
   return (stage > red ? stage : red) + (size_t)(2*cluster_size*kNAcc + 2*kNAcc)*sizeof(double);
 }
-
-template <int THREADS>
-static size_t track_kernel_smem() { return (size_t)kNAcc*THREADS*sizeof(float) + (size_t)(2*kMaxCluster*kNAcc + 2*kNAcc)*sizeof(double); }
-
-static bool track_use_v1() { static int v = -1; if (v < 0) { const char* e = getenv("SDV_TRACK_IMPL"); v = (e && e[0] == 'v' && e[1] == '1') ? 1 : 0; } return v == 1; }
 
 static unsigned track_stagger_ns() { static long v = -1; if (v < 0) { const char* e = getenv("SDV_TRACK_STAGGER_NS"); v = e ? atol(e) : SDV_TRACK_STAGGER_DEFAULT_NS; if (v < 0) v = 0; } return (unsigned)v; }
 template <typename Kern, typename... Extra>
@@ -955,10 +764,9 @@ static cudaError_t launch_track_kern(Kern kern, size_t smem, int threads, TrackJ
 }
 template <int THREADS, int MINB>
 static cudaError_t launch_track_t(TrackJob* jobs_dev, int njobs, const TrackConst* tc_dev, int cluster_size, cudaStream_t st) {
-  if (track_use_v1()) return launch_track_kern(track_cluster_v1_kernel<THREADS, MINB>, track_kernel_smem<THREADS>(), THREADS, jobs_dev, njobs, tc_dev, cluster_size, st);
   // stagger only when the grid fills the co-resident slots of the chip (otherwise there is nothing to desynchronise)
   const unsigned stag = (cluster_size == 1 && njobs > num_sms()) ? track_stagger_ns() : 0u;
-  return launch_track_kern(track_cluster_kernel<THREADS, MINB>, track_kernel_smem_v2<THREADS>(cluster_size), THREADS, jobs_dev, njobs, tc_dev, cluster_size, st, stag);
+  return launch_track_kern(track_cluster_kernel<THREADS, MINB>, track_kernel_smem<THREADS>(cluster_size), THREADS, jobs_dev, njobs, tc_dev, cluster_size, st, stag);
 }
 template <typename Kern>
 static cudaError_t track_attrs(Kern kern, size_t smem) {
@@ -967,7 +775,7 @@ static cudaError_t track_attrs(Kern kern, size_t smem) {
 }
 // threads: 128 (throughput, 4 jobs resident per SM) or 256 (latency)
 #ifndef SDV_TRACK_MINB
-#define SDV_TRACK_MINB 4                    // H100: 4 (128 regs, 80 B spilled) 2.57 ms per 1 056 jobs against 3 (160 regs, no spills) 2.93 ms; DESIGN.md §6
+#define SDV_TRACK_MINB 4                    // H100: 4 (128 regs, 80 B spilled at the time) 2.57 ms per 1 056 jobs against 3 (160 regs, no spills) 2.93 ms; DESIGN.md §6
 #endif
 cudaError_t launch_track_cluster(TrackJob* jobs_dev, int njobs, const TrackConst* tc_dev, int cluster_size, int threads, cudaStream_t st) {
   if (threads == 256) return launch_track_t<256, 1>(jobs_dev, njobs, tc_dev, cluster_size, st);
@@ -981,8 +789,7 @@ cudaError_t kernels_init_device() {
   cudaError_t e = cudaFuncSetAttribute(coarse_res_gs_kernel<kStepThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)kNAcc*kStepThreads*sizeof(float)));
   if (e != cudaSuccess) return e;
 #define SDV_TRACK_ATTRS(T, M) \
-  if ((e = track_attrs(track_cluster_v1_kernel<T, M>, track_kernel_smem<T>())) != cudaSuccess) return e; \
-  if ((e = track_attrs(track_cluster_kernel<T, M>, track_kernel_smem_v2<T>())) != cudaSuccess) return e;
+  if ((e = track_attrs(track_cluster_kernel<T, M>, track_kernel_smem<T>())) != cudaSuccess) return e;
   SDV_TRACK_ATTRS(256, 1) SDV_TRACK_ATTRS(64, 8) SDV_TRACK_ATTRS(128, SDV_TRACK_MINB)
 #undef SDV_TRACK_ATTRS
   return cudaSuccess;
@@ -1059,17 +866,17 @@ __global__ void cd_dilate_kernel(const float* __restrict__ id_in, const float* _
 }
 // (d) normalise + raster-order compaction (:378-423): block counts -> exclusive scan -> scatter
 constexpr int kScanThreads = 256, kScanItems = 4;            // 1024 pixels per block, contiguous per thread
-__device__ __forceinline__ bool cd_valid(const float* id, const float* ws, const float4* ref, const float* ref0, int i, int w, int h, float& idn, float& col) {
+__device__ __forceinline__ bool cd_valid(const float* id, const float* ws, const float* ref, int i, int w, int h, float& idn, float& col) {
   int y = i / w, x = i - y*w;
   if (x < 2 || x >= w-2 || y < 2 || y >= h-2) return false;
   if (!(ws[i] > 0)) return false;
-  idn = id[i] / ws[i]; col = ref0 ? ref0[i] : ref[i].x;
+  idn = id[i] / ws[i]; col = ref[i];
   return isfinite(col) && (idn > 0);
 }
-__global__ void __launch_bounds__(kScanThreads) cd_count_kernel(const float* __restrict__ id, const float* __restrict__ ws, const float4* __restrict__ ref, const float* __restrict__ ref0, int w, int h, int* blockCounts) {
+__global__ void __launch_bounds__(kScanThreads) cd_count_kernel(const float* __restrict__ id, const float* __restrict__ ws, const float* __restrict__ ref, int w, int h, int* blockCounts) {
   __shared__ int s[kScanThreads/32];
   int base = (blockIdx.x*kScanThreads + threadIdx.x)*kScanItems; int c = 0, n = w*h;
-  for (int j = 0; j < kScanItems; j++) { int i = base + j; float a, b; if (i < n && cd_valid(id, ws, ref, ref0, i, w, h, a, b)) c++; }
+  for (int j = 0; j < kScanItems; j++) { int i = base + j; float a, b; if (i < n && cd_valid(id, ws, ref, i, w, h, a, b)) c++; }
   for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
   if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = c;
   __syncthreads();
@@ -1092,12 +899,12 @@ __global__ void cd_scan_kernel(int* blockCounts, int nblocks, int* total) {   //
   }
   if (threadIdx.x == 0) *total = carry;
 }
-__global__ void __launch_bounds__(kScanThreads) cd_emit_kernel(const float* __restrict__ id, const float* __restrict__ ws, const float4* __restrict__ ref, const float* __restrict__ ref0, int w, int h,
+__global__ void __launch_bounds__(kScanThreads) cd_emit_kernel(const float* __restrict__ id, const float* __restrict__ ws, const float* __restrict__ ref, int w, int h,
                                                               const int* __restrict__ blockOffsets, float4* out, int cap) {
   __shared__ int s[kScanThreads/32];
   int base = (blockIdx.x*kScanThreads + threadIdx.x)*kScanItems; int n = w*h;
   float idn[kScanItems], col[kScanItems]; bool ok[kScanItems]; int c = 0;
-  for (int j = 0; j < kScanItems; j++) { int i = base + j; ok[j] = (i < n) && cd_valid(id, ws, ref, ref0, i, w, h, idn[j], col[j]); c += ok[j]; }
+  for (int j = 0; j < kScanItems; j++) { int i = base + j; ok[j] = (i < n) && cd_valid(id, ws, ref, i, w, h, idn[j], col[j]); c += ok[j]; }
   int lane = threadIdx.x & 31, warp = threadIdx.x >> 5; int incl = c;
   for (int o = 1; o < 32; o <<= 1) { int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
   if (lane == 31) s[warp] = incl;
@@ -1126,11 +933,11 @@ void launch_cd_pool(const float* id_lm, const float* ws_lm, float* id_l, float* 
 void launch_cd_dilate(const float* id_in, const float* bak, float* id_out, float* ws_out, int w, int h, int diag, cudaStream_t st) {
   cd_dilate_kernel<<<(w*h+255)/256, 256, 0, st>>>(id_in, bak, id_out, ws_out, w, h, diag);
 }
-void launch_cd_compact(const float* id, const float* ws, const float4* ref, const float* ref0, int w, int h, int* blockCounts, int* total, float4* out, int cap, cudaStream_t st) {
+void launch_cd_compact(const float* id, const float* ws, const float* ref, int w, int h, int* blockCounts, int* total, float4* out, int cap, cudaStream_t st) {
   int nb = cd_num_blocks(w, h);
-  cd_count_kernel<<<nb, kScanThreads, 0, st>>>(id, ws, ref, ref0, w, h, blockCounts);
+  cd_count_kernel<<<nb, kScanThreads, 0, st>>>(id, ws, ref, w, h, blockCounts);
   cd_scan_kernel<<<1, 1024, 0, st>>>(blockCounts, nb, total);
-  cd_emit_kernel<<<nb, kScanThreads, 0, st>>>(id, ws, ref, ref0, w, h, blockCounts, out, cap);
+  cd_emit_kernel<<<nb, kScanThreads, 0, st>>>(id, ws, ref, w, h, blockCounts, out, cap);
 }
 
 __global__ void pack_cloud_kernel(const float* u, const float* v, const float* id, const float* col, int n, float4* out) {

@@ -5,19 +5,19 @@
 namespace sdv {
 
 // pyramid (FrameHessian::makeImages, HessianBlocks.cpp:107-167)
-struct PyrBatchHost { const void* src; float* I0; float* scratch; float4* out; int flags; int pad; };   // mirrors PyrBatch in sdv_kernels.cu
+struct PyrBatchHost { const void* src; float* I0; float* pyr; int flags; int pad; };   // mirrors PyrBatch in sdv_kernels.cu
 // geometric + photometric undistortion tables of the ingest (util/Undistort.cpp): device pointers; G / vignette may be null
 struct UndistortDev { const float* remapX; const float* remapY; const float* G; const float* vignette; int wOrg, hOrg; float factor; };
-size_t pyramid_scratch_floats(int w, int h, int levels);
-void launch_pyramid_batch(const void* batch_dev, int nframes, bool src_u8, const size_t* lvl_off, int w, int h, int levels, cudaStream_t st, const UndistortDev* und = nullptr);
+// all planes of levels >= 1 in one launch (levels > 1; `pyr` of a frame holds level l at lvl_off[l], the offsets of the context); vec: 16-byte aligned inputs / I0
+void launch_pyramid_batch(const void* batch_dev, int nframes, bool src_u8, bool vec, int w, int h, int levels, cudaStream_t st, const UndistortDev* und = nullptr);
 void launch_pyramid_copy0(const void* batch_dev, int nframes, bool src_u8, int w, int h, cudaStream_t st, const UndistortDev* und = nullptr);
-void launch_pyramid_level0_texels(const float* I0, float4* out, int w, int h, cudaStream_t st);
+void launch_grad_texels(const float* I, float4* out, int w, int h, cudaStream_t st);   // packed {I,dx,dy,|grad|^2} texels of one planar level
 void launch_unpack_level(const float4* in, float* dI3, float* ab, int n, cudaStream_t st);
 
 cudaError_t kernels_init_device();        // per-device function attributes of the tracker kernels (called by sdv_create after cudaSetDevice)
 // fused calcRes + calcGSSSE, one launch (CoarseTracker.cpp:486-634, 427-484)
 int  step_kernel_max_grid();
-void launch_coarse_res_gs(const float4* pts, int n, const float4* img, const float* I0, const LevelGeom& g, const EvalParams& ep,
+void launch_coarse_res_gs(const float4* pts, int n, const float* I, const LevelGeom& g, const EvalParams& ep,
                           double* partials, unsigned int* ticket, double* totals, cudaStream_t st);
 
 // device-resident trackNewestCoarse (CoarseTracker.cpp:662-838): njobs clusters of cluster_size CTAs
@@ -32,7 +32,7 @@ void launch_cd_prep(const float* pts4, const int* round_half, int n, int w, floa
 void launch_cd_round(const float4* splats, int n, int* done, int* owner, float* idepth, float* ws, int* remaining, cudaStream_t st);
 void launch_cd_pool(const float* id_lm, const float* ws_lm, float* id_l, float* ws_l, int wl, int hl, int wlm1, cudaStream_t st);
 void launch_cd_dilate(const float* id_in, const float* bak, float* id_out, float* ws_out, int w, int h, int diag, cudaStream_t st);
-void launch_cd_compact(const float* id, const float* ws, const float4* ref, const float* ref0, int w, int h, int* blockCounts, int* total, float4* out, int cap, cudaStream_t st);
+void launch_cd_compact(const float* id, const float* ws, const float* ref, int w, int h, int* blockCounts, int* total, float4* out, int cap, cudaStream_t st);
 void launch_pack_cloud(const float* u, const float* v, const float* id, const float* col, int n, float4* out, cudaStream_t st);
 
 } // namespace sdv

@@ -28,7 +28,7 @@ struct MapDev {                           // device-resident map of one sequence
   int nH, nP; double hostT[kRpMaxHosts][7]; const float* hostI0[kRpMaxHosts]; const sdv_map_pt* pts;
 };
 struct RpJob {
-  const MapDev* map; const float* curI0; const float4* curLvl[kLevels]; double curT[7], curTinv[7];
+  const MapDev* map; const float* cur[kLevels]; double curT[7], curTinv[7];
   float affLL[kRpMaxHosts][2]; int frame_rank[kRpMaxHosts];
   int cur_kf_index, backup, nH, nP; long long pt_off; int error;
 };
@@ -120,7 +120,7 @@ constexpr int kRpWarps = 4;
 #define RP_MATCH_MINB 6
 #endif
 
-__device__ __forceinline__ float cur_pixel(const RpJob& jb, int level, int idx) { return level == 0 ? __ldg(jb.curI0 + idx) : __ldg(&jb.curLvl[level][idx]).x; }
+__device__ __forceinline__ float cur_pixel(const RpJob& jb, int level, int idx) { return __ldg(jb.cur[level] + idx); }
 
 __device__ bool find_match_direct(const RpJob& jb, const RpConst& C, const sdv_map_pt& pt, double2& px_io, RpWarpSmem& sm, const int lane, const double* __restrict__ xf) {
   const MapDev* __restrict__ m = jb.map;
@@ -373,7 +373,7 @@ static int rp_launch(sdv_ctx* c, int n_jobs, const int32_t* slots, const uint64_
     const MapSlot& m = st->maps[slots[k]]; RpJob& j = J[k]; memset(&j, 0, sizeof(j));
     auto it = c->frame_index.find(cur_frames[k]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "reproject job %d: unknown target frame", k);
     const FrameDev& f = c->frames[it->second];
-    j.map = m.dev; j.curI0 = f.I0; for (int l=0;l<c->levels;l++) j.curLvl[l] = (l == 0) ? nullptr : f.lvl[l];
+    j.map = m.dev; for (int l=0;l<c->levels;l++) j.cur[l] = f.img[l];
     for (int i=0;i<7;i++) j.curT[i] = cur_T7[7*k+i];
     const SE3d cur = se3_from7(j.curT); se3_to7(se3_inv(cur), j.curTinv);
     j.cur_kf_index = cur_kf_index ? cur_kf_index[k] : -1; j.backup = backup ? backup[k] : 0; j.nH = m.nH; j.nP = m.nP; j.pt_off = off; off += m.nP;

@@ -23,10 +23,12 @@ void sel_destroy(sdv_ctx* c) {
   for (auto& sl : s->slots) if (sl.mapD) cudaFree(sl.mapD);
   s->eng.io.release(); s->aux.release(); s->eng.destroy(); delete s; c->sel = nullptr;
 }
-static int sel_frame(sdv_ctx* c, uint64_t id, sel::FrameImg& F, long long& need_seq, const char* who) {
+static int sel_frame(sdv_ctx* c, uint64_t id, sel::FrameImg& F, long long& need_seq, const char* who, bool texels = true) {
   auto it = c->frame_index.find(id); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "%s: unknown frame %llu", who, (unsigned long long)id);
-  const FrameDev& f = c->frames[it->second]; if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
-  F.I0 = f.I0; F.L1 = f.lvl[1]; F.L2 = f.lvl[2]; return SDV_OK;
+  FrameDev& f = c->frames[it->second]; if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
+  F.I0 = f.I0; F.L1 = nullptr; F.L2 = nullptr;
+  if (texels) { int rc = ensure_texels(c, f, 1); if (rc) return rc; F.L1 = f.lvl[1]; F.L2 = f.lvl[2]; }   // |grad|^2 of levels 1 and 2 (makeMaps / makeNewTraces read the packed texels)
+  return SDV_OK;
 }
 static int sel_fail(sdv_ctx* c, SelState* s, int rc, const char* who) { return ctx_fail(c, rc == -2 ? SDV_ERR_CAPACITY : SDV_ERR_CUDA, "%s: %s", who, s->eng.err.c_str()); }
 }  // namespace sdv
@@ -67,7 +69,7 @@ int sdv_selector_get_map(sdv_ctx* c, int slot, uint8_t* out) { SDV_GUARD_TRK(c);
 int sdv_selector_make_hists(sdv_ctx* c, uint64_t frame, float* ths_out, float* thsSmoothed_out) { SDV_GUARD_TRK(c);
   if (!c) return SDV_ERR_ARG; SEL_STATE("selector_make_hists");
   CK(cudaSetDevice(c->device));
-  sel::FrameImg F; long long need = 0; { int rc = sel_frame(c, frame, F, need, "selector_make_hists"); if (rc) return rc; }
+  sel::FrameImg F; long long need = 0; { int rc = sel_frame(c, frame, F, need, "selector_make_hists", false); if (rc) return rc; }
   { int rc = join_ingest_upto(c, need); if (rc) return rc; }
   const size_t tf = s->eng.ths_floats(); if (s->aux.reserve(2*sel::Scratch::need(tf, 4), c->st)) return ctx_fail(c, SDV_ERR_CUDA, "selector_make_hists: scratch");
   s->aux.reset(); float* a = s->aux.take<float>(tf); float* b = s->aux.take<float>(tf);
