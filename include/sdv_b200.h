@@ -63,9 +63,16 @@ int  sdv_sync(sdv_ctx* c);                                   /* drain the contex
  * thread, FullSystem::mapMutex) on one side, every other entry (tracking thread, trackMutex) on the other.  Each side is serialised internally and runs on its own
  * stream; calls of the same side from several threads are serialised by the library. */
 /* CoarseTracker::makeK(CalibHessian*) (CoarseTracker.cpp:77-106) and the CalibHessian Reprojector::reprojectMap reads (Reprojector.cpp:117-124): the bundle
- * adjustment optimises the intrinsics at every keyframe, and setCoarseTrackingRef re-derives the tracker's per-level K from them.  Replaces the calibration given
- * to sdv_create for every later tracker / reprojection / structPoseEstimation call of this context (the BA windows carry their own: sdv_ba_set_window). */
+ * adjustment optimises the intrinsics at every keyframe, and setCoarseTrackingRef re-derives the tracker's per-level K from them.  Replaces the context
+ * calibration given to sdv_create: the default K of every later tracker / reprojection / structPoseEstimation call on a slot that has no K of its own
+ * (sdv_set_calib_slots; the BA windows carry their own: sdv_ba_set_window).  Stream-ordered after the work already enqueued. */
 int  sdv_set_calib(sdv_ctx* c, const sdv_calib* K);
+/* CoarseTracker::makeK(CalibHessian*) per tracker instance (CoarseTracker.cpp:77-106): slot slots[i] uses K[i] from now on, for its tracker (calc_res, track,
+ * track_batch, the trackNewCoarse policy) and for the map slot of the same index (reprojection, structPoseEstimation, refine).  One context can so hold
+ * sequences of different cameras (same image size; rectified uploads) and follow each sequence's bundle adjustment.  K == NULL: those slots follow the context
+ * calibration again.  A slot's own K is kept across sdv_set_calib, sdv_tracker_set_ref, sdv_map_set and sdv_map_clear.  All-or-nothing: a bad slot or K
+ * (fx, fy <= 0 or not finite; cx, cy not finite) returns SDV_ERR_ARG and changes no slot.  Stream-ordered after the work already enqueued, like sdv_set_calib. */
+int  sdv_set_calib_slots(sdv_ctx* c, int n, const int32_t* slots, const sdv_calib* K);
 
 /* ---- frames: FrameHessian::makeImages(float* color, CalibHessian*)  FullSystem/HessianBlocks.cpp:107-167 ------------
  * builds the pyramid on the device, keyed by a caller-chosen handle: level 0 is kept as the planar intensity image (its {dx,dy} are
@@ -95,7 +102,7 @@ int  sdv_frame_release(sdv_ctx* c, uint64_t frame);
 /* test hook: copy one level back as AoS {I,dx,dy} (w*h*3 floats) and absSquaredGrad (w*h floats); either may be NULL */
 int  sdv_frame_download(sdv_ctx* c, uint64_t frame, int lvl, float* dI3_out, float* abs_out);
 
-/* ---- tracker reference: CoarseTracker::makeK :77-106 is folded into sdv_create ------------------------------------
+/* ---- tracker reference: CoarseTracker::makeK :77-106 is sdv_create / sdv_set_calib (context) and sdv_set_calib_slots (per instance) -----------
  * CoarseTracker::setCoarseTrackingRef / setCTRefForFirstFrame  CoarseTracker.cpp:636-660 -> makeCoarseDepthL0 :258-425.
  * The PointHessian graph walk (:264-294) stays on the host: the caller passes one row per splat, {u,v,idepth,HdiF},
  * with round_half[i]=0 for `int(u)` (newest-KF sensor points, :270-271) or 1 for `int(u+0.5f)` (:116-117, :285-286). */
@@ -171,6 +178,10 @@ int  sdv_tracker_struct_pose(sdv_ctx* c, int n, const sdv_overlap_pt* pts, int n
                              float* res, int* iterations, int* accepts);
 int  sdv_tracker_struct_pose_batch(sdv_ctx* c, int n_jobs, const int32_t* pt_begin, const sdv_overlap_pt* pts, const int32_t* host_begin,
                                    const double* host_T7, double* curToWorld_io, float* res, int32_t* iterations, int32_t* accepts);
+/* the same with the K of the tracker slot each job belongs to (structPoseEstimation is a CoarseTracker member, CoarseTracker.cpp:949-1007);
+ * slots == NULL is sdv_tracker_struct_pose_batch (every job on the context calibration). */
+int  sdv_tracker_struct_pose_batch_slots(sdv_ctx* c, int n_jobs, const int32_t* slots, const int32_t* pt_begin, const sdv_overlap_pt* pts, const int32_t* host_begin,
+                                         const double* host_T7, double* curToWorld_io, float* res, int32_t* iterations, int32_t* accepts);
 /* ---- fused per-frame refinement (the tail of FullSystem::trackNewCoarse, FullSystem.cpp:482-488): reprojectMap(fh) -> structPoseEstimation
  * without leaving the device.  curToWorld_io: fh->shell->camToWorld from the photometric tracker in, refined pose out; cur_ab = the tracked
  * aff_g2l.  n_matches = overlap_pts.size(), res/iterations/accepts as in sdv_tracker_struct_pose_batch. */

@@ -77,8 +77,8 @@ int shim_set_undistort(const Undistort* u, const float* G256_or_null, const floa
 int shim_ingest_raw(FrameShell* shell, const uint8_t* raw_mono8, float exposure) {
   uint64_t id = (uint64_t)shell->id; return sdv_frame_upload_batch_raw_u8(gpu, 1, &id, &raw_mono8, &exposure);
 }
-// §3c CoarseTracker::makeK (CoarseTracker.cpp:77-106)
-int shim_makeK(CalibHessian* HCalib) { sdv_calib K{HCalib->fxl(), HCalib->fyl(), HCalib->cxl(), HCalib->cyl()}; return sdv_set_calib(gpu, &K); }
+// §3c CoarseTracker::makeK (CoarseTracker.cpp:77-106): a member of each tracker instance, so it sets the K of that instance's slot only
+int shim_makeK(int slot, CalibHessian* HCalib) { sdv_calib K{HCalib->fxl(), HCalib->fyl(), HCalib->cxl(), HCalib->cyl()}; const int32_t s = slot; return sdv_set_calib_slots(gpu, 1, &s, &K); }
 
 // ------------------------------------------------------------------------------------------------ CoarseTracker (CoarseTracker.cpp:649-660, 662-838)
 struct CoarseTracker {
@@ -262,7 +262,7 @@ int shim_activateSelect(const ActivationInputs& in, std::vector<int32_t>& decisi
 // referenced so that -Wunused does not hide a missing call path
 int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const Undistort* u, const uint8_t* raw) {
   std::vector<int32_t> sel, st; Vec5 mr{}; SE3 T; AffLight a;
-  int rc = shim_create(hc) | shim_set_undistort(u, nullptr, nullptr) | shim_ingest_raw(fh->shell, raw, 1.0f) | shim_makeK(&hc);
+  int rc = shim_create(hc) | shim_set_undistort(u, nullptr, nullptr) | shim_ingest_raw(fh->shell, raw, 1.0f) | shim_makeK(fs.coarseTracker->slot, &hc);
   fs.coarseTracker->setCoarseTrackingRef(fs.frameHessians); fs.coarseTracker->trackNewestCoarse(fh, T, a, 3, mr, nullptr);
   std::vector<ImmaturePoint*> imm; std::vector<HostImmatures> hi; rc |= shim_makeNewTraces(fh, sel, imm) | shim_traceNewCoarse(fh, hi);
   std::vector<ActivationGroup> ag; std::vector<float> idp; rc |= shim_activatePoints(ag, st, idp, sel, 7);

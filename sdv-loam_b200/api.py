@@ -55,6 +55,7 @@ def _load():
     L.sdv_pyr_levels.argtypes = [C.c_int, C.c_int]
     L.sdv_sync.argtypes = [_vp]
     L.sdv_set_calib.argtypes = [_vp, C.POINTER(sdv_calib)]
+    L.sdv_set_calib_slots.argtypes = [_vp, C.c_int, _i32p, _vp]
     L.sdv_frame_upload.argtypes = [_vp, C.c_uint64, _vp, C.c_float]
     L.sdv_frame_upload_batch.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _f32p]
     L.sdv_frame_upload_batch_u8.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _f32p]
@@ -75,6 +76,7 @@ def _load():
     L.sdv_reproject_map_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _f64p, _f64p, _i32p, _i32p, _i32p, _vp, C.c_int, _i32p, _i32p, _f64p]
     L.sdv_tracker_refine_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _f64p, _f64p, _vp, C.c_int, _i32p, _f32p, _i32p, _i32p]
     L.sdv_tracker_struct_pose_batch.argtypes = [_vp, C.c_int, _i32p, _vp, _i32p, _f64p, _f64p, _f32p, _i32p, _i32p]
+    L.sdv_tracker_struct_pose_batch_slots.argtypes = [_vp, C.c_int, _vp, _i32p, _vp, _i32p, _f64p, _f64p, _f32p, _i32p, _i32p]
     L.sdv_tracker_track.argtypes = [_vp, C.c_int, C.c_uint64, _f64p, _f64p, C.c_int, _f64p, _f64p, _f64p, C.POINTER(C.c_int), C.POINTER(sdv_track_stats)]
     L.sdv_tracker_track_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _f64p, _f64p, C.c_int, _vp, _f64p, _f64p, _i32p, C.POINTER(sdv_track_stats)]
     L.sdv_last_kernel_ms.argtypes = [_vp]; L.sdv_last_kernel_ms.restype = C.c_float
@@ -156,6 +158,20 @@ class Context:
         """CoarseTracker::makeK / the CalibHessian the Reprojector reads, after the bundle adjustment moved the intrinsics"""
         k = sdv_calib(*[float(x) for x in K]); self._ck(LIB.sdv_set_calib(self.p, C.byref(k))); self.K = tuple(float(x) for x in K)
 
+    def setCalibSlots(self, slots, Ks):
+        """CoarseTracker::makeK per tracker instance: slot slots[i] (its tracker and the map slot of the same index) uses Ks[i] = (fx, fy, cx, cy) from now on,
+        whatever setCalib sets later.  All-or-nothing: a bad slot or K raises SdvError and changes no slot."""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1); Kf = np.asarray(Ks, np.float64).reshape(-1, 4)
+        if len(Kf) != len(sl):
+            raise ValueError(f"{len(sl)} slots but {len(Kf)} calibrations")
+        arr = (sdv_calib * max(len(sl), 1))(*[sdv_calib(*map(float, k)) for k in Kf])
+        self._ck(LIB.sdv_set_calib_slots(self.p, len(sl), sl, C.addressof(arr)))
+
+    def clearCalibSlots(self, slots):
+        """the slots follow the context calibration (setCalib) again"""
+        sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        self._ck(LIB.sdv_set_calib_slots(self.p, len(sl), sl, None))
+
     # Undistort (util/Undistort.cpp) handed over as data; `und` = sdv_loam_b200.undistort.Undistort or anything with wOrg,hOrg,remapX,remapY[,G,vignetteMapInv]
     def setUndistort(self, und, factor: float = 1.0):
         rx = np.ascontiguousarray(und.remapX, np.float32).reshape(-1); ry = np.ascontiguousarray(und.remapY, np.float32).reshape(-1)
@@ -234,6 +250,10 @@ class CoarseTracker:
     def __init__(self, ctx: Context, slot: int = 0):
         self.ctx, self.slot = ctx, slot
 
+    def makeK(self, K):
+        """CoarseTracker::makeK (CoarseTracker.cpp:77-106): this instance tracks (and refines its slot's map) with K = (fx, fy, cx, cy) from now on"""
+        self.ctx.setCalibSlots([self.slot], [K])
+
     def setCoarseTrackingRef(self, ref_frame_id: int, pts, round_half, ref_a: float = 0.0, ref_b: float = 0.0):
         pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 4); rh = np.ascontiguousarray(round_half, np.int32)
         self.ctx._ck(LIB.sdv_tracker_set_ref(self.ctx.p, self.slot, ref_frame_id, len(pts), pts, rh, 0.0, ref_a, ref_b))
@@ -269,7 +289,7 @@ class CoarseTracker:
     def structPoseEstimation(self, curToWorld7, overlap_pts, host_T7):
         """CoarseTracker::structPoseEstimation (CoarseTracker.cpp:949-1007).  overlap_pts: OVERLAP_PT_DTYPE array, host_T7: (nH,7) camToWorld of
         the host keyframes the points index.  Returns dict(T=refined curToWorld, res, iterations, accepts)."""
-        r = structPoseEstimationBatch(self.ctx, np.array(curToWorld7, np.float64).reshape(1, 7), [overlap_pts], [host_T7])
+        r = structPoseEstimationBatch(self.ctx, np.array(curToWorld7, np.float64).reshape(1, 7), [overlap_pts], [host_T7], slots=[self.slot])
         return dict(T=r["T"][0], res=float(r["res"][0]), iterations=int(r["iterations"][0]), accepts=int(r["accepts"][0]))
 
 
@@ -352,8 +372,9 @@ class Reprojector:
         return self.reprojectMapBatch([slot], [cur_frame_id], np.asarray(cur_T7, np.float64).reshape(1, 7), None if cur_ab is None else np.asarray(cur_ab, np.float64).reshape(1, 2), **kw)[0]
 
 
-def structPoseEstimationBatch(ctx, curToWorld7, overlap_pts_list, host_T7_list):
-    """n independent structPoseEstimation calls in one launch (one CTA each): curToWorld7 (n,7) is refined in place."""
+def structPoseEstimationBatch(ctx, curToWorld7, overlap_pts_list, host_T7_list, slots=None):
+    """n independent structPoseEstimation calls in one launch (one CTA each): curToWorld7 (n,7) is refined in place.
+    slots: the tracker slot of each job, whose K it uses (None: the context calibration)."""
     n = len(overlap_pts_list)
     T = np.ascontiguousarray(curToWorld7, np.float64).reshape(n, 7)
     pb = np.zeros(n + 1, np.int32); hb = np.zeros(n + 1, np.int32)
@@ -361,7 +382,9 @@ def structPoseEstimationBatch(ctx, curToWorld7, overlap_pts_list, host_T7_list):
     pts = np.concatenate([np.ascontiguousarray(p, OVERLAP_PT_DTYPE) for p in overlap_pts_list]) if pb[-1] else np.zeros(1, OVERLAP_PT_DTYPE)
     hT = np.ascontiguousarray(np.concatenate([np.asarray(h, np.float64).reshape(-1, 7) for h in host_T7_list]))
     res = np.zeros(n, np.float32); its = np.zeros(n, np.int32); acc = np.zeros(n, np.int32)
-    ctx._ck(LIB.sdv_tracker_struct_pose_batch(ctx.p, n, pb, pts.ctypes.data, hb, hT, T, res, its, acc))
+    sl = None if slots is None else np.ascontiguousarray(slots, np.int32)
+    assert sl is None or sl.shape == (n,)
+    ctx._ck(LIB.sdv_tracker_struct_pose_batch_slots(ctx.p, n, None if sl is None else sl.ctypes.data, pb, pts.ctypes.data, hb, hT, T, res, its, acc))
     return dict(T=T, res=res, iterations=its, accepts=acc)
 
 

@@ -7,6 +7,8 @@
 #include <cstdio>
 #include <cstring>
 #include <cstdarg>
+#include <cmath>
+#include <algorithm>
 
 using namespace sdv;
 
@@ -35,7 +37,7 @@ int sdv_pyr_levels(int w, int h) {               // util/globalCalib.cpp:22-30
 static thread_local char g_create_err[512] = "null context";   // message of the last failed sdv_create on this thread (there is no context to hold it)
 const char* sdv_last_error(sdv_ctx* c) { return c ? c->err : g_create_err; }
 
-static void make_geom(sdv_ctx* c, const sdv_calib* K) {   // CoarseTracker::makeK (CoarseTracker.cpp:77-106)
+static void make_geom(sdv_ctx* c, const sdv_calib* K, int row) {   // CoarseTracker::makeK (CoarseTracker.cpp:77-106) into one row of the geometry table
   float fx[SDV_PYR_LEVELS], fy[SDV_PYR_LEVELS], cx[SDV_PYR_LEVELS], cy[SDV_PYR_LEVELS];
   fx[0]=K->fx; fy[0]=K->fy; cx[0]=K->cx; cy[0]=K->cy;
   for (int l=1;l<c->levels;l++) {
@@ -43,21 +45,44 @@ static void make_geom(sdv_ctx* c, const sdv_calib* K) {   // CoarseTracker::make
     cx[l] = (cx[0]+0.5)/((int)1<<l) - 0.5; cy[l] = (cy[0]+0.5)/((int)1<<l) - 0.5;
   }
   for (int l=0;l<c->levels;l++) {
-    LevelGeom& g = c->tc.geom[l]; g.w = c->w>>l; g.h = c->h>>l; g.fx=fx[l]; g.fy=fy[l]; g.cx=cx[l]; g.cy=cy[l];
+    LevelGeom& g = c->geom[row].g[l]; g.w = c->w>>l; g.h = c->h>>l; g.fx=fx[l]; g.fy=fy[l]; g.cx=cx[l]; g.cy=cy[l];
     float Km[9] = {fx[l],0,cx[l], 0,fy[l],cy[l], 0,0,1}; inv3f(Km, g.Ki);
   }
 }
 
-// CoarseTracker::makeK(HCalib) / the CalibHessian the Reprojector reads (FullSystem::optimize moves the intrinsics at every keyframe): new K for every later call.
-// Stream-ordered after the work already enqueued on the compute stream.
+// rows [lo, hi] of the host mirror to the device, stream-ordered after the work already enqueued on the compute stream (pageable source: staged before the call returns)
+static int upload_geom(sdv_ctx* c, int lo, int hi) {
+  CK(cudaMemcpyAsync(c->geom_dev + lo, &c->geom[lo], (size_t)(hi - lo + 1)*sizeof(GeomRow), cudaMemcpyHostToDevice, c->st));
+  return SDV_OK;
+}
+
+// CoarseTracker::makeK(HCalib) / the CalibHessian the Reprojector reads (FullSystem::optimize moves the intrinsics at every keyframe): the context calibration,
+// used by every later call on a slot without a K of its own.
 int sdv_set_calib(sdv_ctx* c, const sdv_calib* K) { SDV_GUARD_TRK(c);
   if (!c || !K) return SDV_ERR_ARG;
   if (!(K->fx > 0 && K->fy > 0)) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib: focal lengths must be positive");
   CK(cudaSetDevice(c->device));
-  make_geom(c, K);
-  CK(cudaMemcpyAsync(c->tc_dev, &c->tc, sizeof(TrackConst), cudaMemcpyHostToDevice, c->st));   // pageable source: staged before the call returns
-  rp_calib_changed(c);
-  return SDV_OK;
+  make_geom(c, K, 0);
+  return upload_geom(c, 0, 0);
+}
+
+// CoarseTracker::makeK per tracker instance: slot slots[i] uses K[i] (its own row 1 + slot), or the context calibration again when K is NULL.
+// Everything is checked before anything changes.
+int sdv_set_calib_slots(sdv_ctx* c, int n, const int32_t* slots, const sdv_calib* K) { SDV_GUARD_TRK(c);
+  if (!c || n < 0 || (n > 0 && !slots)) return SDV_ERR_ARG;
+  for (int i=0;i<n;i++) {
+    if (slots[i] < 0 || slots[i] >= (int)c->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib_slots: entry %d names slot %d of %d", i, slots[i], (int)c->slots.size());
+    if (K && !(K[i].fx > 0 && K[i].fy > 0 && std::isfinite(K[i].fx) && std::isfinite(K[i].fy) && std::isfinite(K[i].cx) && std::isfinite(K[i].cy)))
+      return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib_slots: entry %d (slot %d): fx, fy must be positive and finite, cx, cy finite", i, slots[i]);
+  }
+  CK(cudaSetDevice(c->device));
+  int lo = (int)c->geom.size(), hi = -1;
+  for (int i=0;i<n;i++) {
+    TrackerSlot& t = c->slots[slots[i]];
+    if (!K) { t.geom_row = 0; continue; }
+    t.geom_row = 1 + slots[i]; make_geom(c, &K[i], t.geom_row); lo = std::min(lo, t.geom_row); hi = std::max(hi, t.geom_row);
+  }
+  return hi >= lo ? upload_geom(c, lo, hi) : SDV_OK;
 }
 
 static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels, const sdv_settings* s_in, int device);
@@ -90,9 +115,12 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
   memset(&c->tc, 0, sizeof(c->tc));
   c->tc.levels = levels; c->tc.huberTH = s.huberTH; c->tc.coarseCutoffTH = s.coarseCutoffTH;
   c->tc.affineOptModeA = s.affineOptModeA; c->tc.affineOptModeB = s.affineOptModeB;
-  make_geom(c, K);
   CK(cudaMalloc(&c->tc_dev, sizeof(TrackConst)));
   CK(cudaMemcpy(c->tc_dev, &c->tc, sizeof(TrackConst), cudaMemcpyHostToDevice));
+  c->geom.assign(s.n_tracker_slots + 1, GeomRow{});                // slot rows are written by sdv_set_calib_slots before a slot points at them
+  make_geom(c, K, 0);
+  CK(cudaMalloc(&c->geom_dev, c->geom.size()*sizeof(GeomRow)));
+  CK(cudaMemcpy(c->geom_dev, c->geom.data(), c->geom.size()*sizeof(GeomRow), cudaMemcpyHostToDevice));
   // frame pool: planar intensity of every level per frame (level 0 + one allocation for levels >= 1), plus the storage of the packed-texel cache of
   // levels >= 1; packed level-0 texels come from a small keyframe pool
   size_t texels = 0; c->lvl_off[0] = 0; for (int l=1;l<levels;l++) { c->lvl_off[l] = texels; texels += (size_t)(w>>l)*(h>>l); }
@@ -113,7 +141,7 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
       size_t cap = (size_t)(w>>l)*(h>>l); if (s.max_ref_points > 0 && (size_t)s.max_ref_points < cap) cap = s.max_ref_points;
       t.cap[l] = (int)cap; t.npts[l] = 0; CK(cudaMalloc(&t.pts[l], cap*sizeof(float4)));
     }
-    t.ref_frame = ~0ull; t.has_totals = false;
+    t.ref_frame = ~0ull; t.has_totals = false; t.geom_row = 0;
   }
   // step-kernel reduction buffers
   CK(cudaMalloc(&c->partials, (size_t)step_kernel_max_grid()*kNAcc*sizeof(double)));
@@ -147,7 +175,7 @@ void sdv_destroy(sdv_ctx* c) {
   cudaFree(c->cd_owner); cudaFree(c->cd_counts); cudaFree(c->cd_scalars); cudaFreeHost(c->cd_scalars_host);
   cudaFree(c->cd_pts4); cudaFree(c->cd_round); cudaFree(c->cd_splats); cudaFree(c->cd_done);
   for (int i=0;i<2;i++) { cudaFree(c->pyr_batch_dev[i]); cudaFreeHost(c->pyr_batch_host[i]); } cudaFree(c->partials); cudaFree(c->ticket); cudaFree(c->totals_dev); cudaFreeHost(c->totals_host);
-  cudaFree(c->tc_dev); cudaFree(c->jobs_dev); cudaFreeHost(c->jobs_host);
+  cudaFree(c->tc_dev); cudaFree(c->geom_dev); cudaFree(c->jobs_dev); cudaFreeHost(c->jobs_host);
   for (int i=0;i<2;i++) cudaFree(c->stage_u8[i]);
   cudaFree(c->und_buf); cudaFree(c->trace_dev);
   for (int i=0;i<sdv_ctx::kIngRing;i++) if (c->ev_ing[i]) cudaEventDestroy(c->ev_ing[i]); for (int i=0;i<2;i++) if (c->ev_cp[i]) cudaEventDestroy(c->ev_cp[i]); if (c->st_cp) cudaStreamDestroy(c->st_cp);
@@ -427,11 +455,12 @@ int sdv_tracker_calc_res(sdv_ctx* c, int slot, uint64_t new_frame, int lvl, cons
   TrackerSlot& t = c->slots[slot];
   FrameDev* f = find_frame(c, new_frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown new frame");
   if (t.ref_frame == ~0ull) return ctx_fail(c, SDV_ERR_STATE, "tracker slot %d has no reference", slot);
-  EvalParams ep; make_eval_params(se3_from7(T), a, b, t.refExposure, f->exposure, t.ref_a, t.ref_b, c->tc.geom[lvl], lvl, cutoffTH, c->tc.huberTH, ep);
+  const LevelGeom& g = slot_geom(c, slot).g[lvl];
+  EvalParams ep; make_eval_params(se3_from7(T), a, b, t.refExposure, f->exposure, t.ref_a, t.ref_b, g, lvl, cutoffTH, c->tc.huberTH, ep);
   { int rcj = join_ingest(c); if (rcj) return rcj; }
   CK(cudaEventRecord(c->ev0, c->st));
   c->launches += 1;
-  launch_coarse_res_gs(t.pts[lvl], t.npts[lvl], f->img[lvl], c->tc.geom[lvl], ep, c->partials, c->ticket, c->totals_dev, c->st);
+  launch_coarse_res_gs(t.pts[lvl], t.npts[lvl], f->img[lvl], g, ep, c->partials, c->ticket, c->totals_dev, c->st);
   CK(cudaEventRecord(c->ev1, c->st));
   CK(cudaMemcpyAsync(c->totals_host, c->totals_dev, kNAcc*sizeof(double), cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st)); CK(cudaGetLastError());
@@ -470,13 +499,13 @@ int sdv_tracker_track_batch(sdv_ctx* c, int n, const int32_t* slots, const uint6
     for (int i=0;i<7;i++) J.T[i] = T_io[7*k+i];
     J.ab[0] = ab_io[2*k]; J.ab[1] = ab_io[2*k+1];
     for (int i=0;i<5;i++) J.minRes[i] = minRes ? minRes[5*k+i] : nan("");
-    J.coarsest = coarsest;
+    J.coarsest = coarsest; J.geom_row = t.geom_row;
   }
   { int rcj = join_ingest_upto(c, need_seq); if (rcj) return rcj; }     // only the uploads that built THESE frames: batch k+1's upload keeps streaming
   c->launches += 2;                                                    // descriptor copy kernel + track_cluster_kernel
   launch_h2d_words(c->jobs_dev, c->jobs_host, (size_t)n*sizeof(TrackJob), c->st);      // kernel copy: not queued behind the next batch's image upload
   CK(cudaEventRecord(c->ev0, c->st));
-  CK(launch_track_cluster(c->jobs_dev, n, c->tc_dev, c->set.cluster_size, c->set.track_threads, c->st));
+  CK(launch_track_cluster(c->jobs_dev, n, c->tc_dev, c->geom_dev, c->set.cluster_size, c->set.track_threads, c->st));
   CK(cudaEventRecord(c->ev1, c->st));
   CK(cudaMemcpyAsync(c->jobs_host, c->jobs_dev, (size_t)n*sizeof(TrackJob), cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st)); CK(cudaGetLastError());

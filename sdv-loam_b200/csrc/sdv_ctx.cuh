@@ -24,6 +24,7 @@ struct TrackerSlot {                      // one CoarseTracker instance (referen
   float4* pts[kLevels]; int npts[kLevels]; int cap[kLevels];
   uint64_t ref_frame; float refExposure; double ref_a, ref_b;   // lastRef, lastRef_aff_g2l
   double totals[kNAcc]; bool has_totals;                        // reduced sums of the last calc_res (what calcGSSSE reads from buf_warped_*)
+  int geom_row;                                                 // row of sdv_ctx::geom this instance's makeK wrote (1 + slot), or 0: the context calibration
 };
 
 struct BAState;                           // sdv_ba.cuh
@@ -42,6 +43,9 @@ struct sdv_ctx {
   static constexpr int kIngRing = 8; cudaEvent_t ev_ing[kIngRing], ev_cp[2]; long long ingest_seq = 0, seq_waited = 0;
   int w, h, levels; sdv_settings set;
   sdv::TrackConst tc; sdv::TrackConst* tc_dev;
+  // geometry table (CoarseTracker::makeK per K): row 0 = the context calibration (sdv_set_calib), row 1 + s = tracker slot s's own K (sdv_set_calib_slots).
+  // Host mirror + device copy; every consumer indexes it with TrackerSlot::geom_row, none derives the geometry from K itself.
+  std::vector<sdv::GeomRow> geom; sdv::GeomRow* geom_dev;
   size_t lvl_off[sdv::kLevels]; size_t frame_texels;
   std::vector<sdv::FrameDev> frames; std::unordered_map<uint64_t,int> frame_index;
   // frames whose device images are referenced by a resident BA window (BAHeader::frames[].img0) or map slot (MapDev::hostI0): refcount per handle.
@@ -75,7 +79,6 @@ namespace sdv {
 void rp_destroy(sdv_ctx* c);
 void sel_destroy(sdv_ctx* c);
 void lidar_destroy(sdv_ctx* c);
-void rp_calib_changed(sdv_ctx* c);             // the Reprojector constants (K, K^-1) are rebuilt from the context calibration at the next call
 int ctx_fail(sdv_ctx* c, int code, const char* fmt, ...);
 void ba_destroy(sdv_ctx* c);
 int  ensure_lvl0(sdv_ctx* c, FrameDev& f);     // build the packed level-0 texels of a frame on demand (keyframes / read-back)
@@ -85,6 +88,7 @@ inline void frame_unpin(sdv_ctx* c, uint64_t id) { auto it = c->pins.find(id); i
 inline bool frame_pinned(const sdv_ctx* c, uint64_t id) { return c->pins.find(id) != c->pins.end(); }
 int  join_ingest(sdv_ctx* c);                  // compute stream waits for every ingest enqueued so far
 int  join_ingest_upto(sdv_ctx* c, long long seq);   // ... for ingest calls <= seq only (frames carry their ingest_seq)
+inline const GeomRow& slot_geom(const sdv_ctx* c, int slot) { return c->geom[c->slots[slot].geom_row]; }   // the K a tracker / map slot uses, at every level
 }
 // entry-point guards (a NULL context falls through to the entry's own argument check)
 #define SDV_GUARD_TRK(c) std::unique_lock<std::recursive_mutex> lk_trk_; if (c) lk_trk_ = std::unique_lock<std::recursive_mutex>((c)->mu_trk)

@@ -186,12 +186,18 @@ struct TrackJob {                         // one trackNewestCoarse call
   float refExposure, newExposure; double ref_a, ref_b;
   double T[7]; double ab[2];              // in: lastToNew_out / aff_g2l_out initial ; out: result (if not aborted)
   double minRes[5]; int coarsest;
+  int geom_row;                           // row of the geometry table (sdv_ctx::geom_dev) this job's tracker slot uses
   double lastRes[5]; double flow[3]; int good;
   long long point_evals[kLevels]; int iterations[kLevels]; int accepts[kLevels];
 };
+static_assert(sizeof(TrackJob) == 432, "geom_row lives in the padding after coarsest: the job descriptor (sdv_track_job_bytes) keeps its size");
 
-struct TrackConst {                       // per-context constants
-  LevelGeom geom[kLevels]; int levels;
+// One row of the geometry table: CoarseTracker::makeK (CoarseTracker.cpp:77-106) of one K at every level.  The table holds one row for the context
+// calibration (row 0) and one per tracker slot (row 1 + slot); a slot without its own K points at row 0.
+struct GeomRow { LevelGeom g[kLevels]; };
+
+struct TrackConst {                       // per-context scalar settings
+  int levels;
   float huberTH, coarseCutoffTH, affineOptModeA, affineOptModeB;
 };
 

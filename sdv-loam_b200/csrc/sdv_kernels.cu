@@ -447,7 +447,8 @@ __constant__ unsigned char kAccRow[45] = {0,0,0,0,0,0,0,0,0, 1,1,1,1,1,1,1,1, 2,
 __constant__ unsigned char kAccCol[45] = {0,1,2,3,4,5,6,7,8, 1,2,3,4,5,6,7,8, 2,3,4,5,6,7,8, 3,4,5,6,7,8, 4,5,6,7,8, 5,6,7,8, 6,7,8, 7,8, 8};
 
 template <int THREADS, int MINB>
-__global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* __restrict__ jobs, const TrackConst* __restrict__ tc_g, unsigned stagger_ns) {
+__global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* __restrict__ jobs, const TrackConst* __restrict__ tc_g, const GeomRow* __restrict__ geom_tab,
+                                                                unsigned stagger_ns) {
   cg::cluster_group cluster = cg::this_cluster();
   const int C = (int)cluster.num_blocks();
   const int rank = (int)cluster.block_rank();
@@ -475,8 +476,11 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
   double* tot    = bsum + kNAcc;                                                         // [kNAcc]
   __shared__ Ctl2 ctl;
   __shared__ TrackConst tc;
+  __shared__ GeomRow geom;                                  // the job's row of the geometry table: the K of its tracker slot at every level
   __shared__ __align__(8) uint64_t full_bar[2];
   for (int i = tid; i < (int)(sizeof(TrackConst)/4); i += THREADS) reinterpret_cast<int*>(&tc)[i] = reinterpret_cast<const int*>(tc_g)[i];
+  { const int* __restrict__ row = reinterpret_cast<const int*>(geom_tab + J.geom_row);
+    for (int i = tid; i < (int)(sizeof(GeomRow)/4); i += THREADS) reinterpret_cast<int*>(&geom)[i] = row[i]; }
   if (tid == 0) {
     ctl.cur = se3_from7(J.T); ctl.a_cur = J.ab[0]; ctl.b_cur = J.ab[1];
     for (int i = 0; i < 5; i++) ctl.lastRes[i] = nan("");
@@ -487,7 +491,7 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  if (tid == 0) make_eval_params(ctl.cur, ctl.a_cur, ctl.b_cur, J.refExposure, J.newExposure, J.ref_a, J.ref_b, tc.geom[ctl.lvl], ctl.lvl,
+  if (tid == 0) make_eval_params(ctl.cur, ctl.a_cur, ctl.b_cur, J.refExposure, J.newExposure, J.ref_a, J.ref_b, geom.g[ctl.lvl], ctl.lvl,
                                  tc.coarseCutoffTH*ctl.lcr, tc.huberTH, ctl.ep);
   __syncthreads();
   if (C > 1) cluster.sync();                                // every CTA of the cluster must be running before the first distributed-shared-memory write
@@ -507,7 +511,7 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
     {
       const float4* __restrict__ pts = J.pts[lvl]; const int n = J.npts[lvl];
       const float* __restrict__ I = J.img[lvl];
-      const LevelGeom& g = tc.geom[lvl];
+      const LevelGeom& g = geom.g[lvl];
       const int K = (n + stride - 1)/stride;                // sweep iterations (uniform over the CTA)
       const int NC = (K + kPtChunk - 1)/kPtChunk;           // point chunks
       auto issue_chunk = [&](int c) {                       // thread 0: TMA bulk copies of chunk c's (<= kPtChunk) blocks into buffer c&1
@@ -703,7 +707,7 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
       }
       SDV_PROF_T(tq4);
       EvalParams ep;
-      if (new_ep) make_eval_params(ep_pose, ep_a, ep_b, J.refExposure, J.newExposure, J.ref_a, J.ref_b, tc.geom[ep_lvl], ep_lvl, tc.coarseCutoffTH*ep_lcr, tc.huberTH, ep);
+      if (new_ep) make_eval_params(ep_pose, ep_a, ep_b, J.refExposure, J.newExposure, J.ref_a, J.ref_b, geom.g[ep_lvl], ep_lvl, tc.coarseCutoffTH*ep_lcr, tc.huberTH, ep);
       __syncwarp();                                          // every lane has read the old control state (racecheck: warp-level WAR on ctl.incn / ctl.haveRepeated otherwise)
       if (L0) {                                              // publish (plain predicated stores; nothing collective follows inside this block)
         ctl.cur = cur; ctl.a_cur = a_cur; ctl.b_cur = b_cur; ctl.cand = cand; ctl.a_cand = a_cand; ctl.b_cand = b_cand;
@@ -754,19 +758,20 @@ static size_t track_kernel_smem(int cluster_size = kMaxCluster) {
 
 static unsigned track_stagger_ns() { static long v = -1; if (v < 0) { const char* e = getenv("SDV_TRACK_STAGGER_NS"); v = e ? atol(e) : SDV_TRACK_STAGGER_DEFAULT_NS; if (v < 0) v = 0; } return (unsigned)v; }
 template <typename Kern, typename... Extra>
-static cudaError_t launch_track_kern(Kern kern, size_t smem, int threads, TrackJob* jobs_dev, int njobs, const TrackConst* tc_dev, int cluster_size, cudaStream_t st, Extra... extra) {
+static cudaError_t launch_track_kern(Kern kern, size_t smem, int threads, TrackJob* jobs_dev, int njobs, const TrackConst* tc_dev, const GeomRow* geom_dev, int cluster_size, cudaStream_t st,
+                                     Extra... extra) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)(njobs*cluster_size)); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = (unsigned)cluster_size; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
   cfg.attrs = at; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kern, jobs_dev, tc_dev, extra...);
+  return cudaLaunchKernelEx(&cfg, kern, jobs_dev, tc_dev, geom_dev, extra...);
 }
 template <int THREADS, int MINB>
-static cudaError_t launch_track_t(TrackJob* jobs_dev, int njobs, const TrackConst* tc_dev, int cluster_size, cudaStream_t st) {
+static cudaError_t launch_track_t(TrackJob* jobs_dev, int njobs, const TrackConst* tc_dev, const GeomRow* geom_dev, int cluster_size, cudaStream_t st) {
   // stagger only when the grid fills the co-resident slots of the chip (otherwise there is nothing to desynchronise)
   const unsigned stag = (cluster_size == 1 && njobs > num_sms()) ? track_stagger_ns() : 0u;
-  return launch_track_kern(track_cluster_kernel<THREADS, MINB>, track_kernel_smem<THREADS>(cluster_size), THREADS, jobs_dev, njobs, tc_dev, cluster_size, st, stag);
+  return launch_track_kern(track_cluster_kernel<THREADS, MINB>, track_kernel_smem<THREADS>(cluster_size), THREADS, jobs_dev, njobs, tc_dev, geom_dev, cluster_size, st, stag);
 }
 template <typename Kern>
 static cudaError_t track_attrs(Kern kern, size_t smem) {
@@ -777,10 +782,10 @@ static cudaError_t track_attrs(Kern kern, size_t smem) {
 #ifndef SDV_TRACK_MINB
 #define SDV_TRACK_MINB 4                    // H100: 4 (128 regs, 80 B spilled at the time) 2.57 ms per 1 056 jobs against 3 (160 regs, no spills) 2.93 ms; DESIGN.md §6
 #endif
-cudaError_t launch_track_cluster(TrackJob* jobs_dev, int njobs, const TrackConst* tc_dev, int cluster_size, int threads, cudaStream_t st) {
-  if (threads == 256) return launch_track_t<256, 1>(jobs_dev, njobs, tc_dev, cluster_size, st);
-  if (threads == 64)  return launch_track_t<64, 8>(jobs_dev, njobs, tc_dev, cluster_size, st);
-  return launch_track_t<128, SDV_TRACK_MINB>(jobs_dev, njobs, tc_dev, cluster_size, st);
+cudaError_t launch_track_cluster(TrackJob* jobs_dev, int njobs, const TrackConst* tc_dev, const GeomRow* geom_dev, int cluster_size, int threads, cudaStream_t st) {
+  if (threads == 256) return launch_track_t<256, 1>(jobs_dev, njobs, tc_dev, geom_dev, cluster_size, st);
+  if (threads == 64)  return launch_track_t<64, 8>(jobs_dev, njobs, tc_dev, geom_dev, cluster_size, st);
+  return launch_track_t<128, SDV_TRACK_MINB>(jobs_dev, njobs, tc_dev, geom_dev, cluster_size, st);
 }
 
 // Function attributes (opt-in dynamic shared memory, non-portable cluster sizes) belong to the CURRENT DEVICE's copy of a kernel: sdv_create calls this

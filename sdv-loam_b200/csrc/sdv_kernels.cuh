@@ -24,7 +24,7 @@ void launch_coarse_res_gs(const float4* pts, int n, const float* I, const LevelG
 // small host->device transfer done by a kernel reading pinned (UVA-mapped) host memory: it does not queue behind bulk cudaMemcpyAsync traffic on the
 // H2D copy engine, so a job-descriptor upload cannot be delayed by the next batch's image upload (DESIGN.md §6)
 void launch_h2d_words(void* dst_dev, const void* src_pinned, size_t bytes, cudaStream_t st);
-cudaError_t launch_track_cluster(TrackJob* jobs_dev, int njobs, const TrackConst* tc_dev, int cluster_size, int threads, cudaStream_t st);
+cudaError_t launch_track_cluster(TrackJob* jobs_dev, int njobs, const TrackConst* tc_dev, const GeomRow* geom_dev, int cluster_size, int threads, cudaStream_t st);
 
 // makeCoarseDepthL0 (CoarseTracker.cpp:258-425)
 int  cd_num_blocks(int w, int h);

@@ -115,7 +115,7 @@ __device__ void ref_hb(RefShared& S, const int pt_begin, const int pt_end, const
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(kRefThreads) struct_pose_kernel(RefineJob* jobs, const sdv_overlap_pt* pts, const double* hostT7, const TrackConst* tc) {
+__global__ void __launch_bounds__(kRefThreads) struct_pose_kernel(RefineJob* jobs, const sdv_overlap_pt* pts, const double* hostT7, const GeomRow* geom_tab) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   RefShared& S = *reinterpret_cast<RefShared*>(smem_raw);
   __shared__ SE3d cur, cand;             // worldToCur_current / worldToCur_new
@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(kRefThreads) struct_pose_kernel(RefineJob* job
   RefineJob& jb = jobs[blockIdx.x];
   const int pt_begin = jb.pt_begin, pt_end = jb.pt_end, nH = jb.nH, host_begin = jb.host_begin; const double* __restrict__ hostT = jb.hostT;   // read once: jb is written below, so the
                                                                         // compiler would otherwise re-load these from global memory inside every loop
-  const LevelGeom g = tc->geom[0];
+  const LevelGeom g = geom_tab[jb.geom_row].g[0];
   const float fxi = g.Ki[0], fyi = g.Ki[4];
   for (int k = threadIdx.x; k < nH; k += blockDim.x) {
     SE3d h = se3_from7(hostT ? hostT + 7*k : hostT7 + 7*(size_t)(host_begin + k)); double R[9]; qmat(h.q, R);
@@ -198,8 +198,8 @@ __global__ void __launch_bounds__(kRefThreads) struct_pose_kernel(RefineJob* job
 cudaError_t refine_init_device() {         // per-device opt-in shared memory size (called by sdv_create after cudaSetDevice)
   return cudaFuncSetAttribute(struct_pose_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RefShared));
 }
-void launch_struct_pose(RefineJob* jobs, int n_jobs, const sdv_overlap_pt* pts, const double* hostT7, const TrackConst* tc, cudaStream_t st) {
-  struct_pose_kernel<<<n_jobs, kRefThreads, sizeof(RefShared), st>>>(jobs, pts, hostT7, tc);
+void launch_struct_pose(RefineJob* jobs, int n_jobs, const sdv_overlap_pt* pts, const double* hostT7, const GeomRow* geom_tab, cudaStream_t st) {
+  struct_pose_kernel<<<n_jobs, kRefThreads, sizeof(RefShared), st>>>(jobs, pts, hostT7, geom_tab);
 }
 
 } // namespace sdv
@@ -217,9 +217,11 @@ static int refine_reserve(sdv_ctx* c, size_t bytes) {
 
 extern "C" {
 
-int sdv_tracker_struct_pose_batch(sdv_ctx* c, int n_jobs, const int32_t* pt_begin, const sdv_overlap_pt* pts, const int32_t* host_begin, const double* host_T7,
-                                  double* curToWorld_io, float* res_out, int32_t* iterations, int32_t* accepts) { SDV_GUARD_TRK(c);
+// slots == NULL: every job uses the context calibration (row 0 of the geometry table)
+int sdv_tracker_struct_pose_batch_slots(sdv_ctx* c, int n_jobs, const int32_t* slots, const int32_t* pt_begin, const sdv_overlap_pt* pts, const int32_t* host_begin,
+                                        const double* host_T7, double* curToWorld_io, float* res_out, int32_t* iterations, int32_t* accepts) { SDV_GUARD_TRK(c);
   if (!c || n_jobs <= 0 || !pt_begin || !host_begin || !host_T7 || !curToWorld_io) return SDV_ERR_ARG;
+  if (slots) for (int k=0;k<n_jobs;k++) if (slots[k] < 0 || slots[k] >= (int)c->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "struct_pose job %d: slot %d of %d", k, slots[k], (int)c->slots.size());
   const int nP = pt_begin[n_jobs], nH = host_begin[n_jobs];
   if (pt_begin[0] != 0 || host_begin[0] != 0 || nP < 0 || nH <= 0 || (nP > 0 && !pts)) return SDV_ERR_ARG;   // both CSRs start at 0: nothing is indexed below it
   for (int k=0;k<n_jobs;k++) {
@@ -234,13 +236,14 @@ int sdv_tracker_struct_pose_batch(sdv_ctx* c, int n_jobs, const int32_t* pt_begi
   unsigned char* hb = (unsigned char*)c->refine_host; unsigned char* db = (unsigned char*)c->refine_dev;
   RefineJob* J = (RefineJob*)(hb + o_jobs);
   for (int k=0;k<n_jobs;k++) { memset(&J[k], 0, sizeof(RefineJob)); for (int i=0;i<7;i++) J[k].T[i] = curToWorld_io[7*k+i];
-    J[k].pt_begin = pt_begin[k]; J[k].pt_end = pt_begin[k+1]; J[k].host_begin = host_begin[k]; J[k].nH = host_begin[k+1]-host_begin[k]; }
+    J[k].pt_begin = pt_begin[k]; J[k].pt_end = pt_begin[k+1]; J[k].host_begin = host_begin[k]; J[k].nH = host_begin[k+1]-host_begin[k];
+    J[k].geom_row = slots ? c->slots[slots[k]].geom_row : 0; }
   if (nP) memcpy(hb + o_pts, pts, (size_t)nP*sizeof(sdv_overlap_pt));
   memcpy(hb + o_host, host_T7, (size_t)nH*7*sizeof(double));
   c->launches += 1;
   CK(cudaMemcpyAsync(db, hb, total, cudaMemcpyHostToDevice, c->st));
   CK(cudaEventRecord(c->ev0, c->st));
-  launch_struct_pose((RefineJob*)(db + o_jobs), n_jobs, (const sdv_overlap_pt*)(db + o_pts), (const double*)(db + o_host), c->tc_dev, c->st);
+  launch_struct_pose((RefineJob*)(db + o_jobs), n_jobs, (const sdv_overlap_pt*)(db + o_pts), (const double*)(db + o_host), c->geom_dev, c->st);
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev1, c->st));
   CK(cudaMemcpyAsync(hb + o_jobs, db + o_jobs, (size_t)n_jobs*sizeof(RefineJob), cudaMemcpyDeviceToHost, c->st));
@@ -249,6 +252,11 @@ int sdv_tracker_struct_pose_batch(sdv_ctx* c, int n_jobs, const int32_t* pt_begi
   for (int k=0;k<n_jobs;k++) { for (int i=0;i<7;i++) curToWorld_io[7*k+i] = J[k].T[i];
     if (res_out) res_out[k] = J[k].res; if (iterations) iterations[k] = J[k].iterations; if (accepts) accepts[k] = J[k].accepts; }
   return SDV_OK;
+}
+
+int sdv_tracker_struct_pose_batch(sdv_ctx* c, int n_jobs, const int32_t* pt_begin, const sdv_overlap_pt* pts, const int32_t* host_begin, const double* host_T7,
+                                  double* curToWorld_io, float* res_out, int32_t* iterations, int32_t* accepts) {
+  return sdv_tracker_struct_pose_batch_slots(c, n_jobs, nullptr, pt_begin, pts, host_begin, host_T7, curToWorld_io, res_out, iterations, accepts);
 }
 
 int sdv_tracker_struct_pose(sdv_ctx* c, int n, const sdv_overlap_pt* pts, int nH, const double* host_T7, double curToWorld_io[7], float* res_out, int* iterations, int* accepts) { SDV_GUARD_TRK(c);

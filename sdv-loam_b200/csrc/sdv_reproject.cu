@@ -29,10 +29,12 @@ struct MapDev {                           // device-resident map of one sequence
 };
 struct RpJob {
   const MapDev* map; const float* cur[kLevels]; double curT[7], curTinv[7];
+  double K[9], Ki[9];                     // the map slot's K (its tracker slot's row of the geometry table at level 0) and K^-1, built on the host (rp_launch)
   float affLL[kRpMaxHosts][2]; int frame_rank[kRpMaxHosts];
   int cur_kf_index, backup, nH, nP; long long pt_off; int error;
+  int geom_row;                           // handed to the structPoseEstimation job of the fused refinement (rp_emit_kernel)
 };
-struct RpConst { double K[9], Ki[9]; int w[kLevels], h[kLevels]; int levels, ncols, ncells; };
+struct RpConst { double K[9], Ki[9]; int w[kLevels], h[kLevels]; int levels, ncols, ncells; };   // K, Ki: the context calibration (geometry row 0), as launch constants
 struct RpScratch { double2* cand_px; float* cand_key; int* cand_cell; unsigned long long* list;   // list: per cell, (key bits << 32) | (frame rank << 27) | point index
                    int* count; int* begin; int* cursor; int* out_pt; double2* out_px;
                    double* xf; };   // xf[job][host][14]: camToWorld_host^-1 and T_cur_ref = camToWorld_cur^-1 * camToWorld_host (7 doubles each), built by rp_project_kernel
@@ -41,15 +43,15 @@ __device__ __forceinline__ void mv3(const double* M, double x, double y, double 
   o[0] = (M[0]*x + M[1]*y) + M[2]*z; o[1] = (M[3]*x + M[4]*y) + M[5]*z; o[2] = (M[6]*x + M[7]*y) + M[8]*z;
 }
 __device__ __forceinline__ void xform(const SE3d& T, const double* p, double* o) { double r[3]; qrot(T.q, p, r); o[0] = r[0]+T.t[0]; o[1] = r[1]+T.t[1]; o[2] = r[2]+T.t[2]; }
-__device__ __forceinline__ void point_world(const RpConst& C, const MapDev* __restrict__ m, const sdv_map_pt& p, double* pw) {   // pixelFrame2PointWorld :570-577
-  double k[3]; mv3(C.Ki, (double)p.u, (double)p.v, 1.0, k);
+__device__ __forceinline__ void point_world(const double* Ki, const MapDev* __restrict__ m, const sdv_map_pt& p, double* pw) {   // pixelFrame2PointWorld :570-577
+  double k[3]; mv3(Ki, (double)p.u, (double)p.v, 1.0, k);
   const double s = (double)(1/p.idepth);
   double r[3] = {k[0]*s, k[1]*s, k[2]*s};
   SE3d c2w = se3_from7(m->hostT[p.host]); xform(c2w, r, pw);
 }
-__device__ __forceinline__ void pixel_from_cam(const RpConst& C, double* c, double* px) {                                        // :579-586 / :603-610
+__device__ __forceinline__ void pixel_from_cam(const double* K, double* c, double* px) {                                          // :579-586 / :603-610
   c[0] = c[0]/c[2]; c[1] = c[1]/c[2]; c[2] = c[2]/c[2];
-  double o[3]; mv3(C.K, c[0], c[1], c[2], o); px[0] = o[0]; px[1] = o[1];
+  double o[3]; mv3(K, c[0], c[1], c[2], o); px[0] = o[0]; px[1] = o[1];
 }
 __device__ __forceinline__ bool in_frame(const RpConst& C, double x, double y, int boundary) {
   if (!isfinite(x) || !isfinite(y) || fabs(x) > 1e9 || fabs(y) > 1e9) return false;
@@ -63,6 +65,12 @@ __device__ __forceinline__ float interp_plane(const float* __restrict__ I, float
 }
 __device__ __forceinline__ float grad_g(float d) { return isfinite(d) ? d : 0.0f; }
 
+template <bool OWN_K>                                                          // OWN_K: as in find_match_direct
+__device__ __forceinline__ void project_point(const RpJob& jb, const RpConst& C, const MapDev* __restrict__ m, const sdv_map_pt& p, double* px) {
+  double pw[3], c[3]; point_world(OWN_K ? jb.Ki : C.Ki, m, p, pw);
+  SE3d w2c = se3_from7(jb.curTinv); xform(w2c, pw, c); pixel_from_cam(OWN_K ? jb.K : C.K, c, px);
+}
+
 __global__ void __launch_bounds__(256) rp_project_kernel(RpJob* __restrict__ jobs, RpConst C, RpScratch S) {
   RpJob& jb = jobs[blockIdx.y]; const MapDev* __restrict__ m = jb.map;
   if (blockIdx.x == 0 && threadIdx.x < jb.nH) {                              // per (frame, keyframe) transforms used by every findMatchDirect attempt (:262)
@@ -74,8 +82,8 @@ __global__ void __launch_bounds__(256) rp_project_kernel(RpJob* __restrict__ job
   const sdv_map_pt p = m->pts[i];
   if (p.host < 0 || p.host >= jb.nH) { jb.error = 1; return; }
   if (jb.frame_rank[p.host] < 0) return;
-  double pw[3], c[3], px[2]; point_world(C, m, p, pw);
-  SE3d w2c = se3_from7(jb.curTinv); xform(w2c, pw, c); pixel_from_cam(C, c, px);
+  double px[2];
+  if (jb.geom_row) project_point<true>(jb, C, m, p, px); else project_point<false>(jb, C, m, p, px);
   if (!in_frame(C, px[0], px[1], 8)) return;
   const int k = (int)(px[1]/kRpCell)*C.ncols + (int)(px[0]/kRpCell);
   const float* __restrict__ I = m->hostI0[p.host]; const int w = C.w[0]; const int idx = (int)(p.v*w + p.u);
@@ -122,25 +130,29 @@ constexpr int kRpWarps = 4;
 
 __device__ __forceinline__ float cur_pixel(const RpJob& jb, int level, int idx) { return __ldg(jb.cur[level] + idx); }
 
+// OWN_K: the job's slot has a K of its own (RpJob::K, Ki in global memory); otherwise the context calibration is read from the launch constants, which the
+// compiler folds into the fp64 instructions as constant-bank operands (reading every job's K from its descriptor cost the fused refinement 4.5 % on an H100)
+template <bool OWN_K>
 __device__ bool find_match_direct(const RpJob& jb, const RpConst& C, const sdv_map_pt& pt, double2& px_io, RpWarpSmem& sm, const int lane, const double* __restrict__ xf) {
+  const double* __restrict__ K = OWN_K ? jb.K : C.K; const double* __restrict__ Ki = OWN_K ? jb.Ki : C.Ki;
   const MapDev* __restrict__ m = jb.map;
   int ref;
   if (jb.nH <= 2) { if (!jb.backup) ref = 0; else if (jb.cur_kf_index == 0) ref = 1; else if (jb.cur_kf_index == 1) ref = 0; else return false; }
   else ref = pt.host;
   const float aLL0 = jb.affLL[ref][0], aLL1 = jb.affLL[ref][1];
-  double pw[3]; point_world(C, m, pt, pw);
+  double pw[3]; point_world(Ki, m, pt, pw);
   const SE3d refInv = se3_from7(xf + ref*14);
   double ptRef[3]; xform(refInv, pw, ptRef);
-  double cR[3] = {ptRef[0], ptRef[1], ptRef[2]}, px[2]; pixel_from_cam(C, cR, px);
+  double cR[3] = {ptRef[0], ptRef[1], ptRef[2]}, px[2]; pixel_from_cam(K, cR, px);
   if (!in_frame(C, px[0], px[1], 4+2)) return false;
   // getWarpMatrixAffine :14-37
   double A[4];
-  { const int hp = 5; double du[3], dv[3]; mv3(C.Ki, px[0]+hp, px[1]+0, 1.0, du); mv3(C.Ki, px[0]+0, px[1]+hp, 1.0, dv);
+  { const int hp = 5; double du[3], dv[3]; mv3(Ki, px[0]+hp, px[1]+0, 1.0, du); mv3(Ki, px[0]+0, px[1]+hp, 1.0, dv);
     const double su = ptRef[2]/du[2], sv = ptRef[2]/dv[2];
     for (int i=0;i<3;i++) { du[i] *= su; dv[i] *= sv; }
     const SE3d Tcr = se3_from7(xf + ref*14 + 7);
     double c0[3], c1[3], c2[3], pc[2], pu[2], pv[2];
-    xform(Tcr, ptRef, c0); pixel_from_cam(C, c0, pc); xform(Tcr, du, c1); pixel_from_cam(C, c1, pu); xform(Tcr, dv, c2); pixel_from_cam(C, c2, pv);
+    xform(Tcr, ptRef, c0); pixel_from_cam(K, c0, pc); xform(Tcr, du, c1); pixel_from_cam(K, c1, pu); xform(Tcr, dv, c2); pixel_from_cam(K, c2, pv);
     A[0] = (pu[0]-pc[0])/hp; A[2] = (pu[1]-pc[1])/hp; A[1] = (pv[0]-pc[0])/hp; A[3] = (pv[1]-pc[1])/hp; }
   int level = 0; { double D = A[0]*A[3] - A[2]*A[1]; while (D > 3.0 && level < C.levels-1) { level += 1; D *= 0.25; } }      // getBestSearchLevel :39-51
   // warpAffine :53-86 (halfpatch 5 -> 10x10 patch with border), values truncated to uint8
@@ -255,7 +267,8 @@ __global__ void __launch_bounds__(32*kRpWarps, RP_MATCH_MINB) rp_match_kernel(co
     last = best; first = false;
     const int bi = (int)(best & 0x7ffffffull);
     double2 px = S.cand_px[jb.pt_off + bi];
-    if (find_match_direct(jb, C, m->pts[bi], px, smem[warp], lane, S.xf + (size_t)blockIdx.y*kRpMaxHosts*14)) { found = bi; fpx = px; break; }
+    const double* xf = S.xf + (size_t)blockIdx.y*kRpMaxHosts*14;
+    if (jb.geom_row ? find_match_direct<true>(jb, C, m->pts[bi], px, smem[warp], lane, xf) : find_match_direct<false>(jb, C, m->pts[bi], px, smem[warp], lane, xf)) { found = bi; fpx = px; break; }
   }
   if (lane == 0) { S.out_pt[cb] = found; S.out_px[cb] = fpx; }
 }
@@ -278,7 +291,7 @@ __global__ void __launch_bounds__(1024) rp_emit_kernel(const RpJob* __restrict__
       sdv_overlap_pt o; o.u = p.u; o.v = p.v; o.idepth = p.idepth; o.host = p.host; o.obs_x = (float)px.x; o.obs_y = (float)px.y; ov[base + run] = o; }
     run++; }
   if (threadIdx.x == 0) { RefineJob& r = rj[blockIdx.x]; for (int i=0;i<7;i++) r.T[i] = jb.curT[i]; r.hostT = &m->hostT[0][0]; r.pt_begin = (int)base; r.pt_end = (int)base + total;
-    r.host_begin = 0; r.nH = jb.nH; r.res = 0; r.iterations = 0; r.accepts = 0; r.num = 0; n_out[blockIdx.x] = total; }
+    r.host_begin = 0; r.nH = jb.nH; r.geom_row = jb.geom_row; r.res = 0; r.iterations = 0; r.accepts = 0; r.num = 0; n_out[blockIdx.x] = total; }
 }
 
 } // namespace sdv
@@ -288,21 +301,23 @@ using namespace sdv;
 
 namespace sdv {
 struct MapSlot { long long ingest_seq = 0; MapDev host_copy; MapDev* dev = nullptr; sdv_map_pt* pts = nullptr; int cap = 0; int nH = 0, nP = 0; uint64_t host_ids[kRpMaxHosts]; double host_ab[kRpMaxHosts][2]; float host_exposure[kRpMaxHosts]; bool set = false; };
-struct RpState { std::vector<MapSlot> maps; void* dev = nullptr; void* host = nullptr; size_t cap = 0, host_cap = 0; RpConst C; bool c_ready = false; };
-static RpState* rp_state(sdv_ctx* c) { if (!c->rp) { c->rp = new RpState(); c->rp->maps.resize(c->slots.size()); } return c->rp; }
+struct RpState { std::vector<MapSlot> maps; void* dev = nullptr; void* host = nullptr; size_t cap = 0, host_cap = 0; RpConst C; };
+static void rp_job_K(const LevelGeom& g, double* K, double* Ki);
+static RpState* rp_state(sdv_ctx* c) {
+  if (!c->rp) { c->rp = new RpState(); c->rp->maps.resize(c->slots.size()); RpConst& C = c->rp->C;
+    C.levels = c->levels; for (int l=0;l<kLevels;l++) { C.w[l] = c->w >> l; C.h[l] = c->h >> l; }
+    C.ncols = (c->w + kRpCell - 1)/kRpCell; C.ncells = C.ncols*((c->h + kRpCell - 1)/kRpCell); }
+  return c->rp;
+}
 void rp_destroy(sdv_ctx* c) { if (!c->rp) return; for (auto& m : c->rp->maps) { if (m.set) for (int k=0;k<m.nH;k++) frame_unpin(c, m.host_ids[k]); cudaFree(m.dev); cudaFree(m.pts); } cudaFree(c->rp->dev); cudaFreeHost(c->rp->host); delete c->rp; c->rp = nullptr; }
-void rp_calib_changed(sdv_ctx* c) { if (c->rp) c->rp->c_ready = false; }
-static void rp_const(sdv_ctx* c, RpState* st) {
-  if (st->c_ready) return; RpConst& C = st->C; const LevelGeom& g = c->tc.geom[0];
-  for (int i=0;i<9;i++) C.K[i] = 0; C.K[0] = (double)g.fx; C.K[2] = (double)g.cx; C.K[4] = (double)g.fy; C.K[5] = (double)g.cy; C.K[8] = 1.0;
-  { const double* A = C.K; double* R = C.Ki;                                   // Eigen fixed 3x3 inverse: cofactors / determinant (K_.inverse(), Reprojector.cpp:565)
+static void rp_job_K(const LevelGeom& g, double* K, double* Ki) {        // the Reprojector's K_ and K_.inverse() (Reprojector.cpp:565) from level 0 of a geometry row
+  for (int i=0;i<9;i++) K[i] = 0; K[0] = (double)g.fx; K[2] = (double)g.cx; K[4] = (double)g.fy; K[5] = (double)g.cy; K[8] = 1.0;
+  { const double* A = K; double* R = Ki;                                       // Eigen fixed 3x3 inverse: cofactors / determinant
 #define COF(i,j) (A[((i+1)%3)*3+((j+1)%3)]*A[((i+2)%3)*3+((j+2)%3)] - A[((i+1)%3)*3+((j+2)%3)]*A[((i+2)%3)*3+((j+1)%3)])
     const double c00 = COF(0,0), c10 = COF(1,0), c20 = COF(2,0); const double det = (c00*A[0] + c10*A[3]) + c20*A[6], invdet = 1.0/det;
     R[0]=c00*invdet; R[1]=c10*invdet; R[2]=c20*invdet; R[3]=COF(0,1)*invdet; R[4]=COF(1,1)*invdet; R[5]=COF(2,1)*invdet; R[6]=COF(0,2)*invdet; R[7]=COF(1,2)*invdet; R[8]=COF(2,2)*invdet;
 #undef COF
   }
-  C.levels = c->levels; for (int l=0;l<kLevels;l++) { C.w[l] = c->w >> l; C.h[l] = c->h >> l; }
-  C.ncols = (c->w + kRpCell - 1)/kRpCell; C.ncells = C.ncols*((c->h + kRpCell - 1)/kRpCell); st->c_ready = true;
 }
 }
 
@@ -347,7 +362,7 @@ int sdv_map_clear(sdv_ctx* c, int slot) { SDV_GUARD_TRK(c);
 struct RpRun { RpScratch S; RpJob* jobs_dev; RpJob* jobs_host; int32_t* h_opt; double2* h_opx; sdv_overlap_pt* ov; RefineJob* rj; RefineJob* rj_host; int* n_out_dev; int* n_out_host; int* cell_order_dev; long long nc; };
 static int rp_launch(sdv_ctx* c, int n_jobs, const int32_t* slots, const uint64_t* cur_frames, const double* cur_T7, const double* cur_ab,
                      const int32_t* cur_kf_index, const int32_t* only_host, const int32_t* backup, RpRun& R) {
-  RpState* st = rp_state(c); rp_const(c, st); const RpConst& C = st->C;
+  RpState* st = rp_state(c); rp_job_K(c->geom[0].g[0], st->C.K, st->C.Ki); const RpConst& C = st->C;
   long long totalP = 0; int maxP = 1;
   for (int k=0;k<n_jobs;k++) { if (slots[k] < 0 || slots[k] >= (int)st->maps.size() || !st->maps[slots[k]].set) return ctx_fail(c, SDV_ERR_STATE, "reproject job %d: map slot %d not set", k, slots[k]);
     totalP += st->maps[slots[k]].nP; maxP = std::max(maxP, st->maps[slots[k]].nP); }
@@ -374,6 +389,7 @@ static int rp_launch(sdv_ctx* c, int n_jobs, const int32_t* slots, const uint64_
     auto it = c->frame_index.find(cur_frames[k]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "reproject job %d: unknown target frame", k);
     const FrameDev& f = c->frames[it->second];
     j.map = m.dev; for (int l=0;l<c->levels;l++) j.cur[l] = f.img[l];
+    rp_job_K(slot_geom(c, slots[k]).g[0], j.K, j.Ki); j.geom_row = c->slots[slots[k]].geom_row;
     for (int i=0;i<7;i++) j.curT[i] = cur_T7[7*k+i];
     const SE3d cur = se3_from7(j.curT); se3_to7(se3_inv(cur), j.curTinv);
     j.cur_kf_index = cur_kf_index ? cur_kf_index[k] : -1; j.backup = backup ? backup[k] : 0; j.nH = m.nH; j.nP = m.nP; j.pt_off = off; off += m.nP;
@@ -435,7 +451,7 @@ int sdv_tracker_refine_batch(sdv_ctx* c, int n_jobs, const int32_t* slots, const
   if (cell_order) { for (int i=0;i<C.ncells;i++) if (cell_order[i] < 0 || cell_order[i] >= C.ncells) return ctx_fail(c, SDV_ERR_ARG, "cell_order[%d] = %d", i, cell_order[i]);
     CK(cudaMemcpyAsync(R.cell_order_dev, cell_order, (size_t)C.ncells*4, cudaMemcpyHostToDevice, s)); }
   rp_emit_kernel<<<n_jobs, 1024, 0, s>>>(R.jobs_dev, C, R.S, cell_order ? R.cell_order_dev : nullptr, max_matches, R.ov, R.rj, R.n_out_dev);
-  launch_struct_pose(R.rj, n_jobs, R.ov, nullptr, c->tc_dev, s);
+  launch_struct_pose(R.rj, n_jobs, R.ov, nullptr, c->geom_dev, s);
   CK(cudaGetLastError()); c->launches += 2;
   CK(cudaEventRecord(c->ev1, s));
   CK(cudaMemcpyAsync(R.rj_host, R.rj, (size_t)n_jobs*sizeof(RefineJob), cudaMemcpyDeviceToHost, s));
