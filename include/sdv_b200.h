@@ -95,6 +95,18 @@ int  sdv_frame_upload_batch_u8(sdv_ctx* c, int n, const uint64_t* frames, const 
  * level-0/level-1 pyramid build are ONE kernel.  Entries that would read outside the raw image are refused (SDV_ERR_ARG). */
 int  sdv_set_undistort(sdv_ctx* c, int w_org, int h_org, const float* remapX, const float* remapY, float factor, const float* G256, const float* vignette_inv);
 int  sdv_frame_upload_batch_raw_u8(sdv_ctx* c, int n, const uint64_t* frames, const uint8_t* const* raw_imgs_worg_horg, const float* exposures);
+/* RAW ingest of several cameras in one context: one Undistort object per calibration file (util/Undistort.cpp:232-334, what src/main.cpp builds once
+ * per sequence), kept side by side.  sdv_set_undistort_cam sets or replaces camera `cam`'s tables, with the arguments and checks of sdv_set_undistort;
+ * the raw size w_org x h_org is per camera, the remap tables always have the context's rectified w*h size.  Replacing a camera is stream-ordered: an
+ * ingest already enqueued finishes with the old tables; the other cameras are untouched.  sdv_set_undistort is this call with cam = 0.
+ * sdv_frame_upload_batch_raw_u8_cams: image k is native w_org x h_org mono8 of camera cams[k], rectified with that camera's tables in the same one
+ * kernel (cams == NULL: every image is camera 0, which is sdv_frame_upload_batch_raw_u8).  Example: the KITTI odometry calibrations (calib/KITTI/00.txt,
+ * 03.txt, 04.txt) come in three raw sizes, 1241x376, 1242x375 and 1226x370, that all crop to 1200x360 with different rectified K: one camera each,
+ * every sequence's tracker slots bound to its camera's K with sdv_set_calib_slots, and all sequences ingested in one batch.  cams is checked before
+ * anything else: an index outside [0, SDV_MAX_CAMERAS) returns SDV_ERR_ARG, a camera that was never set SDV_ERR_STATE, and a refused call changes no frame. */
+#define SDV_MAX_CAMERAS 8
+int  sdv_set_undistort_cam(sdv_ctx* c, int cam, int w_org, int h_org, const float* remapX, const float* remapY, float factor, const float* G256, const float* vignette_inv);
+int  sdv_frame_upload_batch_raw_u8_cams(sdv_ctx* c, int n, const uint64_t* frames, const uint8_t* const* raw_imgs, const int32_t* cams, const float* exposures);
 int  sdv_frame_build_batch_dev(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs_dev, int fmt, const float* exposures);
 /* fmt: 0 float (copied into frame storage), 1 mono8, 2 float ADOPTED as the frame's level-0 plane (zero copy: the buffer must stay
  * valid and unmodified until sdv_frame_release / the handle is re-uploaded — for producers that already write into device memory). */

@@ -77,6 +77,13 @@ int shim_set_undistort(const Undistort* u, const float* G256_or_null, const floa
 int shim_ingest_raw(FrameShell* shell, const uint8_t* raw_mono8, float exposure) {
   uint64_t id = (uint64_t)shell->id; return sdv_frame_upload_batch_raw_u8(gpu, 1, &id, &raw_mono8, &exposure);
 }
+// §4 batched mode, one context for several cameras: tables per camera, each raw image names its camera
+int shim_set_undistort_cam(int cam, const Undistort* u) {
+  return sdv_set_undistort_cam(gpu, cam, u->wOrg, u->hOrg, u->remapX, u->remapY, 1.0f, nullptr, nullptr);
+}
+int shim_ingest_raw_cams(int n, const uint64_t* ids, const uint8_t* const* raw_mono8, const int32_t* cams, const float* exposures) {
+  return sdv_frame_upload_batch_raw_u8_cams(gpu, n, ids, raw_mono8, cams, exposures);
+}
 // §3c CoarseTracker::makeK (CoarseTracker.cpp:77-106): a member of each tracker instance, so it sets the K of that instance's slot only
 int shim_makeK(int slot, CalibHessian* HCalib) { sdv_calib K{HCalib->fxl(), HCalib->fyl(), HCalib->cxl(), HCalib->cyl()}; const int32_t s = slot; return sdv_set_calib_slots(gpu, 1, &s, &K); }
 
@@ -263,6 +270,7 @@ int shim_activateSelect(const ActivationInputs& in, std::vector<int32_t>& decisi
 int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const Undistort* u, const uint8_t* raw) {
   std::vector<int32_t> sel, st; Vec5 mr{}; SE3 T; AffLight a;
   int rc = shim_create(hc) | shim_set_undistort(u, nullptr, nullptr) | shim_ingest_raw(fh->shell, raw, 1.0f) | shim_makeK(fs.coarseTracker->slot, &hc);
+  { const uint64_t id = (uint64_t)fh->shell->id; const int32_t cam = 1; const float ex = 1.0f; rc |= shim_set_undistort_cam(cam, u) | shim_ingest_raw_cams(1, &id, &raw, &cam, &ex); }
   fs.coarseTracker->setCoarseTrackingRef(fs.frameHessians); fs.coarseTracker->trackNewestCoarse(fh, T, a, 3, mr, nullptr);
   std::vector<ImmaturePoint*> imm; std::vector<HostImmatures> hi; rc |= shim_makeNewTraces(fh, sel, imm) | shim_traceNewCoarse(fh, hi);
   std::vector<ActivationGroup> ag; std::vector<float> idp; rc |= shim_activatePoints(ag, st, idp, sel, 7);

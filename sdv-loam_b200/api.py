@@ -62,6 +62,8 @@ def _load():
     L.sdv_frame_build_batch_dev.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), C.c_int, _f32p]
     L.sdv_set_undistort.argtypes = [_vp, C.c_int, C.c_int, _f32p, _f32p, C.c_float, _vp, _vp]
     L.sdv_frame_upload_batch_raw_u8.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _f32p]
+    L.sdv_set_undistort_cam.argtypes = [_vp, C.c_int, C.c_int, C.c_int, _f32p, _f32p, C.c_float, _vp, _vp]
+    L.sdv_frame_upload_batch_raw_u8_cams.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _vp, _f32p]
     L.sdv_track_job_bytes.argtypes = []
     L.sdv_launch_count.argtypes = [_vp]; L.sdv_launch_count.restype = C.c_longlong
     L.sdv_frame_release.argtypes = [_vp, C.c_uint64]
@@ -173,24 +175,28 @@ class Context:
         self._ck(LIB.sdv_set_calib_slots(self.p, len(sl), sl, None))
 
     # Undistort (util/Undistort.cpp) handed over as data; `und` = sdv_loam_b200.undistort.Undistort or anything with wOrg,hOrg,remapX,remapY[,G,vignetteMapInv]
-    def setUndistort(self, und, factor: float = 1.0):
+    # cam: which of the context's SDV_MAX_CAMERAS cameras these tables set or replace (the raw size is per camera, the rectified size is the context's)
+    def setUndistort(self, und, factor: float = 1.0, cam: int = 0):
         rx = np.ascontiguousarray(und.remapX, np.float32).reshape(-1); ry = np.ascontiguousarray(und.remapY, np.float32).reshape(-1)
         assert rx.size == self.w * self.h == ry.size, "remap tables must have the rectified size given to the context"
         G = getattr(und, "G", None); V = getattr(und, "vignetteMapInv", None)
         G = None if G is None else np.ascontiguousarray(G, np.float32); V = None if V is None else np.ascontiguousarray(V, np.float32)
         assert G is None or G.size == 256
         assert V is None or V.size == und.wOrg * und.hOrg
-        self._ck(LIB.sdv_set_undistort(self.p, int(und.wOrg), int(und.hOrg), rx, ry, float(factor), None if G is None else G.ctypes.data, None if V is None else V.ctypes.data))
-        self.wh_org = (int(und.wOrg), int(und.hOrg))
+        self._ck(LIB.sdv_set_undistort_cam(self.p, int(cam), int(und.wOrg), int(und.hOrg), rx, ry, float(factor), None if G is None else G.ctypes.data, None if V is None else V.ctypes.data))
+        self.wh_org = getattr(self, "wh_org", {}); self.wh_org[int(cam)] = (int(und.wOrg), int(und.hOrg))
 
-    def makeImagesRaw(self, frame_id: int, raw, exposure: float = 1.0):
-        """Undistort::undistort<unsigned char> + FrameHessian::makeImages of one native-size mono8 image"""
-        raw = np.ascontiguousarray(raw, np.uint8); assert raw.shape == (self.wh_org[1], self.wh_org[0])
-        self.makeImagesBatch([frame_id], [raw.ctypes.data], [exposure], raw=True); self.sync()
+    def makeImagesRaw(self, frame_id: int, raw, exposure: float = 1.0, cam: int = 0):
+        """Undistort::undistort<unsigned char> + FrameHessian::makeImages of one native-size mono8 image of camera `cam`"""
+        raw = np.ascontiguousarray(raw, np.uint8)
+        if cam in getattr(self, "wh_org", {}):
+            assert raw.shape == (self.wh_org[cam][1], self.wh_org[cam][0]), f"camera {cam} takes {self.wh_org[cam][0]}x{self.wh_org[cam][1]} images"
+        self.makeImagesBatch([frame_id], [raw.ctypes.data], [exposure], raw=True, cams=[cam]); self.sync()
 
-    def makeImagesBatch(self, frame_ids, ptrs, exposures=None, u8=False, device=False, adopt=False, raw=False):
+    def makeImagesBatch(self, frame_ids, ptrs, exposures=None, u8=False, device=False, adopt=False, raw=False, cams=None):
         """Batched makeImages.  ptrs: integer addresses of (h,w) buffers — host (pinned for full-rate, asynchronous H2D)
-        or device (device=True); float32, or mono8 when u8=True; raw=True: native-size mono8 through setUndistort's tables.
+        or device (device=True); float32, or mono8 when u8=True; raw=True: native-size mono8 through setUndistort's tables,
+        image k of camera cams[k] (None: every image is camera 0).
         A uint64 numpy array of addresses avoids per-call list work.  Asynchronous: see sdv_b200.h."""
         n = len(frame_ids)
         ids = np.ascontiguousarray(frame_ids, np.uint64)
@@ -199,7 +205,12 @@ class Context:
         else:
             arr = (_vp * n)(*ptrs)
         ex = self._ones(n) if exposures is None else np.ascontiguousarray(exposures, np.float32)
-        if raw:
+        if raw and cams is not None:
+            cm = np.ascontiguousarray(cams, np.int32).reshape(-1)
+            if len(cm) != n:
+                raise ValueError(f"{n} frames but {len(cm)} camera indices")
+            self._ck(LIB.sdv_frame_upload_batch_raw_u8_cams(self.p, n, ids, arr, cm.ctypes.data, ex))
+        elif raw:
             self._ck(LIB.sdv_frame_upload_batch_raw_u8(self.p, n, ids, arr, ex))
         elif device:
             self._ck(LIB.sdv_frame_build_batch_dev(self.p, n, ids, arr, 1 if u8 else (2 if adopt else 0), ex))

@@ -177,7 +177,8 @@ void sdv_destroy(sdv_ctx* c) {
   for (int i=0;i<2;i++) { cudaFree(c->pyr_batch_dev[i]); cudaFreeHost(c->pyr_batch_host[i]); } cudaFree(c->partials); cudaFree(c->ticket); cudaFree(c->totals_dev); cudaFreeHost(c->totals_host);
   cudaFree(c->tc_dev); cudaFree(c->geom_dev); cudaFree(c->jobs_dev); cudaFreeHost(c->jobs_host);
   for (int i=0;i<2;i++) cudaFree(c->stage_u8[i]);
-  cudaFree(c->und_buf); cudaFree(c->trace_dev);
+  for (float* u : c->und_buf) cudaFree(u);
+  cudaFree(c->trace_dev);
   for (int i=0;i<sdv_ctx::kIngRing;i++) if (c->ev_ing[i]) cudaEventDestroy(c->ev_ing[i]); for (int i=0;i<2;i++) if (c->ev_cp[i]) cudaEventDestroy(c->ev_cp[i]); if (c->st_cp) cudaStreamDestroy(c->st_cp);
   cudaFree(c->refine_dev); cudaFreeHost(c->refine_host);
   rp_destroy(c);
@@ -212,27 +213,35 @@ static int ensure_desc(sdv_ctx* c, int n) {
 static void frame_drop_texels(sdv_ctx* c, FrameDev& f) { if (f.lvl0_slot >= 0) { c->lvl0_free.push_back(f.lvl0_slot); f.lvl0_slot = -1; } f.lvl[0] = nullptr; f.hi_tex = false; }
 
 // kind bit0: mono8 input, bit1: input already in device memory, bit2: adopt the (device, float) buffer as the frame's level-0 plane,
-// bit3: RAW mono8 input of the camera's native size, rectified through the tables of sdv_set_undistort inside the level-0 kernel.
+// bit3: RAW mono8 input of the camera's native size, rectified through the tables of sdv_set_undistort_cam inside the level-0 kernel; image k is camera
+// cams[k] (cams == NULL: camera 0), so the raw byte size, the staging offset and the coalesced copies are per frame.
 // Everything is enqueued on the ingest stream; the compute stream picks it up through ev_in at the next tracker / BA call, so an
 // upload overlaps the tracking of the previous batch.  Every level is a planar intensity image: a pinned-host float upload lands directly in
 // frame storage, levels >= 1 are built by one fused launch, and the consumers form gradients on the fly.
-static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs, const float* exposures, int kind) {
+static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs, const float* exposures, int kind, const int32_t* cams = nullptr) {
   if (!c || n < 0 || !frames || !imgs) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK;
+  const bool raw = (kind & 8), u8 = (kind & 1) || raw, dev = (kind & 2), adopt = (kind & 4) && dev && !u8;
+  if (raw) for (int k=0;k<n;k++) {                                       // before any frame handle is claimed or anything is enqueued: a refused call changes no frame
+    const int cam = cams ? cams[k] : 0;
+    if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "image %d names camera %d (valid: 0..%d)", k, cam, SDV_MAX_CAMERAS - 1);
+    if (!c->und.cam[cam].remapX) return ctx_fail(c, SDV_ERR_STATE, "raw upload before sdv_set_undistort (camera %d has no tables)", cam);
+  }
   CK(cudaSetDevice(c->device));
   const long long seq = c->ingest_seq + 1; const int par = (int)(seq & 1);
   // staging buffers + descriptors of this parity were last used by ingest seq-2: it must have drained before the host rewrites the pinned
   // descriptors (the device-side order copy(seq) after pyramid(seq-2) is enforced on the copy stream below)
   if (seq > 2) CK(cudaEventSynchronize(c->ev_ing[(seq-2) % sdv_ctx::kIngRing]));
   int rc = ensure_desc(c, n); if (rc) return rc;
-  const bool raw = (kind & 8), u8 = (kind & 1) || raw, dev = (kind & 2), adopt = (kind & 4) && dev && !u8;
-  if (raw && !c->has_und) return ctx_fail(c, SDV_ERR_STATE, "raw upload before sdv_set_undistort");
-  const size_t px = (size_t)c->w*c->h, px_in = raw ? (size_t)c->und.wOrg*c->und.hOrg : px;     // bytes of one mono8 input image
-  if (u8 && !dev && (size_t)n*px_in > c->stage_u8_cap[par]) { CK(cudaStreamSynchronize(c->st_in)); cudaFree(c->stage_u8[par]); c->stage_u8[par] = nullptr;
-    c->stage_u8_cap[par] = (size_t)n*px_in; CK(cudaMalloc(&c->stage_u8[par], c->stage_u8_cap[par])); }
+  const size_t px = (size_t)c->w*c->h;
+  auto cam_of = [&](int k) { return raw && cams ? cams[k] : 0; };
+  auto px_in = [&](int k) { const sdv::UndistortDev& u = c->und.cam[cam_of(k)]; return raw ? (size_t)u.wOrg*u.hOrg : px; };   // bytes of mono8 input image k
+  if (u8 && !dev) { size_t total = 0; for (int k=0;k<n;k++) total += px_in(k);
+    if (total > c->stage_u8_cap[par]) { CK(cudaStreamSynchronize(c->st_in)); cudaFree(c->stage_u8[par]); c->stage_u8[par] = nullptr;
+      c->stage_u8_cap[par] = total; CK(cudaMalloc(&c->stage_u8[par], c->stage_u8_cap[par])); } }
   c->cp_dst.clear(); c->cp_src.clear(); c->cp_sz.clear();
   if (c->levels > 1 && ((c->w | c->h) & 1)) return ctx_fail(c, SDV_ERR_ARG, "pyramid needs even image sizes");
-  PyrBatchHost* desc = c->pyr_batch_host[par]; bool vec = true;
+  PyrBatchHost* desc = c->pyr_batch_host[par]; bool vec = true; size_t stage_off = 0;
   for (int k=0;k<n;k++) {
     int idx = -1;
     auto it = c->frame_index.find(frames[k]);
@@ -244,11 +253,11 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
     frame_drop_texels(c, f); f.ingest_seq = seq;
     f.adopted = adopt; f.I0 = adopt ? const_cast<float*>(reinterpret_cast<const float*>(imgs[k])) : f.I0_own; f.img[0] = f.I0;
     PyrBatchHost& b = desc[k];
-    b.pyr = f.pyr; b.I0 = f.I0; b.flags = (f.exposure > 0.f) ? 1 : 0; b.pad = 0;
+    b.pyr = f.pyr; b.I0 = f.I0; b.flags = (f.exposure > 0.f) ? 1 : 0; b.cam = cam_of(k);
     if (dev) b.src = imgs[k];
-    else if (u8) { unsigned char* d8 = c->stage_u8[par] + (size_t)k*px_in; b.src = d8;
-      if (!c->cp_dst.empty() && (unsigned char*)c->cp_src.back() + c->cp_sz.back() == (const unsigned char*)imgs[k] && (unsigned char*)c->cp_dst.back() + c->cp_sz.back() == d8) c->cp_sz.back() += px_in;   // adjacent in host memory: one copy
-      else { c->cp_dst.push_back(d8); c->cp_src.push_back(const_cast<void*>(imgs[k])); c->cp_sz.push_back(px_in); } }
+    else if (u8) { const size_t sz = px_in(k); unsigned char* d8 = c->stage_u8[par] + stage_off; stage_off += sz; b.src = d8;
+      if (!c->cp_dst.empty() && (unsigned char*)c->cp_src.back() + c->cp_sz.back() == (const unsigned char*)imgs[k] && (unsigned char*)c->cp_dst.back() + c->cp_sz.back() == d8) c->cp_sz.back() += sz;   // adjacent in host memory: one copy, whatever the cameras
+      else { c->cp_dst.push_back(d8); c->cp_src.push_back(const_cast<void*>(imgs[k])); c->cp_sz.push_back(sz); } }
     else { b.src = f.I0; c->cp_dst.push_back(f.I0); c->cp_src.push_back(const_cast<void*>(imgs[k])); c->cp_sz.push_back(px*sizeof(float)); }
     vec = vec && ((uintptr_t)b.src % (u8 ? 4 : 16)) == 0 && ((uintptr_t)b.I0 % 16) == 0;   // 4-pixel vector loads / stores of the pyramid kernel
   }
@@ -267,7 +276,7 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
   }
   launch_h2d_words(c->pyr_batch_dev[par], desc, (size_t)n*sizeof(PyrBatchHost), c->st_in);   // kernel copy: a cudaMemcpyAsync here becomes ready only after this batch's bulk copy and
   c->launches += 1;                                                                              // would queue behind the NEXT batch's bulk copy on the H2D engine
-  const UndistortDev* und = raw ? &c->und : nullptr;
+  const UndistortCams* und = raw ? &c->und : nullptr;
   if (c->levels > 1) { launch_pyramid_batch(c->pyr_batch_dev[par], n, u8, vec, c->w, c->h, c->levels, c->st_in, und); c->launches += 1; }
   else if (u8 || (dev && !adopt)) { launch_pyramid_copy0(c->pyr_batch_dev[par], n, u8, c->w, c->h, c->st_in, und); c->launches += 1; }
   CK(cudaGetLastError());
@@ -312,9 +321,10 @@ int sdv_frame_upload_batch(sdv_ctx* c, int n, const uint64_t* frames, const floa
 int sdv_frame_upload_batch_u8(sdv_ctx* c, int n, const uint64_t* frames, const uint8_t* const* imgs, const float* exposures) { SDV_GUARD_TRK(c);
   return frame_ingest(c, n, frames, reinterpret_cast<const void* const*>(imgs), exposures, 1);
 }
-// Undistort (util/Undistort.cpp) as data: the tables the reference builds once per calibration file, kept on the device for the raw-image ingest
-int sdv_set_undistort(sdv_ctx* c, int w_org, int h_org, const float* remapX, const float* remapY, float factor, const float* G256, const float* vignette_inv) { SDV_GUARD_TRK(c);
+// Undistort (util/Undistort.cpp) as data: the tables the reference builds once per calibration file, kept on the device for the raw-image ingest, one entry per camera
+int sdv_set_undistort_cam(sdv_ctx* c, int cam, int w_org, int h_org, const float* remapX, const float* remapY, float factor, const float* G256, const float* vignette_inv) { SDV_GUARD_TRK(c);
   if (!c || w_org < 2 || h_org < 2 || !remapX || !remapY) return SDV_ERR_ARG;
+  if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "camera %d outside 0..%d", cam, SDV_MAX_CAMERAS - 1);
   if (vignette_inv && !G256) return ctx_fail(c, SDV_ERR_ARG, "a vignette map needs a response function (PhotometricUndistorter::processFrame applies it to G[v] only)");
   CK(cudaSetDevice(c->device));
   const size_t px = (size_t)c->w*c->h, po = (size_t)w_org*h_org;
@@ -323,21 +333,27 @@ int sdv_set_undistort(sdv_ctx* c, int w_org, int h_org, const float* remapX, con
     if (x < 0) continue;
     if (!(x > 0 && y > 0 && x < w_org-1 && y < h_org-1)) return ctx_fail(c, SDV_ERR_ARG, "remap table entry %zu (%g,%g) reads outside the %dx%d raw image", i, x, y, w_org, h_org);
   }
-  CK(cudaStreamSynchronize(c->st_in));                                     // an ingest in flight may still read the previous tables
-  cudaFree(c->und_buf); c->und_buf = nullptr; c->has_und = false;
+  CK(cudaStreamSynchronize(c->st_in));                                     // an ingest in flight may still read the previous tables of this camera
+  sdv::UndistortDev& u = c->und.cam[cam];
+  cudaFree(c->und_buf[cam]); c->und_buf[cam] = nullptr; u = {};
   const size_t nfl = 2*px + (G256 ? 256 : 0) + (vignette_inv ? po : 0);
-  CK(cudaMalloc(&c->und_buf, nfl*sizeof(float)));
-  float* p = c->und_buf;
-  CK(cudaMemcpy(p, remapX, px*sizeof(float), cudaMemcpyHostToDevice)); c->und.remapX = p; p += px;
-  CK(cudaMemcpy(p, remapY, px*sizeof(float), cudaMemcpyHostToDevice)); c->und.remapY = p; p += px;
-  c->und.G = nullptr; c->und.vignette = nullptr;
-  if (G256) { CK(cudaMemcpy(p, G256, 256*sizeof(float), cudaMemcpyHostToDevice)); c->und.G = p; p += 256; }
-  if (vignette_inv) { CK(cudaMemcpy(p, vignette_inv, po*sizeof(float), cudaMemcpyHostToDevice)); c->und.vignette = p; p += po; }
-  c->und.wOrg = w_org; c->und.hOrg = h_org; c->und.factor = factor; c->has_und = true;
+  float* p = nullptr; CK(cudaMalloc(&p, nfl*sizeof(float))); c->und_buf[cam] = p;
+  sdv::UndistortDev d = {};
+  CK(cudaMemcpy(p, remapX, px*sizeof(float), cudaMemcpyHostToDevice)); d.remapX = p; p += px;
+  CK(cudaMemcpy(p, remapY, px*sizeof(float), cudaMemcpyHostToDevice)); d.remapY = p; p += px;
+  if (G256) { CK(cudaMemcpy(p, G256, 256*sizeof(float), cudaMemcpyHostToDevice)); d.G = p; p += 256; }
+  if (vignette_inv) { CK(cudaMemcpy(p, vignette_inv, po*sizeof(float), cudaMemcpyHostToDevice)); d.vignette = p; p += po; }
+  d.wOrg = w_org; d.hOrg = h_org; d.factor = factor; u = d;                // set only once every table is on the device
   return SDV_OK;
 }
-int sdv_frame_upload_batch_raw_u8(sdv_ctx* c, int n, const uint64_t* frames, const uint8_t* const* raw_imgs, const float* exposures) { SDV_GUARD_TRK(c);
-  return frame_ingest(c, n, frames, reinterpret_cast<const void* const*>(raw_imgs), exposures, 8);
+int sdv_set_undistort(sdv_ctx* c, int w_org, int h_org, const float* remapX, const float* remapY, float factor, const float* G256, const float* vignette_inv) {
+  return sdv_set_undistort_cam(c, 0, w_org, h_org, remapX, remapY, factor, G256, vignette_inv);
+}
+int sdv_frame_upload_batch_raw_u8_cams(sdv_ctx* c, int n, const uint64_t* frames, const uint8_t* const* raw_imgs, const int32_t* cams, const float* exposures) { SDV_GUARD_TRK(c);
+  return frame_ingest(c, n, frames, reinterpret_cast<const void* const*>(raw_imgs), exposures, 8, cams);
+}
+int sdv_frame_upload_batch_raw_u8(sdv_ctx* c, int n, const uint64_t* frames, const uint8_t* const* raw_imgs, const float* exposures) {
+  return sdv_frame_upload_batch_raw_u8_cams(c, n, frames, raw_imgs, nullptr, exposures);
 }
 int sdv_frame_build_batch_dev(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs_dev, int fmt, const float* exposures) { SDV_GUARD_TRK(c);
   if (fmt < 0 || fmt > 2) return SDV_ERR_ARG;

@@ -53,7 +53,8 @@ struct sdv_ctx {
   std::unordered_map<uint64_t,int> pins;
   unsigned char* stage_u8[2] = {nullptr, nullptr}; size_t stage_u8_cap[2] = {0, 0};   // contiguous mono8 staging per parity (adjacent host images coalesce into one copy)
   int desc_cap; sdv::PyrBatchHost* pyr_batch_dev[2]; sdv::PyrBatchHost* pyr_batch_host[2];     // double-buffered by ingest parity
-  sdv::UndistortDev und = {}; bool has_und = false; float* und_buf = nullptr;       // sdv_set_undistort: remap tables (+ response / vignette) of the raw-image ingest
+  sdv::UndistortCams und = {}; float* und_buf[SDV_MAX_CAMERAS] = {};                 // sdv_set_undistort_cam: per camera, remap tables (+ response / vignette) of the raw-image ingest
+                                                                                    // in one allocation und_buf[k]; a camera is set iff und.cam[k].remapX != nullptr
   std::vector<float4*> lvl0_pool; std::vector<int> lvl0_free;
   std::vector<void*> cp_dst, cp_src; std::vector<size_t> cp_sz; bool no_batch_copy = false;
   std::vector<sdv::TrackerSlot> slots;

@@ -30,7 +30,7 @@ static int num_sms() {
 // ================================================================================================ pyramid
 // Every level of a frame is a planar float intensity plane (level 0: the frame's I0; levels >= 1: the frame's `pyr` allocation at lvl_off[l]).
 // Packed {I,dx,dy,|grad|^2} texels are a derived cache that only keyframe-rate consumers build (grad_texel_kernel).
-struct PyrBatch { const void* src; float* I0; float* pyr; int flags; int pad; };   // per frame: level-0 input (float/u8; may equal I0), level-0 plane, planes of levels >= 1; flags bit0: photometric response applies (exposure > 0)
+struct PyrBatch { const void* src; float* I0; float* pyr; int flags; int cam; };   // per frame: level-0 input (float/u8; may equal I0), level-0 plane, planes of levels >= 1; flags bit0: photometric response applies (exposure > 0); cam: Undistort camera of a RAW input
 static_assert(sizeof(PyrBatch) == sizeof(PyrBatchHost), "PyrBatch mirrors PyrBatchHost");
 
 template <typename T> __device__ __forceinline__ float px_load(const T* p, int i);
@@ -82,8 +82,9 @@ __device__ __forceinline__ float undist_px(const unsigned char* __restrict__ raw
   const float s0 = undist_tap(raw, o, U, photo), s1 = undist_tap(raw, o+1, U, photo), sw = undist_tap(raw, o+U.wOrg, U, photo), sw1 = undist_tap(raw, o+1+U.wOrg, U, photo);
   return xxyy*sw1 + (yy-xxyy)*sw + (xx-xxyy)*s1 + (1-xx-yy+xxyy)*s0;
 }
-__global__ void __launch_bounds__(256) pyr_remap0_kernel(const PyrBatch* __restrict__ batch, UndistortDev U, int n) {
-  const PyrBatch b = batch[blockIdx.y]; const bool photo = (b.flags & 1) && U.G;
+// Each CTA serves one frame and reads that frame's camera entry once (the table is a __grid_constant__ parameter: indexed in place, never copied per thread).
+__global__ void __launch_bounds__(256) pyr_remap0_kernel(const PyrBatch* __restrict__ batch, const __grid_constant__ UndistortCams cams, int n) {
+  const PyrBatch b = batch[blockIdx.y]; const UndistortDev U = cams.cam[b.cam]; const bool photo = (b.flags & 1) && U.G;
   for (int idx = blockIdx.x*blockDim.x + threadIdx.x; idx < n; idx += gridDim.x*blockDim.x) b.I0[idx] = undist_px(reinterpret_cast<const unsigned char*>(b.src), idx, U, photo);
 }
 
@@ -91,14 +92,16 @@ __global__ void __launch_bounds__(256) pyr_remap0_kernel(const PyrBatch* __restr
 // The CTA reads its band of the level-0 input once, keeps levels 1..levels-2 of the band in shared memory and writes every level >= 1 to the frame's planes.
 // Each pixel is 0.25f*(((a+b)+c)+d) of its 2x2 parent quad in the flat-index layout of the per-level filter (parent row 2y, columns 2x, 2x+1 of a level of
 // width wlm1 at 2x + 2y*wlm1), so odd intermediate sizes drop the last column / row exactly as that filter did; a band past the last row of a coarse level
-// simply has fewer (or no) rows there.  Level 0 comes from a float plane (resident or adopted), mono8, or RAW mono8 through the Undistort tables (RAW),
+// simply has fewer (or no) rows there.  Level 0 comes from a float plane (resident or adopted), mono8, or RAW mono8 through its camera's Undistort tables (RAW),
 // and is written to the frame's I0 plane whenever the input is not that plane already.
 // P = level-1 pixels per work item: 2 reads each parent row as one 16-byte (float) / 4-byte (mono8) vector, 1 reads scalars (unaligned input or w % 4 != 0).
 constexpr int kPyrThreads = 256;
 template <typename T, bool RAW, int P>
-__global__ void __launch_bounds__(kPyrThreads) pyr_fused_kernel(const PyrBatch* __restrict__ batch, UndistortDev U, int w, int h, int levels) {
+__global__ void __launch_bounds__(kPyrThreads) pyr_fused_kernel(const PyrBatch* __restrict__ batch, const __grid_constant__ UndistortCams cams, int w, int h, int levels) {
   extern __shared__ float pyr_band[];                       // levels 1..levels-2 of the band: [R1][w1] [R1/2][w2] ...
   const PyrBatch b = batch[blockIdx.y];
+  UndistortDev U{};
+  if constexpr (RAW) U = cams.cam[b.cam];                   // RAW: this frame's camera
   const T* src = reinterpret_cast<const T*>(b.src);
   float* I0 = (RAW || reinterpret_cast<const void*>(b.I0) != b.src) ? b.I0 : nullptr;
   const bool photo = RAW && (b.flags & 1) && U.G;
@@ -163,7 +166,7 @@ static size_t pyr_band_bytes(int w, int levels) {
   return n*sizeof(float);
 }
 template <typename T, bool RAW, int P>
-static void launch_pyr_fused(const PyrBatch* batch_dev, int nframes, int w, int h, int levels, const UndistortDev& U, cudaStream_t st) {
+static void launch_pyr_fused(const PyrBatch* batch_dev, int nframes, int w, int h, int levels, const UndistortCams& U, cudaStream_t st) {
   const size_t smem = pyr_band_bytes(w, levels);
   if (smem > 48*1024) cudaFuncSetAttribute(pyr_fused_kernel<T, RAW, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);   // very wide images; a refusal surfaces as the launch error
   const int R1 = 1 << (levels - 2);
@@ -174,10 +177,10 @@ static void launch_pyr_fused(const PyrBatch* batch_dev, int nframes, int w, int 
 // batch_dev: nframes PyrBatch descriptors in device memory.  src_u8: level-0 input is mono8 (sensor_msgs/Image wire format) instead of float.
 // vec: every level-0 input (and I0 plane written) of the batch is 16-byte aligned; the 4-pixel vector path additionally needs w % 4 == 0.
 // Requires even w,h whenever levels > 1 (pyrLevelsUsed only halves even sizes, globalCalib.cpp:24).
-void launch_pyramid_batch(const void* batch_dev_v, int nframes, bool src_u8, bool vec, int w, int h, int levels, cudaStream_t st, const UndistortDev* und) {
+void launch_pyramid_batch(const void* batch_dev_v, int nframes, bool src_u8, bool vec, int w, int h, int levels, cudaStream_t st, const UndistortCams* und) {
   const PyrBatch* batch_dev = reinterpret_cast<const PyrBatch*>(batch_dev_v);
   if (nframes <= 0 || levels < 2) return;
-  const UndistortDev U = und ? *und : UndistortDev{};
+  const UndistortCams U = und ? *und : UndistortCams{};
   vec = vec && (w % 4 == 0);
   if (und) launch_pyr_fused<unsigned char, true, 1>(batch_dev, nframes, w, h, levels, U, st);
   else if (src_u8) { if (vec) launch_pyr_fused<unsigned char, false, 2>(batch_dev, nframes, w, h, levels, U, st); else launch_pyr_fused<unsigned char, false, 1>(batch_dev, nframes, w, h, levels, U, st); }
@@ -188,7 +191,7 @@ template <typename T> __global__ void pyr_copy0_kernel(const PyrBatch* __restric
   const PyrBatch b = batch[blockIdx.y]; if (reinterpret_cast<const void*>(b.I0) == b.src) return;
   for (int idx = blockIdx.x*blockDim.x + threadIdx.x; idx < n; idx += gridDim.x*blockDim.x) b.I0[idx] = px_load<T>(reinterpret_cast<const T*>(b.src), idx);
 }
-void launch_pyramid_copy0(const void* batch_dev_v, int nframes, bool src_u8, int w, int h, cudaStream_t st, const UndistortDev* und) {
+void launch_pyramid_copy0(const void* batch_dev_v, int nframes, bool src_u8, int w, int h, cudaStream_t st, const UndistortCams* und) {
   const PyrBatch* batch_dev = reinterpret_cast<const PyrBatch*>(batch_dev_v); if (nframes <= 0) return;
   dim3 g((w*h + 255)/256 > 1024 ? 1024 : (w*h + 255)/256, nframes);
   if (und) pyr_remap0_kernel<<<g, 256, 0, st>>>(batch_dev, *und, w*h);
