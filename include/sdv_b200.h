@@ -69,10 +69,17 @@ int  sdv_sync(sdv_ctx* c);                                   /* drain the contex
 int  sdv_set_calib(sdv_ctx* c, const sdv_calib* K);
 /* CoarseTracker::makeK(CalibHessian*) per tracker instance (CoarseTracker.cpp:77-106): slot slots[i] uses K[i] from now on, for its tracker (calc_res, track,
  * track_batch, the trackNewCoarse policy) and for the map slot of the same index (reprojection, structPoseEstimation, refine).  One context can so hold
- * sequences of different cameras (same image size; rectified uploads) and follow each sequence's bundle adjustment.  K == NULL: those slots follow the context
+ * sequences of different cameras (of the context's size; sdv_set_calib_slots_cams for other sizes) and follow each sequence's bundle adjustment.  K == NULL: those slots follow the context
  * calibration again.  A slot's own K is kept across sdv_set_calib, sdv_tracker_set_ref, sdv_map_set and sdv_map_clear.  All-or-nothing: a bad slot or K
  * (fx, fy <= 0 or not finite; cx, cy not finite) returns SDV_ERR_ARG and changes no slot.  Stream-ordered after the work already enqueued, like sdv_set_calib. */
 int  sdv_set_calib_slots(sdv_ctx* c, int n, const int32_t* slots, const sdv_calib* K);
+/* The same, binding slot slots[i] (tracker and map slot) to camera cams[i] as well: its geometry row is built at that camera's rectified size
+ * (sdv_set_camera_size), and every frame it reads must have that size.  cams == NULL is sdv_set_calib_slots (camera 0).  K == NULL with a camera
+ * other than 0, or a camera index outside [0, SDV_MAX_CAMERAS), returns SDV_ERR_ARG (the context calibration has the context size).  Moving a slot
+ * to a camera of another size while it holds a tracker reference (sdv_tracker_set_ref / _set_cloud) or a resident map (sdv_map_set, until
+ * sdv_map_clear) returns SDV_ERR_STATE: those hold frames of its current size.  So the per-keyframe makeK of a slot on camera c passes cams = {c}
+ * (sdv_set_calib_slots would move it back to camera 0 and is refused once the slot is in use).  All-or-nothing. */
+int  sdv_set_calib_slots_cams(sdv_ctx* c, int n, const int32_t* slots, const sdv_calib* K, const int32_t* cams);
 
 /* ---- frames: FrameHessian::makeImages(float* color, CalibHessian*)  FullSystem/HessianBlocks.cpp:107-167 ------------
  * builds the pyramid on the device, keyed by a caller-chosen handle: level 0 is kept as the planar intensity image (its {dx,dy} are
@@ -97,19 +104,36 @@ int  sdv_set_undistort(sdv_ctx* c, int w_org, int h_org, const float* remapX, co
 int  sdv_frame_upload_batch_raw_u8(sdv_ctx* c, int n, const uint64_t* frames, const uint8_t* const* raw_imgs_worg_horg, const float* exposures);
 /* RAW ingest of several cameras in one context: one Undistort object per calibration file (util/Undistort.cpp:232-334, what src/main.cpp builds once
  * per sequence), kept side by side.  sdv_set_undistort_cam sets or replaces camera `cam`'s tables, with the arguments and checks of sdv_set_undistort;
- * the raw size w_org x h_org is per camera, the remap tables always have the context's rectified w*h size.  Replacing a camera is stream-ordered: an
+ * the raw size w_org x h_org is per camera, the remap tables have the camera's rectified size (sdv_set_camera_size; the context's w*h unless set).  Replacing a camera is stream-ordered: an
  * ingest already enqueued finishes with the old tables; the other cameras are untouched.  sdv_set_undistort is this call with cam = 0.
  * sdv_frame_upload_batch_raw_u8_cams: image k is native w_org x h_org mono8 of camera cams[k], rectified with that camera's tables in the same one
- * kernel (cams == NULL: every image is camera 0, which is sdv_frame_upload_batch_raw_u8).  Example: the KITTI odometry calibrations (calib/KITTI/00.txt,
- * 03.txt, 04.txt) come in three raw sizes, 1241x376, 1242x375 and 1226x370, that all crop to 1200x360 with different rectified K: one camera each,
- * every sequence's tracker slots bound to its camera's K with sdv_set_calib_slots, and all sequences ingested in one batch.  cams is checked before
- * anything else: an index outside [0, SDV_MAX_CAMERAS) returns SDV_ERR_ARG, a camera that was never set SDV_ERR_STATE, and a refused call changes no frame. */
+ * kernel (cams == NULL: every image is camera 0, which is sdv_frame_upload_batch_raw_u8), into a frame of that camera's rectified size.  Example: the
+ * KITTI odometry calibrations (calib/KITTI/00.txt, 03.txt, 04.txt) come in three raw sizes, 1241x376, 1242x375 and 1226x370, that all crop to 1200x360
+ * with different rectified K: one camera each, every sequence's tracker slots bound to its camera's K with sdv_set_calib_slots, and all sequences
+ * ingested in one batch.  cams is checked before anything else: an index outside [0, SDV_MAX_CAMERAS) returns SDV_ERR_ARG, a camera that was never set
+ * SDV_ERR_STATE, and a refused call changes no frame. */
 #define SDV_MAX_CAMERAS 8
 int  sdv_set_undistort_cam(sdv_ctx* c, int cam, int w_org, int h_org, const float* remapX, const float* remapY, float factor, const float* G256, const float* vignette_inv);
 int  sdv_frame_upload_batch_raw_u8_cams(sdv_ctx* c, int n, const uint64_t* frames, const uint8_t* const* raw_imgs, const int32_t* cams, const float* exposures);
 int  sdv_frame_build_batch_dev(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs_dev, int fmt, const float* exposures);
 /* fmt: 0 float (copied into frame storage), 1 mono8, 2 float ADOPTED as the frame's level-0 plane (zero copy: the buffer must stay
  * valid and unmodified until sdv_frame_release / the handle is re-uploaded — for producers that already write into device memory). */
+/* Cameras of different rectified sizes in one context (KITTI 1200x360 next to KITTI-360 1400x360).  Camera 0 always has the context size (sdv_create's
+ * w, h); cameras 1..SDV_MAX_CAMERAS-1 start at it.  sdv_set_camera_size gives camera `cam` another rectified size w x h: w <= the context's w, h <= its
+ * h (frame storage is allocated at the context size: create the context at the largest size), and the context's pyramid depth valid at that size (even
+ * w, h when levels > 1, every level non-empty).  Camera 0, a camera index out of range or a size outside these rules return SDV_ERR_ARG; resizing a
+ * camera that has Undistort tables, a resident frame or a bound slot (sdv_set_calib_slots_cams) returns SDV_ERR_STATE.  A refused call changes nothing.
+ * sdv_set_undistort_cam then takes remap tables of that camera's size.  A frame has the size of the camera it was ingested for:
+ * sdv_frame_upload_batch_cams takes host float (fmt 0) or mono8 (fmt 1) images, and sdv_frame_build_batch_dev_cams device images with the fmt values of
+ * sdv_frame_build_batch_dev (fmt 2 adopts a buffer of w_cam*h_cam floats), each at its camera's size.  cams == NULL is camera 0 (the entries without
+ * _cams); every camera index is checked before any frame is claimed or anything is enqueued.
+ * Every per-frame entry compares the frame's size with its slot's and returns SDV_ERR_ARG on a mismatch, changing no state: sdv_tracker_set_ref (ref
+ * frame), calc_res / track / track_batch / sdv_track_new_coarse_batch (new frame), sdv_map_set (host keyframes), sdv_reproject_map_batch /
+ * sdv_tracker_refine_batch (target frame); sdv_ba_set_window needs all frames of one window at one size.  The keyframe-rate candidate management
+ * (selector, makeNewTraces, activation, immature points) works at the context size only and refuses frames of another size with SDV_ERR_ARG. */
+int  sdv_set_camera_size(sdv_ctx* c, int cam, int w, int h);
+int  sdv_frame_upload_batch_cams(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs, const int32_t* cams, int fmt, const float* exposures);
+int  sdv_frame_build_batch_dev_cams(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs_dev, const int32_t* cams, int fmt, const float* exposures);
 int  sdv_frame_release(sdv_ctx* c, uint64_t frame);
 /* test hook: copy one level back as AoS {I,dx,dy} (w*h*3 floats) and absSquaredGrad (w*h floats); either may be NULL */
 int  sdv_frame_download(sdv_ctx* c, uint64_t frame, int lvl, float* dI3_out, float* abs_out);
@@ -165,7 +189,13 @@ int  sdv_tracker_track_batch(sdv_ctx* c, int n, const int32_t* slots, const uint
  *                 there are <= 2 keyframes, :242-250).  cell_order[n_cols*n_rows] is the grid visiting order (the reference shuffles it with
  *                 rand(), :111; NULL = identity); max_matches = (int)(0.8*setting_desiredImmatureDensity).
  *                 Outputs per job k, in visiting order: n_out[k] matches, out_pt[k*cells + i] = index into the slot's points,
- *                 out_px[(k*cells + i)*2] = aligned pixel (it->px). */
+ *                 out_px[(k*cells + i)*2] = aligned pixel (it->px).
+ *                 Cameras of a smaller size (sdv_set_camera_size): n_cols x n_rows and cells are the CONTEXT grid (sdv_reproject_grid), and so is
+ *                 cell_order.  A job whose slot's camera is w x h has the grid ceil(w/25) x ceil(h/25), numbered row-major in its own columns; it walks
+ *                 cell_order and skips every context cell (col, row) = (cell % n_cols, cell / n_cols) with col >= ceil(w/25) or row >= ceil(h/25), and
+ *                 visits the others as its cell row*ceil(w/25) + col.  That subsequence is a permutation of the job's grid, so one context order
+ *                 serves a mixed batch, and the job gets the matches a context of its own size gives for the filtered order.  The output stride
+ *                 stays the context's cells.  sdv_tracker_refine_batch and sdv_track_new_coarse_batch apply the same rule. */
 typedef struct { float u, v, idepth; int32_t host; int32_t type; } sdv_map_pt;
 int  sdv_reproject_grid(sdv_ctx* c, int* n_cols, int* n_rows);
 int  sdv_map_set(sdv_ctx* c, int slot, int nH, const uint64_t* host_frames, const double* host_T7, const double* host_ab, int nP, const sdv_map_pt* pts);
@@ -383,7 +413,7 @@ int  sdv_activate_select_batch(sdv_ctx* c, int n, const int32_t* host_begin, con
  * sdv_lidar_handler_batch: n raw sweeps (one per resident sequence), sweep j = XYZI rows sweep_begin[j] .. sweep_begin[j+1] of xyzi (the decoded PointCloud2, what
  * pcl::fromROSMsg yields; rows with a non-finite coordinate are dropped like pcl::removeNaNFromPointCloud does).  Per sweep: Rlc9 (row-major) / tlc3 = FullSystem::Rlc, tlc
  * (LiDAR -> camera), K4 = FullSystem::fx fy cx cy, lrud_io = FullSystem::left, right, up, down (the running pixel box; 10000, -1, 10000, -1 at start).  The image
- * size is the context's.  Out, per sweep: up to cap rows {Ku, Kv, depth} (doubles, the vCloudPixel pushed into FullSystem::qCloudPixel, same order) at
+ * size, which bounds the pixel box, is the context's (camera 0's), whatever camera size the sequence's frames have.  Out, per sweep: up to cap rows {Ku, Kv, depth} (doubles, the vCloudPixel pushed into FullSystem::qCloudPixel, same order) at
  * cloud3_out[3*j*cap ..], n_out[j] rows, add_feature_point_out[j] = FullSystem::addFeaturePoint (ground ratio > 0.8), stats_out[2j..] = {numGround, size of
  * segmentedCloud} (may be NULL).  The rows feed sdv_make_new_traces_batch and the LiDAR-depth splats of sdv_tracker_set_ref. */
 int  sdv_lidar_init(sdv_ctx* c, int n_scan, int horizon_scan, float ang_res_x, float ang_res_y, float ang_bottom, int ground_scan_ind);

@@ -84,6 +84,20 @@ int shim_set_undistort_cam(int cam, const Undistort* u) {
 int shim_ingest_raw_cams(int n, const uint64_t* ids, const uint8_t* const* raw_mono8, const int32_t* cams, const float* exposures) {
   return sdv_frame_upload_batch_raw_u8_cams(gpu, n, ids, raw_mono8, cams, exposures);
 }
+// §4 cameras of different rectified sizes in one context (created at the largest, KITTI-360's 1400x360): KITTI's 1200x360 on camera 1, its
+// sequences' slots bound to that camera, rectified or device-resident frames of each camera's size
+// §4 the per-keyframe makeK of a slot bound to camera `cam`: the K moves, the camera stays
+int shim_makeK_cam(int slot, int cam, const sdv_calib* K_after_ba) { const int32_t s = slot, c = cam; return sdv_set_calib_slots_cams(gpu, 1, &s, K_after_ba, &c); }
+int shim_kitti_camera(int cam, const Undistort* u, int w, int h /*Undistort::getSize()*/, int n, const int32_t* slots, const sdv_calib* K) {
+  int rc = sdv_set_camera_size(gpu, cam, w, h); if (rc) return rc;
+  rc = shim_set_undistort_cam(cam, u); if (rc) return rc;
+  std::vector<int32_t> cams(n, cam);
+  return sdv_set_calib_slots_cams(gpu, n, slots, K, cams.data());
+}
+int shim_ingest_cams(int n, const uint64_t* ids, const uint8_t* const* mono8, const void* const* dev_float, const int32_t* cams, const float* exposures) {
+  return sdv_frame_upload_batch_cams(gpu, n, ids, reinterpret_cast<const void* const*>(mono8), cams, /*fmt mono8*/1, exposures)
+       | sdv_frame_build_batch_dev_cams(gpu, n, ids, dev_float, cams, /*fmt float*/0, exposures);
+}
 // §3c CoarseTracker::makeK (CoarseTracker.cpp:77-106): a member of each tracker instance, so it sets the K of that instance's slot only
 int shim_makeK(int slot, CalibHessian* HCalib) { sdv_calib K{HCalib->fxl(), HCalib->fyl(), HCalib->cxl(), HCalib->cyl()}; const int32_t s = slot; return sdv_set_calib_slots(gpu, 1, &s, &K); }
 
@@ -271,6 +285,8 @@ int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const 
   std::vector<int32_t> sel, st; Vec5 mr{}; SE3 T; AffLight a;
   int rc = shim_create(hc) | shim_set_undistort(u, nullptr, nullptr) | shim_ingest_raw(fh->shell, raw, 1.0f) | shim_makeK(fs.coarseTracker->slot, &hc);
   { const uint64_t id = (uint64_t)fh->shell->id; const int32_t cam = 1; const float ex = 1.0f; rc |= shim_set_undistort_cam(cam, u) | shim_ingest_raw_cams(1, &id, &raw, &cam, &ex); }
+  { const uint64_t id = (uint64_t)fh->shell->id; const int32_t cam = 2, slot = 3; const float ex = 1.0f; const void* dev = nullptr; const sdv_calib K{hc.fxl(), hc.fyl(), hc.cxl(), hc.cyl()};
+    rc |= shim_kitti_camera(cam, u, 1200, 360, 1, &slot, &K) | shim_ingest_cams(1, &id, &raw, &dev, &cam, &ex) | shim_makeK_cam(slot, cam, &K); }
   fs.coarseTracker->setCoarseTrackingRef(fs.frameHessians); fs.coarseTracker->trackNewestCoarse(fh, T, a, 3, mr, nullptr);
   std::vector<ImmaturePoint*> imm; std::vector<HostImmatures> hi; rc |= shim_makeNewTraces(fh, sel, imm) | shim_traceNewCoarse(fh, hi);
   std::vector<ActivationGroup> ag; std::vector<float> idp; rc |= shim_activatePoints(ag, st, idp, sel, 7);

@@ -56,6 +56,10 @@ def _load():
     L.sdv_sync.argtypes = [_vp]
     L.sdv_set_calib.argtypes = [_vp, C.POINTER(sdv_calib)]
     L.sdv_set_calib_slots.argtypes = [_vp, C.c_int, _i32p, _vp]
+    L.sdv_set_calib_slots_cams.argtypes = [_vp, C.c_int, _i32p, _vp, _vp]
+    L.sdv_set_camera_size.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
+    L.sdv_frame_upload_batch_cams.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _vp, C.c_int, _f32p]
+    L.sdv_frame_build_batch_dev_cams.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _vp, C.c_int, _f32p]
     L.sdv_frame_upload.argtypes = [_vp, C.c_uint64, _vp, C.c_float]
     L.sdv_frame_upload_batch.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _f32p]
     L.sdv_frame_upload_batch_u8.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _f32p]
@@ -121,6 +125,9 @@ def default_settings() -> sdv_settings:
 class Context:
     def __init__(self, K, w: int, h: int, levels: int | None = None, device: int = 0, **settings):
         self.w, self.h = w, h
+        self.cam_wh = {0: (w, h)}          # rectified size per camera (setCameraSize); camera 0 is the context size
+        self.frame_cam = {}                # frame handle -> camera, for frames not on camera 0
+        self.slot_cam = {}                 # tracker / map slot -> camera, for slots not on camera 0 (setCalibSlots)
         self.levels = levels if levels is not None else pyr_levels(w, h)
         s = default_settings()
         for k, v in settings.items():
@@ -150,35 +157,67 @@ class Context:
     def sync(self):
         self._ck(LIB.sdv_sync(self.p))
 
+    def camSize(self, cam: int = 0):
+        """(w, h) of camera `cam`'s frames"""
+        return self.cam_wh.get(int(cam), (self.w, self.h))
+
+    def setCameraSize(self, cam: int, w: int, h: int):
+        """give camera `cam` (1..SDV_MAX_CAMERAS-1) the rectified size w x h <= the context size, at the context's pyramid depth (see sdv_b200.h)"""
+        self._ck(LIB.sdv_set_camera_size(self.p, int(cam), int(w), int(h))); self.cam_wh[int(cam)] = (int(w), int(h))
+
     # FrameHessian::makeImages
-    def makeImages(self, frame_id: int, color, exposure: float = 1.0):
+    def makeImages(self, frame_id: int, color, exposure: float = 1.0, cam: int = 0):
         color = np.ascontiguousarray(color, np.float32)
-        assert color.shape == (self.h, self.w)
-        self._ck(LIB.sdv_frame_upload(self.p, frame_id, color.ctypes.data, exposure))
+        w, h = self.camSize(cam)
+        assert color.shape == (h, w), f"camera {cam} takes {w}x{h} images"
+        if cam == 0:
+            self._ck(LIB.sdv_frame_upload(self.p, frame_id, color.ctypes.data, exposure)); self.frame_cam.pop(frame_id, None)
+        else:
+            self.makeImagesBatch([frame_id], [color.ctypes.data], [exposure], cams=[cam]); self.sync()
 
     def setCalib(self, K):
         """CoarseTracker::makeK / the CalibHessian the Reprojector reads, after the bundle adjustment moved the intrinsics"""
         k = sdv_calib(*[float(x) for x in K]); self._ck(LIB.sdv_set_calib(self.p, C.byref(k))); self.K = tuple(float(x) for x in K)
 
-    def setCalibSlots(self, slots, Ks):
+    def setCalibSlots(self, slots, Ks, cams=None):
         """CoarseTracker::makeK per tracker instance: slot slots[i] (its tracker and the map slot of the same index) uses Ks[i] = (fx, fy, cx, cy) from now on,
-        whatever setCalib sets later.  All-or-nothing: a bad slot or K raises SdvError and changes no slot."""
+        whatever setCalib sets later, and is bound to camera cams[i] (None: camera 0): its frames must have that camera's size.
+        All-or-nothing: a bad slot, K or camera raises SdvError and changes no slot."""
         sl = np.ascontiguousarray(slots, np.int32).reshape(-1); Kf = np.asarray(Ks, np.float64).reshape(-1, 4)
         if len(Kf) != len(sl):
             raise ValueError(f"{len(sl)} slots but {len(Kf)} calibrations")
+        cm = self._cams(cams, len(sl))
         arr = (sdv_calib * max(len(sl), 1))(*[sdv_calib(*map(float, k)) for k in Kf])
-        self._ck(LIB.sdv_set_calib_slots(self.p, len(sl), sl, C.addressof(arr)))
+        self._ck(LIB.sdv_set_calib_slots_cams(self.p, len(sl), sl, C.addressof(arr), None if cm is None else cm.ctypes.data))
+        self._bind(sl, cm)
+
+    def _bind(self, sl, cm):
+        for s, c in zip(sl.tolist(), [0] * len(sl) if cm is None else cm.tolist()):
+            if c:
+                self.slot_cam[s] = c
+            else:
+                self.slot_cam.pop(s, None)
+
+    @staticmethod
+    def _cams(cams, n):
+        if cams is None:
+            return None
+        cm = np.ascontiguousarray(cams, np.int32).reshape(-1)
+        if len(cm) != n:
+            raise ValueError(f"{n} entries but {len(cm)} camera indices")
+        return cm
 
     def clearCalibSlots(self, slots):
         """the slots follow the context calibration (setCalib) again"""
         sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
-        self._ck(LIB.sdv_set_calib_slots(self.p, len(sl), sl, None))
+        self._ck(LIB.sdv_set_calib_slots(self.p, len(sl), sl, None)); self._bind(sl, None)
 
     # Undistort (util/Undistort.cpp) handed over as data; `und` = sdv_loam_b200.undistort.Undistort or anything with wOrg,hOrg,remapX,remapY[,G,vignetteMapInv]
-    # cam: which of the context's SDV_MAX_CAMERAS cameras these tables set or replace (the raw size is per camera, the rectified size is the context's)
+    # cam: which of the context's SDV_MAX_CAMERAS cameras these tables set or replace (the raw size is per camera, the rectified size is the camera's: setCameraSize)
     def setUndistort(self, und, factor: float = 1.0, cam: int = 0):
         rx = np.ascontiguousarray(und.remapX, np.float32).reshape(-1); ry = np.ascontiguousarray(und.remapY, np.float32).reshape(-1)
-        assert rx.size == self.w * self.h == ry.size, "remap tables must have the rectified size given to the context"
+        w, h = self.camSize(cam)
+        assert rx.size == w * h == ry.size, f"remap tables must have camera {cam}'s rectified size {w}x{h}"
         G = getattr(und, "G", None); V = getattr(und, "vignetteMapInv", None)
         G = None if G is None else np.ascontiguousarray(G, np.float32); V = None if V is None else np.ascontiguousarray(V, np.float32)
         assert G is None or G.size == 256
@@ -188,15 +227,15 @@ class Context:
 
     def makeImagesRaw(self, frame_id: int, raw, exposure: float = 1.0, cam: int = 0):
         """Undistort::undistort<unsigned char> + FrameHessian::makeImages of one native-size mono8 image of camera `cam`"""
-        raw = np.ascontiguousarray(raw, np.uint8)
+        raw = np.ascontiguousarray(raw, np.uint8); cam = int(cam)
         if cam in getattr(self, "wh_org", {}):
             assert raw.shape == (self.wh_org[cam][1], self.wh_org[cam][0]), f"camera {cam} takes {self.wh_org[cam][0]}x{self.wh_org[cam][1]} images"
         self.makeImagesBatch([frame_id], [raw.ctypes.data], [exposure], raw=True, cams=[cam]); self.sync()
 
     def makeImagesBatch(self, frame_ids, ptrs, exposures=None, u8=False, device=False, adopt=False, raw=False, cams=None):
         """Batched makeImages.  ptrs: integer addresses of (h,w) buffers — host (pinned for full-rate, asynchronous H2D)
-        or device (device=True); float32, or mono8 when u8=True; raw=True: native-size mono8 through setUndistort's tables,
-        image k of camera cams[k] (None: every image is camera 0).
+        or device (device=True); float32, or mono8 when u8=True; raw=True: native-size mono8 through setUndistort's tables.
+        Image k is camera cams[k] (None: every image is camera 0) and has that camera's size (raw: its raw size).
         A uint64 numpy array of addresses avoids per-call list work.  Asynchronous: see sdv_b200.h."""
         n = len(frame_ids)
         ids = np.ascontiguousarray(frame_ids, np.uint64)
@@ -205,12 +244,24 @@ class Context:
         else:
             arr = (_vp * n)(*ptrs)
         ex = self._ones(n) if exposures is None else np.ascontiguousarray(exposures, np.float32)
-        if raw and cams is not None:
-            cm = np.ascontiguousarray(cams, np.int32).reshape(-1)
-            if len(cm) != n:
-                raise ValueError(f"{n} frames but {len(cm)} camera indices")
-            self._ck(LIB.sdv_frame_upload_batch_raw_u8_cams(self.p, n, ids, arr, cm.ctypes.data, ex))
-        elif raw:
+        cm = self._cams(cams, n)
+        if cm is not None:
+            if raw:
+                self._ck(LIB.sdv_frame_upload_batch_raw_u8_cams(self.p, n, ids, arr, cm.ctypes.data, ex))
+            elif device:
+                self._ck(LIB.sdv_frame_build_batch_dev_cams(self.p, n, ids, arr, cm.ctypes.data, 1 if u8 else (2 if adopt else 0), ex))
+            else:
+                self._ck(LIB.sdv_frame_upload_batch_cams(self.p, n, ids, arr, cm.ctypes.data, 1 if u8 else 0, ex))
+            for i, k in zip(ids.tolist(), cm.tolist()):
+                if k:
+                    self.frame_cam[i] = k
+                else:
+                    self.frame_cam.pop(i, None)
+            return
+        if self.frame_cam:                 # these handles are camera-0 frames now
+            for i in ids.tolist():
+                self.frame_cam.pop(i, None)
+        if raw:
             self._ck(LIB.sdv_frame_upload_batch_raw_u8(self.p, n, ids, arr, ex))
         elif device:
             self._ck(LIB.sdv_frame_build_batch_dev(self.p, n, ids, arr, 1 if u8 else (2 if adopt else 0), ex))
@@ -229,10 +280,11 @@ class Context:
         return int(LIB.sdv_launch_count(self.p))
 
     def releaseFrame(self, frame_id: int):
-        self._ck(LIB.sdv_frame_release(self.p, frame_id))
+        self._ck(LIB.sdv_frame_release(self.p, frame_id)); self.frame_cam.pop(frame_id, None)
 
     def frameLevel(self, frame_id: int, lvl: int):
-        w, h = self.w >> lvl, self.h >> lvl
+        """level lvl of a resident frame at the frame's own (its camera's) size"""
+        w, h = self.camSize(self.frame_cam.get(frame_id, 0)); w, h = w >> lvl, h >> lvl
         dI = np.zeros((h, w, 3), np.float32); ab = np.zeros((h, w), np.float32)
         self._ck(LIB.sdv_frame_download(self.p, frame_id, lvl, dI.ctypes.data, ab.ctypes.data))
         return dI, ab
@@ -262,8 +314,9 @@ class CoarseTracker:
         self.ctx, self.slot = ctx, slot
 
     def makeK(self, K):
-        """CoarseTracker::makeK (CoarseTracker.cpp:77-106): this instance tracks (and refines its slot's map) with K = (fx, fy, cx, cy) from now on"""
-        self.ctx.setCalibSlots([self.slot], [K])
+        """CoarseTracker::makeK (CoarseTracker.cpp:77-106): this instance tracks (and refines its slot's map) with K = (fx, fy, cx, cy) from now on,
+        on the camera its slot is bound to"""
+        self.ctx.setCalibSlots([self.slot], [K], cams=[self.ctx.slot_cam.get(self.slot, 0)])
 
     def setCoarseTrackingRef(self, ref_frame_id: int, pts, round_half, ref_a: float = 0.0, ref_b: float = 0.0):
         pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 4); rh = np.ascontiguousarray(round_half, np.int32)

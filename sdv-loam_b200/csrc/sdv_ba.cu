@@ -104,11 +104,14 @@ int sdv_ba_set_window(sdv_ctx* c, int nF, const uint64_t* frame_ids, const doubl
   SDV_GUARD_TRK(c);                                                           // frame table, pins, level-0 texel pool and the ingest join belong to the tracker domain
   CK(cudaSetDevice(c->device));
   BAState* b; int rc = ba_get(c, &b); if (rc) return rc;
-  for (int f=0; f<nF; f++) if (c->frame_index.find(frame_ids[f]) == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "BA frame %d: unknown frame handle", f);
+  int cam0 = -1;                                                              // one size per window: BAHeader::w/h are the window's frames' size
+  for (int f=0; f<nF; f++) { auto it = c->frame_index.find(frame_ids[f]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "BA frame %d: unknown frame handle", f);
+    const int cam = c->frames[it->second].cam; if (cam0 < 0) cam0 = cam;
+    if (!same_size(c, cam, cam0)) return ctx_fail(c, SDV_ERR_ARG, "BA frame %d is %dx%d but frame 0 is %dx%d: one window holds frames of one size", f, c->cam_w[cam], c->cam_h[cam], c->cam_w[cam0], c->cam_h[cam0]); }
   for (int i=0;i<b->n_pinned;i++) frame_unpin(c, b->pinned[i]);          // the window is being replaced: drop its references, take the new ones
   b->n_pinned = nF; for (int f=0; f<nF; f++) { b->pinned[f] = frame_ids[f]; frame_pin(c, frame_ids[f]); }
   BAHeader* H = b->hdr_host; memset(H, 0, sizeof(BAHeader));
-  H->nF = nF; H->w = c->w; H->h = c->h; H->dim = kCP + 6*nF; b->nF = nF;
+  H->nF = nF; H->w = c->cam_w[cam0]; H->h = c->cam_h[cam0]; H->dim = kCP + 6*nF; b->nF = nF;
   BASettingsDev& s = H->set;
   s.huberTH = c->set.huberTH; s.outlierTHSumComponent = c->set.outlierTHSumComponent; s.idepthFixPrior = c->set.idepthFixPrior;
   s.initialRotPrior = 1e11f; s.initialTransPrior = 1e10f; s.initialCalibHessian = 5e9f;            // settings.cpp:23-27

@@ -37,7 +37,8 @@ int sdv_pyr_levels(int w, int h) {               // util/globalCalib.cpp:22-30
 static thread_local char g_create_err[512] = "null context";   // message of the last failed sdv_create on this thread (there is no context to hold it)
 const char* sdv_last_error(sdv_ctx* c) { return c ? c->err : g_create_err; }
 
-static void make_geom(sdv_ctx* c, const sdv_calib* K, int row) {   // CoarseTracker::makeK (CoarseTracker.cpp:77-106) into one row of the geometry table
+// CoarseTracker::makeK (CoarseTracker.cpp:77-106) into one row of the geometry table, at camera cam's rectified size
+static void make_geom(sdv_ctx* c, const sdv_calib* K, int row, int cam) {
   float fx[SDV_PYR_LEVELS], fy[SDV_PYR_LEVELS], cx[SDV_PYR_LEVELS], cy[SDV_PYR_LEVELS];
   fx[0]=K->fx; fy[0]=K->fy; cx[0]=K->cx; cy[0]=K->cy;
   for (int l=1;l<c->levels;l++) {
@@ -45,7 +46,7 @@ static void make_geom(sdv_ctx* c, const sdv_calib* K, int row) {   // CoarseTrac
     cx[l] = (cx[0]+0.5)/((int)1<<l) - 0.5; cy[l] = (cy[0]+0.5)/((int)1<<l) - 0.5;
   }
   for (int l=0;l<c->levels;l++) {
-    LevelGeom& g = c->geom[row].g[l]; g.w = c->w>>l; g.h = c->h>>l; g.fx=fx[l]; g.fy=fy[l]; g.cx=cx[l]; g.cy=cy[l];
+    LevelGeom& g = c->geom[row].g[l]; g.w = c->cam_w[cam]>>l; g.h = c->cam_h[cam]>>l; g.fx=fx[l]; g.fy=fy[l]; g.cx=cx[l]; g.cy=cy[l];
     float Km[9] = {fx[l],0,cx[l], 0,fy[l],cy[l], 0,0,1}; inv3f(Km, g.Ki);
   }
 }
@@ -62,27 +63,53 @@ int sdv_set_calib(sdv_ctx* c, const sdv_calib* K) { SDV_GUARD_TRK(c);
   if (!c || !K) return SDV_ERR_ARG;
   if (!(K->fx > 0 && K->fy > 0)) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib: focal lengths must be positive");
   CK(cudaSetDevice(c->device));
-  make_geom(c, K, 0);
+  make_geom(c, K, 0, 0);
   return upload_geom(c, 0, 0);
 }
 
-// CoarseTracker::makeK per tracker instance: slot slots[i] uses K[i] (its own row 1 + slot), or the context calibration again when K is NULL.
-// Everything is checked before anything changes.
-int sdv_set_calib_slots(sdv_ctx* c, int n, const int32_t* slots, const sdv_calib* K) { SDV_GUARD_TRK(c);
+// CoarseTracker::makeK per tracker instance: slot slots[i] uses K[i] (its own row 1 + slot, built at camera cams[i]'s size), or the context calibration
+// again when K is NULL (camera 0 only: row 0 has the context size).  Everything is checked before anything changes.
+int sdv_set_calib_slots_cams(sdv_ctx* c, int n, const int32_t* slots, const sdv_calib* K, const int32_t* cams) { SDV_GUARD_TRK(c);
   if (!c || n < 0 || (n > 0 && !slots)) return SDV_ERR_ARG;
   for (int i=0;i<n;i++) {
     if (slots[i] < 0 || slots[i] >= (int)c->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib_slots: entry %d names slot %d of %d", i, slots[i], (int)c->slots.size());
     if (K && !(K[i].fx > 0 && K[i].fy > 0 && std::isfinite(K[i].fx) && std::isfinite(K[i].fy) && std::isfinite(K[i].cx) && std::isfinite(K[i].cy)))
       return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib_slots: entry %d (slot %d): fx, fy must be positive and finite, cx, cy finite", i, slots[i]);
+    const int cam = cams ? cams[i] : 0;
+    if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib_slots: entry %d names camera %d (valid: 0..%d)", i, cam, SDV_MAX_CAMERAS - 1);
+    if (!K && cam != 0) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib_slots: entry %d binds camera %d without a K (the context calibration is camera 0's)", i, cam);
+  }
+  for (int i=0;i<n;i++) {                                                // a slot's reference cloud and resident map hold frames of its current size
+    const TrackerSlot& t = c->slots[slots[i]]; const int cam = cams ? cams[i] : 0;
+    if (!same_size(c, t.cam, cam) && (t.ref_frame != ~0ull || rp_slot_set(c, slots[i])))
+      return ctx_fail(c, SDV_ERR_STATE, "sdv_set_calib_slots: entry %d would move slot %d from camera %d (%dx%d) to camera %d (%dx%d) while its %s holds frames of the old size",
+                      i, slots[i], t.cam, c->cam_w[t.cam], c->cam_h[t.cam], cam, c->cam_w[cam], c->cam_h[cam], t.ref_frame != ~0ull ? "tracker reference" : "map");
   }
   CK(cudaSetDevice(c->device));
   int lo = (int)c->geom.size(), hi = -1;
   for (int i=0;i<n;i++) {
-    TrackerSlot& t = c->slots[slots[i]];
+    TrackerSlot& t = c->slots[slots[i]]; t.cam = cams ? cams[i] : 0;
     if (!K) { t.geom_row = 0; continue; }
-    t.geom_row = 1 + slots[i]; make_geom(c, &K[i], t.geom_row); lo = std::min(lo, t.geom_row); hi = std::max(hi, t.geom_row);
+    t.geom_row = 1 + slots[i]; make_geom(c, &K[i], t.geom_row, t.cam); lo = std::min(lo, t.geom_row); hi = std::max(hi, t.geom_row);
   }
   return hi >= lo ? upload_geom(c, lo, hi) : SDV_OK;
+}
+int sdv_set_calib_slots(sdv_ctx* c, int n, const int32_t* slots, const sdv_calib* K) { return sdv_set_calib_slots_cams(c, n, slots, K, nullptr); }
+
+// A camera's rectified size: at most the context size (frame storage), with the context's pyramid depth.  Refused while anything depends on the old size.
+int sdv_set_camera_size(sdv_ctx* c, int cam, int w, int h) { SDV_GUARD_TRK(c);
+  if (!c) return SDV_ERR_ARG;
+  if (cam == 0) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_camera_size: camera 0 always has the context size %dx%d", c->w, c->h);
+  if (cam < 1 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_camera_size: camera %d outside 1..%d", cam, SDV_MAX_CAMERAS - 1);
+  if (w < 1 || h < 1 || w > c->w || h > c->h) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_camera_size: %dx%d does not fit the context size %dx%d", w, h, c->w, c->h);
+  if (c->levels > 1 && ((w | h) & 1)) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_camera_size: %dx%d: the pyramid needs even image sizes", w, h);
+  if ((w >> (c->levels - 1)) < 1 || (h >> (c->levels - 1)) < 1) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_camera_size: %dx%d has an empty level at the context's %d levels", w, h, c->levels);
+  if (w == c->cam_w[cam] && h == c->cam_h[cam]) return SDV_OK;
+  if (c->und.cam[cam].remapX) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_size: camera %d has Undistort tables of its current size", cam);
+  for (const FrameDev& f : c->frames) if (f.used && f.cam == cam) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_size: camera %d has resident frame %llu", cam, (unsigned long long)f.id);
+  for (size_t s=0;s<c->slots.size();s++) if (c->slots[s].cam == cam) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_size: slot %d is bound to camera %d", (int)s, cam);
+  c->cam_w[cam] = w; c->cam_h[cam] = h;
+  return SDV_OK;
 }
 
 static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels, const sdv_settings* s_in, int device);
@@ -104,6 +131,7 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
   if (s.track_threads != 64 && s.track_threads != 256) s.track_threads = 128;
   if (s.cluster_size > 16) s.cluster_size = 16;
   c->set = s; c->device = device; c->w = w; c->h = h; c->levels = levels;
+  for (int k=0;k<SDV_MAX_CAMERAS;k++) { c->cam_w[k] = w; c->cam_h[k] = h; }
   CK(cudaSetDevice(device));
   CK(kernels_init_device()); CK(refine_init_device());      // per-device function attributes (opt-in shared memory, cluster sizes)
   CK(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking)); CK(cudaStreamCreateWithFlags(&c->st_ba, cudaStreamNonBlocking));
@@ -118,7 +146,7 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
   CK(cudaMalloc(&c->tc_dev, sizeof(TrackConst)));
   CK(cudaMemcpy(c->tc_dev, &c->tc, sizeof(TrackConst), cudaMemcpyHostToDevice));
   c->geom.assign(s.n_tracker_slots + 1, GeomRow{});                // slot rows are written by sdv_set_calib_slots before a slot points at them
-  make_geom(c, K, 0);
+  make_geom(c, K, 0, 0);
   CK(cudaMalloc(&c->geom_dev, c->geom.size()*sizeof(GeomRow)));
   CK(cudaMemcpy(c->geom_dev, c->geom.data(), c->geom.size()*sizeof(GeomRow), cudaMemcpyHostToDevice));
   // frame pool: planar intensity of every level per frame (level 0 + one allocation for levels >= 1), plus the storage of the packed-texel cache of
@@ -127,7 +155,7 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
   c->frame_texels = texels;
   c->frames.resize(s.max_frames);
   for (auto& f : c->frames) {
-    f.used = false; f.adopted = false; f.lvl0_slot = -1; f.hi_tex = false; f.pyr = nullptr; f.base = nullptr; f.ingest_seq = 0;
+    f.used = false; f.adopted = false; f.lvl0_slot = -1; f.hi_tex = false; f.pyr = nullptr; f.base = nullptr; f.ingest_seq = 0; f.cam = 0;
     CK(cudaMalloc(&f.I0_own, (size_t)w*h*sizeof(float))); f.I0 = f.I0_own; f.img[0] = f.I0;
     if (texels) { CK(cudaMalloc(&f.pyr, texels*sizeof(float))); CK(cudaMalloc(&f.base, texels*sizeof(float4))); }
     f.lvl[0] = nullptr; for (int l=1;l<levels;l++) { f.img[l] = f.pyr + c->lvl_off[l]; f.lvl[l] = f.base + c->lvl_off[l]; }
@@ -141,7 +169,7 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
       size_t cap = (size_t)(w>>l)*(h>>l); if (s.max_ref_points > 0 && (size_t)s.max_ref_points < cap) cap = s.max_ref_points;
       t.cap[l] = (int)cap; t.npts[l] = 0; CK(cudaMalloc(&t.pts[l], cap*sizeof(float4)));
     }
-    t.ref_frame = ~0ull; t.has_totals = false; t.geom_row = 0;
+    t.ref_frame = ~0ull; t.has_totals = false; t.geom_row = 0; t.cam = 0;
   }
   // step-kernel reduction buffers
   CK(cudaMalloc(&c->partials, (size_t)step_kernel_max_grid()*kNAcc*sizeof(double)));
@@ -213,8 +241,9 @@ static int ensure_desc(sdv_ctx* c, int n) {
 static void frame_drop_texels(sdv_ctx* c, FrameDev& f) { if (f.lvl0_slot >= 0) { c->lvl0_free.push_back(f.lvl0_slot); f.lvl0_slot = -1; } f.lvl[0] = nullptr; f.hi_tex = false; }
 
 // kind bit0: mono8 input, bit1: input already in device memory, bit2: adopt the (device, float) buffer as the frame's level-0 plane,
-// bit3: RAW mono8 input of the camera's native size, rectified through the tables of sdv_set_undistort_cam inside the level-0 kernel; image k is camera
-// cams[k] (cams == NULL: camera 0), so the raw byte size, the staging offset and the coalesced copies are per frame.
+// bit3: RAW mono8 input of the camera's native size, rectified through the tables of sdv_set_undistort_cam inside the level-0 kernel.
+// Image k is camera cams[k] (cams == NULL: camera 0) and becomes a frame of that camera's rectified size, so the byte size, the staging offset and the
+// coalesced copies are per frame.
 // Everything is enqueued on the ingest stream; the compute stream picks it up through ev_in at the next tracker / BA call, so an
 // upload overlaps the tracking of the previous batch.  Every level is a planar intensity image: a pinned-host float upload lands directly in
 // frame storage, levels >= 1 are built by one fused launch, and the consumers form gradients on the fly.
@@ -222,26 +251,25 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
   if (!c || n < 0 || !frames || !imgs) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK;
   const bool raw = (kind & 8), u8 = (kind & 1) || raw, dev = (kind & 2), adopt = (kind & 4) && dev && !u8;
-  if (raw) for (int k=0;k<n;k++) {                                       // before any frame handle is claimed or anything is enqueued: a refused call changes no frame
-    const int cam = cams ? cams[k] : 0;
-    if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "image %d names camera %d (valid: 0..%d)", k, cam, SDV_MAX_CAMERAS - 1);
-    if (!c->und.cam[cam].remapX) return ctx_fail(c, SDV_ERR_STATE, "raw upload before sdv_set_undistort (camera %d has no tables)", cam);
-  }
+  if (cams) for (int k=0;k<n;k++)                                         // before any frame handle is claimed or anything is enqueued: a refused call changes no frame
+    if (cams[k] < 0 || cams[k] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "image %d names camera %d (valid: 0..%d)", k, cams[k], SDV_MAX_CAMERAS - 1);
+  auto cam_of = [&](int k) { return cams ? cams[k] : 0; };
+  if (raw) for (int k=0;k<n;k++)
+    if (!c->und.cam[cam_of(k)].remapX) return ctx_fail(c, SDV_ERR_STATE, "raw upload before sdv_set_undistort (camera %d has no tables)", cam_of(k));
   CK(cudaSetDevice(c->device));
   const long long seq = c->ingest_seq + 1; const int par = (int)(seq & 1);
   // staging buffers + descriptors of this parity were last used by ingest seq-2: it must have drained before the host rewrites the pinned
   // descriptors (the device-side order copy(seq) after pyramid(seq-2) is enforced on the copy stream below)
   if (seq > 2) CK(cudaEventSynchronize(c->ev_ing[(seq-2) % sdv_ctx::kIngRing]));
   int rc = ensure_desc(c, n); if (rc) return rc;
-  const size_t px = (size_t)c->w*c->h;
-  auto cam_of = [&](int k) { return raw && cams ? cams[k] : 0; };
-  auto px_in = [&](int k) { const sdv::UndistortDev& u = c->und.cam[cam_of(k)]; return raw ? (size_t)u.wOrg*u.hOrg : px; };   // bytes of mono8 input image k
+  auto px = [&](int k) { return (size_t)c->cam_w[cam_of(k)]*c->cam_h[cam_of(k)]; };                  // rectified pixels of frame k
+  auto px_in = [&](int k) { const sdv::UndistortDev& u = c->und.cam[cam_of(k)]; return raw ? (size_t)u.wOrg*u.hOrg : px(k); };   // bytes of mono8 input image k
   if (u8 && !dev) { size_t total = 0; for (int k=0;k<n;k++) total += px_in(k);
     if (total > c->stage_u8_cap[par]) { CK(cudaStreamSynchronize(c->st_in)); cudaFree(c->stage_u8[par]); c->stage_u8[par] = nullptr;
       c->stage_u8_cap[par] = total; CK(cudaMalloc(&c->stage_u8[par], c->stage_u8_cap[par])); } }
   c->cp_dst.clear(); c->cp_src.clear(); c->cp_sz.clear();
   if (c->levels > 1 && ((c->w | c->h) & 1)) return ctx_fail(c, SDV_ERR_ARG, "pyramid needs even image sizes");
-  PyrBatchHost* desc = c->pyr_batch_host[par]; bool vec = true; size_t stage_off = 0;
+  PyrBatchHost* desc = c->pyr_batch_host[par]; bool vec = true; size_t stage_off = 0; int max_w = 0, max_h = 0;
   for (int k=0;k<n;k++) {
     int idx = -1;
     auto it = c->frame_index.find(frames[k]);
@@ -250,16 +278,17 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
     else { for (size_t i=0;i<c->frames.size();i++) if (!c->frames[i].used) { idx = (int)i; break; } }
     if (idx < 0) return ctx_fail(c, SDV_ERR_CAPACITY, "frame pool exhausted (max_frames=%d)", (int)c->frames.size());
     FrameDev& f = c->frames[idx]; f.used = true; f.id = frames[k]; f.exposure = exposures ? exposures[k] : 1.0f; c->frame_index[frames[k]] = idx;
-    frame_drop_texels(c, f); f.ingest_seq = seq;
+    frame_drop_texels(c, f); f.ingest_seq = seq; f.cam = cam_of(k);
     f.adopted = adopt; f.I0 = adopt ? const_cast<float*>(reinterpret_cast<const float*>(imgs[k])) : f.I0_own; f.img[0] = f.I0;
     PyrBatchHost& b = desc[k];
-    b.pyr = f.pyr; b.I0 = f.I0; b.flags = (f.exposure > 0.f) ? 1 : 0; b.cam = cam_of(k);
+    b.pyr = f.pyr; b.I0 = f.I0; b.flags = (f.exposure > 0.f) ? 1 : 0; b.cam = f.cam; b.w = c->cam_w[f.cam]; b.h = c->cam_h[f.cam];
+    max_w = std::max(max_w, b.w); max_h = std::max(max_h, b.h);
     if (dev) b.src = imgs[k];
     else if (u8) { const size_t sz = px_in(k); unsigned char* d8 = c->stage_u8[par] + stage_off; stage_off += sz; b.src = d8;
       if (!c->cp_dst.empty() && (unsigned char*)c->cp_src.back() + c->cp_sz.back() == (const unsigned char*)imgs[k] && (unsigned char*)c->cp_dst.back() + c->cp_sz.back() == d8) c->cp_sz.back() += sz;   // adjacent in host memory: one copy, whatever the cameras
       else { c->cp_dst.push_back(d8); c->cp_src.push_back(const_cast<void*>(imgs[k])); c->cp_sz.push_back(sz); } }
-    else { b.src = f.I0; c->cp_dst.push_back(f.I0); c->cp_src.push_back(const_cast<void*>(imgs[k])); c->cp_sz.push_back(px*sizeof(float)); }
-    vec = vec && ((uintptr_t)b.src % (u8 ? 4 : 16)) == 0 && ((uintptr_t)b.I0 % 16) == 0;   // 4-pixel vector loads / stores of the pyramid kernel
+    else { b.src = f.I0; c->cp_dst.push_back(f.I0); c->cp_src.push_back(const_cast<void*>(imgs[k])); c->cp_sz.push_back(px(k)*sizeof(float)); }
+    vec = vec && ((uintptr_t)b.src % (u8 ? 4 : 16)) == 0 && ((uintptr_t)b.I0 % 16) == 0 && b.w % 4 == 0;   // 4-pixel vector loads / stores of the pyramid kernel
   }
   if (!c->cp_dst.empty()) {                                               // all H2D copies of the batch in ONE runtime call, on the copy stream: PCIe stays busy while the
     if (seq > 2) CK(cudaStreamWaitEvent(c->st_cp, c->ev_ing[(seq-2) % sdv_ctx::kIngRing], 0));   // previous batch's pyramid runs on st_in
@@ -277,8 +306,8 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
   launch_h2d_words(c->pyr_batch_dev[par], desc, (size_t)n*sizeof(PyrBatchHost), c->st_in);   // kernel copy: a cudaMemcpyAsync here becomes ready only after this batch's bulk copy and
   c->launches += 1;                                                                              // would queue behind the NEXT batch's bulk copy on the H2D engine
   const UndistortCams* und = raw ? &c->und : nullptr;
-  if (c->levels > 1) { launch_pyramid_batch(c->pyr_batch_dev[par], n, u8, vec, c->w, c->h, c->levels, c->st_in, und); c->launches += 1; }
-  else if (u8 || (dev && !adopt)) { launch_pyramid_copy0(c->pyr_batch_dev[par], n, u8, c->w, c->h, c->st_in, und); c->launches += 1; }
+  if (c->levels > 1) { launch_pyramid_batch(c->pyr_batch_dev[par], n, u8, vec, c->w, c->h, max_w, max_h, c->levels, c->st_in, und); c->launches += 1; }
+  else if (u8 || (dev && !adopt)) { launch_pyramid_copy0(c->pyr_batch_dev[par], n, u8, max_w, max_h, c->st_in, und); c->launches += 1; }
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev_ing[seq % sdv_ctx::kIngRing], c->st_in)); c->ingest_seq = seq; c->ingest_pending = true;
   return SDV_OK;
@@ -298,7 +327,7 @@ int ensure_lvl0(sdv_ctx* c, FrameDev& f) {        // FrameHessian::dI of a keyfr
   if (c->lvl0_free.empty()) return ctx_fail(c, SDV_ERR_CAPACITY, "keyframe level-0 image pool exhausted (max_kf_images=%d)", (int)c->lvl0_pool.size());
   int rc = join_ingest(c); if (rc) return rc;
   f.lvl0_slot = c->lvl0_free.back(); c->lvl0_free.pop_back(); f.lvl[0] = c->lvl0_pool[f.lvl0_slot];
-  launch_grad_texels(f.I0, f.lvl[0], c->w, c->h, c->st); c->launches += 1;
+  launch_grad_texels(f.I0, f.lvl[0], c->cam_w[f.cam], c->cam_h[f.cam], c->st); c->launches += 1;
   CK(cudaGetLastError());
   return SDV_OK;
 }
@@ -306,11 +335,22 @@ int ensure_texels(sdv_ctx* c, FrameDev& f, int lvl) {   // FrameHessian::dIp / a
   if (lvl == 0) return ensure_lvl0(c, f);
   if (f.hi_tex) return SDV_OK;
   int rc = join_ingest_upto(c, f.ingest_seq); if (rc) return rc;        // only the ingest that built this frame: a later batch keeps streaming
-  for (int l=1;l<c->levels;l++) launch_grad_texels(f.img[l], f.lvl[l], c->w>>l, c->h>>l, c->st);
+  for (int l=1;l<c->levels;l++) launch_grad_texels(f.img[l], f.lvl[l], c->cam_w[f.cam]>>l, c->cam_h[f.cam]>>l, c->st);
   c->launches += c->levels - 1;
   CK(cudaGetLastError());
   f.hi_tex = true;
   return SDV_OK;
+}
+int check_frame_slot(sdv_ctx* c, const FrameDev& f, int slot, const char* who) {
+  const int fc = f.cam, sc = c->slots[slot].cam;
+  if (same_size(c, fc, sc)) return SDV_OK;
+  return ctx_fail(c, SDV_ERR_ARG, "%s: frame %llu is %dx%d (camera %d) but slot %d is bound to camera %d, %dx%d", who, (unsigned long long)f.id,
+                  c->cam_w[fc], c->cam_h[fc], fc, slot, sc, c->cam_w[sc], c->cam_h[sc]);
+}
+int check_frame_ctx(sdv_ctx* c, const FrameDev& f, const char* who) {
+  if (same_size(c, f.cam, 0)) return SDV_OK;
+  return ctx_fail(c, SDV_ERR_ARG, "%s: frame %llu is %dx%d (camera %d); this stage works at the context size %dx%d only", who, (unsigned long long)f.id,
+                  c->cam_w[f.cam], c->cam_h[f.cam], f.cam, c->w, c->h);
 }
 }
 extern "C" {
@@ -327,7 +367,7 @@ int sdv_set_undistort_cam(sdv_ctx* c, int cam, int w_org, int h_org, const float
   if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "camera %d outside 0..%d", cam, SDV_MAX_CAMERAS - 1);
   if (vignette_inv && !G256) return ctx_fail(c, SDV_ERR_ARG, "a vignette map needs a response function (PhotometricUndistorter::processFrame applies it to G[v] only)");
   CK(cudaSetDevice(c->device));
-  const size_t px = (size_t)c->w*c->h, po = (size_t)w_org*h_org;
+  const size_t px = (size_t)c->cam_w[cam]*c->cam_h[cam], po = (size_t)w_org*h_org;   // tables of the camera's rectified size
   for (size_t i=0;i<px;i++) {                                              // Undistort.cpp:871 tests iy against wOrg-1: a table built that way may read below the raw image
     const float x = remapX[i], y = remapY[i];
     if (x < 0) continue;
@@ -355,9 +395,16 @@ int sdv_frame_upload_batch_raw_u8_cams(sdv_ctx* c, int n, const uint64_t* frames
 int sdv_frame_upload_batch_raw_u8(sdv_ctx* c, int n, const uint64_t* frames, const uint8_t* const* raw_imgs, const float* exposures) {
   return sdv_frame_upload_batch_raw_u8_cams(c, n, frames, raw_imgs, nullptr, exposures);
 }
-int sdv_frame_build_batch_dev(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs_dev, int fmt, const float* exposures) { SDV_GUARD_TRK(c);
+int sdv_frame_build_batch_dev_cams(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs_dev, const int32_t* cams, int fmt, const float* exposures) { SDV_GUARD_TRK(c);
   if (fmt < 0 || fmt > 2) return SDV_ERR_ARG;
-  return frame_ingest(c, n, frames, imgs_dev, exposures, 2 | (fmt == 1 ? 1 : 0) | (fmt == 2 ? 4 : 0));
+  return frame_ingest(c, n, frames, imgs_dev, exposures, 2 | (fmt == 1 ? 1 : 0) | (fmt == 2 ? 4 : 0), cams);
+}
+int sdv_frame_build_batch_dev(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs_dev, int fmt, const float* exposures) {
+  return sdv_frame_build_batch_dev_cams(c, n, frames, imgs_dev, nullptr, fmt, exposures);
+}
+int sdv_frame_upload_batch_cams(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs, const int32_t* cams, int fmt, const float* exposures) { SDV_GUARD_TRK(c);
+  if (fmt < 0 || fmt > 1) return SDV_ERR_ARG;
+  return frame_ingest(c, n, frames, imgs, exposures, fmt, cams);
 }
 int sdv_frame_upload(sdv_ctx* c, uint64_t frame, const float* img, float exposure) { SDV_GUARD_TRK(c);
   const float* imgs[1] = {img}; return sdv_frame_upload_batch(c, 1, &frame, imgs, &exposure);
@@ -374,7 +421,7 @@ int sdv_frame_download(sdv_ctx* c, uint64_t frame, int lvl, float* dI3_out, floa
   FrameDev* f = find_frame(c, frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown frame %llu", (unsigned long long)frame);
   { int rcj = join_ingest(c); if (rcj) return rcj; }
   { int rct = ensure_texels(c, *f, lvl); if (rct) return rct; }
-  int n = (c->w>>lvl)*(c->h>>lvl); float *d3 = nullptr, *da = nullptr;
+  int n = (c->cam_w[f->cam]>>lvl)*(c->cam_h[f->cam]>>lvl); float *d3 = nullptr, *da = nullptr;   // the frame's own size
   if (dI3_out) CK(cudaMalloc(&d3, (size_t)3*n*sizeof(float)));
   if (abs_out) CK(cudaMalloc(&da, (size_t)n*sizeof(float)));
   launch_unpack_level(f->lvl[lvl], d3, da, n, c->st);
@@ -393,6 +440,7 @@ int sdv_tracker_set_cloud(sdv_ctx* c, int slot, uint64_t ref_frame, int lvl, int
   TrackerSlot& t = c->slots[slot];
   if (n > t.cap[lvl]) return ctx_fail(c, SDV_ERR_CAPACITY, "cloud of %d points exceeds capacity %d", n, t.cap[lvl]);
   FrameDev* f = find_frame(c, ref_frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown ref frame");
+  { int rcs = check_frame_slot(c, *f, slot, "sdv_tracker_set_cloud"); if (rcs) return rcs; }
   { int rcj = join_ingest(c); if (rcj) return rcj; }
   float* tmp = nullptr; CK(cudaMalloc(&tmp, (size_t)4*(n+1)*sizeof(float)));
   const float* src[4] = {u, v, idepth, color};
@@ -420,9 +468,11 @@ int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const f
   CK(cudaSetDevice(c->device));
   TrackerSlot& t = c->slots[slot];
   FrameDev* f = find_frame(c, ref_frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown ref frame");
+  { int rcs = check_frame_slot(c, *f, slot, "sdv_tracker_set_ref"); if (rcs) return rcs; }
+  const int w = c->cam_w[t.cam], h = c->cam_h[t.cam];      // makeCoarseDepthL0 at the slot's size
   for (int i=0;i<n;i++) {                                   // the reference would write out of bounds here; we refuse instead
     int u = round_half[i] ? (int)(pts4[4*i]+0.5f) : (int)pts4[4*i], v = round_half[i] ? (int)(pts4[4*i+1]+0.5f) : (int)pts4[4*i+1];
-    if (u < 0 || v < 0 || u >= c->w || v >= c->h) return ctx_fail(c, SDV_ERR_ARG, "splat %d (%d,%d) outside the image", i, u, v);
+    if (u < 0 || v < 0 || u >= w || v >= h) return ctx_fail(c, SDV_ERR_ARG, "splat %d (%d,%d) outside the image", i, u, v);
   }
   if (n > c->cd_cap) {
     cudaFree(c->cd_pts4); cudaFree(c->cd_round); cudaFree(c->cd_splats); cudaFree(c->cd_done);
@@ -431,7 +481,6 @@ int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const f
     CK(cudaMalloc(&c->cd_splats, (size_t)c->cd_cap*sizeof(float4))); CK(cudaMalloc(&c->cd_done, (size_t)c->cd_cap*sizeof(int)));
   }
   { int rcj = join_ingest(c); if (rcj) return rcj; }
-  const int w = c->w, h = c->h;
   CK(cudaMemsetAsync(c->cd_id[0], 0, (size_t)w*h*sizeof(float), c->st));
   CK(cudaMemsetAsync(c->cd_ws[0], 0, (size_t)w*h*sizeof(float), c->st));
   if (n > 0) {
@@ -471,6 +520,7 @@ int sdv_tracker_calc_res(sdv_ctx* c, int slot, uint64_t new_frame, int lvl, cons
   TrackerSlot& t = c->slots[slot];
   FrameDev* f = find_frame(c, new_frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown new frame");
   if (t.ref_frame == ~0ull) return ctx_fail(c, SDV_ERR_STATE, "tracker slot %d has no reference", slot);
+  { int rcs = check_frame_slot(c, *f, slot, "sdv_tracker_calc_res"); if (rcs) return rcs; }
   const LevelGeom& g = slot_geom(c, slot).g[lvl];
   EvalParams ep; make_eval_params(se3_from7(T), a, b, t.refExposure, f->exposure, t.ref_a, t.ref_b, g, lvl, cutoffTH, c->tc.huberTH, ep);
   { int rcj = join_ingest(c); if (rcj) return rcj; }
@@ -509,6 +559,7 @@ int sdv_tracker_track_batch(sdv_ctx* c, int n, const int32_t* slots, const uint6
     FrameDev* f = find_frame(c, new_frames[k]); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown new frame (job %d)", k);
     if (f->ingest_seq > need_seq) need_seq = f->ingest_seq;
     if (t.ref_frame == ~0ull) return ctx_fail(c, SDV_ERR_STATE, "tracker slot %d has no reference", slots[k]);
+    { int rcs = check_frame_slot(c, *f, slots[k], "sdv_tracker_track_batch"); if (rcs) return rcs; }
     TrackJob& J = c->jobs_host[k]; memset(&J, 0, sizeof(J));
     for (int l=0;l<c->levels;l++) { J.img[l] = f->img[l]; J.pts[l] = t.pts[l]; J.npts[l] = t.npts[l]; }
     J.refExposure = t.refExposure; J.newExposure = f->exposure; J.ref_a = t.ref_a; J.ref_b = t.ref_b;

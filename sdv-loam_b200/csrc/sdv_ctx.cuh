@@ -18,6 +18,7 @@ struct FrameDev {                         // one FrameHessian's images on the de
   // lvl[0] is a slot of the keyframe level-0 pool (lvl0_slot, -1 if not built); levels >= 1 live in `base` at lvl_off[l] and are valid while hi_tex is set.
   float4* base; float4* lvl[kLevels]; int lvl0_slot; bool hi_tex;
   long long ingest_seq;                   // ingest call that (re)built this frame's pyramid
+  int cam;                                // camera it was ingested for: its size is sdv_ctx::cam_w/cam_h[cam] (storage stays at the context size and lvl_off)
 };
 
 struct TrackerSlot {                      // one CoarseTracker instance (reference keeps two: FullSystem.h coarseTracker / coarseTracker_forNewKF)
@@ -25,6 +26,7 @@ struct TrackerSlot {                      // one CoarseTracker instance (referen
   uint64_t ref_frame; float refExposure; double ref_a, ref_b;   // lastRef, lastRef_aff_g2l
   double totals[kNAcc]; bool has_totals;                        // reduced sums of the last calc_res (what calcGSSSE reads from buf_warped_*)
   int geom_row;                                                 // row of sdv_ctx::geom this instance's makeK wrote (1 + slot), or 0: the context calibration
+  int cam;                                                      // camera of this tracker slot and the map slot of the same index (sdv_set_calib_slots_cams)
 };
 
 struct BAState;                           // sdv_ba.cuh
@@ -42,6 +44,7 @@ struct sdv_ctx {
   // ingest pipeline: H2D copies on st_cp, pyramids on st_in, one completion event per ingest call (ring); a frame remembers the ingest that built it
   static constexpr int kIngRing = 8; cudaEvent_t ev_ing[kIngRing], ev_cp[2]; long long ingest_seq = 0, seq_waited = 0;
   int w, h, levels; sdv_settings set;
+  int cam_w[SDV_MAX_CAMERAS], cam_h[SDV_MAX_CAMERAS];                  // rectified size per camera (sdv_set_camera_size); camera 0 is always w x h
   sdv::TrackConst tc; sdv::TrackConst* tc_dev;
   // geometry table (CoarseTracker::makeK per K): row 0 = the context calibration (sdv_set_calib), row 1 + s = tracker slot s's own K (sdv_set_calib_slots).
   // Host mirror + device copy; every consumer indexes it with TrackerSlot::geom_row, none derives the geometry from K itself.
@@ -90,6 +93,10 @@ inline bool frame_pinned(const sdv_ctx* c, uint64_t id) { return c->pins.find(id
 int  join_ingest(sdv_ctx* c);                  // compute stream waits for every ingest enqueued so far
 int  join_ingest_upto(sdv_ctx* c, long long seq);   // ... for ingest calls <= seq only (frames carry their ingest_seq)
 inline const GeomRow& slot_geom(const sdv_ctx* c, int slot) { return c->geom[c->slots[slot].geom_row]; }   // the K a tracker / map slot uses, at every level
+inline bool same_size(const sdv_ctx* c, int cam_a, int cam_b) { return c->cam_w[cam_a] == c->cam_w[cam_b] && c->cam_h[cam_a] == c->cam_h[cam_b]; }
+int  check_frame_slot(sdv_ctx* c, const FrameDev& f, int slot, const char* who);   // SDV_ERR_ARG (with a message) when frame f's size differs from slot's
+int  check_frame_ctx(sdv_ctx* c, const FrameDev& f, const char* who);              // ... from the context size (keyframe-rate stages)
+bool rp_slot_set(const sdv_ctx* c, int slot);                                     // map slot `slot` holds a resident map (sdv_map_set, not cleared)
 }
 // entry-point guards (a NULL context falls through to the entry's own argument check)
 #define SDV_GUARD_TRK(c) std::unique_lock<std::recursive_mutex> lk_trk_; if (c) lk_trk_ = std::unique_lock<std::recursive_mutex>((c)->mu_trk)

@@ -31,10 +31,15 @@ struct RpJob {
   const MapDev* map; const float* cur[kLevels]; double curT[7], curTinv[7];
   double K[9], Ki[9];                     // the map slot's K (its tracker slot's row of the geometry table at level 0) and K^-1, built on the host (rp_launch)
   float affLL[kRpMaxHosts][2]; int frame_rank[kRpMaxHosts];
-  int cur_kf_index, backup, nH, nP; long long pt_off; int error;
+  int cur_kf_index, backup, nH, nP; long long pt_off;
+  unsigned char error;                    // set by rp_project_kernel: a map point names a host outside [0, nH)
+  unsigned char cam;                      // camera of the map slot: its level-0 size is RpConst::cam_w/cam_h[cam]
   int geom_row;                           // handed to the structPoseEstimation job of the fused refinement (rp_emit_kernel)
 };
-struct RpConst { double K[9], Ki[9]; int w[kLevels], h[kLevels]; int levels, ncols, ncells; };   // K, Ki: the context calibration (geometry row 0), as launch constants
+static_assert(sizeof(RpJob) == 536, "RpJob keeps its size: the camera byte sits beside the one-byte error flag");
+// K, Ki: the context calibration (geometry row 0), as launch constants.  cam_w/cam_h: level-0 size per camera (the job's grid is ceil(w/25) x ceil(h/25));
+// ncols, ncells: the context grid, which strides the per-job outputs and numbers cell_order.
+struct RpConst { double K[9], Ki[9]; int cam_w[SDV_MAX_CAMERAS], cam_h[SDV_MAX_CAMERAS]; int levels, ncols, ncells; };
 struct RpScratch { double2* cand_px; float* cand_key; int* cand_cell; unsigned long long* list;   // list: per cell, (key bits << 32) | (frame rank << 27) | point index
                    int* count; int* begin; int* cursor; int* out_pt; double2* out_px;
                    double* xf; };   // xf[job][host][14]: camToWorld_host^-1 and T_cur_ref = camToWorld_cur^-1 * camToWorld_host (7 doubles each), built by rp_project_kernel
@@ -53,10 +58,10 @@ __device__ __forceinline__ void pixel_from_cam(const double* K, double* c, doubl
   c[0] = c[0]/c[2]; c[1] = c[1]/c[2]; c[2] = c[2]/c[2];
   double o[3]; mv3(K, c[0], c[1], c[2], o); px[0] = o[0]; px[1] = o[1];
 }
-__device__ __forceinline__ bool in_frame(const RpConst& C, double x, double y, int boundary) {
+__device__ __forceinline__ bool in_frame(int w, int h, double x, double y, int boundary) {
   if (!isfinite(x) || !isfinite(y) || fabs(x) > 1e9 || fabs(y) > 1e9) return false;
   const int ox = (int)x, oy = (int)y;
-  return ox >= boundary && ox < C.w[0]-boundary && oy >= boundary && oy < C.h[0]-boundary;
+  return ox >= boundary && ox < w-boundary && oy >= boundary && oy < h-boundary;
 }
 __device__ __forceinline__ float interp_plane(const float* __restrict__ I, float x, float y, int width) {                       // getInterpolatedElement33()[0]
   const int ix = (int)x, iy = (int)y; const float dx = x-ix, dy = y-iy, dxdy = dx*dy;
@@ -84,11 +89,12 @@ __global__ void __launch_bounds__(256) rp_project_kernel(RpJob* __restrict__ job
   if (jb.frame_rank[p.host] < 0) return;
   double px[2];
   if (jb.geom_row) project_point<true>(jb, C, m, p, px); else project_point<false>(jb, C, m, p, px);
-  if (!in_frame(C, px[0], px[1], 8)) return;
-  const int k = (int)(px[1]/kRpCell)*C.ncols + (int)(px[0]/kRpCell);
-  const float* __restrict__ I = m->hostI0[p.host]; const int w = C.w[0]; const int idx = (int)(p.v*w + p.u);
+  const int w = C.cam_w[jb.cam], h = C.cam_h[jb.cam];
+  if (!in_frame(w, h, px[0], px[1], 8)) return;
+  const int k = (int)(px[1]/kRpCell)*((w + kRpCell - 1)/kRpCell) + (int)(px[0]/kRpCell);      // the job's own grid
+  const float* __restrict__ I = m->hostI0[p.host]; const int idx = (int)(p.v*w + p.u);
   float key = 0.f;
-  if (idx >= w && idx < w*(C.h[0]-1)) { const float gx = grad_g(0.5f*(__ldg(I+idx+1) - __ldg(I+idx-1))), gy = grad_g(0.5f*(__ldg(I+idx+w) - __ldg(I+idx-w))); key = sqrtf(gx*gx + gy*gy); }
+  if (idx >= w && idx < w*(h-1)) { const float gx = grad_g(0.5f*(__ldg(I+idx+1) - __ldg(I+idx-1))), gy = grad_g(0.5f*(__ldg(I+idx+w) - __ldg(I+idx-w))); key = sqrtf(gx*gx + gy*gy); }
   S.cand_px[gi] = make_double2(px[0], px[1]); S.cand_key[gi] = key; S.cand_cell[gi] = k;
   atomicAdd(&S.count[(long long)blockIdx.y*C.ncells + k], 1);
 }
@@ -136,6 +142,7 @@ template <bool OWN_K>
 __device__ bool find_match_direct(const RpJob& jb, const RpConst& C, const sdv_map_pt& pt, double2& px_io, RpWarpSmem& sm, const int lane, const double* __restrict__ xf) {
   const double* __restrict__ K = OWN_K ? jb.K : C.K; const double* __restrict__ Ki = OWN_K ? jb.Ki : C.Ki;
   const MapDev* __restrict__ m = jb.map;
+  const int w0 = C.cam_w[jb.cam], h0 = C.cam_h[jb.cam];            // the job's level-0 size (read here: passing it in from the kernel adds spills)
   int ref;
   if (jb.nH <= 2) { if (!jb.backup) ref = 0; else if (jb.cur_kf_index == 0) ref = 1; else if (jb.cur_kf_index == 1) ref = 0; else return false; }
   else ref = pt.host;
@@ -144,7 +151,7 @@ __device__ bool find_match_direct(const RpJob& jb, const RpConst& C, const sdv_m
   const SE3d refInv = se3_from7(xf + ref*14);
   double ptRef[3]; xform(refInv, pw, ptRef);
   double cR[3] = {ptRef[0], ptRef[1], ptRef[2]}, px[2]; pixel_from_cam(K, cR, px);
-  if (!in_frame(C, px[0], px[1], 4+2)) return false;
+  if (!in_frame(w0, h0, px[0], px[1], 4+2)) return false;
   // getWarpMatrixAffine :14-37
   double A[4];
   { const int hp = 5; double du[3], dv[3]; mv3(Ki, px[0]+hp, px[1]+0, 1.0, du); mv3(Ki, px[0]+0, px[1]+hp, 1.0, dv);
@@ -160,7 +167,7 @@ __device__ bool find_match_direct(const RpJob& jb, const RpConst& C, const sdv_m
     const float a00 = (float)(A[3]*invdet), a10 = (float)(-A[2]*invdet), a01 = (float)(-A[1]*invdet), a11 = (float)(A[0]*invdet);
     __syncwarp();
     if (!isnan(a00)) {
-      const float prx = (float)px[0], pry = (float)px[1]; const float* __restrict__ I = m->hostI0[ref]; const int w0 = C.w[0], h0 = C.h[0];
+      const float prx = (float)px[0], pry = (float)px[1]; const float* __restrict__ I = m->hostI0[ref];
       for (int q = lane; q < 100; q += 32) { const int y = q/10, x = q - y*10;
         float p0 = (float)(x-5), p1 = (float)(y-5); p0 *= (1<<level); p1 *= (1<<level);
         const float qx = (a00*p0 + a01*p1) + prx, qy = (a10*p0 + a11*p1) + pry;
@@ -169,7 +176,7 @@ __device__ bool find_match_direct(const RpJob& jb, const RpConst& C, const sdv_m
         sm.pwb[q] = v; } }
     __syncwarp(); }
   double pxs[2] = {px_io.x/(1<<level), px_io.y/(1<<level)};
-  const int wl = C.w[level], hl = C.h[level];
+  const int wl = w0 >> level, hl = h0 >> level;
   const float min_update_squared = (float)(0.03*0.03);
   bool converged = false;
   float u = (float)pxs[0], v = (float)pxs[1], mean_diff = 0;
@@ -178,7 +185,7 @@ __device__ bool find_match_direct(const RpJob& jb, const RpConst& C, const sdv_m
   const float ref0 = sm.pwb[(y0+1)*10 + 1 + x0], ref1 = sm.pwb[(y1+1)*10 + 1 + x1];       // createPatchFromPatchWithBorder :334-344
   bool early_false = false;
   if (pt.type == 1) {                                                          // EDGELET: align1D :346-455
-    const float* __restrict__ I = m->hostI0[ref]; const int w0 = C.w[0]; const int idx = (int)(px[0] + px[1]*w0);
+    const float* __restrict__ I = m->hostI0[ref]; const int idx = (int)(px[0] + px[1]*w0);
     double g0 = (double)grad_g(0.5f*(__ldg(I+idx+1) - __ldg(I+idx-1))), g1 = (double)grad_g(0.5f*(__ldg(I+idx+w0) - __ldg(I+idx-w0)));
     { const double n = sqrt(g0*g0 + g1*g1); g0 /= n; g1 /= n; }
     double d0 = A[0]*g0 + A[1]*g1, d1 = A[2]*g0 + A[3]*g1; { const double n2 = sqrt(d0*d0 + d1*d1); d0 /= n2; d1 /= n2; }
@@ -273,19 +280,29 @@ __global__ void __launch_bounds__(32*kRpWarps, RP_MATCH_MINB) rp_match_kernel(co
   if (lane == 0) { S.out_pt[cb] = found; S.out_px[cb] = fpx; }
 }
 
+// cell `cell` of the context grid (ncols columns) as a cell of a job's grid of jcols x jrows, or -1 when the job's grid does not have it: a job on a smaller
+// camera walks the context's cell_order and skips the cells outside its grid (sdv_b200.h, sdv_reproject_map_batch); on the context grid this is the identity
+__host__ __device__ __forceinline__ int job_cell(int cell, int ncols, int jcols, int jrows) {
+  const int r = cell / ncols, col = cell - r*ncols;
+  return (col < jcols && r < jrows) ? r*jcols + col : -1;
+}
+__host__ __device__ __forceinline__ int grid_dim(int px) { return (px + kRpCell - 1)/kRpCell; }
+
 // Ordered emission of the per-cell results (reprojectMap :147-155): cells are visited in cell_order, every cell with a match contributes one
 // overlap point, the walk stops once more than max_matches were produced.  One CTA per frame; also fills the structPoseEstimation job.
 __global__ void __launch_bounds__(1024) rp_emit_kernel(const RpJob* __restrict__ jobs, RpConst C, RpScratch S, const int* __restrict__ cell_order, int max_matches,
                                                        sdv_overlap_pt* __restrict__ ov, RefineJob* __restrict__ rj, int* __restrict__ n_out) {
   const RpJob& jb = jobs[blockIdx.x]; const MapDev* __restrict__ m = jb.map;
   const long long base = (long long)blockIdx.x*C.ncells; const int per = (C.ncells + 1023)/1024;
+  const int jcols = grid_dim(C.cam_w[jb.cam]), jrows = grid_dim(C.cam_h[jb.cam]);
   __shared__ int part[1024];
-  int s = 0; for (int k = 0; k < per; k++) { const int i = threadIdx.x*per + k; if (i < C.ncells) { const int cell = cell_order ? cell_order[i] : i; s += (S.out_pt[base+cell] >= 0) ? 1 : 0; } }
+  int s = 0; for (int k = 0; k < per; k++) { const int i = threadIdx.x*per + k; if (i < C.ncells) { const int cell = job_cell(cell_order ? cell_order[i] : i, C.ncols, jcols, jrows); s += (cell >= 0 && S.out_pt[base+cell] >= 0) ? 1 : 0; } }
   part[threadIdx.x] = s; __syncthreads();
   for (int o = 1; o < 1024; o <<= 1) { int v = (threadIdx.x >= o) ? part[threadIdx.x-o] : 0; __syncthreads(); part[threadIdx.x] += v; __syncthreads(); }
   int run = part[threadIdx.x] - s;
   const int total = min(part[1023], max_matches + 1);
-  for (int k = 0; k < per; k++) { const int i = threadIdx.x*per + k; if (i >= C.ncells) break; const int cell = cell_order ? cell_order[i] : i;
+  for (int k = 0; k < per; k++) { const int i = threadIdx.x*per + k; if (i >= C.ncells) break; const int cell = job_cell(cell_order ? cell_order[i] : i, C.ncols, jcols, jrows);
+    if (cell < 0) continue;
     const int pi = S.out_pt[base+cell]; if (pi < 0) continue;
     if (run < total) { const sdv_map_pt p = m->pts[pi]; const double2 px = S.out_px[base+cell];
       sdv_overlap_pt o; o.u = p.u; o.v = p.v; o.idepth = p.idepth; o.host = p.host; o.obs_x = (float)px.x; o.obs_y = (float)px.y; ov[base + run] = o; }
@@ -305,10 +322,10 @@ struct RpState { std::vector<MapSlot> maps; void* dev = nullptr; void* host = nu
 static void rp_job_K(const LevelGeom& g, double* K, double* Ki);
 static RpState* rp_state(sdv_ctx* c) {
   if (!c->rp) { c->rp = new RpState(); c->rp->maps.resize(c->slots.size()); RpConst& C = c->rp->C;
-    C.levels = c->levels; for (int l=0;l<kLevels;l++) { C.w[l] = c->w >> l; C.h[l] = c->h >> l; }
-    C.ncols = (c->w + kRpCell - 1)/kRpCell; C.ncells = C.ncols*((c->h + kRpCell - 1)/kRpCell); }
+    C.levels = c->levels; C.ncols = grid_dim(c->w); C.ncells = C.ncols*grid_dim(c->h); }
   return c->rp;
 }
+bool rp_slot_set(const sdv_ctx* c, int slot) { return c->rp && slot < (int)c->rp->maps.size() && c->rp->maps[slot].set; }
 void rp_destroy(sdv_ctx* c) { if (!c->rp) return; for (auto& m : c->rp->maps) { if (m.set) for (int k=0;k<m.nH;k++) frame_unpin(c, m.host_ids[k]); cudaFree(m.dev); cudaFree(m.pts); } cudaFree(c->rp->dev); cudaFreeHost(c->rp->host); delete c->rp; c->rp = nullptr; }
 static void rp_job_K(const LevelGeom& g, double* K, double* Ki) {        // the Reprojector's K_ and K_.inverse() (Reprojector.cpp:565) from level 0 of a geometry row
   for (int i=0;i<9;i++) K[i] = 0; K[0] = (double)g.fx; K[2] = (double)g.cx; K[4] = (double)g.fy; K[5] = (double)g.cy; K[8] = 1.0;
@@ -324,7 +341,7 @@ static void rp_job_K(const LevelGeom& g, double* K, double* Ki) {        // the 
 extern "C" {
 
 int sdv_reproject_grid(sdv_ctx* c, int* n_cols, int* n_rows) { SDV_GUARD_TRK(c);
-  if (!c) return SDV_ERR_ARG; if (n_cols) *n_cols = (c->w + kRpCell - 1)/kRpCell; if (n_rows) *n_rows = (c->h + kRpCell - 1)/kRpCell; return SDV_OK;
+  if (!c) return SDV_ERR_ARG; if (n_cols) *n_cols = grid_dim(c->w); if (n_rows) *n_rows = grid_dim(c->h); return SDV_OK;
 }
 
 int sdv_map_set(sdv_ctx* c, int slot, int nH, const uint64_t* host_frames, const double* host_T7, const double* host_ab, int nP, const sdv_map_pt* pts) { SDV_GUARD_TRK(c);
@@ -335,7 +352,8 @@ int sdv_map_set(sdv_ctx* c, int slot, int nH, const uint64_t* host_frames, const
   if (!m.dev) CK(cudaMalloc(&m.dev, sizeof(MapDev)));
   if (nP > m.cap) { cudaFree(m.pts); m.pts = nullptr; m.cap = nP + nP/4 + 256; CK(cudaMalloc(&m.pts, (size_t)m.cap*sizeof(sdv_map_pt))); }
   { int rcj = join_ingest(c); if (rcj) return rcj; }
-  for (int k=0;k<nH;k++) if (c->frame_index.find(host_frames[k]) == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "map_set: unknown keyframe handle (host %d)", k);
+  for (int k=0;k<nH;k++) { auto it = c->frame_index.find(host_frames[k]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "map_set: unknown keyframe handle (host %d)", k);
+    int rcs = check_frame_slot(c, c->frames[it->second], slot, "sdv_map_set"); if (rcs) return rcs; }
   if (m.set) for (int k=0;k<m.nH;k++) frame_unpin(c, m.host_ids[k]);       // the slot's previous keyframes are no longer referenced by it
   for (int k=0;k<nH;k++) frame_pin(c, host_frames[k]);
   MapDev& h = m.host_copy; memset(&h, 0, sizeof(h)); h.nH = nH; h.nP = nP; h.pts = m.pts; m.ingest_seq = 0;
@@ -362,7 +380,9 @@ int sdv_map_clear(sdv_ctx* c, int slot) { SDV_GUARD_TRK(c);
 struct RpRun { RpScratch S; RpJob* jobs_dev; RpJob* jobs_host; int32_t* h_opt; double2* h_opx; sdv_overlap_pt* ov; RefineJob* rj; RefineJob* rj_host; int* n_out_dev; int* n_out_host; int* cell_order_dev; long long nc; };
 static int rp_launch(sdv_ctx* c, int n_jobs, const int32_t* slots, const uint64_t* cur_frames, const double* cur_T7, const double* cur_ab,
                      const int32_t* cur_kf_index, const int32_t* only_host, const int32_t* backup, RpRun& R) {
-  RpState* st = rp_state(c); rp_job_K(c->geom[0].g[0], st->C.K, st->C.Ki); const RpConst& C = st->C;
+  RpState* st = rp_state(c); rp_job_K(c->geom[0].g[0], st->C.K, st->C.Ki);
+  for (int k=0;k<SDV_MAX_CAMERAS;k++) { st->C.cam_w[k] = c->cam_w[k]; st->C.cam_h[k] = c->cam_h[k]; }
+  const RpConst& C = st->C;
   long long totalP = 0; int maxP = 1;
   for (int k=0;k<n_jobs;k++) { if (slots[k] < 0 || slots[k] >= (int)st->maps.size() || !st->maps[slots[k]].set) return ctx_fail(c, SDV_ERR_STATE, "reproject job %d: map slot %d not set", k, slots[k]);
     totalP += st->maps[slots[k]].nP; maxP = std::max(maxP, st->maps[slots[k]].nP); }
@@ -381,6 +401,7 @@ static int rp_launch(sdv_ctx* c, int n_jobs, const int32_t* slots, const uint64_
   RpJob* J = (RpJob*)(hb + h_jobs); R.jobs_host = J; R.h_opt = (int32_t*)(hb + h_opt); R.h_opx = (double2*)(hb + h_opx); R.rj_host = (RefineJob*)(hb + h_rj); R.n_out_host = (int*)(hb + h_no);
   long long need_seq = 0;
   for (int k=0;k<n_jobs;k++) { auto it = c->frame_index.find(cur_frames[k]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "reproject job %d: unknown target frame", k);
+    { int rcs = check_frame_slot(c, c->frames[it->second], slots[k], "reproject / refine"); if (rcs) return rcs; }
     need_seq = std::max(need_seq, std::max(c->frames[it->second].ingest_seq, st->maps[slots[k]].ingest_seq)); }
   { int rcj = join_ingest_upto(c, need_seq); if (rcj) return rcj; }     // only the uploads these frames came from (a later batch may still be streaming in)
   long long off = 0;
@@ -389,7 +410,7 @@ static int rp_launch(sdv_ctx* c, int n_jobs, const int32_t* slots, const uint64_
     auto it = c->frame_index.find(cur_frames[k]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "reproject job %d: unknown target frame", k);
     const FrameDev& f = c->frames[it->second];
     j.map = m.dev; for (int l=0;l<c->levels;l++) j.cur[l] = f.img[l];
-    rp_job_K(slot_geom(c, slots[k]).g[0], j.K, j.Ki); j.geom_row = c->slots[slots[k]].geom_row;
+    rp_job_K(slot_geom(c, slots[k]).g[0], j.K, j.Ki); j.geom_row = c->slots[slots[k]].geom_row; j.cam = (unsigned char)c->slots[slots[k]].cam;
     for (int i=0;i<7;i++) j.curT[i] = cur_T7[7*k+i];
     const SE3d cur = se3_from7(j.curT); se3_to7(se3_inv(cur), j.curTinv);
     j.cur_kf_index = cur_kf_index ? cur_kf_index[k] : -1; j.backup = backup ? backup[k] : 0; j.nH = m.nH; j.nP = m.nP; j.pt_off = off; off += m.nP;
@@ -434,7 +455,9 @@ int sdv_reproject_map_batch(sdv_ctx* c, int n_jobs, const int32_t* slots, const 
   for (int k=0;k<n_jobs;k++) {
     if (R.jobs_host[k].error) return ctx_fail(c, SDV_ERR_ARG, "reproject job %d: a map point names a host outside [0,%d)", k, R.jobs_host[k].nH);
     int n = 0, matches = 0; int32_t* op = out_pt + (size_t)k*C.ncells; double* ox = out_px + (size_t)k*C.ncells*2;
-    for (int i=0;i<C.ncells;i++) { const int cell = cell_order ? cell_order[i] : i; if (cell < 0 || cell >= C.ncells) return ctx_fail(c, SDV_ERR_ARG, "cell_order[%d] = %d", i, cell);
+    const int jcols = grid_dim(C.cam_w[R.jobs_host[k].cam]), jrows = grid_dim(C.cam_h[R.jobs_host[k].cam]);
+    for (int i=0;i<C.ncells;i++) { int cell = cell_order ? cell_order[i] : i; if (cell < 0 || cell >= C.ncells) return ctx_fail(c, SDV_ERR_ARG, "cell_order[%d] = %d", i, cell);
+      cell = job_cell(cell, C.ncols, jcols, jrows); if (cell < 0) continue;
       const long long cb = (long long)k*C.ncells + cell;
       if (R.h_opt[cb] >= 0) { op[n] = R.h_opt[cb]; ox[2*n] = R.h_opx[cb].x; ox[2*n+1] = R.h_opx[cb].y; n++; matches++; }
       if (matches > max_matches) break; }                                      // Reprojector.cpp:151-153

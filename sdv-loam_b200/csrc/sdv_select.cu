@@ -25,7 +25,8 @@ void sel_destroy(sdv_ctx* c) {
 }
 static int sel_frame(sdv_ctx* c, uint64_t id, sel::FrameImg& F, long long& need_seq, const char* who, bool texels = true) {
   auto it = c->frame_index.find(id); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "%s: unknown frame %llu", who, (unsigned long long)id);
-  FrameDev& f = c->frames[it->second]; if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
+  FrameDev& f = c->frames[it->second]; { int rcs = check_frame_ctx(c, f, who); if (rcs) return rcs; }
+  if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
   F.I0 = f.I0; F.L1 = nullptr; F.L2 = nullptr;
   if (texels) { int rc = ensure_texels(c, f, 1); if (rc) return rc; F.L1 = f.lvl[1]; F.L2 = f.lvl[2]; }   // |grad|^2 of levels 1 and 2 (makeMaps / makeNewTraces read the packed texels)
   return SDV_OK;

@@ -318,6 +318,7 @@ int sdv_immature_init(sdv_ctx* c, uint64_t host_frame, int n, const int32_t* uv,
   if (n == 0) return SDV_OK;
   CK(cudaSetDevice(c->device));
   auto it = c->frame_index.find(host_frame); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_init: unknown host frame %llu", (unsigned long long)host_frame);
+  { int rcs = check_frame_ctx(c, c->frames[it->second], "immature_init"); if (rcs) return rcs; }
   for (int i = 0; i < n; i++) if (uv[2*i] < 2 || uv[2*i+1] < 2 || uv[2*i] >= c->w-3 || uv[2*i+1] >= c->h-3)     // the 8-pattern (+-2) and the +1 bilinear neighbour must stay inside the image
     return ctx_fail(c, SDV_ERR_ARG, "immature_init: candidate %d at (%d,%d) is closer than 3 px to the border", i, uv[2*i], uv[2*i+1]);
   FrameDev& f = c->frames[it->second];
@@ -346,7 +347,8 @@ int sdv_immature_trace_batch(sdv_ctx* c, int n_groups, const uint64_t* frames, c
   std::vector<TraceGroupDev> G(n_groups); std::vector<int> gof(n); long long need_seq = 0;
   for (int g = 0; g < n_groups; g++) {
     auto it = c->frame_index.find(frames[g]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_trace: unknown frame %llu (group %d)", (unsigned long long)frames[g], g);
-    const FrameDev& f = c->frames[it->second]; if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
+    const FrameDev& f = c->frames[it->second]; { int rcs = check_frame_ctx(c, f, "immature_trace"); if (rcs) return rcs; }
+    if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
     G[g].I0 = f.I0; for (int k = 0; k < 9; k++) G[g].KRKi[k] = KRKi9[9*g+k]; for (int k = 0; k < 3; k++) G[g].Kt[k] = Kt3[3*g+k]; G[g].aff[0] = aff2[2*g]; G[g].aff[1] = aff2[2*g+1];
     G[g].pt_begin = pt_begin[g]; G[g].pt_end = pt_begin[g+1];
     for (int i = pt_begin[g]; i < pt_begin[g+1]; i++) gof[i] = g;
@@ -385,7 +387,8 @@ int sdv_immature_optimize_batch(sdv_ctx* c, int n_groups, const int32_t* pt_begi
   std::vector<OptGroupDev> G(n_groups); std::vector<OptTargetDev> T(nt); std::vector<int> gof(n); long long need_seq = 0;
   for (int t = 0; t < nt; t++) {
     auto it = c->frame_index.find(target_frames[t]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_optimize: unknown target frame %llu", (unsigned long long)target_frames[t]);
-    const FrameDev& f = c->frames[it->second]; if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
+    const FrameDev& f = c->frames[it->second]; { int rcs = check_frame_ctx(c, f, "immature_optimize"); if (rcs) return rcs; }
+    if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
     T[t].I0 = f.I0; for (int k = 0; k < 9; k++) T[t].R[k] = pre14[14*t+k]; for (int k = 0; k < 3; k++) T[t].t[k] = pre14[14*t+9+k]; T[t].aff[0] = pre14[14*t+12]; T[t].aff[1] = pre14[14*t+13];
   }
   for (int g = 0; g < n_groups; g++) { G[g].tgt_begin = tgt_begin[g]; G[g].nres = tgt_begin[g+1] - tgt_begin[g]; const float* q = calib6 + 6*g;
