@@ -122,7 +122,7 @@ int  sdv_frame_build_batch_dev(sdv_ctx* c, int n, const uint64_t* frames, const 
  * w, h); cameras 1..SDV_MAX_CAMERAS-1 start at it.  sdv_set_camera_size gives camera `cam` another rectified size w x h: w <= the context's w, h <= its
  * h (frame storage is allocated at the context size: create the context at the largest size), and the context's pyramid depth valid at that size (even
  * w, h when levels > 1, every level non-empty).  Camera 0, a camera index out of range or a size outside these rules return SDV_ERR_ARG; resizing a
- * camera that has Undistort tables, a resident frame or a bound slot (sdv_set_calib_slots_cams) returns SDV_ERR_STATE.  A refused call changes nothing.
+ * camera that has Undistort tables, a resident frame or a bound tracker or selector slot (sdv_set_calib_slots_cams, sdv_selector_set_slot_cams) returns SDV_ERR_STATE.  A refused call changes nothing.
  * sdv_set_undistort_cam then takes remap tables of that camera's size.  A frame has the size of the camera it was ingested for:
  * sdv_frame_upload_batch_cams takes host float (fmt 0) or mono8 (fmt 1) images, and sdv_frame_build_batch_dev_cams device images with the fmt values of
  * sdv_frame_build_batch_dev (fmt 2 adopts a buffer of w_cam*h_cam floats), each at its camera's size.  cams == NULL is camera 0 (the entries without
@@ -130,7 +130,8 @@ int  sdv_frame_build_batch_dev(sdv_ctx* c, int n, const uint64_t* frames, const 
  * Every per-frame entry compares the frame's size with its slot's and returns SDV_ERR_ARG on a mismatch, changing no state: sdv_tracker_set_ref (ref
  * frame), calc_res / track / track_batch / sdv_track_new_coarse_batch (new frame), sdv_map_set (host keyframes), sdv_reproject_map_batch /
  * sdv_tracker_refine_batch (target frame); sdv_ba_set_window needs all frames of one window at one size.  The keyframe-rate candidate management
- * (selector, makeNewTraces, activation, immature points) works at the context size only and refuses frames of another size with SDV_ERR_ARG. */
+ * (selector, makeNewTraces, activation, immature points, LiDAR front-end) names a camera per job (the _cam / _cams entries, sdv_selector_set_slot_cams)
+ * and works at that camera's size; a frame of another size returns SDV_ERR_ARG and changes no state.  The entries without _cam(s) are camera 0. */
 int  sdv_set_camera_size(sdv_ctx* c, int cam, int w, int h);
 int  sdv_frame_upload_batch_cams(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs, const int32_t* cams, int fmt, const float* exposures);
 int  sdv_frame_build_batch_dev_cams(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs_dev, const int32_t* cams, int fmt, const float* exposures);
@@ -277,22 +278,31 @@ typedef struct {
   float energyTH, quality, lastTraceUV[2], lastTracePixelInterval;
   int32_t lastTraceStatus;
 } sdv_immature_pt;
-/* constructor for n candidates at integer pixels uv[2n] of a resident keyframe (>= 3 px from the border, else SDV_ERR_ARG) */
+/* constructor for n candidates at integer pixels uv[2n] of a resident keyframe (>= 3 px from the border, else SDV_ERR_ARG).  _cam: the keyframe is camera cam's
+ * (its size must be that camera's, and the border is that camera's); sdv_immature_init is camera 0. */
 int  sdv_immature_init(sdv_ctx* c, uint64_t host_frame, int n, const int32_t* uv, sdv_immature_pt* out);
+int  sdv_immature_init_cam(sdv_ctx* c, int cam, uint64_t host_frame, int n, const int32_t* uv, sdv_immature_pt* out);
 /* traceOn for n_groups (host keyframe, traced frame) pairs in ONE launch: group g traces pts_io[pt_begin[g] .. pt_begin[g+1]) against frames[g] with
  * KRKi9[9g..] = K R K^-1 (row-major), Kt3[3g..] = K t of hostToNew and aff2[2g..] = AffLight::fromToVecExposure(host, new) — what traceNewCoarse computes per host
- * (:532-538).  Groups may belong to different sequences (batched mode).  pts_io is updated in place; status_out (n points) may be NULL. */
+ * (:532-538).  Groups may belong to different sequences (batched mode).  pts_io is updated in place; status_out (n points) may be NULL.
+ * _cams: group g traces at camera cams[g]'s size (wG[0], hG[0] of its sequence) and frames[g] must have that size; cams == NULL is sdv_immature_trace_batch (camera 0). */
 int  sdv_immature_trace_batch(sdv_ctx* c, int n_groups, const uint64_t* frames, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* aff2,
                               sdv_immature_pt* pts_io, int32_t* status_out);
+int  sdv_immature_trace_batch_cams(sdv_ctx* c, int n_groups, const uint64_t* frames, const int32_t* cams, const int32_t* pt_begin, const float* KRKi9, const float* Kt3,
+                                   const float* aff2, sdv_immature_pt* pts_io, int32_t* status_out);
 /* Activation — PointHessian* FullSystem::optimizeImmaturePoint(ImmaturePoint*, int minObs, ImmaturePointTemporaryResidual*)   FullSystemOptPoint.cpp:18-183
  * over ImmaturePoint::linearizeResidual (ImmaturePoint.cpp:410-476): Gauss-Newton on the inverse depth of a candidate against every other keyframe of the window.
  * Group g = the candidates pts[pt_begin[g] .. pt_begin[g+1]) of ONE host keyframe; its targets are entries tgt_begin[g] .. tgt_begin[g+1]) of target_frames / pre14
  * (frameHessians without the host, window order; pre14 = host->targetPrecalc[target]: PRE_RTll[9] row-major, PRE_tTll[3], PRE_aff_mode[2]); calib6[6g..] = fxl fyl cxl cyl
  * fxli fyli of the CalibHessian.  Outputs per candidate: status 0 = not well constrained (stays immature; the function's `return 0`), -1 = outlier / non-finite
  * (deleted), 1 = activated with idepth_out (setIdepth/setIdepthZero) and res_state_out[k*res_stride + i] = final state of the temporary residual to target i
- * (0 IN -> a PointFrameResidual is created, 1 OOB, 2 OUTLIER; -1 = unused).  The PointHessian / PointFrameResidual objects stay with the caller. */
+ * (0 IN -> a PointFrameResidual is created, 1 OOB, 2 OUTLIER; -1 = unused).  The PointHessian / PointFrameResidual objects stay with the caller.
+ * _cams: group g works at camera cams[g]'s size and every target of the group must have it; cams == NULL is sdv_immature_optimize_batch (camera 0). */
 int  sdv_immature_optimize_batch(sdv_ctx* c, int n_groups, const int32_t* pt_begin, const int32_t* tgt_begin, const uint64_t* target_frames, const float* pre14, const float* calib6,
                                  int min_obs, const sdv_immature_pt* pts, const uint8_t* is_from_sensor, int res_stride, int32_t* status_out, float* idepth_out, int32_t* res_state_out);
+int  sdv_immature_optimize_batch_cams(sdv_ctx* c, int n_groups, const int32_t* pt_begin, const int32_t* tgt_begin, const uint64_t* target_frames, const float* pre14,
+                                      const float* calib6, const int32_t* cams, int min_obs, const sdv_immature_pt* pts, const uint8_t* is_from_sensor, int res_stride,
+                                      int32_t* status_out, float* idepth_out, int32_t* res_state_out);
 
 /* frames + calibration + marginalisation prior:  EnergyFunctional::insertFrame :365-398, setAdjointsF :21-71, HM/bM :88-89.
  * state10 / state_zero10 = FrameHessian::state / state_zero (Vec10: 6 pose, a, b, 2 unused; HessianBlocks.h:141-175),
@@ -376,17 +386,24 @@ int  sdv_ba_get_precalc(sdv_ctx* c, int host, int target, float out27[27], doubl
  * persistent monocular selection map (w*h bytes, values 0 / 1 / 2 / 4 — the reference's float map; zero at birth where the reference's is uninitialised).
  * random_pattern: the w*h bytes of PixelSelector::randomPattern — the caller generates them exactly like the constructor does (srand(3141592); rand() & 0xFF), so the
  * library never touches the process-wide rand() stream.  Reads of thsSmoothed past its (h/32) rows — the reference indexes its uninitialised tail for the last
- * image rows — see zeros here.  LiDAR pixels are rows {Ku, Kv, depth} of doubles, as main.cpp:810-848 pushes them into FullSystem::qCloudPixel. */
+ * image rows — see zeros here.  LiDAR pixels are rows {Ku, Kv, depth} of doubles, as main.cpp:810-848 pushes them into FullSystem::qCloudPixel.
+ * Cameras of another size (sdv_set_camera_size): sdv_selector_set_slot_cams binds slot slots[i] to camera cams[i] (after sdv_selector_init every slot is on
+ * camera 0).  A slot on camera c works at w_c x h_c: its frames must have that size (else SDV_ERR_ARG), its persistent map is w_c*h_c bytes
+ * (sdv_selector_get_map), and its pattern is the first w_c*h_c bytes of random_pattern (what PixelSelector(w_c, h_c) draws after the same srand).  Rebinding
+ * a slot to a camera of another size starts it afresh (map zeroed, currentPotential 3: a new PixelSelector); the same size keeps its state.  A slot or
+ * camera out of range returns SDV_ERR_ARG and changes no slot.  sdv_selector_make_hists_cam: the frame is camera cam's ((w_c/32) x (h_c/32) blocks). */
 typedef struct { float u, v, my_type, score, idepth_fromSensor; int32_t isFromSensor, type; } sdv_new_trace;   /* type: 0 CORNER, 1 EDGELET (ImmaturePoint.h), -1 not assigned (monocular points) */
 int  sdv_selector_init(sdv_ctx* c, const uint8_t* random_pattern, int n_slots);
 int  sdv_selector_potential(sdv_ctx* c, int slot, int set_to /* <= 0: leave */, int* out);
 int  sdv_selector_get_map(sdv_ctx* c, int slot, uint8_t* out_wh);
+int  sdv_selector_set_slot_cams(sdv_ctx* c, int n, const int32_t* slots, const int32_t* cams);
 /* void PixelSelector::makeHists(const FrameHessian*): ths / thsSmoothed of the (w/32) x (h/32) blocks */
 int  sdv_selector_make_hists(sdv_ctx* c, uint64_t frame, float* ths_out, float* thsSmoothed_out);
+int  sdv_selector_make_hists_cam(sdv_ctx* c, int cam, uint64_t frame, float* ths_out, float* thsSmoothed_out);
 /* int PixelSelector::makeMapsFromLidar(fh, map_out, density, recursionsLeft, plot, thFactor, vCloudPixel) for n (slot, frame) pairs at once when cloud_begin != NULL
  * (job j owns cloud rows cloud_begin[j] .. cloud_begin[j+1]; maps_out = the n maps back to back, one byte per cloud row), and
- * int PixelSelector::makeMaps(fh, map_out, density, recursionsLeft, plot, thFactor) when cloud_begin == NULL (maps_out = n maps of w*h bytes; the slot's persistent map
- * is the one written).  makeHists runs first, like `if(fh != gradHistFrame) makeHists(fh)`.  num_have_out[j] = the return value; the slot's currentPotential is updated. */
+ * int PixelSelector::makeMaps(fh, map_out, density, recursionsLeft, plot, thFactor) when cloud_begin == NULL (maps_out = the n maps back to back, job j's at its slot's
+ * camera size w_c*h_c; the slot's persistent map is the one written).  makeHists runs first, like `if(fh != gradHistFrame) makeHists(fh)`.  num_have_out[j] = the return value; the slot's currentPotential is updated. */
 int  sdv_selector_make_maps_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const float* density,
                                   const int32_t* recursions_left, const float* th_factor, uint8_t* maps_out, int32_t* num_have_out);
 /* void FullSystem::makeNewTraces(FrameHessian* newFrame, float*) for n new keyframes (one per sequence / slot) in one call.  density_lidar[j] =
@@ -401,10 +418,15 @@ int  sdv_make_new_traces_batch(sdv_ctx* c, int n, const int32_t* slots, const ui
  * pt_begin[k] .. pt_begin[k+1] = {u, v, idepth_scaled}; KRKi9 / Kt3 per keyframe = K[1] R K[0]^-1, K[1] t of host -> newest, FullSystem.cpp:606-608) and candidate
  * keyframes cand_host_begin[j] .. (their candidates: cand4 rows {u, v, 0.5f*(idepth_max+idepth_min), my_type} that passed the deletion / canActivate tests of
  * :618-645, which are pointer-graph bookkeeping).  decision_out per candidate: 1 = handed to optimizeImmaturePoint (sdv_immature_optimize_batch), 0 = too close to
- * existing points, -1 = projects outside the level-1 image (deleted).  dist_map_out (optional): n maps of (w/2)*(h/2) floats = fwdWarpedIDDistFinal after the walk. */
+ * existing points, -1 = projects outside the level-1 image (deleted).  dist_map_out (optional): n maps of (w/2)*(h/2) floats = fwdWarpedIDDistFinal after the walk.
+ * _cams: sequence j is camera cams[j]'s, its map and walk are at (w_c/2) x (h_c/2) and dist_map_out holds the maps back to back, each at its own size;
+ * cams == NULL is sdv_activate_select_batch (camera 0). */
 int  sdv_activate_select_batch(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,
                                const int32_t* cand_host_begin, const int32_t* cand_begin, const float* cKRKi9, const float* cKt3, const float* cand4, const float* min_act_dist,
                                int32_t* decision_out, float* dist_map_out);
+int  sdv_activate_select_batch_cams(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,
+                                    const int32_t* cand_host_begin, const int32_t* cand_begin, const float* cKRKi9, const float* cKt3, const float* cand4,
+                                    const float* min_act_dist, const int32_t* cams, int32_t* decision_out, float* dist_map_out);
 
 /* =====================================================================================================================
  * LiDAR front-end of the node (SURVEY.md §8f rank 3, second half): void lidarCloudHandler(const sensor_msgs::PointCloud2ConstPtr&)   src/main.cpp:785-858
@@ -413,12 +435,14 @@ int  sdv_activate_select_batch(sdv_ctx* c, int n, const int32_t* host_begin, con
  * sdv_lidar_handler_batch: n raw sweeps (one per resident sequence), sweep j = XYZI rows sweep_begin[j] .. sweep_begin[j+1] of xyzi (the decoded PointCloud2, what
  * pcl::fromROSMsg yields; rows with a non-finite coordinate are dropped like pcl::removeNaNFromPointCloud does).  Per sweep: Rlc9 (row-major) / tlc3 = FullSystem::Rlc, tlc
  * (LiDAR -> camera), K4 = FullSystem::fx fy cx cy, lrud_io = FullSystem::left, right, up, down (the running pixel box; 10000, -1, 10000, -1 at start).  The image
- * size, which bounds the pixel box, is the context's (camera 0's), whatever camera size the sequence's frames have.  Out, per sweep: up to cap rows {Ku, Kv, depth} (doubles, the vCloudPixel pushed into FullSystem::qCloudPixel, same order) at
+ * size, which bounds the pixel box, is camera 0's (the context's); sdv_lidar_handler_batch_cams takes it from camera cams[j] for sweep j.  Out, per sweep: up to cap rows {Ku, Kv, depth} (doubles, the vCloudPixel pushed into FullSystem::qCloudPixel, same order) at
  * cloud3_out[3*j*cap ..], n_out[j] rows, add_feature_point_out[j] = FullSystem::addFeaturePoint (ground ratio > 0.8), stats_out[2j..] = {numGround, size of
  * segmentedCloud} (may be NULL).  The rows feed sdv_make_new_traces_batch and the LiDAR-depth splats of sdv_tracker_set_ref. */
 int  sdv_lidar_init(sdv_ctx* c, int n_scan, int horizon_scan, float ang_res_x, float ang_res_y, float ang_bottom, int ground_scan_ind);
 int  sdv_lidar_handler_batch(sdv_ctx* c, int n, const int32_t* sweep_begin, const float* xyzi, const double* Rlc9, const double* tlc3, const float* K4, int32_t* lrud_io, int cap,
                              double* cloud3_out, int32_t* n_out, int32_t* add_feature_point_out, int32_t* stats_out);
+int  sdv_lidar_handler_batch_cams(sdv_ctx* c, int n, const int32_t* sweep_begin, const float* xyzi, const double* Rlc9, const double* tlc3, const float* K4, const int32_t* cams,
+                                  int32_t* lrud_io, int cap, double* cloud3_out, int32_t* n_out, int32_t* add_feature_point_out, int32_t* stats_out);
 
 #ifdef __cplusplus
 }

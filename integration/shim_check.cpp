@@ -98,6 +98,23 @@ int shim_ingest_cams(int n, const uint64_t* ids, const uint8_t* const* mono8, co
   return sdv_frame_upload_batch_cams(gpu, n, ids, reinterpret_cast<const void* const*>(mono8), cams, /*fmt mono8*/1, exposures)
        | sdv_frame_build_batch_dev_cams(gpu, n, ids, dev_float, cams, /*fmt float*/0, exposures);
 }
+// §4 the keyframe path of a KITTI sequence on camera 1 in a KITTI-360 context: its selector slot bound to camera 1, then every keyframe-rate stage names camera 1
+struct KittiKeyframe { int32_t slot, cam; uint64_t kf, next; std::vector<float> xyzi; double Rlc9[9], tlc3[3]; float K4[4]; int32_t lrud[4]; };
+int shim_kitti_keyframe(KittiKeyframe& k, float density, std::vector<sdv_new_trace>& tr, std::vector<sdv_immature_pt>& imm, std::vector<int32_t>& decision) {
+  int rc = sdv_selector_set_slot_cams(gpu, 1, &k.slot, &k.cam);                               // once per sequence: its PixelSelector works at 1200x360
+  const int32_t sweep_begin[2] = {0, (int32_t)(k.xyzi.size() / 4)}; const int cap = 64 * 1800; std::vector<double> px(3 * (size_t)cap); int32_t n_px = 0, add = 0;
+  rc |= sdv_lidar_handler_batch_cams(gpu, 1, sweep_begin, k.xyzi.data(), k.Rlc9, k.tlc3, k.K4, &k.cam, k.lrud, cap, px.data(), &n_px, &add, nullptr);   // box bounded by 1200x360
+  const int32_t cloud_begin[2] = {0, n_px}; const float dl = density * (float)((k.lrud[1] - k.lrud[0]) * (k.lrud[3] - k.lrud[2])) / (1200.f * 360.f);
+  tr.resize(1 << 15); imm.resize(1 << 15); int32_t n_out = 0, num[2];
+  rc |= sdv_make_new_traces_batch(gpu, 1, &k.slot, &k.kf, cloud_begin, px.data(), &dl, &density, &add, 1 << 15, tr.data(), imm.data(), &n_out, num);   // the slot's camera
+  tr.resize(n_out); imm.resize(n_out);
+  const int32_t pt_begin[2] = {0, n_out}; const float I9[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, z3[3] = {0, 0, 0}, aff[2] = {1, 0};
+  rc |= sdv_immature_trace_batch_cams(gpu, 1, &k.next, &k.cam, pt_begin, I9, z3, aff, imm.data(), nullptr);                    // traceNewCoarse at 1200x360
+  std::vector<float> cand4; for (int i = 0; i < n_out; i++) cand4.insert(cand4.end(), {imm[i].u, imm[i].v, 0.5f * (imm[i].idepth_max + imm[i].idepth_min), tr[i].my_type});
+  const int32_t host_begin[2] = {0, 0}, pt0[1] = {0}, cand_host_begin[2] = {0, 1}, cand_begin[2] = {0, n_out}; const float md = 2.f; decision.resize(n_out);
+  return rc | sdv_activate_select_batch_cams(gpu, 1, host_begin, pt0, nullptr, nullptr, nullptr, cand_host_begin, cand_begin, I9, z3, cand4.data(), &md, &k.cam,
+                                             decision.data(), nullptr);                            // distance map and walk at 600x180
+}
 // §3c CoarseTracker::makeK (CoarseTracker.cpp:77-106): a member of each tracker instance, so it sets the K of that instance's slot only
 int shim_makeK(int slot, CalibHessian* HCalib) { sdv_calib K{HCalib->fxl(), HCalib->fyl(), HCalib->cxl(), HCalib->cyl()}; const int32_t s = slot; return sdv_set_calib_slots(gpu, 1, &s, &K); }
 
@@ -292,6 +309,7 @@ int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const 
   std::vector<ActivationGroup> ag; std::vector<float> idp; rc |= shim_activatePoints(ag, st, idp, sel, 7);
   PixelSelector ps; LidarRig rig{}; std::vector<double> px; std::vector<sdv_new_trace> tr; std::vector<sdv_immature_pt> rc2; ActivationInputs ai; ai.pt_begin = {0}; ai.cand_begin = {0}; ai.currentMinActDist = 2;
   rc |= shim_selector_ctor(ps) | shim_lidarCloudHandler(rig, nullptr, 0, px) | shim_makeNewTraces_whole(fh, rig, px, tr, rc2) | shim_activateSelect(ai, st);
+  { KittiKeyframe k{}; k.slot = 1; k.cam = 1; rc |= shim_kitti_keyframe(k, 1500.f, tr, rc2, st); }
   fs.optimize(6); fs.set_map(0); fs.handover(sel, st); fs.trackNewCoarse(fh); fs.refine_only(fh); shim_frame_destructor(fh);
   return rc;
 }

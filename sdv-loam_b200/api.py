@@ -99,6 +99,13 @@ def _load():
     L.sdv_lidar_init.argtypes = [_vp, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_int]
     L.sdv_lidar_handler_batch.argtypes = [_vp, C.c_int, _i32p, _vp, _f64p, _f64p, _f32p, _i32p, C.c_int, _vp, _i32p, _i32p, _i32p]
     L.sdv_activate_select_batch.argtypes = [_vp, C.c_int, _i32p, _i32p, _vp, _vp, _vp, _i32p, _i32p, _vp, _vp, _vp, _f32p, _vp, _vp]
+    L.sdv_selector_set_slot_cams.argtypes = [_vp, C.c_int, _i32p, _i32p]
+    L.sdv_selector_make_hists_cam.argtypes = [_vp, C.c_int, C.c_uint64, _vp, _vp]
+    L.sdv_activate_select_batch_cams.argtypes = [_vp, C.c_int, _i32p, _i32p, _vp, _vp, _vp, _i32p, _i32p, _vp, _vp, _vp, _f32p, _vp, _vp, _vp]
+    L.sdv_lidar_handler_batch_cams.argtypes = [_vp, C.c_int, _i32p, _vp, _f64p, _f64p, _f32p, _vp, _i32p, C.c_int, _vp, _i32p, _i32p, _i32p]
+    L.sdv_immature_init_cam.argtypes = [_vp, C.c_int, C.c_uint64, C.c_int, _i32p, _vp]
+    L.sdv_immature_trace_batch_cams.argtypes = [_vp, C.c_int, _u64p, _vp, _i32p, _f32p, _f32p, _f32p, _vp, _vp]
+    L.sdv_immature_optimize_batch_cams.argtypes = [_vp, C.c_int, _i32p, _i32p, _u64p, _f32p, _f32p, _vp, C.c_int, _vp, _vp, C.c_int, _i32p, _f32p, _i32p]
     return L
 
 
@@ -592,34 +599,46 @@ IMMATURE_PT_DTYPE = np.dtype([("u", np.float32), ("v", np.float32), ("idepth_min
 IPS_GOOD, IPS_OOB, IPS_OUTLIER, IPS_SKIPPED, IPS_BADCONDITION, IPS_UNINITIALIZED = range(6)
 
 
-def immatureInit(ctx: Context, host_frame_id: int, uv):
-    """ImmaturePoint::ImmaturePoint (ImmaturePoint.cpp:8-36) for integer pixels uv (n,2) of a resident keyframe -> IMMATURE_PT_DTYPE array"""
+def immatureInit(ctx: Context, host_frame_id: int, uv, cam: int = 0):
+    """ImmaturePoint::ImmaturePoint (ImmaturePoint.cpp:8-36) for integer pixels uv (n,2) of a resident keyframe of camera `cam` -> IMMATURE_PT_DTYPE array"""
     uv = np.ascontiguousarray(uv, np.int32).reshape(-1, 2); P = np.zeros(len(uv), IMMATURE_PT_DTYPE)
-    ctx._ck(LIB.sdv_immature_init(ctx.p, host_frame_id, len(uv), uv.reshape(-1), P.ctypes.data))
+    if cam == 0:
+        ctx._ck(LIB.sdv_immature_init(ctx.p, host_frame_id, len(uv), uv.reshape(-1), P.ctypes.data))
+    else:
+        ctx._ck(LIB.sdv_immature_init_cam(ctx.p, int(cam), host_frame_id, len(uv), uv.reshape(-1), P.ctypes.data))
     return P
 
 
-def traceOnBatch(ctx: Context, frame_ids, pt_begin, KRKi, Kt, aff, pts):
+def traceOnBatch(ctx: Context, frame_ids, pt_begin, KRKi, Kt, aff, pts, cams=None):
     """ImmaturePoint::traceOn for every candidate of every (host keyframe, traced frame) group — the loop of FullSystem::traceNewCoarse (FullSystem.cpp:519-552), batched.
-    pts (IMMATURE_PT_DTYPE) is updated in place; returns the statuses."""
+    Group g traces at camera cams[g]'s size (None: camera 0).  pts (IMMATURE_PT_DTYPE) is updated in place; returns the statuses."""
     assert pts.dtype == IMMATURE_PT_DTYPE and pts.flags.c_contiguous
     ng = len(frame_ids); pb = np.ascontiguousarray(pt_begin, np.int32); assert len(pb) == ng + 1 and pb[-1] == len(pts)
-    st = np.zeros(len(pts), np.int32)
-    ctx._ck(LIB.sdv_immature_trace_batch(ctx.p, ng, np.ascontiguousarray(frame_ids, np.uint64), pb, np.ascontiguousarray(KRKi, np.float32).reshape(-1),
-                                         np.ascontiguousarray(Kt, np.float32).reshape(-1), np.ascontiguousarray(aff, np.float32).reshape(-1), pts.ctypes.data, st.ctypes.data))
+    st = np.zeros(len(pts), np.int32); cm = Context._cams(cams, ng)
+    args = (np.ascontiguousarray(frame_ids, np.uint64), pb, np.ascontiguousarray(KRKi, np.float32).reshape(-1), np.ascontiguousarray(Kt, np.float32).reshape(-1),
+            np.ascontiguousarray(aff, np.float32).reshape(-1), pts.ctypes.data, st.ctypes.data)
+    if cm is None:
+        ctx._ck(LIB.sdv_immature_trace_batch(ctx.p, ng, *args))
+    else:
+        ctx._ck(LIB.sdv_immature_trace_batch_cams(ctx.p, ng, args[0], cm.ctypes.data, *args[1:]))
     return st
 
 
-def optimizeImmaturePointBatch(ctx: Context, pt_begin, tgt_begin, target_frame_ids, pre14, calib6, pts, is_from_sensor=None, min_obs=1):
+def optimizeImmaturePointBatch(ctx: Context, pt_begin, tgt_begin, target_frame_ids, pre14, calib6, pts, is_from_sensor=None, min_obs=1, cams=None):
     """FullSystem::optimizeImmaturePoint (FullSystemOptPoint.cpp:18-183) for the candidates of several host keyframes in one launch (group = host; see sdv_b200.h).
+    Group g works at camera cams[g]'s size (None: camera 0); its targets must have that size.
     Returns (status (n,) 0 stay / -1 drop / 1 activate, idepth (n,), res_state (n, stride) with -1 padding)."""
     assert pts.dtype == IMMATURE_PT_DTYPE and pts.flags.c_contiguous
     pb = np.ascontiguousarray(pt_begin, np.int32); tb = np.ascontiguousarray(tgt_begin, np.int32); ng = len(pb) - 1; n = len(pts); assert pb[-1] == n and len(tb) == ng + 1
     stride = max(1, int(np.diff(tb).max())) if ng else 1
     st = np.zeros(n, np.int32); idp = np.zeros(n, np.float32); rs = np.full((n, stride), -1, np.int32)
-    fs = None if is_from_sensor is None else np.ascontiguousarray(is_from_sensor, np.uint8)
-    ctx._ck(LIB.sdv_immature_optimize_batch(ctx.p, ng, pb, tb, np.ascontiguousarray(target_frame_ids, np.uint64), np.ascontiguousarray(pre14, np.float32).reshape(-1),
-                                            np.ascontiguousarray(calib6, np.float32).reshape(-1), min_obs, pts.ctypes.data, None if fs is None else fs.ctypes.data, stride, st, idp, rs.reshape(-1)))
+    fs = None if is_from_sensor is None else np.ascontiguousarray(is_from_sensor, np.uint8); cm = Context._cams(cams, ng)
+    head = (pb, tb, np.ascontiguousarray(target_frame_ids, np.uint64), np.ascontiguousarray(pre14, np.float32).reshape(-1), np.ascontiguousarray(calib6, np.float32).reshape(-1))
+    tail = (min_obs, pts.ctypes.data, None if fs is None else fs.ctypes.data, stride, st, idp, rs.reshape(-1))
+    if cm is None:
+        ctx._ck(LIB.sdv_immature_optimize_batch(ctx.p, ng, *head, *tail))
+    else:
+        ctx._ck(LIB.sdv_immature_optimize_batch_cams(ctx.p, ng, *head, cm.ctypes.data, *tail))
     return st, idp, rs
 
 
@@ -650,31 +669,53 @@ def lidar_density(lrud, wh, desiredImmatureDensity):
 
 
 class PixelSelector:
-    """n_slots PixelSelector + selectionMap pairs (one per resident sequence) of a context: FullSystem/PixelSelector2.cpp, FullSystem.cpp:180-186"""
+    """n_slots PixelSelector + selectionMap pairs (one per resident sequence) of a context: FullSystem/PixelSelector2.cpp, FullSystem.cpp:180-186.
+    Slot s works at its camera's size (cams[s], bindCams; camera 0 by default): its frames, its selection map."""
 
-    def __init__(self, ctx: Context, n_slots: int = 1, pattern=None):
-        self.ctx = ctx; self.n_slots = n_slots
+    def __init__(self, ctx: Context, n_slots: int = 1, pattern=None, cams=None):
+        self.ctx = ctx; self.n_slots = n_slots; self.slot_cam = {}       # slot -> camera, for slots not on camera 0
         self.pattern = np.ascontiguousarray(pattern if pattern is not None else random_pattern(ctx.w, ctx.h), np.uint8); assert self.pattern.size == ctx.w * ctx.h
         ctx._ck(LIB.sdv_selector_init(ctx.p, self.pattern.ctypes.data, n_slots))
+        if cams is not None:
+            self.bindCams(range(n_slots), cams)
+
+    def bindCams(self, slots, cams):
+        """slot slots[i] works at camera cams[i]'s size from now on; moving it to a camera of another size starts it afresh (a new PixelSelector and selectionMap)"""
+        sl = np.ascontiguousarray(list(slots), np.int32).reshape(-1); cm = Context._cams(cams, len(sl))
+        self.ctx._ck(LIB.sdv_selector_set_slot_cams(self.ctx.p, len(sl), sl, cm))
+        for s, c in zip(sl.tolist(), cm.tolist()):
+            if c:
+                self.slot_cam[s] = c
+            else:
+                self.slot_cam.pop(s, None)
+
+    def slotSize(self, slot):
+        return self.ctx.camSize(self.slot_cam.get(int(slot), 0))
 
     def potential(self, slot=0, set_to=None) -> int:
         o = C.c_int(0); self.ctx._ck(LIB.sdv_selector_potential(self.ctx.p, slot, int(set_to) if set_to else 0, C.byref(o))); return o.value
 
     def selectionMap(self, slot=0):
-        o = np.zeros((self.ctx.h, self.ctx.w), np.uint8); self.ctx._ck(LIB.sdv_selector_get_map(self.ctx.p, slot, o.ctypes.data)); return o
+        w, h = self.slotSize(slot); o = np.zeros((h, w), np.uint8); self.ctx._ck(LIB.sdv_selector_get_map(self.ctx.p, slot, o.ctypes.data)); return o
 
-    def makeHists(self, frame_id):
-        n = (self.ctx.w // 32) * (self.ctx.h // 32); a = np.zeros(n, np.float32); b = np.zeros(n, np.float32)
-        self.ctx._ck(LIB.sdv_selector_make_hists(self.ctx.p, frame_id, a.ctypes.data, b.ctypes.data)); return a, b
+    def makeHists(self, frame_id, cam: int = 0):
+        w, h = self.ctx.camSize(cam); n = (w // 32) * (h // 32); a = np.zeros(n, np.float32); b = np.zeros(n, np.float32)
+        self.ctx._ck(LIB.sdv_selector_make_hists_cam(self.ctx.p, int(cam), frame_id, a.ctypes.data, b.ctypes.data)); return a, b
 
     def makeMapsBatch(self, slots, frame_ids, density, recursionsLeft=1, thFactor=1.0, clouds=None):
-        """makeMapsFromLidar (clouds: one (n,3) float64 array {Ku,Kv,depth} per job) or makeMaps (clouds None) for several (slot, frame) pairs -> maps, numHaveSub"""
+        """makeMapsFromLidar (clouds: one (n,3) float64 array {Ku,Kv,depth} per job) or makeMaps (clouds None) for several (slot, frame) pairs -> maps, numHaveSub.
+        makeMaps returns an (n, h, w) array when every slot has the context size, else a list of per-job (h_c, w_c) maps."""
         n = len(slots); sl = np.ascontiguousarray(slots, np.int32); fr = np.ascontiguousarray(frame_ids, np.uint64)
         de = np.ascontiguousarray(np.broadcast_to(density, n), np.float32); rc = np.ascontiguousarray(np.broadcast_to(recursionsLeft, n), np.int32); th = np.ascontiguousarray(np.broadcast_to(thFactor, n), np.float32)
         num = np.zeros(n, np.int32)
         if clouds is None:
-            maps = np.zeros((n, self.ctx.h, self.ctx.w), np.uint8)
-            self.ctx._ck(LIB.sdv_selector_make_maps_batch(self.ctx.p, n, sl, fr, None, None, de, rc, th, maps.ctypes.data, num)); return maps, num
+            whs = [self.slotSize(s) for s in sl.tolist()]
+            if all(wh == (self.ctx.w, self.ctx.h) for wh in whs):
+                maps = np.zeros((n, self.ctx.h, self.ctx.w), np.uint8)
+                self.ctx._ck(LIB.sdv_selector_make_maps_batch(self.ctx.p, n, sl, fr, None, None, de, rc, th, maps.ctypes.data, num)); return maps, num
+            off = np.concatenate([[0], np.cumsum([w * h for w, h in whs])]); flat = np.zeros(int(off[-1]), np.uint8)
+            self.ctx._ck(LIB.sdv_selector_make_maps_batch(self.ctx.p, n, sl, fr, None, None, de, rc, th, flat.ctypes.data, num))
+            return [flat[off[j]:off[j + 1]].reshape(whs[j][1], whs[j][0]) for j in range(n)], num
         cl = [np.ascontiguousarray(c, np.float64).reshape(-1, 3) for c in clouds]; cb = np.concatenate([[0], np.cumsum([len(c) for c in cl])]).astype(np.int32)
         allc = np.ascontiguousarray(np.concatenate(cl) if cb[-1] else np.zeros((1, 3))); maps = np.zeros(max(int(cb[-1]), 1), np.uint8)
         self.ctx._ck(LIB.sdv_selector_make_maps_batch(self.ctx.p, n, sl, fr, cb.ctypes.data, allc.ctypes.data, de, rc, th, maps.ctypes.data, num))
@@ -700,9 +741,9 @@ class PixelSelector:
         return [(out[j, :n_out[j]], imm[j, :n_out[j]]) for j in range(n)], num.reshape(n, 2)
 
 
-def packActivation(seqs):
-    """the flat arrays sdv_activate_select_batch takes, from per-sequence dicts with pt_begin / KRKi / Kt / uvid (source keyframes) and cand_begin / cKRKi / cKt / cand4 /
-    minActDist (candidate keyframes; may be absent)"""
+def packActivation(seqs, cams=None):
+    """the flat arrays sdv_activate_select_batch(_cams) takes, from per-sequence dicts with pt_begin / KRKi / Kt / uvid (source keyframes) and cand_begin / cKRKi / cKt / cand4 /
+    minActDist (candidate keyframes; may be absent); cams: the camera of each sequence (None: camera 0)"""
     hb, pb, gb, cb = [0], [0], [0], [0]; A, B, U, cA, cB, c4, md = [], [], [], [], [], [], []
     f = lambda a, t: np.ascontiguousarray(a, t)
     for q in seqs:
@@ -711,22 +752,32 @@ def packActivation(seqs):
         if len(g) > 1: cA.append(f(q["cKRKi"], np.float32).reshape(-1, 9)); cB.append(f(q["cKt"], np.float32).reshape(-1, 3)); c4.append(f(q["cand4"], np.float32).reshape(-1, 4))
     cat = lambda xs, k: np.ascontiguousarray(np.concatenate(xs) if xs else np.zeros((1, k), np.float32))
     return dict(n=len(seqs), hb=f(hb, np.int32), pb=f(pb, np.int32), A=cat(A, 9), B=cat(B, 3), U=cat(U, 3), gb=f(gb, np.int32), cb=f(cb, np.int32), cA=cat(cA, 9), cB=cat(cB, 3), c4=cat(c4, 4),
-                md=f(md, np.float32), dec=np.zeros(max(cb[-1], 1), np.int32))
+                md=f(md, np.float32), dec=np.zeros(max(cb[-1], 1), np.int32), cams=Context._cams(cams, len(seqs)))
 
 
 def activateSelectPacked(ctx: Context, P, want_maps=False):
-    """sdv_activate_select_batch on arrays packed by packActivation (the decisions land in P['dec'], reused between calls) -> per-sequence views of the decisions (+ maps)"""
-    n = P["n"]; maps = np.zeros((n, ctx.h >> 1, ctx.w >> 1), np.float32) if want_maps else None
-    ctx._ck(LIB.sdv_activate_select_batch(ctx.p, n, P["hb"], P["pb"], P["A"].ctypes.data, P["B"].ctypes.data, P["U"].ctypes.data, P["gb"], P["cb"], P["cA"].ctypes.data, P["cB"].ctypes.data,
-                                          P["c4"].ctypes.data, P["md"], P["dec"].ctypes.data, maps.ctypes.data if want_maps else None))
+    """sdv_activate_select_batch on arrays packed by packActivation (the decisions land in P['dec'], reused between calls) -> per-sequence views of the decisions (+ maps:
+    an (n, h/2, w/2) array when the sequences are on camera 0, else a list of per-sequence level-1 maps at each camera's size)"""
+    n = P["n"]; cm = P.get("cams"); maps = None
+    if cm is None:
+        maps = np.zeros((n, ctx.h >> 1, ctx.w >> 1), np.float32) if want_maps else None; flat = maps
+    elif want_maps:
+        whs = [ctx.camSize(c) for c in cm.tolist()]; off = np.concatenate([[0], np.cumsum([(w >> 1) * (h >> 1) for w, h in whs])]); flat = np.zeros(int(off[-1]), np.float32)
+        maps = [flat[off[j]:off[j + 1]].reshape(whs[j][1] >> 1, whs[j][0] >> 1) for j in range(n)]
+    args = (P["hb"], P["pb"], P["A"].ctypes.data, P["B"].ctypes.data, P["U"].ctypes.data, P["gb"], P["cb"], P["cA"].ctypes.data, P["cB"].ctypes.data, P["c4"].ctypes.data, P["md"])
+    if cm is None:
+        ctx._ck(LIB.sdv_activate_select_batch(ctx.p, n, *args, P["dec"].ctypes.data, flat.ctypes.data if want_maps else None))
+    else:
+        ctx._ck(LIB.sdv_activate_select_batch_cams(ctx.p, n, *args, cm.ctypes.data, P["dec"].ctypes.data, flat.ctypes.data if want_maps else None))
     cb, gb = P["cb"], P["gb"]; out = [P["dec"][cb[gb[j]]:cb[gb[j + 1]]] for j in range(n)]
     return (out, maps) if want_maps else out
 
 
-def activateSelectBatch(ctx: Context, seqs, want_maps=False):
+def activateSelectBatch(ctx: Context, seqs, want_maps=False, cams=None):
     """CoarseDistanceMap::makeDistanceMap + the candidate walk of FullSystem::activatePointsMT for several sequences.  seqs: list of dicts with pt_begin / KRKi / Kt / uvid
-    (source keyframes) and cand_begin / cKRKi / cKt / cand4 / minActDist (candidate keyframes; may be absent).  -> per sequence decisions (+ distance maps)"""
-    r = activateSelectPacked(ctx, packActivation(seqs), want_maps)
+    (source keyframes) and cand_begin / cKRKi / cKt / cand4 / minActDist (candidate keyframes; may be absent); cams: each sequence's camera (None: camera 0).
+    -> per sequence decisions (+ distance maps)"""
+    r = activateSelectPacked(ctx, packActivation(seqs, cams), want_maps)
     return ([d.copy() for d in r[0]], r[1]) if want_maps else [d.copy() for d in r]
 
 
@@ -738,13 +789,14 @@ class LidarFrontEnd:
         self.ctx = ctx; self.n_scan, self.horizon = n_scan, horizon
         ctx._ck(LIB.sdv_lidar_init(ctx.p, n_scan, horizon, ang_res_x, ang_res_y, ang_bottom, groundScanInd))
 
-    def handle(self, sweeps, Rlc, tlc, K4, lruds, cap=None):
-        """sweeps: list of (n,4) float32 XYZI arrays; Rlc (3,3) / tlc (3,) / K4 shared or per sweep; lruds (n,4) running pixel boxes -> list of dicts like the oracle's"""
+    def handle(self, sweeps, Rlc, tlc, K4, lruds, cap=None, cams=None):
+        """sweeps: list of (n,4) float32 XYZI arrays; Rlc (3,3) / tlc (3,) / K4 shared or per sweep; lruds (n,4) running pixel boxes; cams: the camera of each sweep,
+        whose size bounds its pixel box (None: camera 0) -> list of dicts like the oracle's"""
         sw = [np.ascontiguousarray(s, np.float32).reshape(-1, 4) for s in sweeps]; sb = np.concatenate([[0], np.cumsum([len(s) for s in sw])]).astype(np.int32)
         allp = np.ascontiguousarray(np.concatenate(sw) if sb[-1] else np.zeros((1, 4), np.float32))
-        return self.handle_packed(allp, sb, Rlc, tlc, K4, lruds, cap)
+        return self.handle_packed(allp, sb, Rlc, tlc, K4, lruds, cap, cams)
 
-    def handle_packed(self, xyzi_all, sweep_begin, Rlc, tlc, K4, lruds, cap=None):
+    def handle_packed(self, xyzi_all, sweep_begin, Rlc, tlc, K4, lruds, cap=None, cams=None):
         """the same with the sweeps already back to back in ONE host buffer (pinned or not) and their row offsets: nothing is copied on the host"""
         sb = np.ascontiguousarray(sweep_begin, np.int32); n = len(sb) - 1; allp = xyzi_all; assert allp.dtype == np.float32 and allp.flags.c_contiguous
         cap = cap or self.n_scan * self.horizon
@@ -752,5 +804,9 @@ class LidarFrontEnd:
         K = np.ascontiguousarray(np.broadcast_to(np.asarray(K4, np.float32).reshape(-1, 4), (n, 4))).reshape(-1); lr = np.ascontiguousarray(lruds, np.int32).reshape(n, 4).copy()
         if getattr(self, "_out", None) is None or self._out.shape != (n, cap, 3): self._out = np.zeros((n, cap, 3))
         out = self._out; n_out = np.zeros(n, np.int32); add = np.zeros(n, np.int32); st = np.zeros(2 * n, np.int32)
-        self.ctx._ck(LIB.sdv_lidar_handler_batch(self.ctx.p, n, sb, allp.ctypes.data, R, t, K, lr.reshape(-1), cap, out.ctypes.data, n_out, add, st))
+        cm = Context._cams(cams, n)
+        if cm is None:
+            self.ctx._ck(LIB.sdv_lidar_handler_batch(self.ctx.p, n, sb, allp.ctypes.data, R, t, K, lr.reshape(-1), cap, out.ctypes.data, n_out, add, st))
+        else:
+            self.ctx._ck(LIB.sdv_lidar_handler_batch_cams(self.ctx.p, n, sb, allp.ctypes.data, R, t, K, cm.ctypes.data, lr.reshape(-1), cap, out.ctypes.data, n_out, add, st))
         return [dict(cloud_px=out[j, :n_out[j]].copy(), lrud=lr[j], numGround=int(st[2 * j]), n_segmented=int(st[2 * j + 1]), addFeaturePoint=int(add[j])) for j in range(n)]

@@ -108,6 +108,7 @@ int sdv_set_camera_size(sdv_ctx* c, int cam, int w, int h) { SDV_GUARD_TRK(c);
   if (c->und.cam[cam].remapX) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_size: camera %d has Undistort tables of its current size", cam);
   for (const FrameDev& f : c->frames) if (f.used && f.cam == cam) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_size: camera %d has resident frame %llu", cam, (unsigned long long)f.id);
   for (size_t s=0;s<c->slots.size();s++) if (c->slots[s].cam == cam) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_size: slot %d is bound to camera %d", (int)s, cam);
+  { int s; if (sel_cam_bound(c, cam, &s)) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_size: selector slot %d is bound to camera %d", s, cam); }
   c->cam_w[cam] = w; c->cam_h[cam] = h;
   return SDV_OK;
 }
@@ -347,10 +348,10 @@ int check_frame_slot(sdv_ctx* c, const FrameDev& f, int slot, const char* who) {
   return ctx_fail(c, SDV_ERR_ARG, "%s: frame %llu is %dx%d (camera %d) but slot %d is bound to camera %d, %dx%d", who, (unsigned long long)f.id,
                   c->cam_w[fc], c->cam_h[fc], fc, slot, sc, c->cam_w[sc], c->cam_h[sc]);
 }
-int check_frame_ctx(sdv_ctx* c, const FrameDev& f, const char* who) {
-  if (same_size(c, f.cam, 0)) return SDV_OK;
-  return ctx_fail(c, SDV_ERR_ARG, "%s: frame %llu is %dx%d (camera %d); this stage works at the context size %dx%d only", who, (unsigned long long)f.id,
-                  c->cam_w[f.cam], c->cam_h[f.cam], f.cam, c->w, c->h);
+int check_frame_cam(sdv_ctx* c, const FrameDev& f, int cam, const char* who) {
+  if (same_size(c, f.cam, cam)) return SDV_OK;
+  return ctx_fail(c, SDV_ERR_ARG, "%s: frame %llu is %dx%d (camera %d) but the job names camera %d, %dx%d", who, (unsigned long long)f.id,
+                  c->cam_w[f.cam], c->cam_h[f.cam], f.cam, cam, c->cam_w[cam], c->cam_h[cam]);
 }
 }
 extern "C" {

@@ -95,7 +95,8 @@ int  join_ingest_upto(sdv_ctx* c, long long seq);   // ... for ingest calls <= s
 inline const GeomRow& slot_geom(const sdv_ctx* c, int slot) { return c->geom[c->slots[slot].geom_row]; }   // the K a tracker / map slot uses, at every level
 inline bool same_size(const sdv_ctx* c, int cam_a, int cam_b) { return c->cam_w[cam_a] == c->cam_w[cam_b] && c->cam_h[cam_a] == c->cam_h[cam_b]; }
 int  check_frame_slot(sdv_ctx* c, const FrameDev& f, int slot, const char* who);   // SDV_ERR_ARG (with a message) when frame f's size differs from slot's
-int  check_frame_ctx(sdv_ctx* c, const FrameDev& f, const char* who);              // ... from the context size (keyframe-rate stages)
+int  check_frame_cam(sdv_ctx* c, const FrameDev& f, int cam, const char* who);     // ... from camera cam's (keyframe-rate stages: the job names its camera)
+bool sel_cam_bound(const sdv_ctx* c, int cam, int* slot);                          // a selector slot (*slot) is bound to camera cam (sdv_selector_set_slot_cams)
 bool rp_slot_set(const sdv_ctx* c, int slot);                                     // map slot `slot` holds a resident map (sdv_map_set, not cleared)
 }
 // entry-point guards (a NULL context falls through to the entry's own argument check)

@@ -27,19 +27,20 @@ int sdv_lidar_init(sdv_ctx* c, int n_scan, int horizon_scan, float ang_res_x, fl
   return SDV_OK;
 }
 
-int sdv_lidar_handler_batch(sdv_ctx* c, int n, const int32_t* sweep_begin, const float* xyzi, const double* Rlc9, const double* tlc3, const float* K4, int32_t* lrud_io, int cap,
-                            double* cloud3_out, int32_t* n_out, int32_t* add_feature_point_out, int32_t* stats_out) { SDV_GUARD_TRK(c);
+int sdv_lidar_handler_batch_cams(sdv_ctx* c, int n, const int32_t* sweep_begin, const float* xyzi, const double* Rlc9, const double* tlc3, const float* K4, const int32_t* cams,
+                                 int32_t* lrud_io, int cap, double* cloud3_out, int32_t* n_out, int32_t* add_feature_point_out, int32_t* stats_out) { SDV_GUARD_TRK(c);
   if (!c || n < 0 || (n && (!sweep_begin || !Rlc9 || !tlc3 || !K4 || !lrud_io || !cloud3_out || !n_out || cap < 1))) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK;
   LidarState* s = (LidarState*)c->lidar; if (!s) return ctx_fail(c, SDV_ERR_STATE, "lidar_handler: sdv_lidar_init has not been called");
   if (sweep_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler: sweep_begin[0] must be 0");
   for (int j = 0; j < n; j++) { if (sweep_begin[j+1] < sweep_begin[j]) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler: sweep_begin is not ascending at sweep %d", j);
-    if (sweep_begin[j+1] > sweep_begin[j] && !xyzi) return SDV_ERR_ARG; }
+    if (sweep_begin[j+1] > sweep_begin[j] && !xyzi) return SDV_ERR_ARG;
+    if (cams && (cams[j] < 0 || cams[j] >= SDV_MAX_CAMERAS)) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler: sweep %d names camera %d (valid: 0..%d)", j, cams[j], SDV_MAX_CAMERAS - 1); }
   CK(cudaSetDevice(c->device));
   std::vector<lidar::LidarEngine::Sweep> S(n);
   for (int j = 0; j < n; j++) { auto& w = S[j]; w.xyzi_host = xyzi ? xyzi + 4*(size_t)sweep_begin[j] : nullptr; w.n = sweep_begin[j+1] - sweep_begin[j];
     for (int k = 0; k < 9; k++) w.R[k] = Rlc9[9*j+k]; for (int k = 0; k < 3; k++) w.t[k] = tlc3[3*j+k]; for (int k = 0; k < 4; k++) { w.K[k] = K4[4*j+k]; w.lrud[k] = lrud_io[4*j+k]; }
-    w.w = c->w; w.h = c->h; w.out3_host = cloud3_out + 3*(size_t)j*cap; w.cap = cap; }
+    const int cam = cams ? cams[j] : 0; w.w = c->cam_w[cam]; w.h = c->cam_h[cam]; w.out3_host = cloud3_out + 3*(size_t)j*cap; w.cap = cap; }
   const long long l0 = s->eng.launches;
   CK(cudaEventRecord(c->ev0, c->st));
   { int rc = s->eng.handle(S); if (rc) return ctx_fail(c, rc == -2 ? SDV_ERR_CAPACITY : SDV_ERR_CUDA, "lidar_handler: %s", s->eng.err.c_str()); }
@@ -49,6 +50,10 @@ int sdv_lidar_handler_batch(sdv_ctx* c, int n, const int32_t* sweep_begin, const
   for (int j = 0; j < n; j++) { n_out[j] = S[j].n_out; for (int k = 0; k < 4; k++) lrud_io[4*j+k] = S[j].lrud[k]; if (add_feature_point_out) add_feature_point_out[j] = S[j].addFeaturePoint;
     if (stats_out) { stats_out[2*j] = S[j].numGround; stats_out[2*j+1] = S[j].n_segmented; } }
   return SDV_OK;
+}
+int sdv_lidar_handler_batch(sdv_ctx* c, int n, const int32_t* sweep_begin, const float* xyzi, const double* Rlc9, const double* tlc3, const float* K4, int32_t* lrud_io, int cap,
+                            double* cloud3_out, int32_t* n_out, int32_t* add_feature_point_out, int32_t* stats_out) {
+  return sdv_lidar_handler_batch_cams(c, n, sweep_begin, xyzi, Rlc9, tlc3, K4, nullptr, lrud_io, cap, cloud3_out, n_out, add_feature_point_out, stats_out);
 }
 
 }  // extern "C"

@@ -1,10 +1,11 @@
 // sdv_select.cu — C-ABI of the candidate management at keyframe rate (SURVEY.md §8f rank 4 + the caller half of rank 2): binds the engine of sdv_select_core.cuh
 // (kernels + host orchestration; see the header for the reference map and the design) to the context's resident frames and tracker-domain stream.
 //   sdv_selector_init / _potential / _get_map   PixelSelector::PixelSelector, currentPotential, FullSystem::selectionMap      PixelSelector2.cpp:11-26, FullSystem.cpp:180-186
-//   sdv_selector_make_hists                     PixelSelector::makeHists                                                     PixelSelector2.cpp:47-106
+//   sdv_selector_make_hists(_cam)               PixelSelector::makeHists                                                     PixelSelector2.cpp:47-106
 //   sdv_selector_make_maps_batch                PixelSelector::makeMapsFromLidar / makeMaps                                  PixelSelector2.cpp:354-449 / :108-200
 //   sdv_make_new_traces_batch                   FullSystem::makeNewTraces (+ shiTomasiScore, setMask, ImmaturePoint ctor)    FullSystem.cpp:1261-1356, 1540-1583
-//   sdv_activate_select_batch                   CoarseDistanceMap::makeDistanceMap + the candidate walk of activatePointsMT  CoarseTracker.cpp:1139-1282, FullSystem.cpp:600-671
+//   sdv_activate_select_batch(_cams)            CoarseDistanceMap::makeDistanceMap + the candidate walk of activatePointsMT  CoarseTracker.cpp:1139-1282, FullSystem.cpp:600-671
+// A selector slot is bound to a camera (sdv_selector_set_slot_cams; camera 0 after init) and works at that camera's size: its frames, its persistent map.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <vector>
@@ -17,15 +18,20 @@ using namespace sdv;
 static_assert(sizeof(sel::NewTrace) == sizeof(sdv_new_trace) && sizeof(sel::ImmPt) == sizeof(sdv_immature_pt), "engine records mirror the C-ABI structs");
 
 namespace sdv {
-struct SelState { sel::SelEngine eng; std::vector<sel::SelectorSlot> slots; sel::Scratch aux; };
+struct SelState { sel::SelEngine eng; std::vector<sel::SelectorSlot> slots; std::vector<int> cam; sel::Scratch aux; };   // cam[s]: camera of slot s
 void sel_destroy(sdv_ctx* c) {
   SelState* s = (SelState*)c->sel; if (!s) return;
   for (auto& sl : s->slots) if (sl.mapD) cudaFree(sl.mapD);
   s->eng.io.release(); s->aux.release(); s->eng.destroy(); delete s; c->sel = nullptr;
 }
-static int sel_frame(sdv_ctx* c, uint64_t id, sel::FrameImg& F, long long& need_seq, const char* who, bool texels = true) {
+bool sel_cam_bound(const sdv_ctx* c, int cam, int* slot) {
+  const SelState* s = (const SelState*)c->sel; if (!s) return false;
+  for (size_t k = 0; k < s->cam.size(); k++) if (s->cam[k] == cam) { *slot = (int)k; return true; }
+  return false;
+}
+static int sel_frame(sdv_ctx* c, uint64_t id, int cam, sel::FrameImg& F, long long& need_seq, const char* who, bool texels = true) {
   auto it = c->frame_index.find(id); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "%s: unknown frame %llu", who, (unsigned long long)id);
-  FrameDev& f = c->frames[it->second]; { int rcs = check_frame_ctx(c, f, who); if (rcs) return rcs; }
+  FrameDev& f = c->frames[it->second]; { int rcs = check_frame_cam(c, f, cam, who); if (rcs) return rcs; }
   if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
   F.I0 = f.I0; F.L1 = nullptr; F.L2 = nullptr;
   if (texels) { int rc = ensure_texels(c, f, 1); if (rc) return rc; F.L1 = f.lvl[1]; F.L2 = f.lvl[2]; }   // |grad|^2 of levels 1 and 2 (makeMaps / makeNewTraces read the packed texels)
@@ -46,9 +52,22 @@ int sdv_selector_init(sdv_ctx* c, const uint8_t* random_pattern, int n_slots) { 
   sel::SelSet S; S.minGradHistCut = 0.5f; S.minGradHistAdd = 3; S.gradDownweightPerLevel = 0.75f; S.selectDirectionDistribution = 1;            // util/settings.cpp:119-122
   S.outlierTH = c->set.outlierTH; S.outlierTHSumComponent = c->set.outlierTHSumComponent; S.overallEnergyTHWeight = 1;
   if (s->eng.init(c->w, c->h, S, random_pattern, c->st)) { int rc = sel_fail(c, s, -1, "selector_init"); sel_destroy(c); return rc; }
-  s->slots.resize(n_slots);
+  s->slots.resize(n_slots); s->cam.assign(n_slots, 0);
   if (const char* e = getenv("SDV_WALK_THREADS")) { const int t = atoi(e); if (t == 32 || t == 64 || t == 128 || t == 256) s->eng.walk_threads = t; }   // tuning knobs
   if (const char* e = getenv("SDV_FUSE_MAP")) s->eng.fuse_map = atoi(e) != 0;
+  return SDV_OK;
+}
+// Rebinding a slot to a camera of another size starts it afresh (map dropped, currentPotential 3: a new PixelSelector / selectionMap); the same size keeps its state.
+int sdv_selector_set_slot_cams(sdv_ctx* c, int n, const int32_t* slots, const int32_t* cams) { SDV_GUARD_TRK(c);
+  if (!c || n < 0 || (n && (!slots || !cams))) return SDV_ERR_ARG; SEL_STATE("selector_set_slot_cams");
+  for (int i = 0; i < n; i++) {
+    if (slots[i] < 0 || slots[i] >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "selector_set_slot_cams: entry %d names slot %d of %d", i, slots[i], (int)s->slots.size());
+    if (cams[i] < 0 || cams[i] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "selector_set_slot_cams: entry %d names camera %d (valid: 0..%d)", i, cams[i], SDV_MAX_CAMERAS - 1);
+  }
+  CK(cudaSetDevice(c->device));
+  for (int i = 0; i < n; i++) { const int sl = slots[i];
+    if (!same_size(c, s->cam[sl], cams[i])) { sel::SelectorSlot& S = s->slots[sl]; if (S.mapD) { CK(cudaStreamSynchronize(c->st)); CK(cudaFree(S.mapD)); } S = sel::SelectorSlot(); }
+    s->cam[sl] = cams[i]; }
   return SDV_OK;
 }
 int sdv_selector_potential(sdv_ctx* c, int slot, int set_to, int* out) { SDV_GUARD_TRK(c);
@@ -62,28 +81,31 @@ int sdv_selector_get_map(sdv_ctx* c, int slot, uint8_t* out) { SDV_GUARD_TRK(c);
   if (!c || !out) return SDV_ERR_ARG; SEL_STATE("selector_get_map");
   if (slot < 0 || slot >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "selector_get_map: slot %d of %d", slot, (int)s->slots.size());
   CK(cudaSetDevice(c->device));
-  const size_t wh = (size_t)c->w*c->h;
+  const int cam = s->cam[slot]; const size_t wh = (size_t)c->cam_w[cam]*c->cam_h[cam];
   if (!s->slots[slot].mapD) { memset(out, 0, wh); return SDV_OK; }
   CK(cudaMemcpyAsync(out, s->slots[slot].mapD, wh, cudaMemcpyDeviceToHost, c->st)); CK(cudaStreamSynchronize(c->st));
   return SDV_OK;
 }
-int sdv_selector_make_hists(sdv_ctx* c, uint64_t frame, float* ths_out, float* thsSmoothed_out) { SDV_GUARD_TRK(c);
+int sdv_selector_make_hists_cam(sdv_ctx* c, int cam, uint64_t frame, float* ths_out, float* thsSmoothed_out) { SDV_GUARD_TRK(c);
   if (!c) return SDV_ERR_ARG; SEL_STATE("selector_make_hists");
+  if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "selector_make_hists: camera %d (valid: 0..%d)", cam, SDV_MAX_CAMERAS - 1);
   CK(cudaSetDevice(c->device));
-  sel::FrameImg F; long long need = 0; { int rc = sel_frame(c, frame, F, need, "selector_make_hists", false); if (rc) return rc; }
+  sel::FrameImg F; long long need = 0; { int rc = sel_frame(c, frame, cam, F, need, "selector_make_hists", false); if (rc) return rc; }
   { int rc = join_ingest_upto(c, need); if (rc) return rc; }
-  const size_t tf = s->eng.ths_floats(); if (s->aux.reserve(2*sel::Scratch::need(tf, 4), c->st)) return ctx_fail(c, SDV_ERR_CUDA, "selector_make_hists: scratch");
+  const int w = c->cam_w[cam], h = c->cam_h[cam];
+  const size_t tf = sel::SelEngine::ths_floats(w, h); if (s->aux.reserve(2*sel::Scratch::need(tf, 4), c->st)) return ctx_fail(c, SDV_ERR_CUDA, "selector_make_hists: scratch");
   s->aux.reset(); float* a = s->aux.take<float>(tf); float* b = s->aux.take<float>(tf);
   CK(cudaMemsetAsync(a, 0, tf*4, c->st)); CK(cudaMemsetAsync(b, 0, tf*4, c->st));
-  sel::HistJob J{F.I0, a, b}; const long long l0 = s->eng.launches;
+  sel::HistJob J{F.I0, a, b, w, h}; const long long l0 = s->eng.launches;
   if (s->eng.make_hists(1, &J)) return sel_fail(c, s, -1, "selector_make_hists");
   c->launches += s->eng.launches - l0;
-  const int n = (c->w/32)*(c->h/32);
+  const int n = (w/32)*(h/32);
   if (ths_out) CK(cudaMemcpyAsync(ths_out, a, n*4, cudaMemcpyDeviceToHost, c->st));
   if (thsSmoothed_out) CK(cudaMemcpyAsync(thsSmoothed_out, b, n*4, cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st));
   return SDV_OK;
 }
+int sdv_selector_make_hists(sdv_ctx* c, uint64_t frame, float* ths_out, float* thsSmoothed_out) { return sdv_selector_make_hists_cam(c, 0, frame, ths_out, thsSmoothed_out); }
 
 int sdv_selector_make_maps_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const float* density,
                                  const int32_t* recursions_left, const float* th_factor, uint8_t* maps_out, int32_t* num_have_out) { SDV_GUARD_TRK(c);
@@ -95,26 +117,28 @@ int sdv_selector_make_maps_batch(sdv_ctx* c, int n, const int32_t* slots, const 
   for (int j = 0; j < n; j++) { if (slots[j] < 0 || slots[j] >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "selector_make_maps: slot %d of %d", slots[j], (int)s->slots.size());
     for (int k = 0; k < j; k++) if (slots[k] == slots[j]) return ctx_fail(c, SDV_ERR_ARG, "selector_make_maps: slot %d appears twice in one batch", slots[j]); }
   CK(cudaSetDevice(c->device));
-  const size_t wh = (size_t)c->w*c->h, tf = s->eng.ths_floats(); long long need = 0;
-  std::vector<sel::FrameImg> F(n); for (int j = 0; j < n; j++) { int rc = sel_frame(c, frames[j], F[j], need, "selector_make_maps"); if (rc) return rc; }
+  long long need = 0; std::vector<int> jw(n), jh(n);                                   // job j works at its slot's camera size
+  for (int j = 0; j < n; j++) { const int cam = s->cam[slots[j]]; jw[j] = c->cam_w[cam]; jh[j] = c->cam_h[cam]; }
+  std::vector<sel::FrameImg> F(n); for (int j = 0; j < n; j++) { int rc = sel_frame(c, frames[j], s->cam[slots[j]], F[j], need, "selector_make_maps"); if (rc) return rc; }
   { int rc = join_ingest_upto(c, need); if (rc) return rc; }
-  size_t bytes = 1024; for (int j = 0; j < n; j++) { const int m = lidar ? cloud_begin[j+1] - cloud_begin[j] : 0; bytes += 2*sel::Scratch::need(tf, 4) + sel::Scratch::need(3*(size_t)m, 8) + sel::Scratch::need(lidar ? (size_t)std::max(m, 1) : wh, 1); }
+  size_t bytes = 1024; for (int j = 0; j < n; j++) { const int m = lidar ? cloud_begin[j+1] - cloud_begin[j] : 0;
+    bytes += 2*sel::Scratch::need(sel::SelEngine::ths_floats(jw[j], jh[j]), 4) + sel::Scratch::need(3*(size_t)m, 8) + sel::Scratch::need(lidar ? (size_t)std::max(m, 1) : (size_t)jw[j]*jh[j], 1); }
   if (s->aux.reserve(bytes, c->st)) return ctx_fail(c, SDV_ERR_CUDA, "selector_make_maps: scratch");
   s->aux.reset(); std::vector<sel::MapsJobHost> M(n); std::vector<sel::HistJob> Hj(n);
-  for (int j = 0; j < n; j++) { const int m = lidar ? cloud_begin[j+1] - cloud_begin[j] : 0;
+  for (int j = 0; j < n; j++) { const int m = lidar ? cloud_begin[j+1] - cloud_begin[j] : 0; const size_t wh = (size_t)jw[j]*jh[j], tf = sel::SelEngine::ths_floats(jw[j], jh[j]);
     float* a = s->aux.take<float>(tf); float* b = s->aux.take<float>(tf); CK(cudaMemsetAsync(a, 0, tf*4, c->st)); CK(cudaMemsetAsync(b, 0, tf*4, c->st));
     double* cl = nullptr; if (lidar) { cl = s->aux.take<double>(3*(size_t)std::max(m, 1)); if (m) CK(cudaMemcpyAsync(cl, cloud3 + 3*(size_t)cloud_begin[j], 3*(size_t)m*sizeof(double), cudaMemcpyHostToDevice, c->st)); }
     sel::SelectorSlot& sl = s->slots[slots[j]];
     if (!lidar && !sl.mapD) { CK(cudaMalloc((void**)&sl.mapD, wh)); CK(cudaMemsetAsync(sl.mapD, 0, wh, c->st)); }
-    Hj[j] = sel::HistJob{F[j].I0, a, b};
-    M[j].img = F[j]; M[j].thsSm = b; M[j].cloud_dev = cl; M[j].n = m; M[j].map = lidar ? s->aux.take<unsigned char>(std::max(m, 1)) : sl.mapD; M[j].density = density[j];
+    Hj[j] = sel::HistJob{F[j].I0, a, b, jw[j], jh[j]};
+    M[j].img = F[j]; M[j].w = jw[j]; M[j].h = jh[j]; M[j].thsSm = b; M[j].cloud_dev = cl; M[j].n = m; M[j].map = lidar ? s->aux.take<unsigned char>(std::max(m, 1)) : sl.mapD; M[j].density = density[j];
     M[j].recursionsLeft = recursions_left[j]; M[j].thFactor = th_factor[j]; M[j].currentPotential = &sl.currentPotential; M[j].numHaveSub = 0; M[j].passes = 0; }
   const long long l0 = s->eng.launches;
   if (s->eng.make_hists(n, Hj.data())) return sel_fail(c, s, -1, "selector_make_maps");
   if (s->eng.make_maps(M, lidar)) return sel_fail(c, s, -1, "selector_make_maps");
   c->launches += s->eng.launches - l0;
   size_t o = 0;
-  for (int j = 0; j < n; j++) { const size_t sz = lidar ? (size_t)(cloud_begin[j+1] - cloud_begin[j]) : wh;
+  for (int j = 0; j < n; j++) { const size_t sz = lidar ? (size_t)(cloud_begin[j+1] - cloud_begin[j]) : (size_t)jw[j]*jh[j];
     if (sz) CK(cudaMemcpyAsync(maps_out + o, M[j].map, sz, cudaMemcpyDeviceToHost, c->st)); o += sz; if (num_have_out) num_have_out[j] = M[j].numHaveSub; }
   CK(cudaStreamSynchronize(c->st));
   return SDV_OK;
@@ -131,7 +155,7 @@ int sdv_make_new_traces_batch(sdv_ctx* c, int n, const int32_t* slots, const uin
     for (int k = 0; k < j; k++) if (slots[k] == slots[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: slot %d appears twice in one batch", slots[j]); }
   CK(cudaSetDevice(c->device));
   long long need = 0; std::vector<sel::SelEngine::NewTracesJob> J(n);
-  for (int j = 0; j < n; j++) { int rc = sel_frame(c, frames[j], J[j].img, need, "make_new_traces"); if (rc) return rc;
+  for (int j = 0; j < n; j++) { const int cam = s->cam[slots[j]]; int rc = sel_frame(c, frames[j], cam, J[j].img, need, "make_new_traces"); if (rc) return rc; J[j].w = c->cam_w[cam]; J[j].h = c->cam_h[cam];
     J[j].cloud_host = cloud3 ? cloud3 + 3*(size_t)cloud_begin[j] : nullptr; J[j].n = cloud_begin[j+1] - cloud_begin[j]; J[j].slot = &s->slots[slots[j]]; J[j].densityLidar = density_lidar[j];
     J[j].densityDense = density_dense[j]; J[j].addFeaturePoint = add_feature_point[j]; J[j].out_host = (sel::NewTrace*)out + (size_t)j*cap; J[j].imm_host = imm_out ? (sel::ImmPt*)imm_out + (size_t)j*cap : nullptr; J[j].cap = cap; }
   { int rc = join_ingest_upto(c, need); if (rc) return rc; }
@@ -144,14 +168,15 @@ int sdv_make_new_traces_batch(sdv_ctx* c, int n, const int32_t* slots, const uin
   return SDV_OK;
 }
 
-int sdv_activate_select_batch(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,
-                              const int32_t* cand_host_begin, const int32_t* cand_begin, const float* cKRKi9, const float* cKt3, const float* cand4, const float* min_act_dist,
-                              int32_t* decision_out, float* dist_map_out) { SDV_GUARD_TRK(c);
+int sdv_activate_select_batch_cams(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,
+                                   const int32_t* cand_host_begin, const int32_t* cand_begin, const float* cKRKi9, const float* cKt3, const float* cand4, const float* min_act_dist,
+                                   const int32_t* cams, int32_t* decision_out, float* dist_map_out) { SDV_GUARD_TRK(c);
   if (!c || n < 0 || (n && (!host_begin || !pt_begin || !cand_host_begin || !cand_begin || !min_act_dist))) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK; SEL_STATE("activate_select");
   if (host_begin[0] != 0 || cand_host_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "activate_select: host_begin[0] and cand_host_begin[0] must be 0");
+  if (cams) for (int j = 0; j < n; j++) if (cams[j] < 0 || cams[j] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "activate_select: sequence %d names camera %d (valid: 0..%d)", j, cams[j], SDV_MAX_CAMERAS - 1);
   // the engine wants, per sequence, CSR offsets that start at 0: rebase the global ones
-  std::vector<std::vector<int>> pb(n), cb(n); std::vector<sel::SelEngine::ActJob> J(n); const size_t n1 = (size_t)(c->w >> 1)*(c->h >> 1);
+  std::vector<std::vector<int>> pb(n), cb(n); std::vector<sel::SelEngine::ActJob> J(n); size_t map_off = 0;     // distance maps back to back, each at its camera's level-1 size
   for (int j = 0; j < n; j++) {
     const int h0 = host_begin[j], h1 = host_begin[j+1], g0 = cand_host_begin[j], g1 = cand_host_begin[j+1];
     if (h1 < h0 || g1 < g0 || h1 - h0 > 16 || g1 - g0 > 16) return ctx_fail(c, SDV_ERR_ARG, "activate_select: sequence %d has %d source / %d candidate keyframes (0..16)", j, h1 - h0, g1 - g0);
@@ -162,7 +187,8 @@ int sdv_activate_select_batch(sdv_ctx* c, int n, const int32_t* host_begin, cons
     sel::SelEngine::ActJob& a = J[j]; a.nHosts = h1 - h0; a.pt_begin = pb[j].data(); a.KRKi = KRKi9 ? KRKi9 + 9*(size_t)h0 : nullptr; a.Kt = Kt3 ? Kt3 + 3*(size_t)h0 : nullptr;
     a.uvid = uvid ? uvid + 3*(size_t)pt_begin[h0] : nullptr; a.nCandHosts = g1 - g0; a.cand_begin = cb[j].data(); a.cKRKi = cKRKi9 ? cKRKi9 + 9*(size_t)g0 : nullptr; a.cKt = cKt3 ? cKt3 + 3*(size_t)g0 : nullptr;
     a.cand4 = cand4 ? cand4 + 4*(size_t)cand_begin[g0] : nullptr; a.minActDist = min_act_dist[j]; a.decision_host = decision_out ? decision_out + cand_begin[g0] : nullptr;
-    a.map_host = dist_map_out ? dist_map_out + (size_t)j*n1 : nullptr;
+    const int cam = cams ? cams[j] : 0; a.w1 = c->cam_w[cam] >> 1; a.h1 = c->cam_h[cam] >> 1;
+    a.map_host = dist_map_out ? dist_map_out + map_off : nullptr; map_off += (size_t)a.w1*a.h1;
   }
   CK(cudaSetDevice(c->device));
   const long long l0 = s->eng.launches;
@@ -172,6 +198,11 @@ int sdv_activate_select_batch(sdv_ctx* c, int n, const int32_t* host_begin, cons
   if (s->eng.have_ev) c->last_ms = s->eng.last_kernel_ms;                                  // the 43 launches, copies excluded
   c->launches += s->eng.launches - l0;
   return SDV_OK;
+}
+int sdv_activate_select_batch(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,
+                              const int32_t* cand_host_begin, const int32_t* cand_begin, const float* cKRKi9, const float* cKt3, const float* cand4, const float* min_act_dist,
+                              int32_t* decision_out, float* dist_map_out) {
+  return sdv_activate_select_batch_cams(c, n, host_begin, pt_begin, KRKi9, Kt3, uvid, cand_host_begin, cand_begin, cKRKi9, cKt3, cand4, min_act_dist, nullptr, decision_out, dist_map_out);
 }
 
 }  // extern "C"

@@ -33,6 +33,7 @@ struct ImmPt { float u, v, idepth_min, idepth_max, color[8], weights[8], gradH[4
 
 struct SelJob {                          // one select pass of one frame
   FrameImg img; const float* thsSm; const double* cloud; int n;       // cloud == nullptr: dense pass over all pixels
+  int w, h;                              // the frame's (its camera's) size
   int pot, nbx4, nby4, numPotW, numPotH, nslots; float thFactor; int active;
   int *cnt, *off, *slot_of, *list, *mask, *n2start; PtRec* rec;
   unsigned char* map;                    // n bytes (LiDAR) or w*h bytes (dense): 0 / 1 / 2 / 4
@@ -86,9 +87,10 @@ __device__ __forceinline__ void test_rec(const PtRec& r, float thF, float dw1, f
 }
 
 // ---------------------------------------------------------------------------------------------- makeHists
-struct HistJob { const float* I0; float* ths; float* thsSm; };
-__global__ void __launch_bounds__(128) sel_hist_kernel(const HistJob* __restrict__ jobs, int w, int h, SelSet S) {       // CTA per 32x32 block
-  const HistJob J = jobs[blockIdx.y]; const int w32 = w/32, bx = blockIdx.x % w32, by = blockIdx.x / w32;
+struct HistJob { const float* I0; float* ths; float* thsSm; int w = 0, h = 0; };          // w, h: the frame's (its camera's) size; 0: the engine's
+__global__ void __launch_bounds__(128) sel_hist_kernel(const HistJob* __restrict__ jobs, SelSet S) {                    // CTA per 32x32 block of the largest job
+  const HistJob J = jobs[blockIdx.y]; const int w = J.w, h = J.h, w32 = w/32; if ((int)blockIdx.x >= w32*(h/32)) return;
+  const int bx = blockIdx.x % w32, by = blockIdx.x / w32;
   __shared__ int hist[64];
   if (threadIdx.x < 64) hist[threadIdx.x] = 0;
   __syncthreads();
@@ -106,8 +108,8 @@ __global__ void __launch_bounds__(128) sel_hist_kernel(const HistJob* __restrict
     J.ths[bx + by*w32] = q + S.minGradHistAdd;
   }
 }
-__global__ void __launch_bounds__(128) sel_smooth_kernel(const HistJob* __restrict__ jobs, int w, int h) {               // thread per block
-  const HistJob J = jobs[blockIdx.y]; const int w32 = w/32, h32 = h/32, i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= w32*h32) return;
+__global__ void __launch_bounds__(128) sel_smooth_kernel(const HistJob* __restrict__ jobs) {                             // thread per block
+  const HistJob J = jobs[blockIdx.y]; const int w32 = J.w/32, h32 = J.h/32, i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= w32*h32) return;
   const int x = i % w32, y = i / w32; const float* ths = J.ths; float sum = 0, num = 0;
   if (x > 0)     { if (y > 0) { num++; sum += ths[x-1+(y-1)*w32]; } if (y < h32-1) { num++; sum += ths[x-1+(y+1)*w32]; } num++; sum += ths[x-1+y*w32]; }
   if (x < w32-1) { if (y > 0) { num++; sum += ths[x+1+(y-1)*w32]; } if (y < h32-1) { num++; sum += ths[x+1+(y+1)*w32]; } num++; sum += ths[x+1+y*w32]; }
@@ -119,9 +121,10 @@ __global__ void __launch_bounds__(128) sel_smooth_kernel(const HistJob* __restri
 
 // ---------------------------------------------------------------------------------------------- one select pass
 // LiDAR pixels -> records + cell histogram (thread per cloud row)
-__global__ void __launch_bounds__(128) sel_point_kernel(const SelJob* __restrict__ jobs, int w, int h) {
+__global__ void __launch_bounds__(128) sel_point_kernel(const SelJob* __restrict__ jobs) {
   const SelJob J = jobs[blockIdx.y]; if (!J.active || !J.cloud) return;
   const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= J.n) return;
+  const int w = J.w, h = J.h;
   const double cu = J.cloud[3*i], cv = J.cloud[3*i+1]; const float xf = (float)cu, yf = (float)cv;
   PtRec r; r.valid = 0; r.out = i; r.dx = r.dy = r.ag0 = r.ag1 = r.ag2 = r.th0 = 0;
   int slot = -1;
@@ -157,7 +160,7 @@ __global__ void __launch_bounds__(128) sel_scatter_kernel(const SelJob* __restri
 // candidate k of a cell: LiDAR = k-th entry of its (index-sorted) list; dense = k-th pixel of the cell in raster order
 template <bool LIDAR> struct CellIter {
   const SelJob& J; int w, h; int beg, cnt; int x0, y0, mx, my;
-  __device__ CellIter(const SelJob& J_, int w_, int h_, int slot, int cx, int cy) : J(J_), w(w_), h(h_) {
+  __device__ CellIter(const SelJob& J_, int slot, int cx, int cy) : J(J_), w(J_.w), h(J_.h) {
     if (LIDAR) { cnt = J.cnt[slot]; beg = J.off[slot] - cnt; x0 = y0 = mx = my = 0; }
     else { x0 = cx*J.pot; y0 = cy*J.pot; mx = imin_(J.pot, w - x0); my = imin_(J.pot, h - y0); cnt = mx*my; beg = 0; }
   }
@@ -170,13 +173,13 @@ template <bool LIDAR> struct CellIter {
 };
 // per cell: would it produce a level-2 pick, for each of the 16 directions (bit d)?  Exact: arg-max of |grad . dir_d| over the candidates above the level-0
 // threshold, first one wins ties, and the pick only counts when the winner's index is > 0 (PixelSelector2.cpp:319, :592)
-template <bool LIDAR> __global__ void __launch_bounds__(128) sel_cell_kernel(const SelJob* __restrict__ jobs, int w, int h, int dirDist) {
+template <bool LIDAR> __global__ void __launch_bounds__(128) sel_cell_kernel(const SelJob* __restrict__ jobs, int dirDist) {
   const SelJob J = jobs[blockIdx.y]; if (!J.active || (J.cloud != nullptr) != LIDAR) return;
   const int slot = blockIdx.x*blockDim.x + threadIdx.x; if (slot >= J.nslots) return;
   const int blk = slot >> 4, bx = blk % J.nbx4, by = blk / J.nbx4, cx = bx*4 + ((slot>>2)&1)*2 + (slot&1), cy = by*4 + ((slot>>3)&1)*2 + ((slot>>1)&1);
   int m = 0;
   if (cx < J.numPotW && cy < J.numPotH) {
-    CellIter<LIDAR> it(J, w, h, slot, cx, cy);
+    CellIter<LIDAR> it(J, slot, cx, cy);
     if (LIDAR && it.cnt > 1) {                                                           // atomics filled the segment in arbitrary order: restore cloud order
       int* L = J.list + it.beg;
       for (int a = 1; a < it.cnt; a++) { const int v = L[a]; int b = a-1; while (b >= 0 && L[b] > v) { L[b+1] = L[b]; b--; } L[b+1] = v; }
@@ -225,7 +228,7 @@ __global__ void __launch_bounds__(256) sel_n2_kernel(const SelJob* __restrict__ 
   if (threadIdx.x == 0) J.counters[0] = base;
 }
 // thread per 4x4-cell block: the three-level state machine of select / selectFromLidar with the directions now known
-template <bool LIDAR> __global__ void __launch_bounds__(128) sel_block_kernel(const SelJob* __restrict__ jobs, const unsigned char* __restrict__ rp, int w, int h, int dirDist, float dw1) {
+template <bool LIDAR> __global__ void __launch_bounds__(128) sel_block_kernel(const SelJob* __restrict__ jobs, const unsigned char* __restrict__ rp, int dirDist, float dw1) {
   const SelJob J = jobs[blockIdx.y]; if (!J.active || (J.cloud != nullptr) != LIDAR) return;
   const int blk = blockIdx.x*blockDim.x + threadIdx.x; if (blk >= J.nbx4*J.nby4) return;
   const int bx = blk % J.nbx4, by = blk / J.nbx4; const float dw2 = dw1*dw1;
@@ -240,7 +243,7 @@ template <bool LIDAR> __global__ void __launch_bounds__(128) sel_block_kernel(co
       const int slot = (blk << 4) | (sub << 2) | c;
       B.i2 = -1; B.v2 = 0;
       const float* dir2 = kSelDirs[rp[J.n2start[slot]] & 0xF];
-      CellIter<LIDAR> it(J, w, h, slot, cx, cy);
+      CellIter<LIDAR> it(J, slot, cx, cy);
       for (int k = 0; k < it.cnt; k++) { PtRec r; if (!it.get(k, r)) continue; test_rec(r, J.thFactor, dw1, dw2, dirDist, dir2, dir3, dir4, B); }
       if (B.i2 > 0) { J.map[B.i2] = 1; B.v3 = 1e10f; }
     }
@@ -254,9 +257,10 @@ template <bool LIDAR> __global__ void __launch_bounds__(128) sel_block_kernel(co
 // gathers the record of one pixel (threshold, level-0 gradient, the two coarser gradient magnitudes: the scattered loads, now 32 wide), then all lanes replay the
 // three-level state machine over the chunk from shared memory, redundantly and identically (no divergence; lane 0 writes).  A thread-per-block version walks 144 pixels per
 // thread with dependent loads.
-__global__ void __launch_bounds__(32) sel_block_dense_kernel(const SelJob* __restrict__ jobs, const unsigned char* __restrict__ rp, int w, int h, int dirDist, float dw1) {
+__global__ void __launch_bounds__(32) sel_block_dense_kernel(const SelJob* __restrict__ jobs, const unsigned char* __restrict__ rp, int dirDist, float dw1) {
   const SelJob J = jobs[blockIdx.y]; if (!J.active || J.cloud != nullptr) return;
   const int blk = blockIdx.x; if (blk >= J.nbx4*J.nby4) return;
+  const int w = J.w, h = J.h;
   const int bx = blk % J.nbx4, by = blk / J.nbx4, pot = J.pot, pp = pot*pot, npx = 16*pp, lane = threadIdx.x; const float dw2 = dw1*dw1;
   __shared__ PtRec recs[32];
   Best B; B.i2 = B.i3 = B.i4 = -1; B.v2 = B.v3 = B.v4 = 0; int n3 = 0, n4 = 0;
@@ -287,23 +291,24 @@ __global__ void __launch_bounds__(32) sel_block_dense_kernel(const SelJob* __res
   if (lane == 0) { if (n3) atomicAdd(&J.counters[1], n3); if (n4) atomicAdd(&J.counters[2], n4); }
 }
 // random sub-selection (PixelSelector2.cpp:405-423 LiDAR: the pattern is indexed by the pixel; :156-172 dense: by the rank among the selected pixels)
-__global__ void __launch_bounds__(128) sel_sub_lidar_kernel(const SelJob* __restrict__ jobs, const unsigned char* __restrict__ rp, int w) {
+// A w_c x h_c camera's pattern (PixelSelector::PixelSelector(w_c, h_c) re-seeds and draws w_c*h_c bytes) is the first w_c*h_c bytes of the context's: rp serves every job.
+__global__ void __launch_bounds__(128) sel_sub_lidar_kernel(const SelJob* __restrict__ jobs, const unsigned char* __restrict__ rp) {
   const SelJob J = jobs[blockIdx.y]; if (J.charTH < 0 || !J.cloud) return;
   const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= J.n) return;
   if (J.map[i] == 0) return;
-  const int rn = (int)(J.cloud[3*i] + J.cloud[3*i+1]*w);
+  const int rn = (int)(J.cloud[3*i] + J.cloud[3*i+1]*J.w);
   if ((int)rp[rn] > J.charTH) { J.map[i] = 0; atomicAdd(&J.counters[3], 1); }
 }
-__global__ void __launch_bounds__(128) sel_rowcount_kernel(const SelJob* __restrict__ jobs, int w, int h, int* __restrict__ rowcnt /* jobs x h */) {     // thread per image row
+__global__ void __launch_bounds__(128) sel_rowcount_kernel(const SelJob* __restrict__ jobs, int rs, int* __restrict__ rowcnt /* jobs x rs >= every job's h */) {   // thread per image row
   const SelJob J = jobs[blockIdx.y]; if (J.charTH < 0 || J.cloud) return;
-  const int y = blockIdx.x*blockDim.x + threadIdx.x; if (y >= h) return;
+  const int w = J.w, y = blockIdx.x*blockDim.x + threadIdx.x; if (y >= J.h) return;
   int n = 0; for (int x = 0; x < w; x++) n += J.map[y*w + x] != 0;
-  rowcnt[blockIdx.y*h + y] = n;
+  rowcnt[blockIdx.y*rs + y] = n;
 }
-__global__ void __launch_bounds__(128) sel_sub_dense_kernel(const SelJob* __restrict__ jobs, const unsigned char* __restrict__ rp, int w, int h, const int* __restrict__ rowcnt) {
+__global__ void __launch_bounds__(128) sel_sub_dense_kernel(const SelJob* __restrict__ jobs, const unsigned char* __restrict__ rp, int rs, const int* __restrict__ rowcnt) {
   const SelJob J = jobs[blockIdx.y]; if (J.charTH < 0 || J.cloud) return;
-  const int y = blockIdx.x*blockDim.x + threadIdx.x; if (y >= h) return;
-  int rn = 0; for (int r = 0; r < y; r++) rn += rowcnt[blockIdx.y*h + r];
+  const int w = J.w, y = blockIdx.x*blockDim.x + threadIdx.x; if (y >= J.h) return;
+  int rn = 0; for (int r = 0; r < y; r++) rn += rowcnt[blockIdx.y*rs + r];
   int drop = 0;
   for (int x = 0; x < w; x++) if (J.map[y*w + x] != 0) { if ((int)rp[rn] > J.charTH) { J.map[y*w + x] = 0; drop++; } rn++; }
   if (drop) atomicAdd(&J.counters[3], drop);
@@ -312,7 +317,8 @@ __global__ void __launch_bounds__(128) sel_sub_dense_kernel(const SelJob* __rest
 // ---------------------------------------------------------------------------------------------- makeNewTraces
 struct TraceJob {
   FrameImg img; const double* cloud; int n; const unsigned char* mapL; unsigned char* mapD;        // LiDAR selection (n bytes), persistent monocular selection (w*h bytes)
-  int pot;                                                                                          // PixelSelector::currentPotential after both makeMaps calls (setMask)
+  int w, h;                                                                                         // the frame's (its camera's) size
+  int pot;                                                                                         // PixelSelector::currentPotential after both makeMaps calls (setMask)
   float* score; int* flag; int* pos;                                                                // per cloud row
   unsigned char* occ; unsigned char* state; int* cand; int ncand_cap;                              // occupancy mask, per-pixel state of the monocular candidates, their list
   NewTrace* out; ImmPt* imm; int cap;
@@ -358,8 +364,9 @@ __device__ __forceinline__ void paint_mask(unsigned char* occ, int w, int h, int
 __device__ __forceinline__ int float_order_bits(float f) { int b = __float_as_int(f); return b >= 0 ? b : (b ^ 0x7FFFFFFF); }     // monotone float -> int (atomicMax of the scores)
 __device__ __forceinline__ float float_from_order_bits(int b) { return __int_as_float(b >= 0 ? b : (b ^ 0x7FFFFFFF)); }
 // LiDAR loop, part 1 (thread per cloud row): score of every selected pixel, whether its candidate survives (finite pattern), the maximum score
-__global__ void __launch_bounds__(128) nt_lidar_score_kernel(const TraceJob* __restrict__ jobs, int w, int h, SelSet S) {
+__global__ void __launch_bounds__(128) nt_lidar_score_kernel(const TraceJob* __restrict__ jobs, SelSet S) {
   const TraceJob J = jobs[blockIdx.y]; const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= J.n) return;
+  const int w = J.w, h = J.h;
   int keep = 0; float sc = 0;
   if (J.mapL[i] != 0) {
     const int u = (int)J.cloud[3*i], v = (int)J.cloud[3*i+1];
@@ -385,8 +392,9 @@ __global__ void __launch_bounds__(256) nt_scan_kernel(const TraceJob* __restrict
   if (threadIdx.x == 0) J.counts[0] = base;
 }
 // LiDAR loop, part 2: the kept candidates in cloud order -> records, CORNER / EDGELET by score > 0.01f * maxScore (:1328-1335), occupancy mask
-__global__ void __launch_bounds__(128) nt_lidar_emit_kernel(const TraceJob* __restrict__ jobs, int w, int h, SelSet S) {
+__global__ void __launch_bounds__(128) nt_lidar_emit_kernel(const TraceJob* __restrict__ jobs, SelSet S) {
   const TraceJob J = jobs[blockIdx.y]; const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= J.n || !J.flag[i]) return;
+  const int w = J.w, h = J.h;
   const int u = (int)J.cloud[3*i], v = (int)J.cloud[3*i+1], m = J.pos[i];
   const float maxScore = float_from_order_bits(J.counts[3]), threshold = 0.01f;
   if (m < J.cap) {
@@ -398,14 +406,14 @@ __global__ void __launch_bounds__(128) nt_lidar_emit_kernel(const TraceJob* __re
 }
 // monocular loop (:1337-1353): candidates = selected pixels of the persistent map inside the pattern padding, in raster order.  A candidate is dropped when its
 // pattern is not finite or the occupancy mask is set at its pixel — by a LiDAR point, or by a monocular candidate accepted EARLIER in raster order (greedy).
-__global__ void __launch_bounds__(128) nt_dense_state_kernel(const TraceJob* __restrict__ jobs, int w, int h, SelSet S) {   // thread per pixel: state of the monocular candidates
-  const TraceJob J = jobs[blockIdx.y]; const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= w*h) return;
+__global__ void __launch_bounds__(128) nt_dense_state_kernel(const TraceJob* __restrict__ jobs, SelSet S) {   // thread per pixel: state of the monocular candidates
+  const TraceJob J = jobs[blockIdx.y]; const int w = J.w, h = J.h, i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= w*h) return;
   const int y = i / w, x = i - y*w; unsigned char st = 0;
   if (y >= 3 && y < h-4 && x >= 3 && x < w-4 && J.mapD[i] != 0) { ImmPt p; st = (imm_construct(J.img.I0, w, x, y, S, p) && J.occ[i] == 0) ? 1 : 3; }
   J.state[i] = st;
 }
-__global__ void __launch_bounds__(256) nt_dense_resolve_kernel(const TraceJob* __restrict__ jobs, int w, int h, SelSet S) {   // CTA per job
-  const TraceJob J = jobs[blockIdx.x];
+__global__ void __launch_bounds__(256) nt_dense_resolve_kernel(const TraceJob* __restrict__ jobs, SelSet S) {   // CTA per job
+  const TraceJob J = jobs[blockIdx.x]; const int w = J.w, h = J.h;
   __shared__ int sm[512]; __shared__ int base;
   // (1) candidate list in raster order: chunked compaction of state != 0
   if (threadIdx.x == 0) base = 0;
@@ -630,13 +638,14 @@ __global__ void __launch_bounds__(256) act_walk_smem_kernel(const DistJob* __res
 struct SelectorSlot { int currentPotential = 3; unsigned char* mapD = nullptr; };
 
 struct MapsJobHost {                     // one makeMaps / makeMapsFromLidar call
-  FrameImg img; const float* thsSm; const double* cloud_dev; int n; unsigned char* map; float density; int recursionsLeft; float thFactor; int* currentPotential;
-  int numHaveSub;                        // out
+  FrameImg img; int w = 0, h = 0; const float* thsSm; const double* cloud_dev; int n; unsigned char* map; float density; int recursionsLeft; float thFactor; int* currentPotential;
+  int numHaveSub;                       // out
   int passes;                            // out: select passes run (1, or 2 after a recursion)
 };
 
 struct SelEngine {
-  int w = 0, h = 0; SelSet S; cudaStream_t st = nullptr; std::string err;
+  int w = 0, h = 0;                        // the largest image (the pattern's size); every job carries its own size w_j <= w, h_j <= h (a job whose size is 0 has w x h)
+  SelSet S; cudaStream_t st = nullptr; std::string err;
   unsigned char* rp = nullptr;           // randomPattern (device)
   Scratch scr, scr2; long long launches = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr; bool have_ev = false; float last_kernel_ms = 0.f;   // device time of the launches of the last activate() (copies excluded)
@@ -654,23 +663,26 @@ struct SelEngine {
     return 0;
   }
   void destroy() { if (rp) cudaFree(rp); rp = nullptr; scr.release(); scr2.release(); if (have_ev) { cudaEventDestroy(ev0); cudaEventDestroy(ev1); have_ev = false; } }
-  size_t ths_floats() const { const int w32 = w/32, h32 = h/32; return (size_t)w32*(h32+1) + 101; }   // thsSmoothed is read up to one block row / column past its end (zero there)
+  static size_t ths_floats(int w, int h) { const int w32 = w/32, h32 = h/32; return (size_t)w32*(h32+1) + 101; }   // thsSmoothed is read up to one block row / column past its end (zero there)
+  size_t ths_floats() const { return ths_floats(w, h); }
+  template <class J> void size_or_engine(J& j) const { if (!j.w) { j.w = w; j.h = h; } }
 
-  // PixelSelector::makeHists for nj frames: ths / thsSm are device arrays of ths_floats() floats per job, zero-initialised by the caller
+  // PixelSelector::makeHists for nj frames: ths / thsSm are device arrays of ths_floats(w_j, h_j) floats per job, zero-initialised by the caller
   int make_hists(int nj, const HistJob* jobs_host) {
     if (nj <= 0) return 0;
     if (scr2.reserve(Scratch::need(nj, sizeof(HistJob)), st)) { err = "scratch"; return -1; }
     scr2.reset(); HistJob* d = scr2.take<HistJob>(nj);
-    SEL_CK(cudaMemcpyAsync(d, jobs_host, nj*sizeof(HistJob), cudaMemcpyHostToDevice, st));
-    const int w32 = w/32, h32 = h/32;
-    SDV_LAUNCH_SYNC(sel_hist_kernel, dim3(w32*h32, nj), dim3(128), st, d, w, h, S);
-    SDV_LAUNCH(sel_smooth_kernel, dim3((w32*h32 + 127)/128, nj), dim3(128), st, d, w, h);
+    std::vector<HistJob> H(jobs_host, jobs_host + nj); int nb = 0;
+    for (auto& J : H) { size_or_engine(J); nb = std::max(nb, (J.w/32)*(J.h/32)); }
+    SEL_CK(cudaMemcpyAsync(d, H.data(), nj*sizeof(HistJob), cudaMemcpyHostToDevice, st));
+    SDV_LAUNCH_SYNC(sel_hist_kernel, dim3(nb, nj), dim3(128), st, d, S);
+    SDV_LAUNCH(sel_smooth_kernel, dim3((nb + 127)/128, nj), dim3(128), st, d);
     launches += 2; SEL_CK(cudaGetLastError());
     SEL_CK(cudaStreamSynchronize(st));                                                   // jobs_host / scr2 may be reused by the caller
     return 0;
   }
 
-  size_t pass_bytes(int pot, int n, bool lidar) const {
+  static size_t pass_bytes(int pot, int n, bool lidar, int w, int h) {
     const int nbx4 = (w + 4*pot-1)/(4*pot), nby4 = (h + 4*pot-1)/(4*pot); const size_t ns = (size_t)nbx4*nby4*16;
     size_t b = 2*Scratch::need(ns, 4);                                                   // mask, n2start
     if (lidar) b += 2*Scratch::need(ns, 4) + 2*Scratch::need(n, 4) + Scratch::need(n, sizeof(PtRec));
@@ -681,13 +693,13 @@ struct SelEngine {
     const int nj = (int)jobs.size(); n3.assign((size_t)nj*4, 0);
     for (int j0 = 0; j0 < nj; ) {                                                        // chunks bounded by the scratch budget
       size_t bytes = Scratch::need(nj, sizeof(SelJob)) + Scratch::need((size_t)nj*4, 4); int j1 = j0;
-      while (j1 < nj) { const size_t b = pass_bytes(*jobs[j1]->currentPotential, jobs[j1]->n, lidar); if (j1 > j0 && bytes + b > max_scratch) break; bytes += b; j1++; }
+      while (j1 < nj) { const size_t b = pass_bytes(*jobs[j1]->currentPotential, jobs[j1]->n, lidar, jobs[j1]->w, jobs[j1]->h); if (j1 > j0 && bytes + b > max_scratch) break; bytes += b; j1++; }
       if (scr.reserve(bytes, st)) { err = "scratch"; return -1; }
       scr.reset(); const int nc = j1 - j0; std::vector<SelJob> H(nc);
       SelJob* d = scr.take<SelJob>(nc); int* counters = scr.take<int>((size_t)nc*4);
       int maxSlots = 0, maxN = 0, maxBlk = 0; const size_t zero_from = scr.used;
-      for (int k = 0; k < nc; k++) { MapsJobHost& M = *jobs[j0+k]; SelJob& J = H[k]; const int pot = *M.currentPotential;
-        J.img = M.img; J.thsSm = M.thsSm; J.cloud = lidar ? M.cloud_dev : nullptr; J.n = lidar ? M.n : 0; J.pot = pot; J.thFactor = M.thFactor; J.active = 1; J.charTH = -1;
+      for (int k = 0; k < nc; k++) { MapsJobHost& M = *jobs[j0+k]; SelJob& J = H[k]; const int pot = *M.currentPotential, w = M.w, h = M.h;
+        J.img = M.img; J.w = w; J.h = h; J.thsSm = M.thsSm; J.cloud = lidar ? M.cloud_dev : nullptr; J.n = lidar ? M.n : 0; J.pot = pot; J.thFactor = M.thFactor; J.active = 1; J.charTH = -1;
         J.numPotW = (w + pot-1)/pot; J.numPotH = (h + pot-1)/pot; J.nbx4 = (w + 4*pot-1)/(4*pot); J.nby4 = (h + 4*pot-1)/(4*pot); J.nslots = J.nbx4*J.nby4*16;
         J.mask = scr.take<int>(J.nslots); J.n2start = scr.take<int>(J.nslots); J.cnt = J.off = J.slot_of = J.list = nullptr; J.rec = nullptr;
         if (lidar) { J.cnt = scr.take<int>(J.nslots); J.off = scr.take<int>(J.nslots); J.slot_of = scr.take<int>(M.n); J.list = scr.take<int>(M.n); J.rec = scr.take<PtRec>(M.n); }
@@ -699,17 +711,17 @@ struct SelEngine {
       SEL_CK(cudaMemcpyAsync(d, H.data(), nc*sizeof(SelJob), cudaMemcpyHostToDevice, st));
       const int dd = S.selectDirectionDistribution;
       if (lidar) {
-        if (maxN > 0) SDV_LAUNCH(sel_point_kernel, dim3((maxN + 127)/128, nc), dim3(128), st, d, w, h);
+        if (maxN > 0) SDV_LAUNCH(sel_point_kernel, dim3((maxN + 127)/128, nc), dim3(128), st, d);
         SDV_LAUNCH_SYNC(sel_scan_kernel, dim3(nc), dim3(256), st, d);
         if (maxN > 0) SDV_LAUNCH(sel_scatter_kernel, dim3((maxN + 127)/128, nc), dim3(128), st, d);
-        SDV_LAUNCH(sel_cell_kernel<true>, dim3((maxSlots + 127)/128, nc), dim3(128), st, d, w, h, dd);
+        SDV_LAUNCH(sel_cell_kernel<true>, dim3((maxSlots + 127)/128, nc), dim3(128), st, d, dd);
         SDV_LAUNCH_SYNC(sel_n2_kernel, dim3(nc), dim3(256), st, d, rp);
-        SDV_LAUNCH(sel_block_kernel<true>, dim3((maxBlk + 127)/128, nc), dim3(128), st, d, rp, w, h, dd, S.gradDownweightPerLevel);
+        SDV_LAUNCH(sel_block_kernel<true>, dim3((maxBlk + 127)/128, nc), dim3(128), st, d, rp, dd, S.gradDownweightPerLevel);
         launches += 6;
       } else {
-        SDV_LAUNCH(sel_cell_kernel<false>, dim3((maxSlots + 127)/128, nc), dim3(128), st, d, w, h, dd);
+        SDV_LAUNCH(sel_cell_kernel<false>, dim3((maxSlots + 127)/128, nc), dim3(128), st, d, dd);
         SDV_LAUNCH_SYNC(sel_n2_kernel, dim3(nc), dim3(256), st, d, rp);
-        SDV_LAUNCH_SYNC(sel_block_dense_kernel, dim3(maxBlk, nc), dim3(32), st, d, rp, w, h, dd, S.gradDownweightPerLevel);
+        SDV_LAUNCH_SYNC(sel_block_dense_kernel, dim3(maxBlk, nc), dim3(32), st, d, rp, dd, S.gradDownweightPerLevel);
         launches += 3;
       }
       SEL_CK(cudaGetLastError());
@@ -723,6 +735,7 @@ struct SelEngine {
   // the passes and the sub-selection on the device
   int make_maps(std::vector<MapsJobHost>& jobs, bool lidar) {
     const int nj = (int)jobs.size(); if (!nj) return 0;
+    for (auto& M : jobs) size_or_engine(M);
     std::vector<float> numHave(nj, 0), quotia(nj, 0); std::vector<int> ideal(nj, 0), rec(nj); std::vector<MapsJobHost*> act;
     for (int j = 0; j < nj; j++) { rec[j] = jobs[j].recursionsLeft; jobs[j].passes = 0; act.push_back(&jobs[j]); }
     std::vector<int> actIdx(nj); for (int j = 0; j < nj; j++) actIdx[j] = j;
@@ -745,6 +758,7 @@ struct SelEngine {
     // random sub-selection
     std::vector<SelJob> H(nj); bool any = false; int maxN = 0;
     for (int j = 0; j < nj; j++) { SelJob& J = H[j]; J = SelJob(); J.cloud = lidar ? jobs[j].cloud_dev : nullptr; J.n = lidar ? jobs[j].n : 0; J.map = jobs[j].map; J.charTH = -1;
+      J.w = jobs[j].w; J.h = jobs[j].h;
       if (quotia[j] < 0.95) { J.charTH = (int)(unsigned char)(255*quotia[j]); any = true; } maxN = std::max(maxN, J.n); }
     std::vector<int> sub((size_t)nj*4, 0);
     if (any) {
@@ -753,8 +767,9 @@ struct SelEngine {
       for (int j = 0; j < nj; j++) H[j].counters = counters + 4*j;
       SEL_CK(cudaMemsetAsync(counters, 0, (size_t)nj*4*sizeof(int), st));
       SEL_CK(cudaMemcpyAsync(d, H.data(), nj*sizeof(SelJob), cudaMemcpyHostToDevice, st));
-      if (lidar) { if (maxN > 0) SDV_LAUNCH(sel_sub_lidar_kernel, dim3((maxN + 127)/128, nj), dim3(128), st, d, rp, w); launches += 1; }
-      else { SDV_LAUNCH(sel_rowcount_kernel, dim3((h + 127)/128, nj), dim3(128), st, d, w, h, rowcnt); SDV_LAUNCH(sel_sub_dense_kernel, dim3((h + 127)/128, nj), dim3(128), st, d, rp, w, h, rowcnt); launches += 2; }
+      if (lidar) { if (maxN > 0) SDV_LAUNCH(sel_sub_lidar_kernel, dim3((maxN + 127)/128, nj), dim3(128), st, d, rp); launches += 1; }
+      else { int maxH = 0; for (int j = 0; j < nj; j++) maxH = std::max(maxH, H[j].h);                                 // rowcnt rows at the stride h
+        SDV_LAUNCH(sel_rowcount_kernel, dim3((maxH + 127)/128, nj), dim3(128), st, d, h, rowcnt); SDV_LAUNCH(sel_sub_dense_kernel, dim3((maxH + 127)/128, nj), dim3(128), st, d, rp, h, rowcnt); launches += 2; }
       SEL_CK(cudaGetLastError());
       SEL_CK(cudaMemcpyAsync(sub.data(), counters, (size_t)nj*4*sizeof(int), cudaMemcpyDeviceToHost, st));
       SEL_CK(cudaStreamSynchronize(st));
@@ -765,41 +780,44 @@ struct SelEngine {
 
   // ---- FullSystem::makeNewTraces for a batch of new keyframes (one per resident sequence)
   struct NewTracesJob {
-    FrameImg img; const double* cloud_host; int n; SelectorSlot* slot; float densityLidar, densityDense; int addFeaturePoint;
+    FrameImg img; int w = 0, h = 0; const double* cloud_host; int n; SelectorSlot* slot; float densityLidar, densityDense; int addFeaturePoint;   // w, h: the frame's size (= the slot's map)
     NewTrace* out_host; ImmPt* imm_host; int cap;                  // cap: room for the returned points (LiDAR + monocular)
     int n_out, numPoints[2], passes[2];                             // out: points created, {numPointLidar, numPointMonocular}, select passes of the two makeMaps calls
   };
   Scratch io;
   int make_new_traces(std::vector<NewTracesJob>& jobs) {
     const int nj = (int)jobs.size(); if (!nj) return 0;
-    const size_t wh = (size_t)w*h, tf = ths_floats();
-    size_t bytes = Scratch::need(nj, sizeof(TraceJob)) + Scratch::need(nj, sizeof(HistJob)) + 8192;
-    for (auto& j : jobs) bytes += Scratch::need((size_t)3*j.n, 8) + Scratch::need(std::max(j.n, 1), 1) + 2*Scratch::need(tf, 4) + 3*Scratch::need(j.n, 4) + 2*Scratch::need(wh, 1)
+    for (auto& N : jobs) size_or_engine(N);
+    std::vector<size_t> o_ths(nj + 1, 0), o_occ(nj + 1, 0);                                 // per-job ths / thsSm pairs and occupancy masks, each at the job's size
+    for (int j = 0; j < nj; j++) { o_ths[j+1] = o_ths[j] + 2*ths_floats(jobs[j].w, jobs[j].h); o_occ[j+1] = o_occ[j] + (size_t)jobs[j].w*jobs[j].h; }
+    size_t bytes = Scratch::need(nj, sizeof(TraceJob)) + Scratch::need(nj, sizeof(HistJob)) + Scratch::need(o_ths[nj], 4) + Scratch::need(o_occ[nj], 1) + 8192;
+    for (auto& j : jobs) bytes += Scratch::need((size_t)3*j.n, 8) + Scratch::need(std::max(j.n, 1), 1) + 3*Scratch::need(j.n, 4) + Scratch::need((size_t)j.w*j.h, 1)
                               + Scratch::need(j.cap, 4) + Scratch::need(j.cap, sizeof(NewTrace)) + Scratch::need(j.cap, sizeof(ImmPt)) + Scratch::need(4, 4);
     if (io.reserve(bytes, st)) { err = "scratch"; return -1; }
     io.reset(); std::vector<TraceJob> T(nj); std::vector<HistJob> Hj(nj); std::vector<MapsJobHost> ML, MD;
     TraceJob* dT = io.take<TraceJob>(nj);
     // per-type arrays of all jobs back to back: one memset / one upload per call instead of one per keyframe
-    float* ths_all = io.take<float>(2*tf*nj); unsigned char* occ_all = io.take<unsigned char>(wh*nj); int* counts_all = io.take<int>((size_t)4*nj);
+    float* ths_all = io.take<float>(o_ths[nj]); unsigned char* occ_all = io.take<unsigned char>(o_occ[nj]); int* counts_all = io.take<int>((size_t)4*nj);
     size_t tot_cl = 0; for (auto& j : jobs) tot_cl += (size_t)3*std::max(j.n, 0);
     double* cl_all = io.take<double>(std::max(tot_cl, (size_t)1)); size_t off = 0;
-    SEL_CK(cudaMemsetAsync(ths_all, 0, 2*tf*nj*sizeof(float), st)); SEL_CK(cudaMemsetAsync(occ_all, 0, wh*nj, st));
+    SEL_CK(cudaMemsetAsync(ths_all, 0, o_ths[nj]*sizeof(float), st)); SEL_CK(cudaMemsetAsync(occ_all, 0, o_occ[nj], st));
     std::vector<int> c0((size_t)4*nj, 0); for (int j = 0; j < nj; j++) c0[4*j+3] = float_order_bits_host(-1000.0f);
     SEL_CK(cudaMemcpyAsync(counts_all, c0.data(), c0.size()*sizeof(int), cudaMemcpyHostToDevice, st));
-    for (int j = 0; j < nj; j++) { NewTracesJob& N = jobs[j]; TraceJob& J = T[j];
+    int maxWH = 0;
+    for (int j = 0; j < nj; j++) { NewTracesJob& N = jobs[j]; TraceJob& J = T[j]; const size_t wh = (size_t)N.w*N.h, tf = ths_floats(N.w, N.h); maxWH = std::max(maxWH, (int)wh);
       if (!N.slot->mapD) { SEL_CK(cudaMalloc((void**)&N.slot->mapD, wh)); SEL_CK(cudaMemsetAsync(N.slot->mapD, 0, wh, st)); }   // FullSystem::selectionMap: persistent; zero at birth (the reference: uninitialised)
-      double* cl = cl_all + off; unsigned char* mapL = io.take<unsigned char>(std::max(N.n, 1)); float* ths = ths_all + (size_t)2*tf*j; float* thsSm = ths + tf;
+      double* cl = cl_all + off; unsigned char* mapL = io.take<unsigned char>(std::max(N.n, 1)); float* ths = ths_all + o_ths[j]; float* thsSm = ths + tf;
       if (N.n) {                                              // clouds that follow each other in host memory (the C-ABI's layout) travel in ONE copy
         const bool starts_run = (j == 0) || !(jobs[j-1].n > 0 && jobs[j-1].cloud_host + 3*(size_t)jobs[j-1].n == N.cloud_host);
         if (starts_run) { int j2 = j; size_t run = (size_t)3*N.n; while (j2 + 1 < nj && jobs[j2+1].n > 0 && jobs[j2].cloud_host + 3*(size_t)jobs[j2].n == jobs[j2+1].cloud_host) { j2++; run += (size_t)3*jobs[j2].n; }
           SEL_CK(cudaMemcpyAsync(cl, N.cloud_host, run*sizeof(double), cudaMemcpyHostToDevice, st)); }
       }
       off += (size_t)3*std::max(N.n, 0);
-      J.img = N.img; J.cloud = cl; J.n = N.n; J.mapL = mapL; J.mapD = N.slot->mapD; J.score = io.take<float>(N.n); J.flag = io.take<int>(N.n); J.pos = io.take<int>(N.n);
-      J.occ = occ_all + wh*j; J.state = io.take<unsigned char>(wh); J.cand = io.take<int>(N.cap); J.ncand_cap = N.cap;
+      J.img = N.img; J.w = N.w; J.h = N.h; J.cloud = cl; J.n = N.n; J.mapL = mapL; J.mapD = N.slot->mapD; J.score = io.take<float>(N.n); J.flag = io.take<int>(N.n); J.pos = io.take<int>(N.n);
+      J.occ = occ_all + o_occ[j]; J.state = io.take<unsigned char>(wh); J.cand = io.take<int>(N.cap); J.ncand_cap = N.cap;
       J.out = io.take<NewTrace>(N.cap); J.imm = io.take<ImmPt>(N.cap); J.cap = N.cap; J.counts = counts_all + 4*j;
-      Hj[j] = HistJob{N.img.I0, ths, thsSm};
-      MapsJobHost M; M.img = N.img; M.thsSm = thsSm; M.cloud_dev = cl; M.n = N.n; M.map = mapL; M.density = N.densityLidar; M.recursionsLeft = 1; M.thFactor = 1; M.currentPotential = &N.slot->currentPotential;
+      Hj[j] = HistJob{N.img.I0, ths, thsSm, N.w, N.h};
+      MapsJobHost M; M.img = N.img; M.w = N.w; M.h = N.h; M.thsSm = thsSm; M.cloud_dev = cl; M.n = N.n; M.map = mapL; M.density = N.densityLidar; M.recursionsLeft = 1; M.thFactor = 1; M.currentPotential = &N.slot->currentPotential;
       M.numHaveSub = 0; M.passes = 0; ML.push_back(M);
     }
     if (make_hists(nj, Hj.data())) return -1;
@@ -812,11 +830,11 @@ struct SelEngine {
     int maxN = 0;
     for (int j = 0; j < nj; j++) { T[j].pot = jobs[j].slot->currentPotential; maxN = std::max(maxN, T[j].n); }
     SEL_CK(cudaMemcpyAsync(dT, T.data(), nj*sizeof(TraceJob), cudaMemcpyHostToDevice, st));
-    if (maxN > 0) SDV_LAUNCH(nt_lidar_score_kernel, dim3((maxN + 127)/128, nj), dim3(128), st, dT, w, h, S);
+    if (maxN > 0) SDV_LAUNCH(nt_lidar_score_kernel, dim3((maxN + 127)/128, nj), dim3(128), st, dT, S);
     SDV_LAUNCH_SYNC(nt_scan_kernel, dim3(nj), dim3(256), st, dT);
-    if (maxN > 0) SDV_LAUNCH(nt_lidar_emit_kernel, dim3((maxN + 127)/128, nj), dim3(128), st, dT, w, h, S);
-    SDV_LAUNCH(nt_dense_state_kernel, dim3((w*h + 127)/128, nj), dim3(128), st, dT, w, h, S);
-    SDV_LAUNCH_SYNC(nt_dense_resolve_kernel, dim3(nj), dim3(256), st, dT, w, h, S);
+    if (maxN > 0) SDV_LAUNCH(nt_lidar_emit_kernel, dim3((maxN + 127)/128, nj), dim3(128), st, dT, S);
+    SDV_LAUNCH(nt_dense_state_kernel, dim3((maxWH + 127)/128, nj), dim3(128), st, dT, S);
+    SDV_LAUNCH_SYNC(nt_dense_resolve_kernel, dim3(nj), dim3(256), st, dT, S);
     launches += 5; SEL_CK(cudaGetLastError());
     std::vector<int> counts((size_t)nj*4);
     SEL_CK(cudaMemcpyAsync(counts.data(), counts_all, counts.size()*sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -835,20 +853,22 @@ struct SelEngine {
     int nHosts; const int* pt_begin; const float* KRKi; const float* Kt; const float* uvid;                        // host arrays; sources grouped by host keyframe
     int nCandHosts; const int* cand_begin; const float* cKRKi; const float* cKt; const float* cand4; float minActDist;
     int32_t* decision_host; float* map_host;                                                                       // out: per candidate 1 / 0 / -1; optional w1*h1 map after the walk
+    int w1 = 0, h1 = 0;                                                                                            // level-1 size of the sequence's camera
   };
   int activate(std::vector<ActJob>& jobs) {
     const int nj = (int)jobs.size(); if (!nj) return 0;
-    const int w1 = w >> 1, h1 = h >> 1; const size_t n1 = (size_t)w1*h1;
+    for (auto& a : jobs) if (!a.w1) { a.w1 = w >> 1; a.h1 = h >> 1; }
+    size_t n1max = 0; for (auto& a : jobs) n1max = std::max(n1max, (size_t)a.w1*a.h1);
     size_t bytes = Scratch::need(nj, sizeof(DistJob)) + 1024;
     for (auto& a : jobs) { const int np = a.pt_begin[a.nHosts], nc = a.nCandHosts ? a.cand_begin[a.nCandHosts] : 0;
-      bytes += Scratch::need(n1, 4) + Scratch::need(a.nHosts+1, 4) + Scratch::need(12*(size_t)a.nHosts, 4) + Scratch::need(3*(size_t)np, 4)
+      bytes += Scratch::need((size_t)a.w1*a.h1, 4) + Scratch::need(a.nHosts+1, 4) + Scratch::need(12*(size_t)a.nHosts, 4) + Scratch::need(3*(size_t)np, 4)
              + Scratch::need(a.nCandHosts+1, 4) + Scratch::need(12*(size_t)a.nCandHosts, 4) + Scratch::need(4*(size_t)nc, 4) + Scratch::need(3*(size_t)nc, 4) + Scratch::need(nc, 4) + 4096; }
     if (io.reserve(bytes, st)) { err = "scratch"; return -1; }
     io.reset(); std::vector<DistJob> D(nj); DistJob* dD = io.take<DistJob>(nj); int maxP = 0, maxC = 0;
     auto up = [&](const void* src, size_t n) -> void* { char* d = io.take<char>(std::max(n, (size_t)4)); if (n) cudaMemcpyAsync(d, src, n, cudaMemcpyHostToDevice, st); return d; };
     static const int zero1[1] = {0};
     for (int j = 0; j < nj; j++) { ActJob& a = jobs[j]; DistJob& J = D[j]; const int np = a.pt_begin[a.nHosts], nc = a.nCandHosts ? a.cand_begin[a.nCandHosts] : 0;
-      J.d = io.take<int>(n1); J.w1 = w1; J.h1 = h1; J.nHosts = a.nHosts;
+      J.d = io.take<int>((size_t)a.w1*a.h1); J.w1 = a.w1; J.h1 = a.h1; J.nHosts = a.nHosts;
       J.pt_begin = (const int*)up(a.pt_begin, (a.nHosts+1)*sizeof(int)); J.KRKi = (const float*)up(a.KRKi, 9*a.nHosts*sizeof(float)); J.Kt = (const float*)up(a.Kt, 3*a.nHosts*sizeof(float));
       J.uvid = (const float*)up(a.uvid, 3*(size_t)np*sizeof(float));
       J.nCandHosts = a.nCandHosts; J.cand_begin = (const int*)up(a.nCandHosts ? (const void*)a.cand_begin : (const void*)zero1, (a.nCandHosts+1)*sizeof(int));
@@ -856,9 +876,9 @@ struct SelEngine {
       J.minActDist = a.minActDist; J.proj = io.take<int>(3*(size_t)std::max(nc, 1)); J.decision = io.take<int>(std::max(nc, 1));
       maxP = std::max(maxP, np); maxC = std::max(maxC, nc); }
     SEL_CK(cudaMemcpyAsync(dD, D.data(), nj*sizeof(DistJob), cudaMemcpyHostToDevice, st));
-    const int gpx = (int)std::min<size_t>((n1 + 255)/256, 1024);
+    const int gpx = (int)std::min<size_t>((n1max + 255)/256, 1024);
     if (have_ev) cudaEventRecord(ev0, st);
-    const size_t walk_smem = (((n1 + 3) >> 2) + 2048)*sizeof(int);                         // byte map + the two frontier lists
+    const size_t walk_smem = (((n1max + 3) >> 2) + 2048)*sizeof(int);                      // byte map + the two frontier lists, for the largest job
     const bool smem_ok = walk_smem <= max_walk_smem && SDV_SET_SMEM(act_walk_smem_kernel, walk_smem) == 0, fused = smem_ok && fuse_map;
     if (maxC > 0) SDV_LAUNCH(act_project_kernel, dim3((maxC + 127)/128, nj), dim3(128), st, dD);
     if (fused) {                                                                         // ONE kernel per call: distance map built, walked and written back from shared memory
@@ -878,9 +898,9 @@ struct SelEngine {
     std::vector<std::vector<int>> maps(nj);
     for (int j = 0; j < nj; j++) { ActJob& a = jobs[j]; const int nc = a.nCandHosts ? a.cand_begin[a.nCandHosts] : 0;
       if (nc && a.decision_host) SEL_CK(cudaMemcpyAsync(a.decision_host, D[j].decision, (size_t)nc*sizeof(int), cudaMemcpyDeviceToHost, st));
-      if (a.map_host) { maps[j].resize(n1); SEL_CK(cudaMemcpyAsync(maps[j].data(), D[j].d, n1*sizeof(int), cudaMemcpyDeviceToHost, st)); } }
+      if (a.map_host) { maps[j].resize((size_t)a.w1*a.h1); SEL_CK(cudaMemcpyAsync(maps[j].data(), D[j].d, maps[j].size()*sizeof(int), cudaMemcpyDeviceToHost, st)); } }
     SEL_CK(cudaStreamSynchronize(st));
-    for (int j = 0; j < nj; j++) if (jobs[j].map_host) for (size_t i = 0; i < n1; i++) jobs[j].map_host[i] = (float)maps[j][i];
+    for (int j = 0; j < nj; j++) if (jobs[j].map_host) for (size_t i = 0; i < maps[j].size(); i++) jobs[j].map_host[i] = (float)maps[j][i];
     if (have_ev) cudaEventElapsedTime(&last_kernel_ms, ev0, ev1);
     return 0;
   }

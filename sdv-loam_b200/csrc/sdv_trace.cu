@@ -24,7 +24,7 @@ namespace sdv {
 __constant__ int kTracePat[8][2] = {{0,-2},{-1,-1},{1,-1},{-2,0},{0,0},{2,0},{-1,1},{0,2}};   // staticPattern[8], util/settings.cpp:250
 enum { IPS_GOOD = 0, IPS_OOB, IPS_OUTLIER, IPS_SKIPPED, IPS_BADCONDITION, IPS_UNINITIALIZED };
 
-struct TraceGroupDev { const float* I0; float KRKi[9], Kt[3], aff[2]; int pt_begin, pt_end; };   // one (host keyframe, traced frame) pair
+struct TraceGroupDev { const float* I0; float KRKi[9], Kt[3], aff[2]; int pt_begin, pt_end; int w, h; };   // one (host keyframe, traced frame) pair; w, h: its camera's size
 struct TraceSet { float outlierTH, outlierTHSumComponent, overallEnergyTHWeight, huberTH, maxPixSearch; int minTraceTestRadius; float stepsize; int GNIterations;
                   float GNThreshold, extraSlackOnTH, slackInterval, minImprovementFactor; };
 
@@ -207,17 +207,17 @@ __device__ int trace_on(sdv_immature_pt& p, const float* __restrict__ I, int wG0
 }
 
 __global__ void __launch_bounds__(128) imm_trace_kernel(const TraceGroupDev* __restrict__ groups, const int* __restrict__ group_of, int n, sdv_immature_pt* __restrict__ pts, int* __restrict__ status,
-                                                        int w, int h, TraceSet S) {
+                                                        TraceSet S) {
   const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= n) return;
   const TraceGroupDev& G = groups[group_of[i]];
   sdv_immature_pt p = pts[i];
-  const int st = trace_on(p, G.I0, w, h, G.KRKi, G.Kt, G.aff, S);
+  const int st = trace_on(p, G.I0, G.w, G.h, G.KRKi, G.Kt, G.aff, S);
   pts[i] = p; status[i] = st;
 }
 
 // ---- activation: FullSystem::optimizeImmaturePoint (FullSystemOptPoint.cpp:18-183) over ImmaturePoint::linearizeResidual (ImmaturePoint.cpp:410-476)
 struct OptTargetDev { const float* I0; float R[9], t[3], aff[2]; };          // target image + FrameFramePrecalc {PRE_RTll, PRE_tTll, PRE_aff_mode} of (host,target)
-struct OptGroupDev { int tgt_begin, nres; float fxl, fyl, cxl, cyl, fxli, fyli; };
+struct OptGroupDev { int tgt_begin, nres; float fxl, fyl, cxl, cyl, fxli, fyli; int w, h; };    // w, h: the size of the group's camera (every target's)
 enum { RS_IN = 0, RS_OOB, RS_OUTLIER };
 struct TmpResDev { int state_state; double state_energy; int state_NewState; double state_NewEnergy; };
 
@@ -256,9 +256,9 @@ __device__ double linearize_residual(const sdv_immature_pt& p, const OptTargetDe
 constexpr int kOptMaxRes = SDV_MAX_FRAMES_WINDOW;
 __global__ void __launch_bounds__(64) imm_optimize_kernel(const OptGroupDev* __restrict__ groups, const OptTargetDev* __restrict__ targets, const int* __restrict__ group_of, int n,
                                                            const sdv_immature_pt* __restrict__ pts, const unsigned char* __restrict__ from_sensor, int min_obs, int res_stride,
-                                                           int* __restrict__ status, float* __restrict__ idepth_out, int* __restrict__ res_state, int w, int h, float huberTH) {
+                                                           int* __restrict__ status, float* __restrict__ idepth_out, int* __restrict__ res_state, float huberTH) {
   const int k = blockIdx.x*blockDim.x + threadIdx.x; if (k >= n) return;
-  const OptGroupDev G = groups[group_of[k]]; const OptTargetDev* T = targets + G.tgt_begin; const int nres = G.nres;
+  const OptGroupDev G = groups[group_of[k]]; const OptTargetDev* T = targets + G.tgt_begin; const int nres = G.nres, w = G.w, h = G.h;
   const sdv_immature_pt p = pts[k]; const bool isFromSensor = from_sensor && from_sensor[k];
   const float minIdepthH_act = 100; const int GNIts = 3;                      // util/settings.cpp:41,133
   TmpResDev res[kOptMaxRes];
@@ -313,13 +313,15 @@ static int trace_scratch(sdv_ctx* c, size_t bytes) {
 
 extern "C" {
 
-int sdv_immature_init(sdv_ctx* c, uint64_t host_frame, int n, const int32_t* uv, sdv_immature_pt* out) { SDV_GUARD_TRK(c);
+int sdv_immature_init_cam(sdv_ctx* c, int cam, uint64_t host_frame, int n, const int32_t* uv, sdv_immature_pt* out) { SDV_GUARD_TRK(c);
   if (!c || n < 0 || (n && (!uv || !out))) return SDV_ERR_ARG;
+  if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "immature_init: camera %d (valid: 0..%d)", cam, SDV_MAX_CAMERAS - 1);
   if (n == 0) return SDV_OK;
   CK(cudaSetDevice(c->device));
   auto it = c->frame_index.find(host_frame); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_init: unknown host frame %llu", (unsigned long long)host_frame);
-  { int rcs = check_frame_ctx(c, c->frames[it->second], "immature_init"); if (rcs) return rcs; }
-  for (int i = 0; i < n; i++) if (uv[2*i] < 2 || uv[2*i+1] < 2 || uv[2*i] >= c->w-3 || uv[2*i+1] >= c->h-3)     // the 8-pattern (+-2) and the +1 bilinear neighbour must stay inside the image
+  { int rcs = check_frame_cam(c, c->frames[it->second], cam, "immature_init"); if (rcs) return rcs; }
+  const int w = c->cam_w[cam], h = c->cam_h[cam];
+  for (int i = 0; i < n; i++) if (uv[2*i] < 2 || uv[2*i+1] < 2 || uv[2*i] >= w-3 || uv[2*i+1] >= h-3)     // the 8-pattern (+-2) and the +1 bilinear neighbour must stay inside the image
     return ctx_fail(c, SDV_ERR_ARG, "immature_init: candidate %d at (%d,%d) is closer than 3 px to the border", i, uv[2*i], uv[2*i+1]);
   FrameDev& f = c->frames[it->second];
   { int rc = join_ingest_upto(c, f.ingest_seq); if (rc) return rc; }
@@ -327,17 +329,19 @@ int sdv_immature_init(sdv_ctx* c, uint64_t host_frame, int n, const int32_t* uv,
   { int rc = trace_scratch(c, bytes); if (rc) return rc; }
   char* d = (char*)c->trace_dev;
   CK(cudaMemcpyAsync(d, uv, o_pts, cudaMemcpyHostToDevice, c->st));
-  imm_init_kernel<<<(n + 127)/128, 128, 0, c->st>>>(f.I0, c->w, c->h, n, (const int*)d, (sdv_immature_pt*)(d + o_pts), trace_settings(c)); c->launches += 1;
+  imm_init_kernel<<<(n + 127)/128, 128, 0, c->st>>>(f.I0, w, h, n, (const int*)d, (sdv_immature_pt*)(d + o_pts), trace_settings(c)); c->launches += 1;
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, d + o_pts, (size_t)n*sizeof(sdv_immature_pt), cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st));
   return SDV_OK;
 }
+int sdv_immature_init(sdv_ctx* c, uint64_t host_frame, int n, const int32_t* uv, sdv_immature_pt* out) { return sdv_immature_init_cam(c, 0, host_frame, n, uv, out); }
 
-int sdv_immature_trace_batch(sdv_ctx* c, int n_groups, const uint64_t* frames, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* aff2,
-                             sdv_immature_pt* pts_io, int32_t* status_out) { SDV_GUARD_TRK(c);
+int sdv_immature_trace_batch_cams(sdv_ctx* c, int n_groups, const uint64_t* frames, const int32_t* cams, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* aff2,
+                                  sdv_immature_pt* pts_io, int32_t* status_out) { SDV_GUARD_TRK(c);
   if (!c || n_groups < 0 || (n_groups && (!frames || !pt_begin || !KRKi9 || !Kt3 || !aff2))) return SDV_ERR_ARG;
   if (n_groups == 0) return SDV_OK;
+  if (cams) for (int g = 0; g < n_groups; g++) if (cams[g] < 0 || cams[g] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "immature_trace: group %d names camera %d (valid: 0..%d)", g, cams[g], SDV_MAX_CAMERAS - 1);
   if (pt_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "immature_trace: pt_begin[0] must be 0");
   for (int g = 0; g < n_groups; g++) if (pt_begin[g+1] < pt_begin[g]) return ctx_fail(c, SDV_ERR_ARG, "immature_trace: pt_begin is not ascending at group %d", g);
   const int n = pt_begin[n_groups];
@@ -347,9 +351,9 @@ int sdv_immature_trace_batch(sdv_ctx* c, int n_groups, const uint64_t* frames, c
   std::vector<TraceGroupDev> G(n_groups); std::vector<int> gof(n); long long need_seq = 0;
   for (int g = 0; g < n_groups; g++) {
     auto it = c->frame_index.find(frames[g]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_trace: unknown frame %llu (group %d)", (unsigned long long)frames[g], g);
-    const FrameDev& f = c->frames[it->second]; { int rcs = check_frame_ctx(c, f, "immature_trace"); if (rcs) return rcs; }
+    const int cam = cams ? cams[g] : 0; const FrameDev& f = c->frames[it->second]; { int rcs = check_frame_cam(c, f, cam, "immature_trace"); if (rcs) return rcs; }
     if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
-    G[g].I0 = f.I0; for (int k = 0; k < 9; k++) G[g].KRKi[k] = KRKi9[9*g+k]; for (int k = 0; k < 3; k++) G[g].Kt[k] = Kt3[3*g+k]; G[g].aff[0] = aff2[2*g]; G[g].aff[1] = aff2[2*g+1];
+    G[g].w = c->cam_w[cam]; G[g].h = c->cam_h[cam]; G[g].I0 = f.I0; for (int k = 0; k < 9; k++) G[g].KRKi[k] = KRKi9[9*g+k]; for (int k = 0; k < 3; k++) G[g].Kt[k] = Kt3[3*g+k]; G[g].aff[0] = aff2[2*g]; G[g].aff[1] = aff2[2*g+1];
     G[g].pt_begin = pt_begin[g]; G[g].pt_end = pt_begin[g+1];
     for (int i = pt_begin[g]; i < pt_begin[g+1]; i++) gof[i] = g;
   }
@@ -362,7 +366,7 @@ int sdv_immature_trace_batch(sdv_ctx* c, int n_groups, const uint64_t* frames, c
   CK(cudaMemcpyAsync(d + o_of, gof.data(), (size_t)n*sizeof(int), cudaMemcpyHostToDevice, c->st));
   CK(cudaMemcpyAsync(d + o_pts, pts_io, (size_t)n*sizeof(sdv_immature_pt), cudaMemcpyHostToDevice, c->st));
   CK(cudaEventRecord(c->ev0, c->st));
-  imm_trace_kernel<<<(n + 127)/128, 128, 0, c->st>>>((const TraceGroupDev*)(d + o_g), (const int*)(d + o_of), n, (sdv_immature_pt*)(d + o_pts), (int*)(d + o_st), c->w, c->h, trace_settings(c));
+  imm_trace_kernel<<<(n + 127)/128, 128, 0, c->st>>>((const TraceGroupDev*)(d + o_g), (const int*)(d + o_of), n, (sdv_immature_pt*)(d + o_pts), (int*)(d + o_st), trace_settings(c));
   c->launches += 1;
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev1, c->st));
@@ -372,11 +376,15 @@ int sdv_immature_trace_batch(sdv_ctx* c, int n_groups, const uint64_t* frames, c
   CK(cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   return SDV_OK;
 }
+int sdv_immature_trace_batch(sdv_ctx* c, int n_groups, const uint64_t* frames, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* aff2,
+                             sdv_immature_pt* pts_io, int32_t* status_out) { return sdv_immature_trace_batch_cams(c, n_groups, frames, nullptr, pt_begin, KRKi9, Kt3, aff2, pts_io, status_out); }
 
-int sdv_immature_optimize_batch(sdv_ctx* c, int n_groups, const int32_t* pt_begin, const int32_t* tgt_begin, const uint64_t* target_frames, const float* pre14, const float* calib6,
-                                int min_obs, const sdv_immature_pt* pts, const uint8_t* is_from_sensor, int res_stride, int32_t* status_out, float* idepth_out, int32_t* res_state_out) { SDV_GUARD_TRK(c);
+int sdv_immature_optimize_batch_cams(sdv_ctx* c, int n_groups, const int32_t* pt_begin, const int32_t* tgt_begin, const uint64_t* target_frames, const float* pre14, const float* calib6,
+                                     const int32_t* cams, int min_obs, const sdv_immature_pt* pts, const uint8_t* is_from_sensor, int res_stride, int32_t* status_out, float* idepth_out,
+                                     int32_t* res_state_out) { SDV_GUARD_TRK(c);
   if (!c || n_groups < 0 || (n_groups && (!pt_begin || !tgt_begin || !target_frames || !pre14 || !calib6))) return SDV_ERR_ARG;
   if (n_groups == 0) return SDV_OK;
+  if (cams) for (int g = 0; g < n_groups; g++) if (cams[g] < 0 || cams[g] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "immature_optimize: group %d names camera %d (valid: 0..%d)", g, cams[g], SDV_MAX_CAMERAS - 1);
   if (pt_begin[0] != 0 || tgt_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "immature_optimize: pt_begin[0] and tgt_begin[0] must be 0");
   for (int g = 0; g < n_groups; g++) { if (pt_begin[g+1] < pt_begin[g] || tgt_begin[g+1] < tgt_begin[g]) return ctx_fail(c, SDV_ERR_ARG, "immature_optimize: offsets not ascending at group %d", g);
     const int nres = tgt_begin[g+1] - tgt_begin[g]; if (nres > kOptMaxRes || nres > res_stride) return ctx_fail(c, SDV_ERR_ARG, "immature_optimize: group %d has %d targets (max %d, res_stride %d)", g, nres, kOptMaxRes, res_stride); }
@@ -385,14 +393,15 @@ int sdv_immature_optimize_batch(sdv_ctx* c, int n_groups, const int32_t* pt_begi
   if (!pts || !status_out || !idepth_out || !res_state_out || res_stride < 1) return SDV_ERR_ARG;
   CK(cudaSetDevice(c->device));
   std::vector<OptGroupDev> G(n_groups); std::vector<OptTargetDev> T(nt); std::vector<int> gof(n); long long need_seq = 0;
+  std::vector<int> cam_of(nt, 0); if (cams) for (int g = 0; g < n_groups; g++) for (int t = tgt_begin[g]; t < tgt_begin[g+1]; t++) cam_of[t] = cams[g];
   for (int t = 0; t < nt; t++) {
     auto it = c->frame_index.find(target_frames[t]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_optimize: unknown target frame %llu", (unsigned long long)target_frames[t]);
-    const FrameDev& f = c->frames[it->second]; { int rcs = check_frame_ctx(c, f, "immature_optimize"); if (rcs) return rcs; }
+    const FrameDev& f = c->frames[it->second]; { int rcs = check_frame_cam(c, f, cam_of[t], "immature_optimize"); if (rcs) return rcs; }
     if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
     T[t].I0 = f.I0; for (int k = 0; k < 9; k++) T[t].R[k] = pre14[14*t+k]; for (int k = 0; k < 3; k++) T[t].t[k] = pre14[14*t+9+k]; T[t].aff[0] = pre14[14*t+12]; T[t].aff[1] = pre14[14*t+13];
   }
   for (int g = 0; g < n_groups; g++) { G[g].tgt_begin = tgt_begin[g]; G[g].nres = tgt_begin[g+1] - tgt_begin[g]; const float* q = calib6 + 6*g;
-    G[g].fxl = q[0]; G[g].fyl = q[1]; G[g].cxl = q[2]; G[g].cyl = q[3]; G[g].fxli = q[4]; G[g].fyli = q[5];
+    G[g].fxl = q[0]; G[g].fyl = q[1]; G[g].cxl = q[2]; G[g].cyl = q[3]; G[g].fxli = q[4]; G[g].fyli = q[5]; const int cam = cams ? cams[g] : 0; G[g].w = c->cam_w[cam]; G[g].h = c->cam_h[cam];
     for (int i = pt_begin[g]; i < pt_begin[g+1]; i++) gof[i] = g; }
   { int rc = join_ingest_upto(c, need_seq); if (rc) return rc; }
   auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
@@ -407,7 +416,7 @@ int sdv_immature_optimize_batch(sdv_ctx* c, int n_groups, const int32_t* pt_begi
   CK(cudaMemcpyAsync(d + o_pts, pts, (size_t)n*sizeof(sdv_immature_pt), cudaMemcpyHostToDevice, c->st));
   CK(cudaEventRecord(c->ev0, c->st));
   imm_optimize_kernel<<<(n + 63)/64, 64, 0, c->st>>>((const OptGroupDev*)(d + o_g), (const OptTargetDev*)(d + o_t), (const int*)(d + o_of), n, (const sdv_immature_pt*)(d + o_pts),
-      is_from_sensor ? (const unsigned char*)(d + o_fs) : nullptr, min_obs, res_stride, (int*)(d + o_st), (float*)(d + o_id), (int*)(d + o_rs), c->w, c->h, c->set.huberTH);
+      is_from_sensor ? (const unsigned char*)(d + o_fs) : nullptr, min_obs, res_stride, (int*)(d + o_st), (float*)(d + o_id), (int*)(d + o_rs), c->set.huberTH);
   c->launches += 1;
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev1, c->st));
@@ -417,6 +426,10 @@ int sdv_immature_optimize_batch(sdv_ctx* c, int n_groups, const int32_t* pt_begi
   CK(cudaStreamSynchronize(c->st));
   CK(cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   return SDV_OK;
+}
+int sdv_immature_optimize_batch(sdv_ctx* c, int n_groups, const int32_t* pt_begin, const int32_t* tgt_begin, const uint64_t* target_frames, const float* pre14, const float* calib6,
+                                int min_obs, const sdv_immature_pt* pts, const uint8_t* is_from_sensor, int res_stride, int32_t* status_out, float* idepth_out, int32_t* res_state_out) {
+  return sdv_immature_optimize_batch_cams(c, n_groups, pt_begin, tgt_begin, target_frames, pre14, calib6, nullptr, min_obs, pts, is_from_sensor, res_stride, status_out, idepth_out, res_state_out);
 }
 
 }  // extern "C"
