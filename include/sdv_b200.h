@@ -133,6 +133,19 @@ int  sdv_frame_build_batch_dev(sdv_ctx* c, int n, const uint64_t* frames, const 
  * (selector, makeNewTraces, activation, immature points, LiDAR front-end) names a camera per job (the _cam / _cams entries, sdv_selector_set_slot_cams)
  * and works at that camera's size; a frame of another size returns SDV_ERR_ARG and changes no state.  The entries without _cam(s) are camera 0. */
 int  sdv_set_camera_size(sdv_ctx* c, int cam, int w, int h);
+/* Cameras of different pyramid depths in one context (pyrLevelsUsed, util/globalCalib.cpp:22-30: KITTI-CARLA's 1392x1024 has 5 levels, KITTI's 1200x360 4).
+ * sdv_create's `levels` is the STORAGE depth: every frame is built to it, whatever its camera.  A camera's depth is what its tracker / map slots and jobs
+ * use, as the reference's pyrLevelsUsed: sdv_tracker_set_ref builds clouds for that many levels, trackNewestCoarse starts at depth - 1 by default
+ * (sdv_tracker_track_batch_levels, sdv_track_new_coarse_batch: FullSystem.cpp:421), and the Reprojector's search level is capped at depth - 1
+ * (Reprojector.cpp:268; sdv_reproject_map_batch, sdv_tracker_refine_batch).  sdv_tracker_set_cloud / _get_cloud / _calc_res refuse a level at or past the
+ * slot camera's depth, sdv_frame_download one at or past the frame camera's depth (SDV_ERR_ARG).  BA and immature points read level 0, the activation
+ * walk and distance map level 1, the selector levels 0..2: they do not depend on the depth.
+ * sdv_set_camera_levels gives camera `cam` (camera 0 included) the depth `levels` in 1..the context's `levels`; every camera starts at the context's
+ * depth.  The reference rule is levels = sdv_pyr_levels(w_cam, h_cam).  A size valid for sdv_set_camera_size is valid at every smaller depth.  A camera
+ * or depth out of range returns SDV_ERR_ARG; SDV_ERR_STATE while a tracker slot bound to the camera holds a reference or a resident map (built at the old
+ * depth), or for a depth below 3 while a selector slot is bound to the camera (sdv_selector_set_slot_cams refuses such a camera with SDV_ERR_ARG).
+ * A refused call changes nothing.  sdv_set_calib_slots_cams refuses to move a slot holding a reference or map to a camera of another size OR depth. */
+int  sdv_set_camera_levels(sdv_ctx* c, int cam, int levels);
 int  sdv_frame_upload_batch_cams(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs, const int32_t* cams, int fmt, const float* exposures);
 int  sdv_frame_build_batch_dev_cams(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs_dev, const int32_t* cams, int fmt, const float* exposures);
 int  sdv_frame_release(sdv_ctx* c, uint64_t frame);
@@ -176,6 +189,12 @@ int  sdv_tracker_track(sdv_ctx* c, int slot, uint64_t new_frame, double T_io[7],
 int  sdv_tracker_track_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* new_frames, double* T_io, double* ab_io,
                              int coarsest, const double* minResForAbort, double* lastRes, double* flow, int32_t* good,
                              sdv_track_stats* stats);
+/* the same with a coarsest level per job: job k starts at coarsest[k]; coarsest == NULL starts every job at its slot camera's depth - 1 (pyrLevelsUsed-1,
+ * sdv_set_camera_levels).  sdv_tracker_track_batch is this call with its scalar for every job.  A level at or past a job's depth, or >= 5
+ * (CoarseTracker.cpp:672), returns SDV_ERR_ARG before anything is enqueued. */
+int  sdv_tracker_track_batch_levels(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* new_frames, double* T_io, double* ab_io,
+                                    const int32_t* coarsest, const double* minResForAbort, double* lastRes, double* flow, int32_t* good,
+                                    sdv_track_stats* stats);
 /* ---- map reprojection + direct feature alignment (SURVEY.md §8 a10): the Reprojector of FullSystem::trackNewCoarse / makeKeyFrame
  *   void Reprojector::reprojectMap(FrameHessian* frame, std::vector<std::pair<PointHessian*, Eigen::Vector2d>>& overlap_pts)     Reprojector.cpp:117-156
  *   void Reprojector::backprojectMap(FrameHessian* ref_frame, FrameHessian* frame, overlap_pts&)                                   :158-185

@@ -115,6 +115,15 @@ int shim_kitti_keyframe(KittiKeyframe& k, float density, std::vector<sdv_new_tra
   return rc | sdv_activate_select_batch_cams(gpu, 1, host_begin, pt0, nullptr, nullptr, nullptr, cand_host_begin, cand_begin, I9, z3, cand4.data(), &md, &k.cam,
                                              decision.data(), nullptr);                            // distance map and walk at 600x180
 }
+// §4 cameras of different pyramid depths (KITTI-CARLA 1392x1024 at 5 levels next to KITTI at 4, in a 1400x1024 context at 5): each camera at pyrLevelsUsed
+int shim_camera_depths(int n_cams, const int* w, const int* h) {
+  int rc = 0;
+  for (int cam = 0; cam < n_cams; cam++) rc |= sdv_set_camera_levels(gpu, cam, sdv_pyr_levels(w[cam], h[cam]));
+  return rc;
+}
+int shim_track_own_depths(int n, const int32_t* slots, const uint64_t* frames, double* T, double* ab, double* lastRes, double* flow, int32_t* good) {
+  return sdv_tracker_track_batch_levels(gpu, n, slots, frames, T, ab, /*each job at its camera's depth - 1*/nullptr, nullptr, lastRes, flow, good, nullptr);
+}
 // §3c CoarseTracker::makeK (CoarseTracker.cpp:77-106): a member of each tracker instance, so it sets the K of that instance's slot only
 int shim_makeK(int slot, CalibHessian* HCalib) { sdv_calib K{HCalib->fxl(), HCalib->fyl(), HCalib->cxl(), HCalib->cyl()}; const int32_t s = slot; return sdv_set_calib_slots(gpu, 1, &s, &K); }
 

@@ -58,6 +58,7 @@ def _load():
     L.sdv_set_calib_slots.argtypes = [_vp, C.c_int, _i32p, _vp]
     L.sdv_set_calib_slots_cams.argtypes = [_vp, C.c_int, _i32p, _vp, _vp]
     L.sdv_set_camera_size.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
+    L.sdv_set_camera_levels.argtypes = [_vp, C.c_int, C.c_int]
     L.sdv_frame_upload_batch_cams.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _vp, C.c_int, _f32p]
     L.sdv_frame_build_batch_dev_cams.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _vp, C.c_int, _f32p]
     L.sdv_frame_upload.argtypes = [_vp, C.c_uint64, _vp, C.c_float]
@@ -85,6 +86,7 @@ def _load():
     L.sdv_tracker_struct_pose_batch_slots.argtypes = [_vp, C.c_int, _vp, _i32p, _vp, _i32p, _f64p, _f64p, _f32p, _i32p, _i32p]
     L.sdv_tracker_track.argtypes = [_vp, C.c_int, C.c_uint64, _f64p, _f64p, C.c_int, _f64p, _f64p, _f64p, C.POINTER(C.c_int), C.POINTER(sdv_track_stats)]
     L.sdv_tracker_track_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _f64p, _f64p, C.c_int, _vp, _f64p, _f64p, _i32p, C.POINTER(sdv_track_stats)]
+    L.sdv_tracker_track_batch_levels.argtypes = [_vp, C.c_int, _i32p, _u64p, _f64p, _f64p, _vp, _vp, _f64p, _f64p, _i32p, C.POINTER(sdv_track_stats)]
     L.sdv_last_kernel_ms.argtypes = [_vp]; L.sdv_last_kernel_ms.restype = C.c_float
     L.sdv_immature_init.argtypes = [_vp, C.c_uint64, C.c_int, _i32p, _vp]
     L.sdv_immature_trace_batch.argtypes = [_vp, C.c_int, _u64p, _i32p, _f32p, _f32p, _f32p, _vp, _vp]
@@ -135,7 +137,8 @@ class Context:
         self.cam_wh = {0: (w, h)}          # rectified size per camera (setCameraSize); camera 0 is the context size
         self.frame_cam = {}                # frame handle -> camera, for frames not on camera 0
         self.slot_cam = {}                 # tracker / map slot -> camera, for slots not on camera 0 (setCalibSlots)
-        self.levels = levels if levels is not None else pyr_levels(w, h)
+        self.levels = levels if levels is not None else pyr_levels(w, h)     # storage depth: every frame is built to it
+        self.cam_levels = {}               # pyramid depth per camera, for cameras not at the context's (setCameraLevels)
         s = default_settings()
         for k, v in settings.items():
             if not hasattr(s, k):
@@ -171,6 +174,22 @@ class Context:
     def setCameraSize(self, cam: int, w: int, h: int):
         """give camera `cam` (1..SDV_MAX_CAMERAS-1) the rectified size w x h <= the context size, at the context's pyramid depth (see sdv_b200.h)"""
         self._ck(LIB.sdv_set_camera_size(self.p, int(cam), int(w), int(h))); self.cam_wh[int(cam)] = (int(w), int(h))
+
+    def camLevels(self, cam: int = 0) -> int:
+        """pyramid depth (pyrLevelsUsed) of camera `cam`: what its tracker / map slots and jobs use"""
+        return self.cam_levels.get(int(cam), self.levels)
+
+    def setCameraLevels(self, cam: int, levels: int):
+        """give camera `cam` (0..SDV_MAX_CAMERAS-1) the pyramid depth `levels` in 1..self.levels; the reference rule is pyr_levels(*camSize(cam)) (see sdv_b200.h)"""
+        self._ck(LIB.sdv_set_camera_levels(self.p, int(cam), int(levels)))
+        if int(levels) == self.levels:
+            self.cam_levels.pop(int(cam), None)
+        else:
+            self.cam_levels[int(cam)] = int(levels)
+
+    def _check_level(self, lvl: int, cam: int, what: str):
+        if not 0 <= lvl < self.camLevels(cam):
+            raise SdvError(f"sdv error -1: {what}: level {lvl}, but camera {cam} has {self.camLevels(cam)} levels")
 
     # FrameHessian::makeImages
     def makeImages(self, frame_id: int, color, exposure: float = 1.0, cam: int = 0):
@@ -290,8 +309,9 @@ class Context:
         self._ck(LIB.sdv_frame_release(self.p, frame_id)); self.frame_cam.pop(frame_id, None)
 
     def frameLevel(self, frame_id: int, lvl: int):
-        """level lvl of a resident frame at the frame's own (its camera's) size"""
-        w, h = self.camSize(self.frame_cam.get(frame_id, 0)); w, h = w >> lvl, h >> lvl
+        """level lvl (below its camera's depth) of a resident frame at the frame's own (its camera's) size"""
+        cam = self.frame_cam.get(frame_id, 0); self._check_level(lvl, cam, "frameLevel")
+        w, h = self.camSize(cam); w, h = w >> lvl, h >> lvl
         dI = np.zeros((h, w, 3), np.float32); ab = np.zeros((h, w), np.float32)
         self._ck(LIB.sdv_frame_download(self.p, frame_id, lvl, dI.ctypes.data, ab.ctypes.data))
         return dI, ab
@@ -301,6 +321,7 @@ class Context:
 
     def trackBatch(self, slots, frame_ids, T, ab, coarsest=None, minRes=None):
         """n independent trackNewestCoarse calls in one launch.  T (n,7), ab (n,2) are updated in place.
+        coarsest: None starts each job at its slot camera's depth - 1 (pyrLevelsUsed-1); an int is that level for every job; a sequence one level per job.
         slots / frame_ids may be pre-built contiguous int32 / uint64 arrays (no per-call Python work beyond the C call)."""
         n = len(slots)
         slots = np.ascontiguousarray(slots, np.int32); ids = np.ascontiguousarray(frame_ids, np.uint64)
@@ -309,8 +330,14 @@ class Context:
         lastRes = np.empty((n, 5)); flow = np.empty((n, 3)); good = np.empty(n, np.int32)
         stats = np.empty(n, TRACK_STATS_DTYPE)
         mr = None if minRes is None else np.ascontiguousarray(minRes, np.float64).ctypes.data
-        self._ck(LIB.sdv_tracker_track_batch(self.p, n, slots, ids, T, ab, self.levels - 1 if coarsest is None else coarsest,
-                                             mr, lastRes, flow, good, stats.ctypes.data_as(C.POINTER(sdv_track_stats))))
+        sp = stats.ctypes.data_as(C.POINTER(sdv_track_stats))
+        if isinstance(coarsest, (int, np.integer)):
+            self._ck(LIB.sdv_tracker_track_batch(self.p, n, slots, ids, T, ab, int(coarsest), mr, lastRes, flow, good, sp))
+        else:
+            co = None if coarsest is None else np.ascontiguousarray(coarsest, np.int32).reshape(-1)
+            if co is not None and len(co) != n:
+                raise ValueError(f"{n} jobs but {len(co)} coarsest levels")
+            self._ck(LIB.sdv_tracker_track_batch_levels(self.p, n, slots, ids, T, ab, None if co is None else co.ctypes.data, mr, lastRes, flow, good, sp))
         return dict(good=good.astype(bool), lastResiduals=lastRes, flow=flow, evals=stats["point_evals"], iterations=stats["iterations"], accepts=stats["accepts"])
 
 
@@ -319,6 +346,14 @@ class CoarseTracker:
 
     def __init__(self, ctx: Context, slot: int = 0):
         self.ctx, self.slot = ctx, slot
+
+    @property
+    def levels(self) -> int:
+        """pyrLevelsUsed of this instance: its slot camera's depth"""
+        return self.ctx.camLevels(self.ctx.slot_cam.get(self.slot, 0))
+
+    def _check_level(self, lvl: int, what: str):
+        self.ctx._check_level(lvl, self.ctx.slot_cam.get(self.slot, 0), what)
 
     def makeK(self, K):
         """CoarseTracker::makeK (CoarseTracker.cpp:77-106): this instance tracks (and refines its slot's map) with K = (fx, fy, cx, cy) from now on,
@@ -330,18 +365,18 @@ class CoarseTracker:
         self.ctx._ck(LIB.sdv_tracker_set_ref(self.ctx.p, self.slot, ref_frame_id, len(pts), pts, rh, 0.0, ref_a, ref_b))
 
     def setCloud(self, ref_frame_id: int, lvl: int, u, v, idepth, color, ref_a: float = 0.0, ref_b: float = 0.0):
-        a = [np.ascontiguousarray(x, np.float32) for x in (u, v, idepth, color)]
+        self._check_level(lvl, "setCloud"); a = [np.ascontiguousarray(x, np.float32) for x in (u, v, idepth, color)]
         self.ctx._ck(LIB.sdv_tracker_set_cloud(self.ctx.p, self.slot, ref_frame_id, lvl, len(a[0]), *a, ref_a, ref_b))
 
     def cloud(self, lvl: int):
-        n = C.c_int(0)
+        self._check_level(lvl, "cloud"); n = C.c_int(0)
         self.ctx._ck(LIB.sdv_tracker_get_cloud(self.ctx.p, self.slot, lvl, C.byref(n), None, None, None, None))
         a = [np.zeros(max(n.value, 1), np.float32) for _ in range(4)]
         self.ctx._ck(LIB.sdv_tracker_get_cloud(self.ctx.p, self.slot, lvl, C.byref(n), *[x.ctypes.data for x in a]))
         return [x[:n.value] for x in a]
 
     def calcRes(self, new_frame_id: int, lvl: int, T7, a: float, b: float, cutoffTH: float):
-        rs = np.zeros(6)
+        self._check_level(lvl, "calcRes"); rs = np.zeros(6)
         self.ctx._ck(LIB.sdv_tracker_calc_res(self.ctx.p, self.slot, new_frame_id, lvl, np.ascontiguousarray(T7, np.float64), a, b, cutoffTH, rs))
         return rs
 

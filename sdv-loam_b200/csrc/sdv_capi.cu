@@ -79,11 +79,12 @@ int sdv_set_calib_slots_cams(sdv_ctx* c, int n, const int32_t* slots, const sdv_
     if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib_slots: entry %d names camera %d (valid: 0..%d)", i, cam, SDV_MAX_CAMERAS - 1);
     if (!K && cam != 0) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib_slots: entry %d binds camera %d without a K (the context calibration is camera 0's)", i, cam);
   }
-  for (int i=0;i<n;i++) {                                                // a slot's reference cloud and resident map hold frames of its current size
+  for (int i=0;i<n;i++) {                                                // a slot's reference cloud and resident map hold frames of its current size, built at its current depth
     const TrackerSlot& t = c->slots[slots[i]]; const int cam = cams ? cams[i] : 0;
-    if (!same_size(c, t.cam, cam) && (t.ref_frame != ~0ull || rp_slot_set(c, slots[i])))
-      return ctx_fail(c, SDV_ERR_STATE, "sdv_set_calib_slots: entry %d would move slot %d from camera %d (%dx%d) to camera %d (%dx%d) while its %s holds frames of the old size",
-                      i, slots[i], t.cam, c->cam_w[t.cam], c->cam_h[t.cam], cam, c->cam_w[cam], c->cam_h[cam], t.ref_frame != ~0ull ? "tracker reference" : "map");
+    if (!same_size_depth(c, t.cam, cam) && (t.ref_frame != ~0ull || rp_slot_set(c, slots[i])))
+      return ctx_fail(c, SDV_ERR_STATE, "sdv_set_calib_slots: entry %d would move slot %d from camera %d (%dx%d, %d levels) to camera %d (%dx%d, %d levels) while its %s holds frames of the old camera",
+                      i, slots[i], t.cam, c->cam_w[t.cam], c->cam_h[t.cam], c->cam_levels[t.cam], cam, c->cam_w[cam], c->cam_h[cam], c->cam_levels[cam],
+                      t.ref_frame != ~0ull ? "tracker reference" : "map");
   }
   CK(cudaSetDevice(c->device));
   int lo = (int)c->geom.size(), hi = -1;
@@ -113,6 +114,21 @@ int sdv_set_camera_size(sdv_ctx* c, int cam, int w, int h) { SDV_GUARD_TRK(c);
   return SDV_OK;
 }
 
+// A camera's pyramid depth (pyrLevelsUsed): what its tracker / map slots and jobs use, at most the context's storage depth.  Refused while a slot of the
+// camera holds clouds or a map built at the old depth, and below the selector's 3 levels while a selector slot is bound to it.
+int sdv_set_camera_levels(sdv_ctx* c, int cam, int levels) { SDV_GUARD_TRK(c);
+  if (!c) return SDV_ERR_ARG;
+  if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_camera_levels: camera %d outside 0..%d", cam, SDV_MAX_CAMERAS - 1);
+  if (levels < 1 || levels > c->levels) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_camera_levels: %d levels outside 1..%d (the context's storage depth)", levels, c->levels);
+  if (levels == c->cam_levels[cam]) return SDV_OK;
+  for (size_t s=0;s<c->slots.size();s++) if (c->slots[s].cam == cam && (c->slots[s].ref_frame != ~0ull || rp_slot_set(c, (int)s)))
+    return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_levels: slot %d of camera %d holds a %s built at %d levels", (int)s, cam,
+                    c->slots[s].ref_frame != ~0ull ? "tracker reference" : "map", c->cam_levels[cam]);
+  { int s; if (levels < 3 && sel_cam_bound(c, cam, &s)) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_levels: selector slot %d is bound to camera %d and reads levels 0..2", s, cam); }
+  c->cam_levels[cam] = levels;
+  return SDV_OK;
+}
+
 static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels, const sdv_settings* s_in, int device);
 int sdv_create(const sdv_calib* K, int w, int h, int levels, const sdv_settings* s_in, int device, sdv_ctx** out) {
   if (out) *out = nullptr;
@@ -132,7 +148,7 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
   if (s.track_threads != 64 && s.track_threads != 256) s.track_threads = 128;
   if (s.cluster_size > 16) s.cluster_size = 16;
   c->set = s; c->device = device; c->w = w; c->h = h; c->levels = levels;
-  for (int k=0;k<SDV_MAX_CAMERAS;k++) { c->cam_w[k] = w; c->cam_h[k] = h; }
+  for (int k=0;k<SDV_MAX_CAMERAS;k++) { c->cam_w[k] = w; c->cam_h[k] = h; c->cam_levels[k] = levels; }
   CK(cudaSetDevice(device));
   CK(kernels_init_device()); CK(refine_init_device());      // per-device function attributes (opt-in shared memory, cluster sizes)
   CK(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking)); CK(cudaStreamCreateWithFlags(&c->st_ba, cudaStreamNonBlocking));
@@ -420,6 +436,7 @@ int sdv_frame_download(sdv_ctx* c, uint64_t frame, int lvl, float* dI3_out, floa
   if (!c || lvl < 0 || lvl >= c->levels) return SDV_ERR_ARG;
   CK(cudaSetDevice(c->device));
   FrameDev* f = find_frame(c, frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown frame %llu", (unsigned long long)frame);
+  if (lvl >= c->cam_levels[f->cam]) return ctx_fail(c, SDV_ERR_ARG, "sdv_frame_download: level %d of frame %llu, whose camera %d has %d levels", lvl, (unsigned long long)frame, f->cam, c->cam_levels[f->cam]);
   { int rcj = join_ingest(c); if (rcj) return rcj; }
   { int rct = ensure_texels(c, *f, lvl); if (rct) return rct; }
   int n = (c->cam_w[f->cam]>>lvl)*(c->cam_h[f->cam]>>lvl); float *d3 = nullptr, *da = nullptr;   // the frame's own size
@@ -437,6 +454,7 @@ int sdv_frame_download(sdv_ctx* c, uint64_t frame, int lvl, float* dI3_out, floa
 int sdv_tracker_set_cloud(sdv_ctx* c, int slot, uint64_t ref_frame, int lvl, int n, const float* u, const float* v,
                           const float* idepth, const float* color, double ref_a, double ref_b) { SDV_GUARD_TRK(c);
   if (!c || slot < 0 || slot >= (int)c->slots.size() || lvl < 0 || lvl >= c->levels || n < 0) return SDV_ERR_ARG;
+  if (lvl >= slot_levels(c, slot)) return ctx_fail(c, SDV_ERR_ARG, "sdv_tracker_set_cloud: level %d, but slot %d's camera has %d levels", lvl, slot, slot_levels(c, slot));
   CK(cudaSetDevice(c->device));
   TrackerSlot& t = c->slots[slot];
   if (n > t.cap[lvl]) return ctx_fail(c, SDV_ERR_CAPACITY, "cloud of %d points exceeds capacity %d", n, t.cap[lvl]);
@@ -454,6 +472,7 @@ int sdv_tracker_set_cloud(sdv_ctx* c, int slot, uint64_t ref_frame, int lvl, int
 
 int sdv_tracker_get_cloud(sdv_ctx* c, int slot, int lvl, int* n_out, float* u, float* v, float* idepth, float* color) { SDV_GUARD_TRK(c);
   if (!c || slot < 0 || slot >= (int)c->slots.size() || lvl < 0 || lvl >= c->levels || !n_out) return SDV_ERR_ARG;
+  if (lvl >= slot_levels(c, slot)) return ctx_fail(c, SDV_ERR_ARG, "sdv_tracker_get_cloud: level %d, but slot %d's camera has %d levels", lvl, slot, slot_levels(c, slot));
   CK(cudaSetDevice(c->device));
   TrackerSlot& t = c->slots[slot]; int n = t.npts[lvl]; *n_out = n;
   if (!u || n == 0) return SDV_OK;
@@ -470,7 +489,7 @@ int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const f
   TrackerSlot& t = c->slots[slot];
   FrameDev* f = find_frame(c, ref_frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown ref frame");
   { int rcs = check_frame_slot(c, *f, slot, "sdv_tracker_set_ref"); if (rcs) return rcs; }
-  const int w = c->cam_w[t.cam], h = c->cam_h[t.cam];      // makeCoarseDepthL0 at the slot's size
+  const int w = c->cam_w[t.cam], h = c->cam_h[t.cam], L = c->cam_levels[t.cam];   // makeCoarseDepthL0 at the slot's size, for its camera's pyrLevelsUsed levels
   for (int i=0;i<n;i++) {                                   // the reference would write out of bounds here; we refuse instead
     int u = round_half[i] ? (int)(pts4[4*i]+0.5f) : (int)pts4[4*i], v = round_half[i] ? (int)(pts4[4*i+1]+0.5f) : (int)pts4[4*i+1];
     if (u < 0 || v < 0 || u >= w || v >= h) return ctx_fail(c, SDV_ERR_ARG, "splat %d (%d,%d) outside the image", i, u, v);
@@ -496,20 +515,20 @@ int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const f
       if (c->cd_scalars_host[0] == 0) break;
     }
   }
-  for (int l=1;l<c->levels;l++) launch_cd_pool(c->cd_id[l-1], c->cd_ws[l-1], c->cd_id[l], c->cd_ws[l], w>>l, h>>l, w>>(l-1), c->st);
-  for (int l=0;l<c->levels;l++) {
+  for (int l=1;l<L;l++) launch_cd_pool(c->cd_id[l-1], c->cd_ws[l-1], c->cd_id[l], c->cd_ws[l], w>>l, h>>l, w>>(l-1), c->st);
+  for (int l=0;l<L;l++) {
     launch_cd_dilate(c->cd_id[l], c->cd_ws[l], c->cd_id2[l], c->cd_ws2[l], w>>l, h>>l, l < 2 ? 1 : 0, c->st);
     launch_cd_compact(c->cd_id2[l], c->cd_ws2[l], f->img[l], w>>l, h>>l, c->cd_counts, c->cd_scalars + 1 + l, t.pts[l], t.cap[l], c->st);
   }
   CK(cudaMemcpyAsync(c->cd_scalars_host, c->cd_scalars, 8*sizeof(int), cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st));
   CK(cudaGetLastError());
-  for (int l=0;l<c->levels;l++) if (c->cd_scalars_host[1+l] > t.cap[l]) {
+  for (int l=0;l<L;l++) if (c->cd_scalars_host[1+l] > t.cap[l]) {
     // the emit kernel never wrote past cap[l], but the slot's clouds are now a truncated mix: invalidate the slot instead of leaving it half-updated
     t.ref_frame = ~0ull; t.has_totals = false; for (int k=0;k<c->levels;k++) t.npts[k] = 0;
     return ctx_fail(c, SDV_ERR_CAPACITY, "level %d cloud (%d) exceeds capacity %d (max_ref_points); slot %d has no reference now", l, c->cd_scalars_host[1+l], t.cap[l], slot);
   }
-  for (int l=0;l<c->levels;l++) t.npts[l] = c->cd_scalars_host[1+l];
+  for (int l=0;l<c->levels;l++) t.npts[l] = l < L ? c->cd_scalars_host[1+l] : 0;       // levels past the camera's depth are never read
   t.ref_frame = ref_frame; t.ref_a = ref_a; t.ref_b = ref_b; t.refExposure = f->exposure; t.has_totals = false;
   return SDV_OK;
 }
@@ -517,6 +536,7 @@ int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const f
 // ------------------------------------------------------------------------------------------------ calcRes / calcGSSSE
 int sdv_tracker_calc_res(sdv_ctx* c, int slot, uint64_t new_frame, int lvl, const double T[7], double a, double b, float cutoffTH, double rs_out[6]) { SDV_GUARD_TRK(c);
   if (!c || slot < 0 || slot >= (int)c->slots.size() || lvl < 0 || lvl >= c->levels || !T || !rs_out) return SDV_ERR_ARG;
+  if (lvl >= slot_levels(c, slot)) return ctx_fail(c, SDV_ERR_ARG, "sdv_tracker_calc_res: level %d, but slot %d's camera has %d levels", lvl, slot, slot_levels(c, slot));
   CK(cudaSetDevice(c->device));
   TrackerSlot& t = c->slots[slot];
   FrameDev* f = find_frame(c, new_frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown new frame");
@@ -545,9 +565,11 @@ int sdv_tracker_calc_gs(sdv_ctx* c, int slot, int /*lvl*/, double H[64], double 
 }
 
 // ------------------------------------------------------------------------------------------------ trackNewestCoarse
-int sdv_tracker_track_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* new_frames, double* T_io, double* ab_io, int coarsest,
-                            const double* minRes, double* lastRes, double* flow, int32_t* good, sdv_track_stats* stats) { SDV_GUARD_TRK(c);
-  if (!c || n <= 0 || !slots || !new_frames || !T_io || !ab_io || coarsest < 0 || coarsest >= c->levels || coarsest >= 5) return SDV_ERR_ARG;
+// coarsest: job k starts its LM at coarsest[k]; NULL: at its slot camera's depth - 1 (FullSystem.cpp:421, coarseTracker->trackNewestCoarse(.., pyrLevelsUsed-1, ..)).
+// all_coarsest >= 0 (sdv_tracker_track_batch): that level for every job.  Every level is checked against its job's depth before anything is enqueued.
+static int track_batch_impl(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* new_frames, double* T_io, double* ab_io, const int32_t* coarsest, int all_coarsest,
+                            const double* minRes, double* lastRes, double* flow, int32_t* good, sdv_track_stats* stats) {
+  if (!c || n <= 0 || !slots || !new_frames || !T_io || !ab_io) return SDV_ERR_ARG;
   CK(cudaSetDevice(c->device));
   if (n > c->jobs_cap) {
     cudaFree(c->jobs_dev); cudaFreeHost(c->jobs_host); c->jobs_cap = n;
@@ -561,13 +583,16 @@ int sdv_tracker_track_batch(sdv_ctx* c, int n, const int32_t* slots, const uint6
     if (f->ingest_seq > need_seq) need_seq = f->ingest_seq;
     if (t.ref_frame == ~0ull) return ctx_fail(c, SDV_ERR_STATE, "tracker slot %d has no reference", slots[k]);
     { int rcs = check_frame_slot(c, *f, slots[k], "sdv_tracker_track_batch"); if (rcs) return rcs; }
+    const int L = slot_levels(c, slots[k]), co = all_coarsest >= 0 ? all_coarsest : (coarsest ? coarsest[k] : L - 1);
+    if (co < 0 || co >= L || co >= 5)                                   // CoarseTracker.cpp:672: assert(coarsestLvl < 5 && coarsestLvl < pyrLevelsUsed)
+      return ctx_fail(c, SDV_ERR_ARG, "sdv_tracker_track_batch: job %d starts at level %d, but slot %d's camera has %d levels (and the tracker at most 5)", k, co, slots[k], L);
     TrackJob& J = c->jobs_host[k]; memset(&J, 0, sizeof(J));
     for (int l=0;l<c->levels;l++) { J.img[l] = f->img[l]; J.pts[l] = t.pts[l]; J.npts[l] = t.npts[l]; }
     J.refExposure = t.refExposure; J.newExposure = f->exposure; J.ref_a = t.ref_a; J.ref_b = t.ref_b;
     for (int i=0;i<7;i++) J.T[i] = T_io[7*k+i];
     J.ab[0] = ab_io[2*k]; J.ab[1] = ab_io[2*k+1];
     for (int i=0;i<5;i++) J.minRes[i] = minRes ? minRes[5*k+i] : nan("");
-    J.coarsest = coarsest; J.geom_row = t.geom_row;
+    J.coarsest = co; J.geom_row = t.geom_row;
   }
   { int rcj = join_ingest_upto(c, need_seq); if (rcj) return rcj; }     // only the uploads that built THESE frames: batch k+1's upload keeps streaming
   c->launches += 2;                                                    // descriptor copy kernel + track_cluster_kernel
@@ -588,6 +613,15 @@ int sdv_tracker_track_batch(sdv_ctx* c, int n, const int32_t* slots, const uint6
     if (stats) for (int l=0;l<SDV_PYR_LEVELS;l++) { stats[k].point_evals[l] = J.point_evals[l]; stats[k].iterations[l] = J.iterations[l]; stats[k].accepts[l] = J.accepts[l]; }
   }
   return SDV_OK;
+}
+int sdv_tracker_track_batch_levels(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* new_frames, double* T_io, double* ab_io, const int32_t* coarsest,
+                                   const double* minRes, double* lastRes, double* flow, int32_t* good, sdv_track_stats* stats) { SDV_GUARD_TRK(c);
+  return track_batch_impl(c, n, slots, new_frames, T_io, ab_io, coarsest, -1, minRes, lastRes, flow, good, stats);
+}
+int sdv_tracker_track_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* new_frames, double* T_io, double* ab_io, int coarsest,
+                            const double* minRes, double* lastRes, double* flow, int32_t* good, sdv_track_stats* stats) { SDV_GUARD_TRK(c);
+  if (!c || coarsest < 0 || coarsest >= c->levels || coarsest >= 5) return SDV_ERR_ARG;
+  return track_batch_impl(c, n, slots, new_frames, T_io, ab_io, nullptr, coarsest, minRes, lastRes, flow, good, stats);
 }
 int sdv_tracker_track(sdv_ctx* c, int slot, uint64_t new_frame, double T_io[7], double ab_io[2], int coarsest, const double minRes[5],
                       double lastRes[5], double flow[3], int* good, sdv_track_stats* stats) { SDV_GUARD_TRK(c);

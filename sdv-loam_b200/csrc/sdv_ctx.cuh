@@ -45,6 +45,7 @@ struct sdv_ctx {
   static constexpr int kIngRing = 8; cudaEvent_t ev_ing[kIngRing], ev_cp[2]; long long ingest_seq = 0, seq_waited = 0;
   int w, h, levels; sdv_settings set;
   int cam_w[SDV_MAX_CAMERAS], cam_h[SDV_MAX_CAMERAS];                  // rectified size per camera (sdv_set_camera_size); camera 0 is always w x h
+  int cam_levels[SDV_MAX_CAMERAS];                                     // pyramid depth per camera (sdv_set_camera_levels), 1..levels: what its slots and jobs use; frames are stored at `levels`
   sdv::TrackConst tc; sdv::TrackConst* tc_dev;
   // geometry table (CoarseTracker::makeK per K): row 0 = the context calibration (sdv_set_calib), row 1 + s = tracker slot s's own K (sdv_set_calib_slots).
   // Host mirror + device copy; every consumer indexes it with TrackerSlot::geom_row, none derives the geometry from K itself.
@@ -93,7 +94,11 @@ inline bool frame_pinned(const sdv_ctx* c, uint64_t id) { return c->pins.find(id
 int  join_ingest(sdv_ctx* c);                  // compute stream waits for every ingest enqueued so far
 int  join_ingest_upto(sdv_ctx* c, long long seq);   // ... for ingest calls <= seq only (frames carry their ingest_seq)
 inline const GeomRow& slot_geom(const sdv_ctx* c, int slot) { return c->geom[c->slots[slot].geom_row]; }   // the K a tracker / map slot uses, at every level
+// frames are depth-agnostic (stored at the context's depth): a frame fits a camera of the same size.  A tracker / map slot holds clouds built at its camera's
+// depth as well: it may only keep them on a camera of the same size and depth.
 inline bool same_size(const sdv_ctx* c, int cam_a, int cam_b) { return c->cam_w[cam_a] == c->cam_w[cam_b] && c->cam_h[cam_a] == c->cam_h[cam_b]; }
+inline bool same_size_depth(const sdv_ctx* c, int cam_a, int cam_b) { return same_size(c, cam_a, cam_b) && c->cam_levels[cam_a] == c->cam_levels[cam_b]; }
+inline int slot_levels(const sdv_ctx* c, int slot) { return c->cam_levels[c->slots[slot].cam]; }   // pyrLevelsUsed of a tracker / map slot
 int  check_frame_slot(sdv_ctx* c, const FrameDev& f, int slot, const char* who);   // SDV_ERR_ARG (with a message) when frame f's size differs from slot's
 int  check_frame_cam(sdv_ctx* c, const FrameDev& f, int cam, const char* who);     // ... from camera cam's (keyframe-rate stages: the job names its camera)
 bool sel_cam_bound(const sdv_ctx* c, int cam, int* slot);                          // a selector slot (*slot) is bound to camera cam (sdv_selector_set_slot_cams)

@@ -63,7 +63,6 @@ extern "C" int sdv_track_hypothesis(const sdv_track_new_coarse_io* io, int i, do
 extern "C" int sdv_track_new_coarse_batch(sdv_ctx* c, int n, sdv_track_new_coarse_io* io, const int32_t* cell_order, int max_matches) {
   if (!c || n <= 0 || !io) return SDV_ERR_ARG;
   const float setting_reTrackThreshold = 1.5f;                                           // settings.cpp:130
-  const int coarsest = c->levels - 1;
   struct St { TryGen gen; int ntries; SE3d try0; double achieved[5]; bool haveOneGood, done; SE3d lastF_2_fh; double aff[2]; double flow[3]; int tryIterations; };
   std::vector<St> st(n);
   size_t maxTries = 0;
@@ -77,7 +76,8 @@ extern "C" int sdv_track_new_coarse_batch(sdv_ctx* c, int n, sdv_track_new_coars
     slots.resize(m); frames.resize(m); good.resize(m); T.resize(7*m); ab.resize(2*m); minRes.resize(5*m); lastRes.resize(5*m); flow.resize(3*m);
     for (int a=0;a<m;a++) { const int k = act[a]; slots[a] = io[k].slot; frames[a] = io[k].frame; se3_to7(i == 0 ? st[k].try0 : make_try(st[k].gen, (int)i), &T[7*a]);
       ab[2*a] = io[k].aff_last[0]; ab[2*a+1] = io[k].aff_last[1]; for (int l=0;l<5;l++) minRes[5*a+l] = st[k].achieved[l]; }
-    int rc = sdv_tracker_track_batch(c, m, slots.data(), frames.data(), T.data(), ab.data(), coarsest, minRes.data(), lastRes.data(), flow.data(), good.data(), nullptr);
+    // every sequence starts at its own slot camera's pyrLevelsUsed-1 (:421, :429)
+    int rc = sdv_tracker_track_batch_levels(c, m, slots.data(), frames.data(), T.data(), ab.data(), nullptr, minRes.data(), lastRes.data(), flow.data(), good.data(), nullptr);
     if (rc) return rc;
     for (int a=0;a<m;a++) { const int k = act[a]; St& s = st[k]; s.tryIterations++;
       const double* lr = &lastRes[5*a];

@@ -38,8 +38,9 @@ struct RpJob {
 };
 static_assert(sizeof(RpJob) == 536, "RpJob keeps its size: the camera byte sits beside the one-byte error flag");
 // K, Ki: the context calibration (geometry row 0), as launch constants.  cam_w/cam_h: level-0 size per camera (the job's grid is ceil(w/25) x ceil(h/25));
-// ncols, ncells: the context grid, which strides the per-job outputs and numbers cell_order.
-struct RpConst { double K[9], Ki[9]; int cam_w[SDV_MAX_CAMERAS], cam_h[SDV_MAX_CAMERAS]; int levels, ncols, ncells; };
+// cam_levels: pyramid depth per camera (getBestSearchLevel's cap is the job camera's depth - 1); ncols, ncells: the context grid, which strides the per-job
+// outputs and numbers cell_order.
+struct RpConst { double K[9], Ki[9]; int cam_w[SDV_MAX_CAMERAS], cam_h[SDV_MAX_CAMERAS], cam_levels[SDV_MAX_CAMERAS]; int ncols, ncells; };
 struct RpScratch { double2* cand_px; float* cand_key; int* cand_cell; unsigned long long* list;   // list: per cell, (key bits << 32) | (frame rank << 27) | point index
                    int* count; int* begin; int* cursor; int* out_pt; double2* out_px;
                    double* xf; };   // xf[job][host][14]: camToWorld_host^-1 and T_cur_ref = camToWorld_cur^-1 * camToWorld_host (7 doubles each), built by rp_project_kernel
@@ -142,7 +143,8 @@ template <bool OWN_K>
 __device__ bool find_match_direct(const RpJob& jb, const RpConst& C, const sdv_map_pt& pt, double2& px_io, RpWarpSmem& sm, const int lane, const double* __restrict__ xf) {
   const double* __restrict__ K = OWN_K ? jb.K : C.K; const double* __restrict__ Ki = OWN_K ? jb.Ki : C.Ki;
   const MapDev* __restrict__ m = jb.map;
-  const int w0 = C.cam_w[jb.cam], h0 = C.cam_h[jb.cam];            // the job's level-0 size (read here: passing it in from the kernel adds spills)
+  // the job's level-0 size and getBestSearchLevel's cap (read here: passing them in from the kernel, or reading the depth where it is used, adds spills)
+  const int w0 = C.cam_w[jb.cam], h0 = C.cam_h[jb.cam], max_level = C.cam_levels[jb.cam] - 1;
   int ref;
   if (jb.nH <= 2) { if (!jb.backup) ref = 0; else if (jb.cur_kf_index == 0) ref = 1; else if (jb.cur_kf_index == 1) ref = 0; else return false; }
   else ref = pt.host;
@@ -161,7 +163,7 @@ __device__ bool find_match_direct(const RpJob& jb, const RpConst& C, const sdv_m
     double c0[3], c1[3], c2[3], pc[2], pu[2], pv[2];
     xform(Tcr, ptRef, c0); pixel_from_cam(K, c0, pc); xform(Tcr, du, c1); pixel_from_cam(K, c1, pu); xform(Tcr, dv, c2); pixel_from_cam(K, c2, pv);
     A[0] = (pu[0]-pc[0])/hp; A[2] = (pu[1]-pc[1])/hp; A[1] = (pv[0]-pc[0])/hp; A[3] = (pv[1]-pc[1])/hp; }
-  int level = 0; { double D = A[0]*A[3] - A[2]*A[1]; while (D > 3.0 && level < C.levels-1) { level += 1; D *= 0.25; } }      // getBestSearchLevel :39-51
+  int level = 0; { double D = A[0]*A[3] - A[2]*A[1]; while (D > 3.0 && level < max_level) { level += 1; D *= 0.25; } }   // getBestSearchLevel :39-51, :268
   // warpAffine :53-86 (halfpatch 5 -> 10x10 patch with border), values truncated to uint8
   { const double det = A[0]*A[3] - A[2]*A[1], invdet = 1.0/det;
     const float a00 = (float)(A[3]*invdet), a10 = (float)(-A[2]*invdet), a01 = (float)(-A[1]*invdet), a11 = (float)(A[0]*invdet);
@@ -322,7 +324,7 @@ struct RpState { std::vector<MapSlot> maps; void* dev = nullptr; void* host = nu
 static void rp_job_K(const LevelGeom& g, double* K, double* Ki);
 static RpState* rp_state(sdv_ctx* c) {
   if (!c->rp) { c->rp = new RpState(); c->rp->maps.resize(c->slots.size()); RpConst& C = c->rp->C;
-    C.levels = c->levels; C.ncols = grid_dim(c->w); C.ncells = C.ncols*grid_dim(c->h); }
+    C.ncols = grid_dim(c->w); C.ncells = C.ncols*grid_dim(c->h); }
   return c->rp;
 }
 bool rp_slot_set(const sdv_ctx* c, int slot) { return c->rp && slot < (int)c->rp->maps.size() && c->rp->maps[slot].set; }
@@ -381,7 +383,7 @@ struct RpRun { RpScratch S; RpJob* jobs_dev; RpJob* jobs_host; int32_t* h_opt; d
 static int rp_launch(sdv_ctx* c, int n_jobs, const int32_t* slots, const uint64_t* cur_frames, const double* cur_T7, const double* cur_ab,
                      const int32_t* cur_kf_index, const int32_t* only_host, const int32_t* backup, RpRun& R) {
   RpState* st = rp_state(c); rp_job_K(c->geom[0].g[0], st->C.K, st->C.Ki);
-  for (int k=0;k<SDV_MAX_CAMERAS;k++) { st->C.cam_w[k] = c->cam_w[k]; st->C.cam_h[k] = c->cam_h[k]; }
+  for (int k=0;k<SDV_MAX_CAMERAS;k++) { st->C.cam_w[k] = c->cam_w[k]; st->C.cam_h[k] = c->cam_h[k]; st->C.cam_levels[k] = c->cam_levels[k]; }
   const RpConst& C = st->C;
   long long totalP = 0; int maxP = 1;
   for (int k=0;k<n_jobs;k++) { if (slots[k] < 0 || slots[k] >= (int)st->maps.size() || !st->maps[slots[k]].set) return ctx_fail(c, SDV_ERR_STATE, "reproject job %d: map slot %d not set", k, slots[k]);

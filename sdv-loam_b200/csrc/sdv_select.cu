@@ -46,6 +46,7 @@ extern "C" {
 int sdv_selector_init(sdv_ctx* c, const uint8_t* random_pattern, int n_slots) { SDV_GUARD_TRK(c);
   if (!c || !random_pattern || n_slots < 1) return SDV_ERR_ARG;
   if (c->levels < 3) return ctx_fail(c, SDV_ERR_ARG, "selector_init: the selector reads pyramid levels 0..2 (context has %d levels)", c->levels);
+  if (c->cam_levels[0] < 3) return ctx_fail(c, SDV_ERR_ARG, "selector_init: the selector reads pyramid levels 0..2 and binds every slot to camera 0, which has %d levels", c->cam_levels[0]);
   CK(cudaSetDevice(c->device));
   sel_destroy(c);
   SelState* s = new SelState(); c->sel = s;
@@ -63,6 +64,7 @@ int sdv_selector_set_slot_cams(sdv_ctx* c, int n, const int32_t* slots, const in
   for (int i = 0; i < n; i++) {
     if (slots[i] < 0 || slots[i] >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "selector_set_slot_cams: entry %d names slot %d of %d", i, slots[i], (int)s->slots.size());
     if (cams[i] < 0 || cams[i] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "selector_set_slot_cams: entry %d names camera %d (valid: 0..%d)", i, cams[i], SDV_MAX_CAMERAS - 1);
+    if (c->cam_levels[cams[i]] < 3) return ctx_fail(c, SDV_ERR_ARG, "selector_set_slot_cams: entry %d names camera %d of %d levels (the selector reads levels 0..2)", i, cams[i], c->cam_levels[cams[i]]);
   }
   CK(cudaSetDevice(c->device));
   for (int i = 0; i < n; i++) { const int sl = slots[i];
