@@ -322,6 +322,45 @@ int  sdv_immature_optimize_batch(sdv_ctx* c, int n_groups, const int32_t* pt_beg
 int  sdv_immature_optimize_batch_cams(sdv_ctx* c, int n_groups, const int32_t* pt_begin, const int32_t* tgt_begin, const uint64_t* target_frames, const float* pre14,
                                       const float* calib6, const int32_t* cams, int min_obs, const sdv_immature_pt* pts, const uint8_t* is_from_sensor, int res_stride,
                                       int32_t* status_out, float* idepth_out, int32_t* res_state_out);
+/* ---- device-resident immature points: FrameHessian::immaturePoints (HessianBlocks.h) kept on the device, one block per host keyframe, keyed by its frame handle.
+ * The records are made on the device (makeNewTraces), traced there every frame (traceNewCoarse) and never need to visit the host; the entries above copy every
+ * record to the device and back per call.  A block holds, per point, the sdv_immature_pt record and the sdv_immature_meta record below, in the order of
+ * host->immaturePoints.  Tracker call domain.  The pool grows at keyframe rate only (set, make_new_traces_store); the per-frame trace never allocates.
+ * A host with no block returns SDV_ERR_NOFRAME from every entry that names it; a refused call changes no block.
+ * sdv_immature_store_set    replaces host_frame's block by pts[n] (+ meta[n]; NULL: my_type 1, type -1, not from the sensor); n == 0 leaves an empty block.
+ *                           The frame need not be resident: the records carry all the trace reads of their host.
+ * sdv_immature_store_count  counts_out[i] = size of hosts[i]'s block, for n hosts.
+ * sdv_immature_store_get    reads host_frame's block back in its current order; *n_out = its size (also when SDV_ERR_CAPACITY: cap < size, nothing copied);
+ *                           pts_out / meta_out may each be NULL.
+ * sdv_immature_store_drop   drops the blocks of n hosts: the keyframe leaves the window (FullSystem::marginalizeFrame -> FrameHessian::release deletes its immaturePoints,
+ *                           HessianBlocks.cpp:90-105). */
+typedef struct { float my_type; int32_t type; int32_t isFromSensor; float idepth_fromSensor; } sdv_immature_meta;   /* ImmaturePoint members of the activation / PointHessian ctor */
+int  sdv_immature_store_set(sdv_ctx* c, uint64_t host_frame, int n, const sdv_immature_pt* pts, const sdv_immature_meta* meta);
+int  sdv_immature_store_count(sdv_ctx* c, int n, const uint64_t* hosts, int32_t* counts_out);
+int  sdv_immature_store_get(sdv_ctx* c, uint64_t host_frame, int cap, sdv_immature_pt* pts_out, sdv_immature_meta* meta_out, int32_t* n_out);
+int  sdv_immature_store_drop(sdv_ctx* c, int n, const uint64_t* hosts);
+/* FullSystem::traceNewCoarse (FullSystem.cpp:519-552) on the store: group g traces every point of hosts[g]'s block into frames[g] (camera cams[g]'s size; NULL: camera 0)
+ * with KRKi9[9g..], Kt3[3g..], aff2[2g..] as sdv_immature_trace_batch_cams takes them (:534-538); ImmaturePoint::traceOn (ImmaturePoint.cpp:50-352) updates the records in
+ * place.  Groups of several sequences and cameras go into one launch; a host may appear in one group per call (else SDV_ERR_ARG).  counts_out (may be NULL):
+ * counts_out[6g + s] = the points of group g whose lastTraceStatus is s afterwards (0 GOOD .. 5 UNINITIALIZED: trace_good, trace_oob, ... of :543-548).
+ * No record crosses PCIe; the call returns without waiting for the device unless counts_out is given.  Until that kernel has run, re-ingesting a traced frame
+ * (or a frame into its storage after sdv_frame_release) is ordered after it on the device, and releasing an adopted frame waits for it on the host. */
+/* void FullSystem::activatePointsMT() (FullSystem.cpp:598-720) on the store, after the currentMinActDist update (:571-592, which reads ef->nPoints and stays with the caller),
+ * for n sequences.  Sequence j's window is hosts[host_begin[j] .. host_begin[j+1]) in frameHessians order, newest last (1..16 keyframes, at most SDV_MAX_FRAMES_WINDOW
+ * targets each); per window host: flagged[] = flaggedForMarginalization, cKRKi9 / cKt3 = K[1] R K[0]^-1, K[1] t of host -> newest (:606-610).  The ACTIVE-point sources
+ * of the distance map (src_host_begin per sequence, src_pt_begin, KRKi9, Kt3, uvid) and min_act_dist[j] as sdv_activate_select_batch_cams takes them; pre14 = the
+ * (host, target) rows of sdv_immature_optimize_batch, host-major over each window, targets in window order without the host; calib6[6j..]; cams[j] (NULL: camera 0).
+ * On the device: the deletion / canActivate filter (:612-645, setting_minTraceQuality 3), the distance map and walk (:647-671; a candidate projecting outside level 1 is
+ * deleted), optimizeImmaturePoint with minObs 1 on the accepted ones, the post pass (:683-707: activated, -1 and OOB points leave the store) and the swap-with-back
+ * compaction of every host's block (:709-720).  Out, in toOptimize order, for the activated points only: act_host (index into hosts), act_idx (idxInImmaturePoints before
+ * the compaction), the record and meta, act_idepth, act_res_state[k*SDV_MAX_FRAMES_WINDOW + t] (state of the residual to target t, -1 padding); n_act_out[j] per sequence;
+ * counts_out[g] (may be NULL) = host g's block size after the compaction.  More than cap activated points return SDV_ERR_CAPACITY and change nothing. */
+int  sdv_activate_points_store_batch(sdv_ctx* c, int n, const int32_t* host_begin, const uint64_t* hosts, const int32_t* flagged, const float* cKRKi9, const float* cKt3,
+                                     const int32_t* src_host_begin, const int32_t* src_pt_begin, const float* KRKi9, const float* Kt3, const float* uvid, const float* min_act_dist,
+                                     const float* pre14, const float* calib6, const int32_t* cams, int cap, int32_t* n_act_out, int32_t* act_host, int32_t* act_idx,
+                                     sdv_immature_pt* act_pts, sdv_immature_meta* act_meta, float* act_idepth, int32_t* act_res_state, int32_t* counts_out);
+int  sdv_immature_trace_store_batch(sdv_ctx* c, int n_groups, const uint64_t* hosts, const uint64_t* frames, const int32_t* cams, const float* KRKi9, const float* Kt3,
+                                    const float* aff2, int32_t* counts_out);
 
 /* frames + calibration + marginalisation prior:  EnergyFunctional::insertFrame :365-398, setAdjointsF :21-71, HM/bM :88-89.
  * state10 / state_zero10 = FrameHessian::state / state_zero (Vec10: 6 pose, a, b, 2 unused; HessianBlocks.h:141-175),
@@ -432,6 +471,12 @@ int  sdv_selector_make_maps_batch(sdv_ctx* c, int n, const int32_t* slots, const
  * n_out[j] = how many; num_points2[2j..] = {numPointLidar, numPointMonocular}.  SDV_ERR_CAPACITY when cap is too small. */
 int  sdv_make_new_traces_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const float* density_lidar,
                                const float* density_dense, const int32_t* add_feature_point, int cap, sdv_new_trace* out, sdv_immature_pt* imm_out, int32_t* n_out, int32_t* num_points2);
+/* The same with the points deposited into the immature-point store (sdv_immature_store_set) instead of returned: job j's points, in creation order, replace the block of
+ * frames[j], with what the host does around the call in the reference applied on the device — for LiDAR points idepth_fromSensor = 1.0/depth and
+ * idepth_min = idepth_max = idepth_fromSensor (FullSystem.cpp:1313-1317), lastTraceStatus = IPS_SKIPPED (makeKeyFrame, :1080-1084); meta = {my_type, type, isFromSensor,
+ * idepth_fromSensor} of the sdv_new_trace record.  n_out / num_points2 as above; cap bounds the points of a job as above.  A frame named twice returns SDV_ERR_ARG. */
+int  sdv_make_new_traces_store_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const float* density_lidar,
+                                     const float* density_dense, const int32_t* add_feature_point, int cap, int32_t* n_out, int32_t* num_points2);
 /* The selection half of void FullSystem::activatePointsMT() for n sequences: CoarseDistanceMap::makeDistanceMap from the ACTIVE points of the other keyframes, then the
  * candidate walk :600-671 with addIntoDistFinal after every accept.  Sequence j owns source keyframes host_begin[j] .. host_begin[j+1] (their points: uvid rows
  * pt_begin[k] .. pt_begin[k+1] = {u, v, idepth_scaled}; KRKi9 / Kt3 per keyframe = K[1] R K[0]^-1, K[1] t of host -> newest, FullSystem.cpp:606-608) and candidate

@@ -306,6 +306,47 @@ int shim_activateSelect(const ActivationInputs& in, std::vector<int32_t>& decisi
                                    in.cand4.data(), &in.currentMinActDist, decision.data(), nullptr);   // 1 -> toOptimize.push_back(ph), 0 -> skipped, -1 -> delete ph (:653-669)
 }
 
+// ------------------------------------------------------------------------------------------------ device-resident immature points (sdv_immature_store_*)
+// host->immaturePoints keeps only a count; the records live in the context's store block of the host, keyed by its frame id.
+struct StoreHost { FrameHessian* host; int32_t cam; int32_t nImmature; Mat33f KRKi; Vec3f Kt; Vec2f aff; };    // per host: what :532-538 computes
+// makeKeyFrame -> makeNewTraces (FullSystem.cpp:1273-1356) + the SKIPPED loop (:1080-1084): the new keyframe's points go straight into its block
+int shim_makeNewTraces_store(FrameHessian* newFrame, const LidarRig& fsys, int32_t slot, const std::vector<double>& vCloudPixel3, int32_t& nImmature) {
+  const int32_t cloud_begin[2] = {0, (int32_t)(vCloudPixel3.size()/3)}, add = fsys.addFeaturePoint ? 1 : 0; const uint64_t id = (uint64_t)newFrame->shell->id;
+  const int lidarArea = (fsys.right - fsys.left)*(fsys.down - fsys.up), imageArea = wG[0]*hG[0];
+  const float dl = ((float)lidarArea/(float)imageArea) * setting_desiredImmatureDensity, dd = setting_desiredImmatureDensity; int32_t num[2];
+  return sdv_make_new_traces_store_batch(gpu, 1, &slot, &id, cloud_begin, vCloudPixel3.data(), &dl, &dd, &add, 1 << 14, &nImmature, num);
+}
+// FullSystem::traceNewCoarse (FullSystem.cpp:519-552): every host of the window in one launch, nothing copied; counts only when the caller logs them (:543-548)
+int shim_traceNewCoarse_store(FrameHessian* fh, const std::vector<StoreHost>& hosts, std::vector<int32_t>* counts6) {
+  std::vector<uint64_t> hid, frames; std::vector<int32_t> cams; std::vector<float> KRKi, Kt, aff;
+  for (const StoreHost& h : hosts) {
+    hid.push_back((uint64_t)h.host->shell->id); frames.push_back((uint64_t)fh->shell->id); cams.push_back(h.cam);
+    KRKi.insert(KRKi.end(), h.KRKi.m, h.KRKi.m + 9); for (int i = 0; i < 3; i++) Kt.push_back((float)h.Kt[i]); aff.push_back(h.aff.v[0]); aff.push_back(h.aff.v[1]);
+  }
+  if (counts6) counts6->resize(6*hosts.size());
+  return sdv_immature_trace_store_batch(gpu, (int)hosts.size(), hid.data(), frames.data(), cams.data(), KRKi.data(), Kt.data(), aff.data(), counts6 ? counts6->data() : nullptr);
+}
+// FullSystem::marginalizeFrame -> FrameHessian::release (HessianBlocks.cpp:90-105): the keyframe's immature points go with it
+int shim_drop_immatures(FrameHessian* fh) { const uint64_t id = (uint64_t)fh->shell->id; return sdv_immature_store_drop(gpu, 1, &id); }
+// read-back of a block (debugging, plotting): the records in host->immaturePoints order
+int shim_read_immatures(FrameHessian* host, std::vector<sdv_immature_pt>& pts, std::vector<sdv_immature_meta>& meta) {
+  const uint64_t id = (uint64_t)host->shell->id; int32_t n = 0; int rc = sdv_immature_store_count(gpu, 1, &id, &n); if (rc) return rc;
+  pts.resize(n); meta.resize(n); return sdv_immature_store_get(gpu, id, n, pts.data(), meta.data(), &n);
+}
+// activatePointsMT (FullSystem.cpp:598-720) on the store for one window; the caller builds PointHessians from the activated records
+int shim_activatePoints_store(const std::vector<uint64_t>& window, const std::vector<int32_t>& flagged, const ActivationInputs& in, const std::vector<float>& pre14, const float calib6[6],
+                              std::vector<sdv_immature_pt>& act, std::vector<float>& idepth, std::vector<int32_t>& res_state, std::vector<int32_t>& counts) {
+  const int32_t host_begin[2] = {0, (int32_t)window.size()}, src_host_begin[2] = {0, (int32_t)in.pt_begin.size() - 1}; const int cap = 4096; int32_t n_act = 0;
+  std::vector<int32_t> ah(cap), ai(cap); std::vector<sdv_immature_meta> am(cap); act.resize(cap); idepth.resize(cap); res_state.resize((size_t)cap*SDV_MAX_FRAMES_WINDOW); counts.resize(window.size());
+  int rc = sdv_activate_points_store_batch(gpu, 1, host_begin, window.data(), flagged.data(), in.cKRKi9.data(), in.cKt3.data(), src_host_begin, in.pt_begin.data(), in.KRKi9.data(), in.Kt3.data(),
+                                           in.uvid.data(), &in.currentMinActDist, pre14.data(), calib6, nullptr, cap, &n_act, ah.data(), ai.data(), act.data(), am.data(), idepth.data(),
+                                           res_state.data(), counts.data());
+  act.resize(n_act); idepth.resize(n_act); return rc;
+}
+int shim_set_immatures(FrameHessian* host, const std::vector<sdv_immature_pt>& pts, const std::vector<sdv_immature_meta>& meta) {
+  return sdv_immature_store_set(gpu, (uint64_t)host->shell->id, (int)pts.size(), pts.data(), meta.empty() ? nullptr : meta.data());
+}
+
 // referenced so that -Wunused does not hide a missing call path
 int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const Undistort* u, const uint8_t* raw) {
   std::vector<int32_t> sel, st; Vec5 mr{}; SE3 T; AffLight a;
@@ -319,6 +360,10 @@ int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const 
   PixelSelector ps; LidarRig rig{}; std::vector<double> px; std::vector<sdv_new_trace> tr; std::vector<sdv_immature_pt> rc2; ActivationInputs ai; ai.pt_begin = {0}; ai.cand_begin = {0}; ai.currentMinActDist = 2;
   rc |= shim_selector_ctor(ps) | shim_lidarCloudHandler(rig, nullptr, 0, px) | shim_makeNewTraces_whole(fh, rig, px, tr, rc2) | shim_activateSelect(ai, st);
   { KittiKeyframe k{}; k.slot = 1; k.cam = 1; rc |= shim_kitti_keyframe(k, 1500.f, tr, rc2, st); }
+  { std::vector<StoreHost> sh; std::vector<sdv_immature_meta> me; int32_t ni = 0;
+    rc |= shim_makeNewTraces_store(fh, rig, 0, px, ni) | shim_traceNewCoarse_store(fh, sh, &st) | shim_read_immatures(fh, rc2, me) | shim_set_immatures(fh, rc2, me) | shim_drop_immatures(fh);
+    std::vector<float> idp2; std::vector<int32_t> rs2, cn2; const float cal6[6] = {1, 1, 0, 0, 1, 1};
+    rc |= shim_activatePoints_store({(uint64_t)fh->shell->id}, {0}, ai, {}, cal6, rc2, idp2, rs2, cn2); }
   fs.optimize(6); fs.set_map(0); fs.handover(sel, st); fs.trackNewCoarse(fh); fs.refine_only(fh); shim_frame_destructor(fh);
   return rc;
 }

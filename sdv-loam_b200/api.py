@@ -108,6 +108,14 @@ def _load():
     L.sdv_immature_init_cam.argtypes = [_vp, C.c_int, C.c_uint64, C.c_int, _i32p, _vp]
     L.sdv_immature_trace_batch_cams.argtypes = [_vp, C.c_int, _u64p, _vp, _i32p, _f32p, _f32p, _f32p, _vp, _vp]
     L.sdv_immature_optimize_batch_cams.argtypes = [_vp, C.c_int, _i32p, _i32p, _u64p, _f32p, _f32p, _vp, C.c_int, _vp, _vp, C.c_int, _i32p, _f32p, _i32p]
+    L.sdv_immature_store_set.argtypes = [_vp, C.c_uint64, C.c_int, _vp, _vp]
+    L.sdv_immature_store_count.argtypes = [_vp, C.c_int, _u64p, _i32p]
+    L.sdv_immature_store_get.argtypes = [_vp, C.c_uint64, C.c_int, _vp, _vp, C.POINTER(C.c_int32)]
+    L.sdv_immature_store_drop.argtypes = [_vp, C.c_int, _u64p]
+    L.sdv_immature_trace_store_batch.argtypes = [_vp, C.c_int, _u64p, _u64p, _vp, _f32p, _f32p, _f32p, _vp]
+    L.sdv_activate_points_store_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _i32p, _f32p, _f32p, _i32p, _i32p, _vp, _vp, _vp, _f32p, _f32p, _f32p, _vp, C.c_int, _i32p,
+                                                  _vp, _vp, _vp, _vp, _vp, _vp, _vp]
+    L.sdv_make_new_traces_store_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _i32p, _vp, _f32p, _f32p, _i32p, C.c_int, _i32p, _i32p]
     return L
 
 
@@ -677,6 +685,69 @@ def optimizeImmaturePointBatch(ctx: Context, pt_begin, tgt_begin, target_frame_i
     return st, idp, rs
 
 
+IMMATURE_META_DTYPE = np.dtype([("my_type", np.float32), ("type", np.int32), ("isFromSensor", np.int32), ("idepth_fromSensor", np.float32)])
+
+
+class ImmatureStore:
+    """host->immaturePoints of every keyframe of a context, kept on the device: one block per host keyframe, keyed by its frame id (sdv_immature_store_*).
+    The records never need to come back to the host: PixelSelector.makeNewTracesStore fills a block, traceStoreBatch traces blocks in place, drop forgets them."""
+
+    def __init__(self, ctx: Context):
+        self.ctx = ctx
+
+    def set(self, host_frame_id: int, pts, meta=None):
+        """replace the block of host_frame_id by pts (IMMATURE_PT_DTYPE) and meta (IMMATURE_META_DTYPE; None: my_type 1, type -1, not from the sensor)"""
+        p = np.ascontiguousarray(pts, IMMATURE_PT_DTYPE); m = None if meta is None else np.ascontiguousarray(meta, IMMATURE_META_DTYPE)
+        assert m is None or len(m) == len(p)
+        self.ctx._ck(LIB.sdv_immature_store_set(self.ctx.p, int(host_frame_id), len(p), p.ctypes.data if len(p) else None, None if m is None else m.ctypes.data))
+
+    def count(self, host_frame_ids):
+        h = np.ascontiguousarray(np.atleast_1d(host_frame_ids), np.uint64); o = np.zeros(len(h), np.int32)
+        self.ctx._ck(LIB.sdv_immature_store_count(self.ctx.p, len(h), h, o)); return o
+
+    def get(self, host_frame_id: int):
+        """(records, meta) of the block of host_frame_id in its current order"""
+        n = self.count([host_frame_id])[0]; P = np.zeros(n, IMMATURE_PT_DTYPE); M = np.zeros(n, IMMATURE_META_DTYPE); no = C.c_int32(0)
+        self.ctx._ck(LIB.sdv_immature_store_get(self.ctx.p, int(host_frame_id), int(n), P.ctypes.data, M.ctypes.data, C.byref(no))); return P, M
+
+    def drop(self, host_frame_ids):
+        h = np.ascontiguousarray(np.atleast_1d(host_frame_ids), np.uint64); self.ctx._ck(LIB.sdv_immature_store_drop(self.ctx.p, len(h), h))
+
+
+def traceStoreBatch(ctx: Context, host_frame_ids, frame_ids, KRKi, Kt, aff, cams=None, counts=False):
+    """FullSystem::traceNewCoarse on the store: group g traces every point of host_frame_ids[g]'s block into frame_ids[g] (camera cams[g]; None: camera 0), in place.
+    counts=True waits for the device and returns the (n, 6) per-status counts after the trace (column s: lastTraceStatus == s); else returns None at once."""
+    ng = len(host_frame_ids); cm = Context._cams(cams, ng); co = np.zeros((ng, 6), np.int32) if counts else None
+    ctx._ck(LIB.sdv_immature_trace_store_batch(ctx.p, ng, np.ascontiguousarray(host_frame_ids, np.uint64), np.ascontiguousarray(frame_ids, np.uint64), None if cm is None else cm.ctypes.data,
+                                               np.ascontiguousarray(KRKi, np.float32).reshape(-1), np.ascontiguousarray(Kt, np.float32).reshape(-1),
+                                               np.ascontiguousarray(aff, np.float32).reshape(-1), None if co is None else co.ctypes.data))
+    return co
+
+
+def activateStoreBatch(ctx: Context, seqs, cams=None, cap=1 << 16):
+    """FullSystem::activatePointsMT (FullSystem.cpp:598-720) on the ImmatureStore for several sequences.  seqs: dicts with hosts (window keyframe ids, newest last), flagged,
+    cKRKi / cKt (per host), the distance-map sources pt_begin / KRKi / Kt / uvid as activateSelectBatch takes them, minActDist, pre14 ((host, target) rows, host-major,
+    targets = the window without the host), calib6.  -> dict of per-sequence lists: host (index into the sequence's hosts), idx, pts, meta, idepth, res_state (k, nH-1),
+    and counts (block sizes after the compaction)"""
+    f = lambda a, t: np.ascontiguousarray(a, t); n = len(seqs); P = packActivation(seqs, cams)
+    hb = f(np.concatenate([[0], np.cumsum([len(q["hosts"]) for q in seqs])]), np.int32); NH = int(hb[-1])
+    hosts = f(np.concatenate([q["hosts"] for q in seqs]), np.uint64); fl = f(np.concatenate([q["flagged"] for q in seqs]), np.int32)
+    cA = f(np.concatenate([np.asarray(q["cKRKi"], np.float32).reshape(-1, 9) for q in seqs]), np.float32); cB = f(np.concatenate([np.asarray(q["cKt"], np.float32).reshape(-1, 3) for q in seqs]), np.float32)
+    pre = f(np.concatenate([np.asarray(q["pre14"], np.float32).reshape(-1, 14) for q in seqs] + [np.zeros((1, 14), np.float32)]), np.float32)
+    cal = f(np.stack([np.asarray(q["calib6"], np.float32) for q in seqs]), np.float32); R = 8
+    n_act = np.zeros(n, np.int32); ah = np.zeros(cap, np.int32); ai = np.zeros(cap, np.int32); ap = np.zeros(cap, IMMATURE_PT_DTYPE); am = np.zeros(cap, IMMATURE_META_DTYPE)
+    aid = np.zeros(cap, np.float32); ars = np.zeros((cap, R), np.int32); cnt = np.zeros(NH, np.int32); cm = P["cams"]
+    ctx._ck(LIB.sdv_activate_points_store_batch(ctx.p, n, hb, hosts, fl, cA, cB, P["hb"], P["pb"], P["A"].ctypes.data, P["B"].ctypes.data, P["U"].ctypes.data, P["md"], pre, cal,
+                                                None if cm is None else cm.ctypes.data, cap, n_act, ah.ctypes.data, ai.ctypes.data, ap.ctypes.data, am.ctypes.data, aid.ctypes.data,
+                                                ars.ctypes.data, cnt.ctypes.data))
+    out = dict(host=[], idx=[], pts=[], meta=[], idepth=[], res_state=[], counts=[]); o = 0
+    for j in range(n):
+        a = slice(o, o + n_act[j]); o += n_act[j]; nH = len(seqs[j]["hosts"])
+        out["host"].append(ah[a] - hb[j]); out["idx"].append(ai[a].copy()); out["pts"].append(ap[a].copy()); out["meta"].append(am[a].copy())
+        out["idepth"].append(aid[a].copy()); out["res_state"].append(ars[a, :nH - 1].copy()); out["counts"].append(cnt[hb[j]:hb[j + 1]].copy())
+    return out
+
+
 def coarseTrackingLogLine(frame_id: int, timestamp: float, ab_exposure: float, result: dict) -> str:
     """One line of the reference's coarseTrackingLog (FullSystem.cpp:500-513, written when setting_logStuff is on):
     id timestamp ab_exposure camToWorld.log()[6] a b achievedRes[0] tryIterations — `result` is one element of trackNewCoarseBatch's return."""
@@ -774,6 +845,16 @@ class PixelSelector:
                                                   np.ascontiguousarray(np.broadcast_to(density_lidar, n), np.float32), np.ascontiguousarray(np.broadcast_to(density_dense, n), np.float32),
                                                   np.ascontiguousarray(np.broadcast_to(add_feature_point, n), np.int32), cap, out.ctypes.data, imm.ctypes.data, n_out, num))
         return [(out[j, :n_out[j]], imm[j, :n_out[j]]) for j in range(n)], num.reshape(n, 2)
+
+    def makeNewTracesStore(self, slots, frame_ids, clouds, density_lidar, density_dense, add_feature_point, cap=1 << 14):
+        """FullSystem::makeNewTraces for one new keyframe per slot, the points deposited into the ImmatureStore block of frame_ids[j] (sensor points with their LiDAR
+        depth and status SKIPPED, as makeNewTraces / makeKeyFrame leave them) -> points per job (n,), numPoints (n,2)"""
+        n = len(slots); cl = [np.ascontiguousarray(c, np.float64).reshape(-1, 3) for c in clouds]; cb = np.concatenate([[0], np.cumsum([len(c) for c in cl])]).astype(np.int32)
+        allc = np.ascontiguousarray(np.concatenate(cl) if cb[-1] else np.zeros((1, 3))); n_out = np.zeros(n, np.int32); num = np.zeros(2 * n, np.int32)
+        self.ctx._ck(LIB.sdv_make_new_traces_store_batch(self.ctx.p, n, np.ascontiguousarray(slots, np.int32), np.ascontiguousarray(frame_ids, np.uint64), cb, allc.ctypes.data,
+                                                        np.ascontiguousarray(np.broadcast_to(density_lidar, n), np.float32), np.ascontiguousarray(np.broadcast_to(density_dense, n), np.float32),
+                                                        np.ascontiguousarray(np.broadcast_to(add_feature_point, n), np.int32), cap, n_out, num))
+        return n_out, num.reshape(n, 2)
 
 
 def packActivation(seqs, cams=None):

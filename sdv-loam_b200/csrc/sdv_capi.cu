@@ -172,7 +172,7 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
   c->frame_texels = texels;
   c->frames.resize(s.max_frames);
   for (auto& f : c->frames) {
-    f.used = false; f.adopted = false; f.lvl0_slot = -1; f.hi_tex = false; f.pyr = nullptr; f.base = nullptr; f.ingest_seq = 0; f.cam = 0;
+    f.used = false; f.adopted = false; f.trk_async = false; f.lvl0_slot = -1; f.hi_tex = false; f.pyr = nullptr; f.base = nullptr; f.ingest_seq = 0; f.cam = 0;
     CK(cudaMalloc(&f.I0_own, (size_t)w*h*sizeof(float))); f.I0 = f.I0_own; f.img[0] = f.I0;
     if (texels) { CK(cudaMalloc(&f.pyr, texels*sizeof(float))); CK(cudaMalloc(&f.base, texels*sizeof(float4))); }
     f.lvl[0] = nullptr; for (int l=1;l<levels;l++) { f.img[l] = f.pyr + c->lvl_off[l]; f.lvl[l] = f.base + c->lvl_off[l]; }
@@ -229,8 +229,10 @@ void sdv_destroy(sdv_ctx* c) {
   rp_destroy(c);
   sel_destroy(c);
   lidar_destroy(c);
+  imm_store_destroy(c);
   ba_destroy(c);
   if (c->ba_ev0) cudaEventDestroy(c->ba_ev0); if (c->ba_ev1) cudaEventDestroy(c->ba_ev1); if (c->ev_xdom) cudaEventDestroy(c->ev_xdom); if (c->st_ba) cudaStreamDestroy(c->st_ba);
+  if (c->ev_trk_async) cudaEventDestroy(c->ev_trk_async);
   if (c->ev0) cudaEventDestroy(c->ev0); if (c->ev1) cudaEventDestroy(c->ev1); if (c->ev_in) cudaEventDestroy(c->ev_in); if (c->st) cudaStreamDestroy(c->st); if (c->st_in) cudaStreamDestroy(c->st_in);
   cudaGetLastError();                                      // a partially built context may have produced benign errors above: do not leave them sticky
   delete c;
@@ -294,6 +296,7 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
       if (frame_pinned(c, frames[k])) return ctx_fail(c, SDV_ERR_STATE, "frame %llu is referenced by a resident BA window / map slot and cannot be re-uploaded", (unsigned long long)frames[k]); }
     else { for (size_t i=0;i<c->frames.size();i++) if (!c->frames[i].used) { idx = (int)i; break; } }
     if (idx < 0) return ctx_fail(c, SDV_ERR_CAPACITY, "frame pool exhausted (max_frames=%d)", (int)c->frames.size());
+    { int rcf = frame_fence(c, c->frames[idx], c->st_cp, c->st_in, c->frames[idx].adopted); if (rcf) return rcf; }   // an earlier trace may still read its storage
     FrameDev& f = c->frames[idx]; f.used = true; f.id = frames[k]; f.exposure = exposures ? exposures[k] : 1.0f; c->frame_index[frames[k]] = idx;
     frame_drop_texels(c, f); f.ingest_seq = seq; f.cam = cam_of(k);
     f.adopted = adopt; f.I0 = adopt ? const_cast<float*>(reinterpret_cast<const float*>(imgs[k])) : f.I0_own; f.img[0] = f.I0;
@@ -331,6 +334,14 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
 }
 }  // extern "C"
 namespace sdv {
+int frame_fence(sdv_ctx* c, FrameDev& f, cudaStream_t a, cudaStream_t b, bool host_wait) {
+  if (!f.trk_async || !c->ev_trk_async) return SDV_OK;
+  if (host_wait) { CK(cudaEventSynchronize(c->ev_trk_async)); f.trk_async = false; return SDV_OK; }
+  if (a) CK(cudaStreamWaitEvent(a, c->ev_trk_async, 0));
+  if (b) CK(cudaStreamWaitEvent(b, c->ev_trk_async, 0));
+  if (a || b) f.trk_async = false;                                       // the writers of the new contents are ordered after the readers
+  return SDV_OK;
+}
 int join_ingest_upto(sdv_ctx* c, long long seq) {  // the compute stream waits for ingest calls <= seq (st_in is in order, so one event covers all earlier ones)
   if (seq > c->ingest_seq) seq = c->ingest_seq;
   if (seq <= c->seq_waited) return SDV_OK;
@@ -430,6 +441,7 @@ int sdv_frame_release(sdv_ctx* c, uint64_t frame) { SDV_GUARD_TRK(c);
   if (!c) return SDV_ERR_ARG;
   auto it = c->frame_index.find(frame); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown frame %llu", (unsigned long long)frame);
   if (frame_pinned(c, frame)) return ctx_fail(c, SDV_ERR_STATE, "frame %llu is referenced by a resident BA window / map slot: replace or clear that window / map first", (unsigned long long)frame);
+  { int rcf = frame_fence(c, c->frames[it->second], nullptr, nullptr, c->frames[it->second].adopted); if (rcf) return rcf; }   // the caller may reuse an adopted buffer at once
   FrameDev& f = c->frames[it->second]; f.used = false; frame_drop_texels(c, f); f.adopted = false; f.I0 = f.I0_own; f.img[0] = f.I0; c->frame_index.erase(it); return SDV_OK;
 }
 int sdv_frame_download(sdv_ctx* c, uint64_t frame, int lvl, float* dI3_out, float* abs_out) { SDV_GUARD_TRK(c);

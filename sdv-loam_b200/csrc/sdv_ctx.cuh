@@ -19,6 +19,7 @@ struct FrameDev {                         // one FrameHessian's images on the de
   float4* base; float4* lvl[kLevels]; int lvl0_slot; bool hi_tex;
   long long ingest_seq;                   // ingest call that (re)built this frame's pyramid
   int cam;                                // camera it was ingested for: its size is sdv_ctx::cam_w/cam_h[cam] (storage stays at the context size and lvl_off)
+  bool trk_async;                         // read by tracker-stream work that may still be pending (sdv_ctx::ev_trk_async marks its end)
 };
 
 struct TrackerSlot {                      // one CoarseTracker instance (reference keeps two: FullSystem.h coarseTracker / coarseTracker_forNewKF)
@@ -70,6 +71,8 @@ struct sdv_ctx {
   float last_ms;
   void* refine_dev = nullptr; void* refine_host = nullptr; size_t refine_cap = 0;      // staging of sdv_tracker_struct_pose_batch
   void* trace_dev = nullptr; size_t trace_cap = 0;                                  // scratch of the immature-point calls (sdv_trace.cu)
+  cudaEvent_t ev_trk_async = nullptr;           // recorded on st after the last call that returned with a kernel still reading frames (FrameDev::trk_async)
+  void* imm_store = nullptr;                    // sdv::ImmStore: device-resident immature points, one block per host keyframe (sdv_trace.cu)
   void* lidar = nullptr;                        // sdv::LidarState: engine of the LiDAR front-end (sdv_lidar.cu)
   void* sel = nullptr;                          // sdv::SelState: PixelSelector slots + engine of the candidate management (sdv_select.cu)
   sdv::RpState* rp = nullptr;                   // map slots + scratch of the Reprojector path (sdv_reproject.cu)
@@ -84,6 +87,15 @@ namespace sdv {
 void rp_destroy(sdv_ctx* c);
 void sel_destroy(sdv_ctx* c);
 void lidar_destroy(sdv_ctx* c);
+void imm_store_destroy(sdv_ctx* c);
+// makeNewTraces into the store: job j's n[j] records (sel::NewTrace / sel::ImmPt device arrays, stream-ordered on c->st) replace the block of hosts[j]
+int  imm_store_deposit(sdv_ctx* c, int nj, const uint64_t* hosts, const int* n, const void* const* new_trace_dev, const void* const* imm_dev);
+int  sel_activate_select(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,
+                         const int32_t* cand_host_begin, const int32_t* cand_begin, const float* cKRKi9, const float* cKt3, const float* cand4, const float* cand4_dev,
+                         const float* min_act_dist, const int32_t* cams, int32_t* decision_out, float* dist_map_out);
+// frames read by a tracker-stream call that returned before its kernel ran (sdv_immature_trace_store_batch without counts) carry FrameDev::trk_async; frame_fence
+// makes an ingest that overwrites such a frame wait for that work on the device, and waits on the host before an adopted buffer is handed back
+int  frame_fence(sdv_ctx* c, FrameDev& f, cudaStream_t a, cudaStream_t b, bool host_wait);
 int ctx_fail(sdv_ctx* c, int code, const char* fmt, ...);
 void ba_destroy(sdv_ctx* c);
 int  ensure_lvl0(sdv_ctx* c, FrameDev& f);     // build the packed level-0 texels of a frame on demand (keyframes / read-back)

@@ -146,33 +146,55 @@ int sdv_selector_make_maps_batch(sdv_ctx* c, int n, const int32_t* slots, const 
   return SDV_OK;
 }
 
-int sdv_make_new_traces_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const float* density_lidar,
-                              const float* density_dense, const int32_t* add_feature_point, int cap, sdv_new_trace* out, sdv_immature_pt* imm_out, int32_t* n_out, int32_t* num_points2) { SDV_GUARD_TRK(c);
-  if (!c || n < 0 || (n && (!slots || !frames || !cloud_begin || !density_lidar || !density_dense || !add_feature_point || !out || !n_out || cap < 1))) return SDV_ERR_ARG;
+}  // extern "C"
+// makeNewTraces for n jobs; out == nullptr: the records go into the immature-point store (block of frames[j]) instead of to the caller
+static int make_new_traces(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const float* density_lidar,
+                           const float* density_dense, const int32_t* add_feature_point, int cap, sdv_new_trace* out, sdv_immature_pt* imm_out, int32_t* n_out, int32_t* num_points2) {
   if (n == 0) return SDV_OK; SEL_STATE("make_new_traces");
   if (cloud_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: cloud_begin[0] must be 0");
   for (int j = 0; j < n; j++) { if (cloud_begin[j+1] < cloud_begin[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: cloud_begin is not ascending at job %d", j);
     if (cloud_begin[j+1] > cloud_begin[j] && !cloud3) return SDV_ERR_ARG;
     if (slots[j] < 0 || slots[j] >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: slot %d of %d", slots[j], (int)s->slots.size());
-    for (int k = 0; k < j; k++) if (slots[k] == slots[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: slot %d appears twice in one batch", slots[j]); }
+    for (int k = 0; k < j; k++) if (slots[k] == slots[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: slot %d appears twice in one batch", slots[j]);
+    if (!out) for (int k = 0; k < j; k++) if (frames[k] == frames[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces_store: frame %llu appears twice in one batch", (unsigned long long)frames[j]); }
   CK(cudaSetDevice(c->device));
   long long need = 0; std::vector<sel::SelEngine::NewTracesJob> J(n);
   for (int j = 0; j < n; j++) { const int cam = s->cam[slots[j]]; int rc = sel_frame(c, frames[j], cam, J[j].img, need, "make_new_traces"); if (rc) return rc; J[j].w = c->cam_w[cam]; J[j].h = c->cam_h[cam];
     J[j].cloud_host = cloud3 ? cloud3 + 3*(size_t)cloud_begin[j] : nullptr; J[j].n = cloud_begin[j+1] - cloud_begin[j]; J[j].slot = &s->slots[slots[j]]; J[j].densityLidar = density_lidar[j];
-    J[j].densityDense = density_dense[j]; J[j].addFeaturePoint = add_feature_point[j]; J[j].out_host = (sel::NewTrace*)out + (size_t)j*cap; J[j].imm_host = imm_out ? (sel::ImmPt*)imm_out + (size_t)j*cap : nullptr; J[j].cap = cap; }
+    J[j].densityDense = density_dense[j]; J[j].addFeaturePoint = add_feature_point[j]; J[j].out_host = out ? (sel::NewTrace*)out + (size_t)j*cap : nullptr;
+    J[j].imm_host = (out && imm_out) ? (sel::ImmPt*)imm_out + (size_t)j*cap : nullptr; J[j].cap = cap; }
   { int rc = join_ingest_upto(c, need); if (rc) return rc; }
   const long long l0 = s->eng.launches;
   CK(cudaEventRecord(c->ev0, c->st));
   { int rc = s->eng.make_new_traces(J); if (rc) return sel_fail(c, s, rc, "make_new_traces"); }
+  if (!out) {                                                                            // device-output path: the records go from the engine's scratch into the store
+    std::vector<int> cnt(n); std::vector<const void*> nt(n), im(n);
+    for (int j = 0; j < n; j++) { cnt[j] = J[j].n_out; nt[j] = J[j].out_dev; im[j] = J[j].imm_dev; }
+    int rc = imm_store_deposit(c, n, frames, cnt.data(), nt.data(), im.data()); if (rc) return rc;
+  }
   CK(cudaEventRecord(c->ev1, c->st)); CK(cudaStreamSynchronize(c->st)); CK(cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   c->launches += s->eng.launches - l0;
   for (int j = 0; j < n; j++) { n_out[j] = J[j].n_out; if (num_points2) { num_points2[2*j] = J[j].numPoints[0]; num_points2[2*j+1] = J[j].numPoints[1]; } }
   return SDV_OK;
 }
+extern "C" {
+int sdv_make_new_traces_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const float* density_lidar,
+                              const float* density_dense, const int32_t* add_feature_point, int cap, sdv_new_trace* out, sdv_immature_pt* imm_out, int32_t* n_out, int32_t* num_points2) { SDV_GUARD_TRK(c);
+  if (!c || n < 0 || (n && (!slots || !frames || !cloud_begin || !density_lidar || !density_dense || !add_feature_point || !out || !n_out || cap < 1))) return SDV_ERR_ARG;
+  return make_new_traces(c, n, slots, frames, cloud_begin, cloud3, density_lidar, density_dense, add_feature_point, cap, out, imm_out, n_out, num_points2);
+}
+int sdv_make_new_traces_store_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const float* density_lidar,
+                                    const float* density_dense, const int32_t* add_feature_point, int cap, int32_t* n_out, int32_t* num_points2) { SDV_GUARD_TRK(c);
+  if (!c || n < 0 || (n && (!slots || !frames || !cloud_begin || !density_lidar || !density_dense || !add_feature_point || !n_out || cap < 1))) return SDV_ERR_ARG;
+  return make_new_traces(c, n, slots, frames, cloud_begin, cloud3, density_lidar, density_dense, add_feature_point, cap, nullptr, nullptr, n_out, num_points2);
+}
 
-int sdv_activate_select_batch_cams(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,
-                                   const int32_t* cand_host_begin, const int32_t* cand_begin, const float* cKRKi9, const float* cKt3, const float* cand4, const float* min_act_dist,
-                                   const int32_t* cams, int32_t* decision_out, float* dist_map_out) { SDV_GUARD_TRK(c);
+}  // extern "C"
+namespace sdv {
+// makeDistanceMap + the candidate walk; cand4_dev != nullptr: the cand4 rows are device memory (the activation on the immature-point store)
+int sel_activate_select(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,
+                        const int32_t* cand_host_begin, const int32_t* cand_begin, const float* cKRKi9, const float* cKt3, const float* cand4, const float* cand4_dev,
+                        const float* min_act_dist, const int32_t* cams, int32_t* decision_out, float* dist_map_out) {
   if (!c || n < 0 || (n && (!host_begin || !pt_begin || !cand_host_begin || !cand_begin || !min_act_dist))) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK; SEL_STATE("activate_select");
   if (host_begin[0] != 0 || cand_host_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "activate_select: host_begin[0] and cand_host_begin[0] must be 0");
@@ -185,10 +207,10 @@ int sdv_activate_select_batch_cams(sdv_ctx* c, int n, const int32_t* host_begin,
     for (int k = h0; k <= h1; k++) { if (k > h0 && pt_begin[k] < pt_begin[k-1]) return ctx_fail(c, SDV_ERR_ARG, "activate_select: pt_begin is not ascending"); pb[j].push_back(pt_begin[k] - pt_begin[h0]); }
     for (int k = g0; k <= g1; k++) { if (k > g0 && cand_begin[k] < cand_begin[k-1]) return ctx_fail(c, SDV_ERR_ARG, "activate_select: cand_begin is not ascending"); cb[j].push_back(cand_begin[k] - cand_begin[g0]); }
     const int np = pb[j].back(), nc = cb[j].back();
-    if ((np && (!KRKi9 || !Kt3 || !uvid)) || (nc && (!cKRKi9 || !cKt3 || !cand4 || !decision_out))) return SDV_ERR_ARG;
+    if ((np && (!KRKi9 || !Kt3 || !uvid)) || (nc && (!cKRKi9 || !cKt3 || (!cand4 && !cand4_dev) || !decision_out))) return SDV_ERR_ARG;
     sel::SelEngine::ActJob& a = J[j]; a.nHosts = h1 - h0; a.pt_begin = pb[j].data(); a.KRKi = KRKi9 ? KRKi9 + 9*(size_t)h0 : nullptr; a.Kt = Kt3 ? Kt3 + 3*(size_t)h0 : nullptr;
     a.uvid = uvid ? uvid + 3*(size_t)pt_begin[h0] : nullptr; a.nCandHosts = g1 - g0; a.cand_begin = cb[j].data(); a.cKRKi = cKRKi9 ? cKRKi9 + 9*(size_t)g0 : nullptr; a.cKt = cKt3 ? cKt3 + 3*(size_t)g0 : nullptr;
-    a.cand4 = cand4 ? cand4 + 4*(size_t)cand_begin[g0] : nullptr; a.minActDist = min_act_dist[j]; a.decision_host = decision_out ? decision_out + cand_begin[g0] : nullptr;
+    a.cand4 = cand4 ? cand4 + 4*(size_t)cand_begin[g0] : nullptr; a.cand4_dev = cand4_dev ? cand4_dev + 4*(size_t)cand_begin[g0] : nullptr; a.minActDist = min_act_dist[j]; a.decision_host = decision_out ? decision_out + cand_begin[g0] : nullptr;
     const int cam = cams ? cams[j] : 0; a.w1 = c->cam_w[cam] >> 1; a.h1 = c->cam_h[cam] >> 1;
     a.map_host = dist_map_out ? dist_map_out + map_off : nullptr; map_off += (size_t)a.w1*a.h1;
   }
@@ -200,6 +222,13 @@ int sdv_activate_select_batch_cams(sdv_ctx* c, int n, const int32_t* host_begin,
   if (s->eng.have_ev) c->last_ms = s->eng.last_kernel_ms;                                  // the 43 launches, copies excluded
   c->launches += s->eng.launches - l0;
   return SDV_OK;
+}
+}  // namespace sdv
+extern "C" {
+int sdv_activate_select_batch_cams(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,
+                                   const int32_t* cand_host_begin, const int32_t* cand_begin, const float* cKRKi9, const float* cKt3, const float* cand4, const float* min_act_dist,
+                                   const int32_t* cams, int32_t* decision_out, float* dist_map_out) { SDV_GUARD_TRK(c);
+  return sel_activate_select(c, n, host_begin, pt_begin, KRKi9, Kt3, uvid, cand_host_begin, cand_begin, cKRKi9, cKt3, cand4, nullptr, min_act_dist, cams, decision_out, dist_map_out);
 }
 int sdv_activate_select_batch(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,
                               const int32_t* cand_host_begin, const int32_t* cand_begin, const float* cKRKi9, const float* cKt3, const float* cand4, const float* min_act_dist,

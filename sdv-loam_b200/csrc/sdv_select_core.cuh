@@ -783,6 +783,8 @@ struct SelEngine {
     FrameImg img; int w = 0, h = 0; const double* cloud_host; int n; SelectorSlot* slot; float densityLidar, densityDense; int addFeaturePoint;   // w, h: the frame's size (= the slot's map)
     NewTrace* out_host; ImmPt* imm_host; int cap;                  // cap: room for the returned points (LiDAR + monocular)
     int n_out, numPoints[2], passes[2];                             // out: points created, {numPointLidar, numPointMonocular}, select passes of the two makeMaps calls
+    const NewTrace* out_dev = nullptr; const ImmPt* imm_dev = nullptr;   // out: the n_out records on the device (engine scratch, valid until the next engine call);
+                                                                    // out_host == nullptr: they stay there (device-output path)
   };
   Scratch io;
   int make_new_traces(std::vector<NewTracesJob>& jobs) {
@@ -841,7 +843,8 @@ struct SelEngine {
     SEL_CK(cudaStreamSynchronize(st));
     for (int j = 0; j < nj; j++) { NewTracesJob& N = jobs[j]; N.n_out = counts[4*j] + counts[4*j+1];
       if (counts[4*j+2] >= N.cap || N.n_out > N.cap) { err = "make_new_traces: output capacity too small"; return -2; }
-      if (N.n_out) { SEL_CK(cudaMemcpyAsync(N.out_host, T[j].out, (size_t)N.n_out*sizeof(NewTrace), cudaMemcpyDeviceToHost, st));
+      N.out_dev = T[j].out; N.imm_dev = T[j].imm;
+      if (N.n_out && N.out_host) { SEL_CK(cudaMemcpyAsync(N.out_host, T[j].out, (size_t)N.n_out*sizeof(NewTrace), cudaMemcpyDeviceToHost, st));
                      if (N.imm_host) SEL_CK(cudaMemcpyAsync(N.imm_host, T[j].imm, (size_t)N.n_out*sizeof(ImmPt), cudaMemcpyDeviceToHost, st)); } }
     SEL_CK(cudaStreamSynchronize(st));
     return 0;
@@ -854,6 +857,7 @@ struct SelEngine {
     int nCandHosts; const int* cand_begin; const float* cKRKi; const float* cKt; const float* cand4; float minActDist;
     int32_t* decision_host; float* map_host;                                                                       // out: per candidate 1 / 0 / -1; optional w1*h1 map after the walk
     int w1 = 0, h1 = 0;                                                                                            // level-1 size of the sequence's camera
+    const float* cand4_dev = nullptr;                                                                              // device-input path: the cand4 rows already on the device
   };
   int activate(std::vector<ActJob>& jobs) {
     const int nj = (int)jobs.size(); if (!nj) return 0;
@@ -872,7 +876,7 @@ struct SelEngine {
       J.pt_begin = (const int*)up(a.pt_begin, (a.nHosts+1)*sizeof(int)); J.KRKi = (const float*)up(a.KRKi, 9*a.nHosts*sizeof(float)); J.Kt = (const float*)up(a.Kt, 3*a.nHosts*sizeof(float));
       J.uvid = (const float*)up(a.uvid, 3*(size_t)np*sizeof(float));
       J.nCandHosts = a.nCandHosts; J.cand_begin = (const int*)up(a.nCandHosts ? (const void*)a.cand_begin : (const void*)zero1, (a.nCandHosts+1)*sizeof(int));
-      J.cKRKi = (const float*)up(a.cKRKi, 9*a.nCandHosts*sizeof(float)); J.cKt = (const float*)up(a.cKt, 3*a.nCandHosts*sizeof(float)); J.cand4 = (const float*)up(a.cand4, 4*(size_t)nc*sizeof(float));
+      J.cKRKi = (const float*)up(a.cKRKi, 9*a.nCandHosts*sizeof(float)); J.cKt = (const float*)up(a.cKt, 3*a.nCandHosts*sizeof(float)); J.cand4 = a.cand4_dev ? a.cand4_dev : (const float*)up(a.cand4, 4*(size_t)nc*sizeof(float));
       J.minActDist = a.minActDist; J.proj = io.take<int>(3*(size_t)std::max(nc, 1)); J.decision = io.take<int>(std::max(nc, 1));
       maxP = std::max(maxP, np); maxC = std::max(maxC, nc); }
     SEL_CK(cudaMemcpyAsync(dD, D.data(), nj*sizeof(DistJob), cudaMemcpyHostToDevice, st));

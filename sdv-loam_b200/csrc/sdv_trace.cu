@@ -13,7 +13,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
+#include <string.h>
 #include <vector>
+#include <algorithm>
 #include "sdv_ctx.cuh"
 
 using namespace sdv;
@@ -309,6 +311,161 @@ static int trace_scratch(sdv_ctx* c, size_t bytes) {
   CK(cudaStreamSynchronize(c->st)); cudaFree(c->trace_dev); c->trace_dev = nullptr; c->trace_cap = 0;
   CK(cudaMalloc(&c->trace_dev, bytes + bytes/2)); c->trace_cap = bytes + bytes/2; return SDV_OK;
 }
+
+// ---- the immature-point store: host->immaturePoints of every keyframe kept on the device (sdv_immature_store_*, sdv_immature_trace_store_batch)
+// A block keeps each record in two arrays split by what traceOn does with the fields: ImmRO (92 B) it only reads, ImmRW (28 B) it writes.  A per-frame trace
+// therefore writes 28 B per point instead of 120, and a point that is already OOB (traceOn returns at once) costs one 4-byte status read.
+struct ImmRO { float u, v, color[8], weights[8], gradH[4], energyTH; };
+struct ImmRW { float idepth_min, idepth_max, quality, lastTraceUV[2], lastTracePixelInterval; int32_t status; };
+static_assert(sizeof(ImmRO) + sizeof(ImmRW) == sizeof(sdv_immature_pt) && sizeof(sdv_immature_meta) == 16, "store layout");
+__host__ __device__ __forceinline__ void imm_split(const sdv_immature_pt& p, ImmRO& a, ImmRW& b) {
+  a.u = p.u; a.v = p.v; for (int k = 0; k < 8; k++) { a.color[k] = p.color[k]; a.weights[k] = p.weights[k]; } for (int k = 0; k < 4; k++) a.gradH[k] = p.gradH[k]; a.energyTH = p.energyTH;
+  b.idepth_min = p.idepth_min; b.idepth_max = p.idepth_max; b.quality = p.quality; b.lastTraceUV[0] = p.lastTraceUV[0]; b.lastTraceUV[1] = p.lastTraceUV[1];
+  b.lastTracePixelInterval = p.lastTracePixelInterval; b.status = p.lastTraceStatus;
+}
+__host__ __device__ __forceinline__ void imm_join(const ImmRO& a, const ImmRW& b, sdv_immature_pt& p) {
+  p.u = a.u; p.v = a.v; for (int k = 0; k < 8; k++) { p.color[k] = a.color[k]; p.weights[k] = a.weights[k]; } for (int k = 0; k < 4; k++) p.gradH[k] = a.gradH[k]; p.energyTH = a.energyTH;
+  p.idepth_min = b.idepth_min; p.idepth_max = b.idepth_max; p.quality = b.quality; p.lastTraceUV[0] = b.lastTraceUV[0]; p.lastTraceUV[1] = b.lastTraceUV[1];
+  p.lastTracePixelInterval = b.lastTracePixelInterval; p.lastTraceStatus = b.status;
+}
+struct ImmBlock { ImmRO* ro = nullptr; ImmRW* rw = nullptr; sdv_immature_meta* meta = nullptr; int n = 0, cap = 0; };   // one allocation: ro | rw | meta, cap points each
+struct ImmStore { std::unordered_map<uint64_t, ImmBlock> blocks; std::vector<ImmBlock> spare; };                       // spare: blocks of dropped hosts, reused before allocating
+void imm_store_destroy(sdv_ctx* c) {
+  ImmStore* S = (ImmStore*)c->imm_store; if (!S) return;
+  for (auto& kv : S->blocks) cudaFree(kv.second.ro);
+  for (auto& b : S->spare) cudaFree(b.ro);
+  delete S; c->imm_store = nullptr;
+}
+static ImmStore* imm_store(sdv_ctx* c) { if (!c->imm_store) c->imm_store = new ImmStore(); return (ImmStore*)c->imm_store; }
+static size_t al16(size_t b) { return (b + 15) & ~(size_t)15; }
+// Room for hosts that are about to receive new contents, in two phases so that a refused call changes no block.  imm_store_plan picks, per host, its own block
+// if large enough, else the smallest free spare that fits, else a new allocation; before allocating it frees the spares too small for the request (a drive
+// whose point counts grow does not keep every block it outgrew).  Nothing visible changes until imm_store_commit; on failure the new allocations become spares.
+// Stream-ordered reuse: every reader and writer of a block runs on c->st.
+struct ImmPlan { uint64_t host; int n; ImmBlock b; bool own; };
+static ImmBlock imm_block_layout(char* p, int cap) {
+  ImmBlock nb; const size_t o_rw = al16((size_t)cap*sizeof(ImmRO)), o_m = o_rw + al16((size_t)cap*sizeof(ImmRW));
+  nb.ro = (ImmRO*)p; nb.rw = (ImmRW*)(p + o_rw); nb.meta = (sdv_immature_meta*)(p + o_m); nb.cap = cap; return nb;
+}
+static size_t imm_block_bytes(int cap) { return al16((size_t)cap*sizeof(ImmRO)) + al16((size_t)cap*sizeof(ImmRW)) + (size_t)cap*sizeof(sdv_immature_meta); }
+static int imm_store_plan(sdv_ctx* c, ImmStore* S, int nh, const uint64_t* hosts, const int* n, std::vector<ImmPlan>& P) {
+  P.assign(nh, ImmPlan()); std::vector<char> taken(S->spare.size(), 0); std::vector<ImmBlock> fresh;
+  auto fail = [&](int rc) { for (auto& b : fresh) S->spare.push_back(b); return rc; };
+  for (int j = 0; j < nh; j++) {
+    ImmPlan& q = P[j]; q.host = hosts[j]; q.n = n[j]; auto it = S->blocks.find(hosts[j]);
+    if (it != S->blocks.end() && it->second.cap >= n[j]) { q.b = it->second; q.own = true; continue; }
+    q.own = false; int best = -1;
+    for (int k = 0; k < (int)S->spare.size(); k++) if (!taken[k] && S->spare[k].cap >= n[j] && (best < 0 || S->spare[k].cap < S->spare[best].cap)) best = k;
+    if (best >= 0) { taken[best] = 1; q.b = S->spare[best]; continue; }
+    bool small = false; for (int k = 0; k < (int)S->spare.size(); k++) small |= !taken[k] && S->spare[k].cap < n[j];
+    if (small) {                                                                         // spares this request outgrew: give their memory back first
+      if (cudaStreamSynchronize(c->st) != cudaSuccess) return fail(ctx_fail(c, SDV_ERR_CUDA, "immature store: stream synchronise"));
+      std::vector<ImmBlock> keep; std::vector<char> kt;
+      for (int k = 0; k < (int)S->spare.size(); k++) { if (!taken[k] && S->spare[k].cap < n[j]) cudaFree(S->spare[k].ro); else { keep.push_back(S->spare[k]); kt.push_back(taken[k]); } }
+      S->spare.swap(keep); taken.swap(kt);
+    }
+    const int cap = std::max(256, n[j] + n[j]/4); char* p = nullptr;
+    if (cudaMalloc((void**)&p, imm_block_bytes(cap)) != cudaSuccess) { cudaGetLastError(); return fail(ctx_fail(c, SDV_ERR_CUDA, "immature store: cudaMalloc of %d points", cap)); }
+    q.b = imm_block_layout(p, cap); fresh.push_back(q.b);
+  }
+  for (int k = (int)taken.size() - 1; k >= 0; k--) if (taken[k]) S->spare.erase(S->spare.begin() + k);   // the spares now in a plan
+  return SDV_OK;
+}
+// the plan's blocks and counts become the hosts' blocks; a host that moved leaves its old block as a spare
+static void imm_store_commit(ImmStore* S, std::vector<ImmPlan>& P) {
+  for (ImmPlan& q : P) {
+    auto it = S->blocks.find(q.host); q.b.n = q.n;
+    if (it == S->blocks.end()) S->blocks[q.host] = q.b;
+    else { if (!q.own) S->spare.push_back(it->second); it->second = q.b; }
+  }
+}
+// a failed call after imm_store_plan: blocks it took from the spares or allocated go back to the spares
+static void imm_store_abandon(ImmStore* S, std::vector<ImmPlan>& P) { for (ImmPlan& q : P) if (!q.own) S->spare.push_back(q.b); }
+
+// makeNewTraces into the store: the records of the selector engine (sdv_new_trace + sdv_immature_pt) with FullSystem.cpp:1313-1317 and :1080-1084 applied
+struct DepositJob { const sdv_new_trace* t; const sdv_immature_pt* p; ImmRO* ro; ImmRW* rw; sdv_immature_meta* meta; int n; };
+__global__ void __launch_bounds__(128) imm_deposit_kernel(const DepositJob* __restrict__ jobs) {
+  const DepositJob J = jobs[blockIdx.y]; const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= J.n) return;
+  const sdv_new_trace t = J.t[i]; sdv_immature_pt p = J.p[i];
+  if (t.isFromSensor) { p.idepth_min = p.idepth_max = t.idepth_fromSensor; p.lastTraceStatus = IPS_SKIPPED; }   // idepth_max = idepth_fromSensor*1.0: the float survives the double product
+  ImmRO a; ImmRW b; imm_split(p, a, b); J.ro[i] = a; J.rw[i] = b;
+  sdv_immature_meta m; m.my_type = t.my_type; m.type = t.type; m.isFromSensor = t.isFromSensor; m.idepth_fromSensor = t.idepth_fromSensor; J.meta[i] = m;
+}
+int imm_store_deposit(sdv_ctx* c, int nj, const uint64_t* hosts, const int* n, const void* const* nt_dev, const void* const* imm_dev) {
+  ImmStore* S = imm_store(c); std::vector<ImmPlan> P; { int rc = imm_store_plan(c, S, nj, hosts, n, P); if (rc) return rc; }
+  std::vector<DepositJob> D(nj); int maxN = 0;
+  for (int j = 0; j < nj; j++) { D[j] = DepositJob{(const sdv_new_trace*)nt_dev[j], (const sdv_immature_pt*)imm_dev[j], P[j].b.ro, P[j].b.rw, P[j].b.meta, n[j]}; maxN = std::max(maxN, n[j]); }
+  if (maxN > 0) {
+    { int rc = trace_scratch(c, nj*sizeof(DepositJob)); if (rc) { imm_store_abandon(S, P); return rc; } }
+    if (cudaMemcpyAsync(c->trace_dev, D.data(), nj*sizeof(DepositJob), cudaMemcpyHostToDevice, c->st) != cudaSuccess) { imm_store_abandon(S, P); CK(cudaGetLastError()); }
+    imm_deposit_kernel<<<dim3((maxN + 127)/128, nj), 128, 0, c->st>>>((const DepositJob*)c->trace_dev); c->launches += 1;
+    if (cudaGetLastError() != cudaSuccess) { imm_store_abandon(S, P); return ctx_fail(c, SDV_ERR_CUDA, "immature store: deposit launch"); }
+  }
+  imm_store_commit(S, P);
+  return SDV_OK;
+}
+
+// traceNewCoarse on the store: thread per point of all groups; the group is found by binary search over the groups' starts.  Calls trace_on, as imm_trace_kernel does.
+struct TraceStoreGroupDev { const float* I0; float KRKi[9], Kt[3], aff[2]; int w, h; const ImmRO* ro; ImmRW* rw; };
+__global__ void __launch_bounds__(128) imm_trace_store_kernel(const TraceStoreGroupDev* __restrict__ groups, const int* __restrict__ gbeg, int n_groups, int n, TraceSet S,
+                                                              int* __restrict__ counts) {
+  const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= n) return;
+  int lo = 0, hi = n_groups - 1;
+  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (__ldg(gbeg + mid) <= i) lo = mid; else hi = mid - 1; }   // the last group starting at or before i: empty groups drop out
+  const TraceStoreGroupDev& G = groups[lo]; const int k = i - __ldg(gbeg + lo);
+  int st = G.rw[k].status;
+  if (st != IPS_OOB) {                                                                   // traceOn returns an OOB point unchanged (ImmaturePoint.cpp:52)
+    sdv_immature_pt p; imm_join(G.ro[k], G.rw[k], p);
+    st = trace_on(p, G.I0, G.w, G.h, G.KRKi, G.Kt, G.aff, S);
+    ImmRO a; ImmRW b; imm_split(p, a, b); G.rw[k] = b;
+  }
+  if (counts && (unsigned)st < 6u) atomicAdd(counts + 6*lo + st, 1);
+}
+
+// ---- activatePointsMT on the store (FullSystem.cpp:598-720), device side: the filter of :612-645, gathers, the post pass's compaction
+struct ActHostDev { const ImmRO* ro; const ImmRW* rw; const sdv_immature_meta* meta; int newest, flagged; };
+enum { ACT_KEEP = 0, ACT_DELETE = 1, ACT_CAND = 2 };
+__device__ __forceinline__ int group_of_point(const int* __restrict__ gbeg, int n_groups, int i) {
+  int lo = 0, hi = n_groups - 1;
+  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (__ldg(gbeg + mid) <= i) lo = mid; else hi = mid - 1; }
+  return lo;
+}
+// per point: code = class | lastTraceStatus << 4, and for a candidate its cand4 row {u, v, 0.5f*(idepth_max+idepth_min), my_type}
+__global__ void __launch_bounds__(128) imm_act_filter_kernel(const ActHostDev* __restrict__ hosts, const int* __restrict__ gbeg, int n_hosts, int n, float minTraceQuality,
+                                                             int* __restrict__ code, float4* __restrict__ rows) {
+  const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= n) return;
+  const int g = group_of_point(gbeg, n_hosts, i); const ActHostDev& H = hosts[g]; const int k = i - __ldg(gbeg + g);
+  const ImmRW b = H.rw[k]; const sdv_immature_meta m = H.meta[k]; int cls = ACT_KEEP;
+  if (!(m.isFromSensor == 0 && H.newest)) {                                                  // :617 non-sensor points of the newest keyframe are skipped
+    if (!isfinite(b.idepth_max) || b.status == IPS_OUTLIER) cls = ACT_DELETE;              // :621
+    else {
+      const bool canActivate = (b.status == IPS_GOOD || b.status == IPS_SKIPPED || b.status == IPS_BADCONDITION || b.status == IPS_OOB)
+                               && b.lastTracePixelInterval < 8 && b.quality > minTraceQuality && (b.idepth_max+b.idepth_min) > 0;     // :630-636
+      if (!canActivate) cls = (H.flagged || b.status == IPS_OOB) ? ACT_DELETE : ACT_KEEP;  // :641
+      else { cls = ACT_CAND; const ImmRO a = H.ro[k]; rows[i] = make_float4(a.u, a.v, 0.5f*(b.idepth_max+b.idepth_min), m.my_type); }
+    }
+  }
+  code[i] = cls | (b.status << 4);
+}
+__global__ void __launch_bounds__(128) imm_act_rows_kernel(const float4* __restrict__ rows, const int* __restrict__ idx, int n, float4* __restrict__ out) {
+  const int k = blockIdx.x*blockDim.x + threadIdx.x; if (k < n) out[k] = rows[idx[k]];
+}
+// toOptimize k = point idx[k] of the call's point numbering: its full record, meta and isFromSensor byte
+__global__ void __launch_bounds__(128) imm_act_gather_kernel(const ActHostDev* __restrict__ hosts, const int* __restrict__ gbeg, int n_hosts, const int* __restrict__ idx, int n,
+                                                             sdv_immature_pt* __restrict__ pts, sdv_immature_meta* __restrict__ meta, unsigned char* __restrict__ fs) {
+  const int k = blockIdx.x*blockDim.x + threadIdx.x; if (k >= n) return;
+  const int i = idx[k], g = group_of_point(gbeg, n_hosts, i); const ActHostDev& H = hosts[g]; const int j = i - __ldg(gbeg + g);
+  sdv_immature_pt p; imm_join(H.ro[j], H.rw[j], p); pts[k] = p; const sdv_immature_meta m = H.meta[j]; meta[k] = m; fs[k] = m.isFromSensor ? 1 : 0;
+}
+// compaction: the new block of host g is its old entries perm[nbeg[g] ..] in that order; pass 0 gathers into scratch, pass 1 writes back in place
+struct ActBlockDev { ImmRO* ro; ImmRW* rw; sdv_immature_meta* meta; };
+__global__ void __launch_bounds__(128) imm_act_permute_kernel(const ActBlockDev* __restrict__ blocks, const int* __restrict__ nbeg, int n_hosts, const int* __restrict__ perm, int n,
+                                                              ImmRO* __restrict__ sro, ImmRW* __restrict__ srw, sdv_immature_meta* __restrict__ smeta, int pass) {
+  const int k = blockIdx.x*blockDim.x + threadIdx.x; if (k >= n) return;
+  const int g = group_of_point(nbeg, n_hosts, k); const ActBlockDev& B = blocks[g]; const int j = k - __ldg(nbeg + g);
+  if (pass == 0) { const int o = perm[k]; sro[k] = B.ro[o]; srw[k] = B.rw[o]; smeta[k] = B.meta[o]; }
+  else { B.ro[j] = sro[k]; B.rw[j] = srw[k]; B.meta[j] = smeta[k]; }
+}
 }  // namespace sdv
 
 extern "C" {
@@ -432,4 +589,213 @@ int sdv_immature_optimize_batch(sdv_ctx* c, int n_groups, const int32_t* pt_begi
   return sdv_immature_optimize_batch_cams(c, n_groups, pt_begin, tgt_begin, target_frames, pre14, calib6, nullptr, min_obs, pts, is_from_sensor, res_stride, status_out, idepth_out, res_state_out);
 }
 
+// ---- the immature-point store
+int sdv_immature_store_set(sdv_ctx* c, uint64_t host_frame, int n, const sdv_immature_pt* pts, const sdv_immature_meta* meta) { SDV_GUARD_TRK(c);
+  if (!c || n < 0 || (n && !pts)) return SDV_ERR_ARG;
+  CK(cudaSetDevice(c->device));
+  std::vector<ImmRO> a(n); std::vector<ImmRW> b(n); std::vector<sdv_immature_meta> m(n);
+  for (int i = 0; i < n; i++) { imm_split(pts[i], a[i], b[i]); m[i] = meta ? meta[i] : sdv_immature_meta{1.f, -1, 0, 0.f}; }
+  ImmStore* S = imm_store(c); std::vector<ImmPlan> P; { int rc = imm_store_plan(c, S, 1, &host_frame, &n, P); if (rc) return rc; }
+  if (n) {                                                                               // pageable sources: staged before the copies return
+    const ImmBlock& blk = P[0].b;
+    if (cudaMemcpyAsync(blk.ro, a.data(), (size_t)n*sizeof(ImmRO), cudaMemcpyHostToDevice, c->st) != cudaSuccess ||
+        cudaMemcpyAsync(blk.rw, b.data(), (size_t)n*sizeof(ImmRW), cudaMemcpyHostToDevice, c->st) != cudaSuccess ||
+        cudaMemcpyAsync(blk.meta, m.data(), (size_t)n*sizeof(sdv_immature_meta), cudaMemcpyHostToDevice, c->st) != cudaSuccess) {
+      imm_store_abandon(S, P); cudaGetLastError(); return ctx_fail(c, SDV_ERR_CUDA, "immature_store_set: copies");
+    }
+  }
+  imm_store_commit(S, P);
+  return SDV_OK;
+}
+int sdv_immature_store_count(sdv_ctx* c, int n, const uint64_t* hosts, int32_t* counts_out) { SDV_GUARD_TRK(c);
+  if (!c || n < 0 || (n && (!hosts || !counts_out))) return SDV_ERR_ARG;
+  const ImmStore* S = (const ImmStore*)c->imm_store;
+  for (int i = 0; i < n; i++) if (!S || !S->blocks.count(hosts[i])) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_store_count: host %llu has no block", (unsigned long long)hosts[i]);
+  for (int i = 0; i < n; i++) counts_out[i] = S->blocks.at(hosts[i]).n;
+  return SDV_OK;
+}
+int sdv_immature_store_get(sdv_ctx* c, uint64_t host_frame, int cap, sdv_immature_pt* pts_out, sdv_immature_meta* meta_out, int32_t* n_out) { SDV_GUARD_TRK(c);
+  if (!c || !n_out || cap < 0) return SDV_ERR_ARG;
+  const ImmStore* S = (const ImmStore*)c->imm_store; auto it = S ? S->blocks.find(host_frame) : decltype(S->blocks.end())();
+  if (!S || it == S->blocks.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_store_get: host %llu has no block", (unsigned long long)host_frame);
+  const ImmBlock& blk = it->second; const int n = blk.n; *n_out = n;
+  if (cap < n) return ctx_fail(c, SDV_ERR_CAPACITY, "immature_store_get: host %llu holds %d points, room for %d", (unsigned long long)host_frame, n, cap);
+  if (n == 0 || (!pts_out && !meta_out)) return SDV_OK;
+  CK(cudaSetDevice(c->device));
+  std::vector<ImmRO> a(pts_out ? n : 0); std::vector<ImmRW> b(pts_out ? n : 0);
+  if (pts_out) { CK(cudaMemcpyAsync(a.data(), blk.ro, (size_t)n*sizeof(ImmRO), cudaMemcpyDeviceToHost, c->st)); CK(cudaMemcpyAsync(b.data(), blk.rw, (size_t)n*sizeof(ImmRW), cudaMemcpyDeviceToHost, c->st)); }
+  if (meta_out) CK(cudaMemcpyAsync(meta_out, blk.meta, (size_t)n*sizeof(sdv_immature_meta), cudaMemcpyDeviceToHost, c->st));
+  CK(cudaStreamSynchronize(c->st));
+  if (pts_out) for (int i = 0; i < n; i++) imm_join(a[i], b[i], pts_out[i]);
+  return SDV_OK;
+}
+int sdv_immature_store_drop(sdv_ctx* c, int n, const uint64_t* hosts) { SDV_GUARD_TRK(c);
+  if (!c || n < 0 || (n && !hosts)) return SDV_ERR_ARG;
+  ImmStore* S = (ImmStore*)c->imm_store;
+  for (int i = 0; i < n; i++) if (!S || !S->blocks.count(hosts[i])) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_store_drop: host %llu has no block", (unsigned long long)hosts[i]);
+  for (int i = 0; i < n; i++) { auto it = S->blocks.find(hosts[i]); if (it == S->blocks.end()) continue;          // named twice
+    S->spare.push_back(it->second); S->blocks.erase(it); }
+  return SDV_OK;
+}
+
+int sdv_immature_trace_store_batch(sdv_ctx* c, int n_groups, const uint64_t* hosts, const uint64_t* frames, const int32_t* cams, const float* KRKi9, const float* Kt3,
+                                   const float* aff2, int32_t* counts_out) { SDV_GUARD_TRK(c);
+  if (!c || n_groups < 0 || (n_groups && (!hosts || !frames || !KRKi9 || !Kt3 || !aff2))) return SDV_ERR_ARG;
+  if (n_groups == 0) return SDV_OK;
+  if (cams) for (int g = 0; g < n_groups; g++) if (cams[g] < 0 || cams[g] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "immature_trace_store: group %d names camera %d (valid: 0..%d)", g, cams[g], SDV_MAX_CAMERAS - 1);
+  const ImmStore* S = (const ImmStore*)c->imm_store;
+  std::vector<TraceStoreGroupDev> G(n_groups); std::vector<int> gbeg(n_groups + 1, 0); long long need_seq = 0;
+  std::unordered_map<uint64_t, int> seen; seen.reserve(2*n_groups);
+  for (int g = 0; g < n_groups; g++) {
+    auto bt = S ? S->blocks.find(hosts[g]) : decltype(S->blocks.end())();
+    if (!S || bt == S->blocks.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_trace_store: host %llu has no block (group %d)", (unsigned long long)hosts[g], g);
+    if (!seen.emplace(hosts[g], g).second) return ctx_fail(c, SDV_ERR_ARG, "immature_trace_store: host %llu in groups %d and %d", (unsigned long long)hosts[g], seen[hosts[g]], g);
+    auto it = c->frame_index.find(frames[g]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_trace_store: unknown frame %llu (group %d)", (unsigned long long)frames[g], g);
+    const int cam = cams ? cams[g] : 0; const FrameDev& f = c->frames[it->second]; { int rcs = check_frame_cam(c, f, cam, "immature_trace_store"); if (rcs) return rcs; }
+    if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
+    const ImmBlock& blk = bt->second; TraceStoreGroupDev& D = G[g];
+    D.I0 = f.I0; D.w = c->cam_w[cam]; D.h = c->cam_h[cam]; D.ro = blk.ro; D.rw = blk.rw;
+    for (int k = 0; k < 9; k++) D.KRKi[k] = KRKi9[9*g+k]; for (int k = 0; k < 3; k++) D.Kt[k] = Kt3[3*g+k]; D.aff[0] = aff2[2*g]; D.aff[1] = aff2[2*g+1];
+    gbeg[g+1] = gbeg[g] + blk.n;
+  }
+  const int n = gbeg[n_groups];
+  if (n == 0) { if (counts_out) memset(counts_out, 0, (size_t)6*n_groups*sizeof(int32_t)); return SDV_OK; }
+  CK(cudaSetDevice(c->device));
+  { int rc = join_ingest_upto(c, need_seq); if (rc) return rc; }
+  const size_t o_b = al16(n_groups*sizeof(TraceStoreGroupDev)), o_c = o_b + al16((n_groups + 1)*sizeof(int)), bytes = o_c + (size_t)6*n_groups*sizeof(int);
+  { int rc = trace_scratch(c, bytes); if (rc) return rc; }
+  char* d = (char*)c->trace_dev;
+  CK(cudaMemcpyAsync(d, G.data(), n_groups*sizeof(TraceStoreGroupDev), cudaMemcpyHostToDevice, c->st));       // pageable sources: staged before the calls return
+  CK(cudaMemcpyAsync(d + o_b, gbeg.data(), (n_groups + 1)*sizeof(int), cudaMemcpyHostToDevice, c->st));
+  if (counts_out) CK(cudaMemsetAsync(d + o_c, 0, (size_t)6*n_groups*sizeof(int), c->st));
+  CK(cudaEventRecord(c->ev0, c->st));
+  imm_trace_store_kernel<<<(n + 127)/128, 128, 0, c->st>>>((const TraceStoreGroupDev*)d, (const int*)(d + o_b), n_groups, n, trace_settings(c), counts_out ? (int*)(d + o_c) : nullptr);
+  c->launches += 1;
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(c->ev1, c->st));
+  if (counts_out) {
+    CK(cudaMemcpyAsync(counts_out, d + o_c, (size_t)6*n_groups*sizeof(int), cudaMemcpyDeviceToHost, c->st));
+    CK(cudaStreamSynchronize(c->st)); CK(cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
+  } else {                                                                               // returns with the kernel pending: a re-ingest or release of a traced frame waits for it
+    if (!c->ev_trk_async) CK(cudaEventCreateWithFlags(&c->ev_trk_async, cudaEventDisableTiming));
+    CK(cudaEventRecord(c->ev_trk_async, c->st));
+    for (int g = 0; g < n_groups; g++) c->frames[c->frame_index[frames[g]]].trk_async = true;
+  }
+  return SDV_OK;
+}
+
+}  // extern "C"
+
+extern "C" {
+int sdv_activate_points_store_batch(sdv_ctx* c, int n, const int32_t* host_begin, const uint64_t* hosts, const int32_t* flagged, const float* cKRKi9, const float* cKt3,
+                                    const int32_t* src_host_begin, const int32_t* src_pt_begin, const float* KRKi9, const float* Kt3, const float* uvid, const float* min_act_dist,
+                                    const float* pre14, const float* calib6, const int32_t* cams, int cap, int32_t* n_act_out, int32_t* act_host, int32_t* act_idx,
+                                    sdv_immature_pt* act_pts, sdv_immature_meta* act_meta, float* act_idepth, int32_t* act_res_state, int32_t* counts_out) { SDV_GUARD_TRK(c);
+  if (!c || n < 0 || cap < 0 || (n && (!host_begin || !hosts || !flagged || !cKRKi9 || !cKt3 || !src_host_begin || !src_pt_begin || !min_act_dist || !pre14 || !calib6 || !n_act_out)))
+    return SDV_ERR_ARG;
+  if (n == 0) return SDV_OK;
+  if (cap > 0 && (!act_host || !act_idx || !act_pts || !act_meta || !act_idepth || !act_res_state)) return SDV_ERR_ARG;
+  if (!c->sel) return ctx_fail(c, SDV_ERR_STATE, "activate_points_store: sdv_selector_init has not been called");
+  if (cams) for (int j = 0; j < n; j++) if (cams[j] < 0 || cams[j] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "activate_points_store: sequence %d names camera %d (valid: 0..%d)", j, cams[j], SDV_MAX_CAMERAS - 1);
+  if (host_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "activate_points_store: host_begin[0] must be 0");
+  for (int j = 0; j < n; j++) { const int nH = host_begin[j+1] - host_begin[j];
+    if (nH < 1 || nH > 16 || nH - 1 > SDV_MAX_FRAMES_WINDOW) return ctx_fail(c, SDV_ERR_ARG, "activate_points_store: sequence %d has %d keyframes (1..16, at most %d targets)", j, nH, SDV_MAX_FRAMES_WINDOW); }
+  const int NH = host_begin[n]; const ImmStore* S = (const ImmStore*)c->imm_store;
+  std::vector<int> seq_of(NH), gbeg(NH + 1, 0), pre_begin(n + 1, 0); std::vector<const FrameDev*> F(NH); std::vector<ActHostDev> HD(NH); long long need_seq = 0;
+  std::unordered_map<uint64_t, int> seen; seen.reserve(2*NH);
+  for (int j = 0; j < n; j++) { const int nH = host_begin[j+1] - host_begin[j]; pre_begin[j+1] = pre_begin[j] + nH*(nH - 1);
+    for (int g = host_begin[j]; g < host_begin[j+1]; g++) { seq_of[g] = j;
+      auto bt = S ? S->blocks.find(hosts[g]) : decltype(S->blocks.end())();
+      if (!S || bt == S->blocks.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "activate_points_store: host %llu has no block", (unsigned long long)hosts[g]);
+      if (!seen.emplace(hosts[g], g).second) return ctx_fail(c, SDV_ERR_ARG, "activate_points_store: host %llu appears twice", (unsigned long long)hosts[g]);
+      auto it = c->frame_index.find(hosts[g]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "activate_points_store: keyframe %llu is not resident", (unsigned long long)hosts[g]);
+      const FrameDev& f = c->frames[it->second]; { int rcs = check_frame_cam(c, f, cams ? cams[j] : 0, "activate_points_store"); if (rcs) return rcs; }
+      if (f.ingest_seq > need_seq) need_seq = f.ingest_seq; F[g] = &f;
+      const ImmBlock& blk = bt->second; HD[g] = ActHostDev{blk.ro, blk.rw, blk.meta, g == host_begin[j+1] - 1 ? 1 : 0, flagged[g] ? 1 : 0}; gbeg[g+1] = gbeg[g] + blk.n; } }
+  const int N = gbeg[NH];
+  CK(cudaSetDevice(c->device));
+  { int rc = join_ingest_upto(c, need_seq); if (rc) return rc; }
+  // scratch, sized once for every phase
+  const size_t nN = (size_t)std::max(N, 1), R = SDV_MAX_FRAMES_WINDOW; size_t off = 0;
+  auto take = [&](size_t b) { const size_t o = off; off += al16(b); return o; };
+  const size_t o_hd = take(NH*sizeof(ActHostDev)), o_gb = take((NH + 1)*sizeof(int)), o_code = take(nN*4), o_rows = take(nN*16), o_c4 = take(nN*16), o_idx = take(nN*4),
+               o_og = take(NH*sizeof(OptGroupDev)), o_ot = take((size_t)pre_begin[n]*sizeof(OptTargetDev) + 16), o_gof = take(nN*4), o_pts = take(nN*sizeof(sdv_immature_pt)),
+               o_meta = take(nN*16), o_fs = take(nN), o_st = take(nN*4), o_id = take(nN*4), o_rs = take(nN*R*4), o_perm = take(nN*4), o_nb = take((NH + 1)*sizeof(int)),
+               o_bd = take(NH*sizeof(ActBlockDev)), o_sro = take(nN*sizeof(ImmRO)), o_srw = take(nN*sizeof(ImmRW)), o_sme = take(nN*16), bytes = off;
+  { int rc = trace_scratch(c, bytes); if (rc) return rc; }
+  char* d = (char*)c->trace_dev;
+  // (1) the filter of :612-645 on the device; the host reads one code per point back (class and status, 4 bytes), no record
+  std::vector<int> code(nN, 0);
+  CK(cudaMemcpyAsync(d + o_hd, HD.data(), NH*sizeof(ActHostDev), cudaMemcpyHostToDevice, c->st));
+  CK(cudaMemcpyAsync(d + o_gb, gbeg.data(), (NH + 1)*sizeof(int), cudaMemcpyHostToDevice, c->st));
+  if (N) { imm_act_filter_kernel<<<(N + 127)/128, 128, 0, c->st>>>((const ActHostDev*)(d + o_hd), (const int*)(d + o_gb), NH, N, 3.0f /* setting_minTraceQuality, settings.cpp:131 */,
+                                                                 (int*)(d + o_code), (float4*)(d + o_rows)); c->launches += 1; CK(cudaGetLastError());
+           CK(cudaMemcpyAsync(code.data(), d + o_code, (size_t)N*4, cudaMemcpyDeviceToHost, c->st)); }
+  CK(cudaStreamSynchronize(c->st));
+  // (2) makeDistanceMap + the walk (:597-671) over the candidates, rows gathered on the device in host-then-point order
+  std::vector<int> cidx, cand_begin(NH + 1, 0);
+  for (int g = 0; g < NH; g++) { for (int i = gbeg[g]; i < gbeg[g+1]; i++) if ((code[i] & 3) == ACT_CAND) cidx.push_back(i); cand_begin[g+1] = (int)cidx.size(); }
+  const int NC = (int)cidx.size(); std::vector<int32_t> decision(std::max(NC, 1), 0);
+  if (NC) { CK(cudaMemcpyAsync(d + o_idx, cidx.data(), (size_t)NC*4, cudaMemcpyHostToDevice, c->st));
+            imm_act_rows_kernel<<<(NC + 127)/128, 128, 0, c->st>>>((const float4*)(d + o_rows), (const int*)(d + o_idx), NC, (float4*)(d + o_c4)); c->launches += 1; CK(cudaGetLastError()); }
+  { int rc = sel_activate_select(c, n, src_host_begin, src_pt_begin, KRKi9, Kt3, uvid, host_begin, cand_begin.data(), cKRKi9, cKt3, nullptr, (const float*)(d + o_c4), min_act_dist, cams,
+                                 decision.data(), nullptr); if (rc) return rc; }
+  // (3) optimizeImmaturePoint (min_obs 1) on the accepted candidates, toOptimize order, read from the store
+  std::vector<int> oidx, ohost; std::vector<int> opt_of(NC, -1);
+  for (int k = 0; k < NC; k++) if (decision[k] == 1) { opt_of[k] = (int)oidx.size(); oidx.push_back(cidx[k]); }
+  const int NO = (int)oidx.size(); std::vector<int> gof(std::max(NO, 1)); std::vector<OptGroupDev> OG(NH); std::vector<OptTargetDev> OT(pre_begin[n]);
+  { int k = 0; for (int g = 0; g < NH; g++) while (k < NO && oidx[k] < gbeg[g+1]) gof[k++] = g; }
+  for (int g = 0; g < NH; g++) { const int j = seq_of[g], h0 = host_begin[j], nH = host_begin[j+1] - h0, h = g - h0, cam = cams ? cams[j] : 0; const float* q = calib6 + 6*j;
+    OptGroupDev& G = OG[g]; G.tgt_begin = pre_begin[j] + h*(nH - 1); G.nres = nH - 1; G.fxl = q[0]; G.fyl = q[1]; G.cxl = q[2]; G.cyl = q[3]; G.fxli = q[4]; G.fyli = q[5]; G.w = c->cam_w[cam]; G.h = c->cam_h[cam];
+    int t = 0; for (int tg = h0; tg < h0 + nH; tg++) { if (tg == g) continue; OptTargetDev& T = OT[G.tgt_begin + t]; const float* r = pre14 + 14*(size_t)(G.tgt_begin + t); t++;
+      T.I0 = F[tg]->I0; for (int e = 0; e < 9; e++) T.R[e] = r[e]; for (int e = 0; e < 3; e++) T.t[e] = r[9+e]; T.aff[0] = r[12]; T.aff[1] = r[13]; } }
+  std::vector<sdv_immature_pt> opts(NO); std::vector<sdv_immature_meta> ometa(NO); std::vector<int> ost(NO); std::vector<float> oid(NO); std::vector<int> ors((size_t)NO*R);
+  if (NO) {
+    CK(cudaMemcpyAsync(d + o_idx, oidx.data(), (size_t)NO*4, cudaMemcpyHostToDevice, c->st));
+    CK(cudaMemcpyAsync(d + o_og, OG.data(), NH*sizeof(OptGroupDev), cudaMemcpyHostToDevice, c->st));
+    if (!OT.empty()) CK(cudaMemcpyAsync(d + o_ot, OT.data(), OT.size()*sizeof(OptTargetDev), cudaMemcpyHostToDevice, c->st));
+    CK(cudaMemcpyAsync(d + o_gof, gof.data(), (size_t)NO*4, cudaMemcpyHostToDevice, c->st));
+    imm_act_gather_kernel<<<(NO + 127)/128, 128, 0, c->st>>>((const ActHostDev*)(d + o_hd), (const int*)(d + o_gb), NH, (const int*)(d + o_idx), NO, (sdv_immature_pt*)(d + o_pts),
+                                                            (sdv_immature_meta*)(d + o_meta), (unsigned char*)(d + o_fs));
+    imm_optimize_kernel<<<(NO + 63)/64, 64, 0, c->st>>>((const OptGroupDev*)(d + o_og), (const OptTargetDev*)(d + o_ot), (const int*)(d + o_gof), NO, (const sdv_immature_pt*)(d + o_pts),
+                                                        (const unsigned char*)(d + o_fs), 1, (int)R, (int*)(d + o_st), (float*)(d + o_id), (int*)(d + o_rs), c->set.huberTH);
+    c->launches += 2; CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(ost.data(), d + o_st, (size_t)NO*4, cudaMemcpyDeviceToHost, c->st)); CK(cudaMemcpyAsync(oid.data(), d + o_id, (size_t)NO*4, cudaMemcpyDeviceToHost, c->st));
+    CK(cudaMemcpyAsync(ors.data(), d + o_rs, (size_t)NO*R*4, cudaMemcpyDeviceToHost, c->st));
+    CK(cudaMemcpyAsync(opts.data(), d + o_pts, (size_t)NO*sizeof(sdv_immature_pt), cudaMemcpyDeviceToHost, c->st));
+    CK(cudaMemcpyAsync(ometa.data(), d + o_meta, (size_t)NO*16, cudaMemcpyDeviceToHost, c->st));
+    CK(cudaStreamSynchronize(c->st));
+  }
+  std::vector<int> nact(n, 0); int total = 0; for (int k = 0; k < NO; k++) if (ost[k] == 1) { nact[seq_of[gof[k]]]++; total++; }
+  if (total > cap) return ctx_fail(c, SDV_ERR_CAPACITY, "activate_points_store: %d points activated, room for %d", total, cap);    // nothing has changed yet
+  // (4) the post pass (:683-707) and the swap-with-back compaction of every host's vector (:709-720)
+  std::vector<char> dead(nN, 0);
+  for (int i = 0; i < N; i++) if ((code[i] & 3) == ACT_DELETE) dead[i] = 1;
+  for (int k = 0; k < NC; k++) if (decision[k] == -1) dead[cidx[k]] = 1;
+  for (int k = 0; k < NO; k++) if (ost[k] == 1 || ost[k] == -1 || (code[oidx[k]] >> 4) == IPS_OOB) dead[oidx[k]] = 1;
+  std::vector<int> perm, nbeg(NH + 1, 0); std::vector<ActBlockDev> BD(NH);
+  for (int g = 0; g < NH; g++) { std::vector<int> v(gbeg[g+1] - gbeg[g]); for (size_t i = 0; i < v.size(); i++) v[i] = (int)i;
+    for (int i = 0; i < (int)v.size(); i++) if (dead[gbeg[g] + v[i]]) { v[i] = v.back(); v.pop_back(); i--; }
+    perm.insert(perm.end(), v.begin(), v.end()); nbeg[g+1] = (int)perm.size(); BD[g] = ActBlockDev{const_cast<ImmRO*>(HD[g].ro), const_cast<ImmRW*>(HD[g].rw), const_cast<sdv_immature_meta*>(HD[g].meta)}; }
+  const int NP = (int)perm.size();
+  if (NP) {
+    CK(cudaMemcpyAsync(d + o_perm, perm.data(), (size_t)NP*4, cudaMemcpyHostToDevice, c->st)); CK(cudaMemcpyAsync(d + o_nb, nbeg.data(), (NH + 1)*sizeof(int), cudaMemcpyHostToDevice, c->st));
+    CK(cudaMemcpyAsync(d + o_bd, BD.data(), NH*sizeof(ActBlockDev), cudaMemcpyHostToDevice, c->st));
+    for (int pass = 0; pass < 2; pass++)
+      imm_act_permute_kernel<<<(NP + 127)/128, 128, 0, c->st>>>((const ActBlockDev*)(d + o_bd), (const int*)(d + o_nb), NH, (const int*)(d + o_perm), NP, (ImmRO*)(d + o_sro),
+                                                                (ImmRW*)(d + o_srw), (sdv_immature_meta*)(d + o_sme), pass);
+    c->launches += 2; CK(cudaGetLastError());
+  }
+  ImmStore* SW = (ImmStore*)c->imm_store;
+  for (int g = 0; g < NH; g++) { SW->blocks[hosts[g]].n = nbeg[g+1] - nbeg[g]; if (counts_out) counts_out[g] = nbeg[g+1] - nbeg[g]; }
+  // activated points, toOptimize order: what new PointHessian(ph) copies, its idepth and the residual states of FullSystemOptPoint.cpp:157-177
+  int o = 0;
+  for (int k = 0; k < NO; k++) if (ost[k] == 1) { const int g = gof[k];
+    act_host[o] = g; act_idx[o] = oidx[k] - gbeg[g]; act_pts[o] = opts[k]; act_meta[o] = ometa[k]; act_idepth[o] = oid[k];
+    for (size_t r = 0; r < R; r++) act_res_state[(size_t)o*R + r] = ors[(size_t)k*R + r];
+    o++; }
+  for (int j = 0; j < n; j++) n_act_out[j] = nact[j];
+  CK(cudaStreamSynchronize(c->st));
+  return SDV_OK;
+}
 }  // extern "C"
