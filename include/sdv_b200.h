@@ -455,6 +455,11 @@ int  sdv_selector_init(sdv_ctx* c, const uint8_t* random_pattern, int n_slots);
 int  sdv_selector_potential(sdv_ctx* c, int slot, int set_to /* <= 0: leave */, int* out);
 int  sdv_selector_get_map(sdv_ctx* c, int slot, uint8_t* out_wh);
 int  sdv_selector_set_slot_cams(sdv_ctx* c, int n, const int32_t* slots, const int32_t* cams);
+/* The running LiDAR pixel box FullSystem::left, right, up, down (FullSystem.h:191-194) belongs to the sequence, like selectionMap: every selector slot keeps
+ * one on the device.  It is {10000, -1, 10000, -1} when the slot is created (sdv_selector_init) and whenever a rebind to a camera of another size starts the
+ * slot afresh; sdv_lidar_handler_rows_batch reads and updates it.  set_to (may be NULL: leave) writes it, stream-ordered after the handler calls enqueued
+ * so far (a mid-drive start); lrud_out (may be NULL) reads it back, waiting for those calls.  A slot out of range returns SDV_ERR_ARG. */
+int  sdv_selector_lidar_box(sdv_ctx* c, int slot, const int32_t* set_to, int32_t* lrud_out);
 /* void PixelSelector::makeHists(const FrameHessian*): ths / thsSmoothed of the (w/32) x (h/32) blocks */
 int  sdv_selector_make_hists(sdv_ctx* c, uint64_t frame, float* ths_out, float* thsSmoothed_out);
 int  sdv_selector_make_hists_cam(sdv_ctx* c, int cam, uint64_t frame, float* ths_out, float* thsSmoothed_out);
@@ -477,6 +482,16 @@ int  sdv_make_new_traces_batch(sdv_ctx* c, int n, const int32_t* slots, const ui
  * idepth_fromSensor} of the sdv_new_trace record.  n_out / num_points2 as above; cap bounds the points of a job as above.  A frame named twice returns SDV_ERR_ARG. */
 int  sdv_make_new_traces_store_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const float* density_lidar,
                                      const float* density_dense, const int32_t* add_feature_point, int cap, int32_t* n_out, int32_t* num_points2);
+/* FullSystem::makeNewTraces (FullSystem.cpp:1273-1356) fed from the LiDAR row sets (sdv_lidar_handler_rows_batch): sdv_make_new_traces_store_batch with job j's rows,
+ * box and flag taken from frames[j]'s row set, which never leaves the device — density_lidar = ((float)((right-left)*(down-up)) / (float)(w_c*h_c)) * desired_density[j]
+ * from the set's box and the slot camera's size (:1287-1290), density_dense = desired_density[j], add_feature_point = the set's addFeaturePoint.  Outputs and rules
+ * as sdv_make_new_traces_store_batch.  A frame without a row set returns SDV_ERR_NOFRAME, an overflowed set SDV_ERR_CAPACITY; either way no block and no selector
+ * state changes.  The call waits for the device (the potential adaptation runs on the host), after reading every job's header in one copy.
+ * Difference from the reference: there, addFeaturePoint and the box are whatever the LATEST lidarCloudHandler left; here they are the snapshot taken with frames[j]'s
+ * sweep.  The two agree whenever a frame's keyframe work runs before the next sweep is handled — the sequential order of process() (main.cpp:470-508), and what
+ * the host-row path gives. */
+int  sdv_make_new_traces_rows_store_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const float* desired_density, int cap, int32_t* n_out,
+                                          int32_t* num_points2);
 /* The selection half of void FullSystem::activatePointsMT() for n sequences: CoarseDistanceMap::makeDistanceMap from the ACTIVE points of the other keyframes, then the
  * candidate walk :600-671 with addIntoDistFinal after every accept.  Sequence j owns source keyframes host_begin[j] .. host_begin[j+1] (their points: uvid rows
  * pt_begin[k] .. pt_begin[k+1] = {u, v, idepth_scaled}; KRKi9 / Kt3 per keyframe = K[1] R K[0]^-1, K[1] t of host -> newest, FullSystem.cpp:606-608) and candidate
@@ -507,6 +522,25 @@ int  sdv_lidar_handler_batch(sdv_ctx* c, int n, const int32_t* sweep_begin, cons
                              double* cloud3_out, int32_t* n_out, int32_t* add_feature_point_out, int32_t* stats_out);
 int  sdv_lidar_handler_batch_cams(sdv_ctx* c, int n, const int32_t* sweep_begin, const float* xyzi, const double* Rlc9, const double* tlc3, const float* K4, const int32_t* cams,
                                   int32_t* lrud_io, int cap, double* cloud3_out, int32_t* n_out, int32_t* add_feature_point_out, int32_t* stats_out);
+/* Row sets: FullSystem::qCloudPixel on the device, keyed by frame handle.  lidarCloudHandler (main.cpp:785-858) pushes a sweep's rows, process() pairs the front
+ * image with the front cloud and pops both after addActiveFrame (main.cpp:470-508); keying the rows by the handle the paired image gets makes that pairing
+ * explicit and lets a sweep be ingested ahead of its image (the frame need not be resident).  A set holds up to its deposit's cap rows {Ku, Kv, depth} (doubles,
+ * the reference's order) and a header: the true row count (also past cap), an overflow mark, the running box {left, right, up, down} as it stood after this
+ * sweep, addFeaturePoint, numGround and the size of segmentedCloud.  A deposit under an existing handle replaces its set.  Blocks are reused in place when the
+ * new cap fits, else a spare or a new allocation with headroom is taken; dropped sets become spares.  Tracker call domain.
+ * sdv_lidar_handler_rows_batch: the handler of sdv_lidar_handler_batch_cams writing into row sets.  Sweep j belongs to the sequence on selector slot slots[j]: its
+ * camera is the slot's (its size bounds the box, main.cpp:828), the box is the slot's (sdv_selector_lidar_box) and is updated on the device, the rows go into
+ * frames[j]'s set.  Refused before anything is enqueued, changing nothing: sdv_lidar_init or sdv_selector_init missing (SDV_ERR_STATE); a slot out of range,
+ * a slot or a frame named twice, cap < 1 (SDV_ERR_ARG).  Without stats_out the call enqueues and returns: the sweep upload goes on the copy stream, so it
+ * overlaps tracking already enqueued, and the kernels wait for it by event.  Pinned xyzi must stay valid until the next call that synchronises (as for the image
+ * uploads).  With stats_out it waits and fills {rows, numGround, n_segmented, addFeaturePoint, overflow} per sweep.  More rows than cap keep the true count in
+ * the header and mark the set; nothing is written past cap, and every consumer of the set returns SDV_ERR_CAPACITY.
+ * sdv_lidar_rows_get: frame's rows (cap: room in cloud3_out; cloud3_out NULL: header only), *n_out = the true count, the box and the flag; waits.
+ * sdv_lidar_rows_drop: qCloudPixel.pop() (main.cpp:507) for n frames.  A handle without a set returns SDV_ERR_NOFRAME from both and changes nothing. */
+int  sdv_lidar_handler_rows_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* sweep_begin, const float* xyzi, const double* Rlc9,
+                                  const double* tlc3, const float* K4, int cap, int32_t* stats_out);
+int  sdv_lidar_rows_get(sdv_ctx* c, uint64_t frame, int cap, double* cloud3_out, int32_t* n_out, int32_t* lrud_out, int32_t* add_feature_point_out);
+int  sdv_lidar_rows_drop(sdv_ctx* c, int n, const uint64_t* frames);
 
 #ifdef __cplusplus
 }

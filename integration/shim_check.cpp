@@ -347,6 +347,27 @@ int shim_set_immatures(FrameHessian* host, const std::vector<sdv_immature_pt>& p
   return sdv_immature_store_set(gpu, (uint64_t)host->shell->id, (int)pts.size(), pts.data(), meta.empty() ? nullptr : meta.data());
 }
 
+// ------------------------------------------------------------------------------------------------ LiDAR row sets (sdv_lidar_handler_rows_batch, sdv_lidar_rows_*)
+// FullSystem::qCloudPixel holds frame handles; the rows, the box FullSystem::left/right/up/down (FullSystem.h:191-194) and addFeaturePoint stay on the device
+struct RowsQueue { std::vector<uint64_t> qCloudPixel; int32_t slot; };
+// void lidarCloudHandler(const sensor_msgs::PointCloud2ConstPtr&)  main.cpp:785-858: the sweep is deposited under the id its paired image will get; nothing waits
+int shim_lidarCloudHandler_rows(RowsQueue& fsys, const LidarRig& rig, uint64_t next_frame_id, const float* xyzi, int n) {
+  const int32_t sweep_begin[2] = {0, n}; const float K4[4] = {rig.fx, rig.fy, rig.cx, rig.cy};
+  int rc = sdv_lidar_handler_rows_batch(gpu, 1, &fsys.slot, &next_frame_id, sweep_begin, xyzi, rig.Rlc, rig.tlc, K4, /*cap*/64*1800, nullptr);
+  if (!rc) fsys.qCloudPixel.push_back(next_frame_id);                                     // -> fullSystem->qCloudPixel.push(vCloudPixel)
+  return rc;
+}
+// void FullSystem::makeNewTraces(FrameHessian* newFrame, float*)  FullSystem.cpp:1273-1356: rows, box and addFeaturePoint of newFrame's set; points into its store block
+int shim_makeNewTraces_rows(FrameHessian* newFrame, const RowsQueue& fsys, int32_t& nImmature) {
+  const uint64_t id = (uint64_t)newFrame->shell->id; const float dens = setting_desiredImmatureDensity; int32_t num[2];
+  return sdv_make_new_traces_rows_store_batch(gpu, 1, &fsys.slot, &id, &dens, 1 << 14, &nImmature, num);
+}
+// process() (main.cpp:470-508): after addActiveFrame, qCloudPixel.pop() with the image
+int shim_process_pop(RowsQueue& fsys) {
+  if (fsys.qCloudPixel.empty()) return SDV_OK;
+  const uint64_t id = fsys.qCloudPixel.front(); fsys.qCloudPixel.erase(fsys.qCloudPixel.begin()); return sdv_lidar_rows_drop(gpu, 1, &id);
+}
+
 // referenced so that -Wunused does not hide a missing call path
 int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const Undistort* u, const uint8_t* raw) {
   std::vector<int32_t> sel, st; Vec5 mr{}; SE3 T; AffLight a;
@@ -364,6 +385,7 @@ int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const 
     rc |= shim_makeNewTraces_store(fh, rig, 0, px, ni) | shim_traceNewCoarse_store(fh, sh, &st) | shim_read_immatures(fh, rc2, me) | shim_set_immatures(fh, rc2, me) | shim_drop_immatures(fh);
     std::vector<float> idp2; std::vector<int32_t> rs2, cn2; const float cal6[6] = {1, 1, 0, 0, 1, 1};
     rc |= shim_activatePoints_store({(uint64_t)fh->shell->id}, {0}, ai, {}, cal6, rc2, idp2, rs2, cn2); }
+  { RowsQueue q{{}, 0}; int32_t ni = 0; rc |= shim_lidarCloudHandler_rows(q, rig, (uint64_t)fh->shell->id, nullptr, 0) | shim_makeNewTraces_rows(fh, q, ni) | shim_process_pop(q); }
   fs.optimize(6); fs.set_map(0); fs.handover(sel, st); fs.trackNewCoarse(fh); fs.refine_only(fh); shim_frame_destructor(fh);
   return rc;
 }

@@ -116,6 +116,11 @@ def _load():
     L.sdv_activate_points_store_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _i32p, _f32p, _f32p, _i32p, _i32p, _vp, _vp, _vp, _f32p, _f32p, _f32p, _vp, C.c_int, _i32p,
                                                   _vp, _vp, _vp, _vp, _vp, _vp, _vp]
     L.sdv_make_new_traces_store_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _i32p, _vp, _f32p, _f32p, _i32p, C.c_int, _i32p, _i32p]
+    L.sdv_selector_lidar_box.argtypes = [_vp, C.c_int, _vp, _vp]
+    L.sdv_lidar_handler_rows_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _i32p, _vp, _f64p, _f64p, _f32p, C.c_int, _vp]
+    L.sdv_lidar_rows_get.argtypes = [_vp, C.c_uint64, C.c_int, _vp, C.POINTER(C.c_int32), _vp, C.POINTER(C.c_int32)]
+    L.sdv_lidar_rows_drop.argtypes = [_vp, C.c_int, _u64p]
+    L.sdv_make_new_traces_rows_store_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _f32p, C.c_int, _i32p, _i32p]
     return L
 
 
@@ -856,6 +861,19 @@ class PixelSelector:
                                                         np.ascontiguousarray(np.broadcast_to(add_feature_point, n), np.int32), cap, n_out, num))
         return n_out, num.reshape(n, 2)
 
+    def lidarBox(self, slot=0, set_to=None):
+        """FullSystem::left, right, up, down of the sequence on `slot` (set_to: write it first, e.g. for a start in mid-drive) -> int32 (4,)"""
+        o = np.zeros(4, np.int32); st = None if set_to is None else np.ascontiguousarray(set_to, np.int32).reshape(4)
+        self.ctx._ck(LIB.sdv_selector_lidar_box(self.ctx.p, int(slot), None if st is None else st.ctypes.data, o.ctypes.data)); return o
+
+    def makeNewTracesRowsStore(self, slots, frame_ids, desired_density, cap=1 << 14):
+        """makeNewTracesStore fed from the LiDAR row sets of frame_ids (LidarFrontEnd.handleRows): rows, box and addFeaturePoint of each frame's set, which never come
+        to the host; density_lidar follows from the set's box and the slot's camera size -> points per job (n,), numPoints (n,2)"""
+        n = len(slots); n_out = np.zeros(n, np.int32); num = np.zeros(2 * n, np.int32)
+        self.ctx._ck(LIB.sdv_make_new_traces_rows_store_batch(self.ctx.p, n, np.ascontiguousarray(slots, np.int32), np.ascontiguousarray(frame_ids, np.uint64),
+                                                             np.ascontiguousarray(np.broadcast_to(desired_density, n), np.float32), cap, n_out, num))
+        return n_out, num.reshape(n, 2)
+
 
 def packActivation(seqs, cams=None):
     """the flat arrays sdv_activate_select_batch(_cams) takes, from per-sequence dicts with pt_begin / KRKi / Kt / uvid (source keyframes) and cand_begin / cKRKi / cKt / cand4 /
@@ -926,3 +944,35 @@ class LidarFrontEnd:
         else:
             self.ctx._ck(LIB.sdv_lidar_handler_batch_cams(self.ctx.p, n, sb, allp.ctypes.data, R, t, K, cm.ctypes.data, lr.reshape(-1), cap, out.ctypes.data, n_out, add, st))
         return [dict(cloud_px=out[j, :n_out[j]].copy(), lrud=lr[j], numGround=int(st[2 * j]), n_segmented=int(st[2 * j + 1]), addFeaturePoint=int(add[j])) for j in range(n)]
+
+    def handleRows(self, slots, frame_ids, sweeps, Rlc, tlc, K4, cap=None, stats=False, sweep_begin=None):
+        """the handler writing into row sets (FullSystem::qCloudPixel on the device): sweep j belongs to the sequence on selector slot slots[j] (its camera, its pixel box),
+        its rows go into frame_ids[j]'s set.  sweeps: list of (n,4) float32 XYZI arrays, or with sweep_begin ONE packed host buffer (pinned or not: pinned memory must stay
+        valid until the next call that synchronises).  stats=False: enqueue and return None; True: wait -> per sweep dict rows, numGround, n_segmented,
+        addFeaturePoint, overflow"""
+        if sweep_begin is None:
+            sw = [np.ascontiguousarray(s, np.float32).reshape(-1, 4) for s in sweeps]; sb = np.concatenate([[0], np.cumsum([len(s) for s in sw])]).astype(np.int32)
+            allp = np.ascontiguousarray(np.concatenate(sw) if sb[-1] else np.zeros((1, 4), np.float32))
+        else:
+            sb = np.ascontiguousarray(sweep_begin, np.int32); allp = sweeps; assert allp.dtype == np.float32 and allp.flags.c_contiguous
+        n = len(sb) - 1; cap = cap or self.n_scan * self.horizon
+        R = np.ascontiguousarray(np.broadcast_to(np.asarray(Rlc, np.float64).reshape(-1, 9), (n, 9))).reshape(-1); t = np.ascontiguousarray(np.broadcast_to(np.asarray(tlc, np.float64).reshape(-1, 3), (n, 3))).reshape(-1)
+        K = np.ascontiguousarray(np.broadcast_to(np.asarray(K4, np.float32).reshape(-1, 4), (n, 4))).reshape(-1); st = np.zeros((n, 5), np.int32) if stats else None
+        self.ctx._ck(LIB.sdv_lidar_handler_rows_batch(self.ctx.p, n, np.ascontiguousarray(slots, np.int32), np.ascontiguousarray(frame_ids, np.uint64), sb, allp.ctypes.data, R, t, K, cap,
+                                                      None if st is None else st.ctypes.data))
+        if st is None:
+            return None
+        return [dict(rows=int(r[0]), numGround=int(r[1]), n_segmented=int(r[2]), addFeaturePoint=int(r[3]), overflow=int(r[4])) for r in st]
+
+    def rows(self, frame_id):
+        """frame_id's row set -> dict like handle()'s: cloud_px (the rows), lrud (the box after its sweep), addFeaturePoint"""
+        n = C.c_int32(0); add = C.c_int32(0); lr = np.zeros(4, np.int32)
+        self.ctx._ck(LIB.sdv_lidar_rows_get(self.ctx.p, int(frame_id), 0, None, C.byref(n), lr.ctypes.data, C.byref(add)))
+        out = np.zeros((n.value, 3))
+        if n.value:
+            self.ctx._ck(LIB.sdv_lidar_rows_get(self.ctx.p, int(frame_id), n.value, out.ctypes.data, C.byref(n), None, None))
+        return dict(cloud_px=out, lrud=lr, addFeaturePoint=int(add.value))
+
+    def dropRows(self, frame_ids):
+        """qCloudPixel.pop() for frame_ids (main.cpp:507)"""
+        f = np.ascontiguousarray(np.atleast_1d(frame_ids), np.uint64); self.ctx._ck(LIB.sdv_lidar_rows_drop(self.ctx.p, len(f), f))

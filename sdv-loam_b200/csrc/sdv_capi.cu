@@ -229,6 +229,7 @@ void sdv_destroy(sdv_ctx* c) {
   rp_destroy(c);
   sel_destroy(c);
   lidar_destroy(c);
+  lidar_rows_destroy(c);
   imm_store_destroy(c);
   ba_destroy(c);
   if (c->ba_ev0) cudaEventDestroy(c->ba_ev0); if (c->ba_ev1) cudaEventDestroy(c->ba_ev1); if (c->ev_xdom) cudaEventDestroy(c->ev_xdom); if (c->st_ba) cudaStreamDestroy(c->st_ba);

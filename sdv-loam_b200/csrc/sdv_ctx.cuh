@@ -74,6 +74,7 @@ struct sdv_ctx {
   cudaEvent_t ev_trk_async = nullptr;           // recorded on st after the last call that returned with a kernel still reading frames (FrameDev::trk_async)
   void* imm_store = nullptr;                    // sdv::ImmStore: device-resident immature points, one block per host keyframe (sdv_trace.cu)
   void* lidar = nullptr;                        // sdv::LidarState: engine of the LiDAR front-end (sdv_lidar.cu)
+  void* lidar_rows = nullptr;                   // sdv::RowStore: LiDAR pixel rows per frame handle, FullSystem::qCloudPixel on the device (sdv_lidar.cu)
   void* sel = nullptr;                          // sdv::SelState: PixelSelector slots + engine of the candidate management (sdv_select.cu)
   sdv::RpState* rp = nullptr;                   // map slots + scratch of the Reprojector path (sdv_reproject.cu)
   sdv::BAState* ba = nullptr;                   // selected back-end window
@@ -88,6 +89,14 @@ void rp_destroy(sdv_ctx* c);
 void sel_destroy(sdv_ctx* c);
 void lidar_destroy(sdv_ctx* c);
 void imm_store_destroy(sdv_ctx* c);
+void lidar_rows_destroy(sdv_ctx* c);
+// the header of a frame's LiDAR row set as the handler left it (sdv_lidar_handler_rows_batch)
+struct LidarRowsInfo { int rows, overflow, lrud[4], addFeaturePoint, numGround, n_segmented, room; };   // rows: true count; room: rows the set can hold
+// row sets of frames[j]: their device rows and headers (one copy back, waits for the tracker stream); SDV_ERR_NOFRAME for a frame without a set
+int  lidar_rows_fetch(sdv_ctx* c, int n, const uint64_t* frames, const double** rows_dev, LidarRowsInfo* info, const char* who);
+int  sel_n_slots(const sdv_ctx* c);                                                      // selector slots (sdv_selector_init), -1 without a selector
+// selector slot `slot` (in range): its camera and its running LiDAR pixel box FullSystem::left/right/up/down (4 ints on the device)
+void sel_slot_box(const sdv_ctx* c, int slot, int* cam, int** box_dev);
 // makeNewTraces into the store: job j's n[j] records (sel::NewTrace / sel::ImmPt device arrays, stream-ordered on c->st) replace the block of hosts[j]
 int  imm_store_deposit(sdv_ctx* c, int nj, const uint64_t* hosts, const int* n, const void* const* new_trace_dev, const void* const* imm_dev);
 int  sel_activate_select(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,

@@ -10,6 +10,8 @@
 //                                     the row set, like lineCountFlag), feasibility = size >= 30 or (size >= 5 and >= 3 rows)
 //   lidarCloudHandler   :785-858   -> lf_keep_kernel (Rlc p + tlc in fp64, pinhole projection in float, image bounds), lf_scan_kernel (raster-order compaction),
 //                                     lf_emit_kernel (rows {Ku, Kv, depth}, running pixel box by atomicMin/Max, ground count -> addFeaturePoint)
+// Two host paths share the nine launches: handle() copies the rows and the box back and waits; handle_rows() (the row sets of sdv_lidar.cu) writes the rows into a
+// caller-owned device block, seeds the box from device memory (lf_rows_seed_kernel), writes a header and the box back (lf_rows_finalize_kernel) and need not wait.
 // Float math: the reference's build resolves atan2 / sqrt / sin / cos of floats to the float overloads (FullSystem.h:19 includes <math.h>).  sqrtf and the divisions are IEEE
 // on both sides; atan2f is NOT specified by IEEE, so the device carries a restatement of the C library's algorithm (fdlibm e_atan2f.c / s_atanf.c — float operations
 // only, bit-identical to glibc 2.39's atan2f on 2e7 random arguments, tests/test_select_emu_cpu.py::test_atan2f_matches_libm); sinf / cosf are only ever taken of the two
@@ -185,49 +187,114 @@ __global__ void __launch_bounds__(128) lf_emit_kernel(const LidarJob* __restrict
   if (f == 2) atomicAdd(&J.counters[1], 1);
 }
 
+// ---- device-output path (sdv_lidar_handler_rows_batch): the rows go straight into a row set's block, the running pixel box is read from and written back to
+// device memory (the selector slot's), and nothing waits for the device
+struct RowsHdr { int rows, overflow, left, right, up, down, addFeaturePoint, numGround, n_segmented, pad_[7]; };   // 64 B ahead of the block's rows; rows: the true count
+struct RowsJob { int* counters; int* box; RowsHdr* hdr; int cap; };
+__global__ void __launch_bounds__(128) lf_rows_seed_kernel(const RowsJob* __restrict__ jobs, int nj) {            // thread per sweep: the box as the previous sweep left it
+  const int j = blockIdx.x*blockDim.x + threadIdx.x; if (j >= nj) return;
+  const RowsJob R = jobs[j];
+  for (int k = 0; k < 4; k++) R.counters[2+k] = R.box[k];
+}
+__global__ void __launch_bounds__(128) lf_rows_finalize_kernel(const RowsJob* __restrict__ jobs, int nj) {        // thread per sweep: header + the slot's new box
+  const int j = blockIdx.x*blockDim.x + threadIdx.x; if (j >= nj) return;
+  const RowsJob R = jobs[j]; const int* c = R.counters; RowsHdr h;
+  h.rows = c[0]; h.overflow = c[0] > R.cap ? 1 : 0; h.left = c[2]; h.right = c[3]; h.up = c[4]; h.down = c[5]; h.numGround = c[1]; h.n_segmented = c[6];
+  h.addFeaturePoint = ((float)c[1] / (float)c[0] > 0.8) ? 1 : 0;                                                     // :851-854, the host path's expression (0/0: NaN, 0)
+  for (int k = 0; k < 7; k++) h.pad_[k] = 0;
+  *R.hdr = h;
+  for (int k = 0; k < 4; k++) R.box[k] = c[2+k];
+}
+#ifdef SDV_EMU
+static inline cudaError_t cudaStreamWaitEvent(cudaStream_t, cudaEvent_t, unsigned) { return 0; }                   // one host thread: every copy and launch is in order already
+#endif
+
 // ================================================================================================ host engine
 struct LidarEngine {
   LidarSet S; cudaStream_t st = nullptr; std::string err; Scratch io; long long launches = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr; bool have_ev = false; float last_kernel_ms = 0.f;   // device time of the nine launches of the last handle() (copies excluded)
+  cudaStream_t st_up = nullptr;                                                                 // copy stream of the device-output path's sweep uploads (nullptr: st)
+  cudaEvent_t ev_up = nullptr, ev_done = nullptr; bool have_sync_ev = false;                    // uploads done / the kernels of the last call done (they read the staging)
   // sinf / cosf of the two angular resolutions come from the host's libm (only these four values are ever needed)
   void init(int n_scan, int horizon, float ang_res_x, float ang_res_y, float ang_bottom, int groundScanInd, cudaStream_t st_) {
     if (!have_ev) { have_ev = (cudaEventCreate(&ev0) == cudaSuccess && cudaEventCreate(&ev1) == cudaSuccess); }
+    if (!have_sync_ev) { have_sync_ev = (cudaEventCreate(&ev_up) == cudaSuccess && cudaEventCreate(&ev_done) == cudaSuccess); }
     st = st_; S.N = n_scan; S.H = horizon; S.ang_res_x = ang_res_x; S.ang_res_y = ang_res_y; S.ang_bottom = ang_bottom; S.groundScanInd = groundScanInd; S.sensorMountAngle = 0.0f;
     S.segmentTheta = (float)(60.0/180.0*M_PI); const float ax = (float)(ang_res_x / 180.0 * M_PI), ay = (float)(ang_res_y / 180.0 * M_PI);           // main.cpp:118-122
     S.sinX = sinf(ax); S.cosX = cosf(ax); S.sinY = sinf(ay); S.cosY = cosf(ay); S.validPointNum = 5; S.validLineNum = 3;
   }
-  void destroy() { io.release(); if (have_ev) { cudaEventDestroy(ev0); cudaEventDestroy(ev1); have_ev = false; } }
+  void destroy() { io.release(); if (have_ev) { cudaEventDestroy(ev0); cudaEventDestroy(ev1); have_ev = false; }
+                   if (have_sync_ev) { cudaEventDestroy(ev_up); cudaEventDestroy(ev_done); have_sync_ev = false; } }
   struct Sweep { const float* xyzi_host; int n; double R[9], t[3]; float K[4]; int w, h; int lrud[4];      // in (lrud: FullSystem::left/right/up/down, updated)
-                 double* out3_host; int cap; int n_out, numGround, n_segmented, addFeaturePoint; };        // out
+                 double* out3_host; int cap; int n_out, numGround, n_segmented, addFeaturePoint;          // out
+                 int* box_dev = nullptr; RowsHdr* hdr_dev = nullptr; double* out3_dev = nullptr; };      // device-output path: the slot's box, the row set's header and rows
+  // host path: waits, copies the rows to out3_host and the box to lrud
   int handle(std::vector<Sweep>& sw) {
     const int nj = (int)sw.size(); if (!nj) return 0;
+    std::vector<LidarJob> J; int* counters_all = nullptr;
+    if (enqueue(sw, false, st, J, counters_all)) return -1;
+    std::vector<int> cnt((size_t)nj*8);
+    SEL_CK(cudaMemcpyAsync(cnt.data(), counters_all, cnt.size()*sizeof(int), cudaMemcpyDeviceToHost, st));
+    SEL_CK(cudaStreamSynchronize(st));
+    if (have_ev) cudaEventElapsedTime(&last_kernel_ms, ev0, ev1);
+    for (int j = 0; j < nj; j++) { Sweep& s = sw[j]; const int* c = &cnt[8*j]; s.n_out = c[0]; s.numGround = c[1]; for (int k = 0; k < 4; k++) s.lrud[k] = c[2+k]; s.n_segmented = c[6];
+      s.addFeaturePoint = ((float)s.numGround / (float)s.n_out > 0.8) ? 1 : 0;                                 // :851-854
+      if (s.n_out > s.cap) { err = "lidar: output capacity too small"; return -2; }
+      if (s.n_out) SEL_CK(cudaMemcpyAsync(s.out3_host, J[j].out3, 3*(size_t)s.n_out*sizeof(double), cudaMemcpyDeviceToHost, st)); }
+    SEL_CK(cudaStreamSynchronize(st));
+    return 0;
+  }
+  // device-output path: sweep j's rows go to sw[j].out3_dev (at most cap), its header to hdr_dev, the box is read from and written back to box_dev (4 ints).
+  // stats5 == nullptr: enqueue and return; else wait and fill {rows, numGround, n_segmented, addFeaturePoint, overflow} per sweep
+  int handle_rows(std::vector<Sweep>& sw, int* stats5) {
+    const int nj = (int)sw.size(); if (!nj) return 0;
+    std::vector<LidarJob> J; int* counters_all = nullptr;
+    if (enqueue(sw, true, st_up ? st_up : st, J, counters_all)) return -1;
+    if (!stats5) return 0;
+    std::vector<int> cnt((size_t)nj*8);
+    SEL_CK(cudaMemcpyAsync(cnt.data(), counters_all, cnt.size()*sizeof(int), cudaMemcpyDeviceToHost, st));
+    SEL_CK(cudaStreamSynchronize(st));
+    if (have_ev) cudaEventElapsedTime(&last_kernel_ms, ev0, ev1);
+    for (int j = 0; j < nj; j++) { const int* c = &cnt[8*j]; int* o = stats5 + 5*j;
+      o[0] = c[0]; o[1] = c[1]; o[2] = c[6]; o[3] = ((float)c[1] / (float)c[0] > 0.8) ? 1 : 0; o[4] = c[0] > sw[j].cap ? 1 : 0; }
+    return 0;
+  }
+  // scratch, job table, sweep uploads (on `up`; the kernels wait for them by event when up != st) and the nine launches of one call; rows: the device-output
+  // path (rows into out3_dev, box seeded from and written back to box_dev, header)
+  int enqueue(std::vector<Sweep>& sw, bool rows, cudaStream_t up, std::vector<LidarJob>& J, int*& counters_all) {
+    const int nj = (int)sw.size();
     if (S.N > 128 || S.groundScanInd >= S.N) { err = "lidar: at most 128 rings, groundScanInd < rings"; return -1; }
-    const size_t m = (size_t)S.N*S.H; size_t bytes = Scratch::need(nj, sizeof(LidarJob)) + 1024;
+    const size_t m = (size_t)S.N*S.H; size_t bytes = Scratch::need(nj, sizeof(LidarJob)) + Scratch::need(nj, sizeof(RowsJob)) + 1024;
     for (auto& s : sw) bytes += Scratch::need(std::max(s.n, 1), 16) + 5*Scratch::need(m, 4) + Scratch::need(m, 16) + 2*Scratch::need(m, 1) + Scratch::need(2*m, 8) + Scratch::need(2*m, 4)
-                              + Scratch::need(3*(size_t)s.cap, 8) + Scratch::need(8, 4) + 1024;
+                              + (rows ? 0 : Scratch::need(3*(size_t)s.cap, 8)) + Scratch::need(8, 4) + 1024;
     if (io.reserve(bytes, st)) { err = "scratch"; return -1; }
-    io.reset(); std::vector<LidarJob> J(nj); LidarJob* dJ = io.take<LidarJob>(nj); int maxN = 0;
+    io.reset(); J.assign(nj, LidarJob()); LidarJob* dJ = io.take<LidarJob>(nj); RowsJob* dR = io.take<RowsJob>(nj); int maxN = 0;
     // per-type arrays of all sweeps back to back: one memset / one counter upload / one counter read-back per call instead of one per sweep
-    int* cellIdx_all = io.take<int>(m*nj); int* counters_all = io.take<int>((size_t)8*nj); std::vector<int> c0((size_t)8*nj, 0);
+    int* cellIdx_all = io.take<int>(m*nj); counters_all = io.take<int>((size_t)8*nj); std::vector<int> c0((size_t)8*nj, 0); std::vector<RowsJob> R(rows ? nj : 0);
     size_t tot_pts = 0; for (auto& s : sw) tot_pts += (size_t)std::max(s.n, 0);
     float4* pts_all = io.take<float4>(std::max(tot_pts, (size_t)1)); size_t off = 0;
+    if (up != st && have_sync_ev) SEL_CK(cudaStreamWaitEvent(up, ev_done, 0));            // the staging is rewritten only after the last call's kernels have read it
     for (int j = 0; j < nj; j++) { Sweep& s = sw[j]; LidarJob& L = J[j];
       float4* pts = pts_all + off;
       if (s.n) {                                              // sweeps that follow each other in host memory (the C-ABI's layout) travel in ONE copy
         int j2 = j; size_t run = (size_t)s.n;
         const bool starts_run = (j == 0) || !(sw[j-1].n > 0 && sw[j-1].xyzi_host + 4*(size_t)sw[j-1].n == s.xyzi_host);
         if (starts_run) { while (j2 + 1 < nj && sw[j2+1].n > 0 && sw[j2].xyzi_host + 4*(size_t)sw[j2].n == sw[j2+1].xyzi_host) { j2++; run += (size_t)sw[j2].n; }
-          SEL_CK(cudaMemcpyAsync(pts, s.xyzi_host, run*16, cudaMemcpyHostToDevice, st)); }
+          SEL_CK(cudaMemcpyAsync(pts, s.xyzi_host, run*16, cudaMemcpyHostToDevice, up)); }
       }
       off += (size_t)std::max(s.n, 0);
       L.pts = pts; L.n = s.n; L.cellIdx = cellIdx_all + (size_t)j*m; L.range = io.take<float>(m); L.cloud = io.take<float4>(m); L.ground = io.take<signed char>(m); L.parent = io.take<int>(m); L.csize = io.take<int>(m);
       L.rowmask = io.take<unsigned long long>(2*m); L.flag = io.take<unsigned char>(m); L.pos = io.take<int>(m); L.kuv = io.take<float>(2*m);
       for (int k = 0; k < 9; k++) L.R[k] = s.R[k]; for (int k = 0; k < 3; k++) L.t[k] = s.t[k]; L.fx = s.K[0]; L.fy = s.K[1]; L.cx = s.K[2]; L.cy = s.K[3]; L.w = s.w; L.h = s.h;
-      L.out3 = io.take<double>(3*(size_t)std::max(s.cap, 1)); L.cap = s.cap; L.counters = counters_all + 8*j;
-      for (int k = 0; k < 4; k++) c0[8*j+2+k] = s.lrud[k];
+      L.out3 = rows ? s.out3_dev : io.take<double>(3*(size_t)std::max(s.cap, 1)); L.cap = s.cap; L.counters = counters_all + 8*j;
+      if (rows) R[j] = RowsJob{L.counters, s.box_dev, s.hdr_dev, s.cap};
+      else for (int k = 0; k < 4; k++) c0[8*j+2+k] = s.lrud[k];
       maxN = std::max(maxN, s.n); }
+    if (up != st) { SEL_CK(cudaEventRecord(ev_up, up)); SEL_CK(cudaStreamWaitEvent(st, ev_up, 0)); }
     SEL_CK(cudaMemcpyAsync(counters_all, c0.data(), c0.size()*sizeof(int), cudaMemcpyHostToDevice, st)); SEL_CK(cudaMemsetAsync(cellIdx_all, 0xFF, m*nj*sizeof(int), st));
     SEL_CK(cudaMemcpyAsync(dJ, J.data(), nj*sizeof(LidarJob), cudaMemcpyHostToDevice, st));
+    if (rows) { SEL_CK(cudaMemcpyAsync(dR, R.data(), nj*sizeof(RowsJob), cudaMemcpyHostToDevice, st));
+                SDV_LAUNCH(lf_rows_seed_kernel, dim3((nj + 127)/128), dim3(128), st, dR, nj); launches += 1; }
     const dim3 gc((unsigned)((m + 127)/128), nj), b128(128);
     if (have_ev) cudaEventRecord(ev0, st);
     if (maxN > 0) SDV_LAUNCH(lf_project_kernel, dim3((maxN + 127)/128, nj), b128, st, dJ, S);
@@ -240,16 +307,10 @@ struct LidarEngine {
     SDV_LAUNCH_SYNC(lf_scan_kernel, dim3(nj), dim3(256), st, dJ, S);
     SDV_LAUNCH(lf_emit_kernel, gc, b128, st, dJ, S);
     if (have_ev) cudaEventRecord(ev1, st);
-    launches += 9; SEL_CK(cudaGetLastError());
-    std::vector<int> cnt((size_t)nj*8);
-    SEL_CK(cudaMemcpyAsync(cnt.data(), counters_all, cnt.size()*sizeof(int), cudaMemcpyDeviceToHost, st));
-    SEL_CK(cudaStreamSynchronize(st));
-    if (have_ev) cudaEventElapsedTime(&last_kernel_ms, ev0, ev1);
-    for (int j = 0; j < nj; j++) { Sweep& s = sw[j]; const int* c = &cnt[8*j]; s.n_out = c[0]; s.numGround = c[1]; for (int k = 0; k < 4; k++) s.lrud[k] = c[2+k]; s.n_segmented = c[6];
-      s.addFeaturePoint = ((float)s.numGround / (float)s.n_out > 0.8) ? 1 : 0;                                 // :851-854
-      if (s.n_out > s.cap) { err = "lidar: output capacity too small"; return -2; }
-      if (s.n_out) SEL_CK(cudaMemcpyAsync(s.out3_host, J[j].out3, 3*(size_t)s.n_out*sizeof(double), cudaMemcpyDeviceToHost, st)); }
-    SEL_CK(cudaStreamSynchronize(st));
+    launches += 9;
+    if (rows) { SDV_LAUNCH(lf_rows_finalize_kernel, dim3((nj + 127)/128), dim3(128), st, dR, nj); launches += 1; }
+    if (have_sync_ev) SEL_CK(cudaEventRecord(ev_done, st));
+    SEL_CK(cudaGetLastError());
     return 0;
   }
   // debugging / test read-back of the images of job 0 of the last call is not kept: tests compare the pixel rows, the box, the counts

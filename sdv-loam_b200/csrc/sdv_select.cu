@@ -18,10 +18,13 @@ using namespace sdv;
 static_assert(sizeof(sel::NewTrace) == sizeof(sdv_new_trace) && sizeof(sel::ImmPt) == sizeof(sdv_immature_pt), "engine records mirror the C-ABI structs");
 
 namespace sdv {
-struct SelState { sel::SelEngine eng; std::vector<sel::SelectorSlot> slots; std::vector<int> cam; sel::Scratch aux; };   // cam[s]: camera of slot s
+struct SelState { sel::SelEngine eng; std::vector<sel::SelectorSlot> slots; std::vector<int> cam; sel::Scratch aux;   // cam[s]: camera of slot s
+                  int* boxD = nullptr; };                                                // FullSystem::left/right/up/down of every slot (4 ints each, device), FullSystem.h:191-194
+static const int32_t kBox0[4] = {10000, -1, 10000, -1};                                   // their initial values
 void sel_destroy(sdv_ctx* c) {
   SelState* s = (SelState*)c->sel; if (!s) return;
   for (auto& sl : s->slots) if (sl.mapD) cudaFree(sl.mapD);
+  cudaFree(s->boxD);
   s->eng.io.release(); s->aux.release(); s->eng.destroy(); delete s; c->sel = nullptr;
 }
 bool sel_cam_bound(const sdv_ctx* c, int cam, int* slot) {
@@ -37,6 +40,8 @@ static int sel_frame(sdv_ctx* c, uint64_t id, int cam, sel::FrameImg& F, long lo
   if (texels) { int rc = ensure_texels(c, f, 1); if (rc) return rc; F.L1 = f.lvl[1]; F.L2 = f.lvl[2]; }   // |grad|^2 of levels 1 and 2 (makeMaps / makeNewTraces read the packed texels)
   return SDV_OK;
 }
+int sel_n_slots(const sdv_ctx* c) { const SelState* s = (const SelState*)c->sel; return s ? (int)s->slots.size() : -1; }
+void sel_slot_box(const sdv_ctx* c, int slot, int* cam, int** box_dev) { const SelState* s = (const SelState*)c->sel; *cam = s->cam[slot]; *box_dev = s->boxD + 4*(size_t)slot; }
 static int sel_fail(sdv_ctx* c, SelState* s, int rc, const char* who) { return ctx_fail(c, rc == -2 ? SDV_ERR_CAPACITY : SDV_ERR_CUDA, "%s: %s", who, s->eng.err.c_str()); }
 }  // namespace sdv
 #define SEL_STATE(who) SelState* s = (SelState*)c->sel; if (!s) return ctx_fail(c, SDV_ERR_STATE, who ": sdv_selector_init has not been called")
@@ -54,11 +59,15 @@ int sdv_selector_init(sdv_ctx* c, const uint8_t* random_pattern, int n_slots) { 
   S.outlierTH = c->set.outlierTH; S.outlierTHSumComponent = c->set.outlierTHSumComponent; S.overallEnergyTHWeight = 1;
   if (s->eng.init(c->w, c->h, S, random_pattern, c->st)) { int rc = sel_fail(c, s, -1, "selector_init"); sel_destroy(c); return rc; }
   s->slots.resize(n_slots); s->cam.assign(n_slots, 0);
+  { std::vector<int32_t> b0((size_t)4*n_slots); for (size_t k = 0; k < b0.size(); k++) b0[k] = kBox0[k & 3];
+    if (cudaMalloc((void**)&s->boxD, b0.size()*sizeof(int32_t)) != cudaSuccess || cudaMemcpy(s->boxD, b0.data(), b0.size()*sizeof(int32_t), cudaMemcpyHostToDevice) != cudaSuccess) {
+      cudaGetLastError(); sel_destroy(c); return ctx_fail(c, SDV_ERR_CUDA, "selector_init: pixel boxes of %d slots", n_slots); } }
   if (const char* e = getenv("SDV_WALK_THREADS")) { const int t = atoi(e); if (t == 32 || t == 64 || t == 128 || t == 256) s->eng.walk_threads = t; }   // tuning knobs
   if (const char* e = getenv("SDV_FUSE_MAP")) s->eng.fuse_map = atoi(e) != 0;
   return SDV_OK;
 }
-// Rebinding a slot to a camera of another size starts it afresh (map dropped, currentPotential 3: a new PixelSelector / selectionMap); the same size keeps its state.
+// Rebinding a slot to a camera of another size starts it afresh (map dropped, currentPotential 3, LiDAR pixel box at its initial value: a new PixelSelector /
+// selectionMap / sequence); the same size keeps its state.
 int sdv_selector_set_slot_cams(sdv_ctx* c, int n, const int32_t* slots, const int32_t* cams) { SDV_GUARD_TRK(c);
   if (!c || n < 0 || (n && (!slots || !cams))) return SDV_ERR_ARG; SEL_STATE("selector_set_slot_cams");
   for (int i = 0; i < n; i++) {
@@ -68,7 +77,8 @@ int sdv_selector_set_slot_cams(sdv_ctx* c, int n, const int32_t* slots, const in
   }
   CK(cudaSetDevice(c->device));
   for (int i = 0; i < n; i++) { const int sl = slots[i];
-    if (!same_size(c, s->cam[sl], cams[i])) { sel::SelectorSlot& S = s->slots[sl]; if (S.mapD) { CK(cudaStreamSynchronize(c->st)); CK(cudaFree(S.mapD)); } S = sel::SelectorSlot(); }
+    if (!same_size(c, s->cam[sl], cams[i])) { sel::SelectorSlot& S = s->slots[sl]; if (S.mapD) { CK(cudaStreamSynchronize(c->st)); CK(cudaFree(S.mapD)); } S = sel::SelectorSlot();
+      CK(cudaMemcpyAsync(s->boxD + 4*(size_t)sl, kBox0, sizeof(kBox0), cudaMemcpyHostToDevice, c->st)); }
     s->cam[sl] = cams[i]; }
   return SDV_OK;
 }
@@ -77,6 +87,14 @@ int sdv_selector_potential(sdv_ctx* c, int slot, int set_to, int* out) { SDV_GUA
   if (slot < 0 || slot >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "selector_potential: slot %d of %d", slot, (int)s->slots.size());
   if (set_to > 0) s->slots[slot].currentPotential = set_to;
   if (out) *out = s->slots[slot].currentPotential;
+  return SDV_OK;
+}
+int sdv_selector_lidar_box(sdv_ctx* c, int slot, const int32_t* set_to, int32_t* lrud_out) { SDV_GUARD_TRK(c);
+  if (!c) return SDV_ERR_ARG; SEL_STATE("selector_lidar_box");
+  if (slot < 0 || slot >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "selector_lidar_box: slot %d of %d", slot, (int)s->slots.size());
+  CK(cudaSetDevice(c->device));
+  if (set_to) CK(cudaMemcpyAsync(s->boxD + 4*(size_t)slot, set_to, 4*sizeof(int32_t), cudaMemcpyHostToDevice, c->st));   // stream-ordered: after the handlers enqueued so far
+  if (lrud_out) { CK(cudaMemcpyAsync(lrud_out, s->boxD + 4*(size_t)slot, 4*sizeof(int32_t), cudaMemcpyDeviceToHost, c->st)); CK(cudaStreamSynchronize(c->st)); }
   return SDV_OK;
 }
 int sdv_selector_get_map(sdv_ctx* c, int slot, uint8_t* out) { SDV_GUARD_TRK(c);
@@ -149,18 +167,19 @@ int sdv_selector_make_maps_batch(sdv_ctx* c, int n, const int32_t* slots, const 
 }  // extern "C"
 // makeNewTraces for n jobs; out == nullptr: the records go into the immature-point store (block of frames[j]) instead of to the caller
 static int make_new_traces(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const float* density_lidar,
-                           const float* density_dense, const int32_t* add_feature_point, int cap, sdv_new_trace* out, sdv_immature_pt* imm_out, int32_t* n_out, int32_t* num_points2) {
+                           const float* density_dense, const int32_t* add_feature_point, int cap, sdv_new_trace* out, sdv_immature_pt* imm_out, int32_t* n_out, int32_t* num_points2,
+                           const double* const* cloud_dev = nullptr /* job j's rows on the device (row sets), instead of cloud3 */) {
   if (n == 0) return SDV_OK; SEL_STATE("make_new_traces");
   if (cloud_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: cloud_begin[0] must be 0");
   for (int j = 0; j < n; j++) { if (cloud_begin[j+1] < cloud_begin[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: cloud_begin is not ascending at job %d", j);
-    if (cloud_begin[j+1] > cloud_begin[j] && !cloud3) return SDV_ERR_ARG;
+    if (cloud_begin[j+1] > cloud_begin[j] && !cloud3 && !cloud_dev) return SDV_ERR_ARG;
     if (slots[j] < 0 || slots[j] >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: slot %d of %d", slots[j], (int)s->slots.size());
     for (int k = 0; k < j; k++) if (slots[k] == slots[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: slot %d appears twice in one batch", slots[j]);
     if (!out) for (int k = 0; k < j; k++) if (frames[k] == frames[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces_store: frame %llu appears twice in one batch", (unsigned long long)frames[j]); }
   CK(cudaSetDevice(c->device));
   long long need = 0; std::vector<sel::SelEngine::NewTracesJob> J(n);
   for (int j = 0; j < n; j++) { const int cam = s->cam[slots[j]]; int rc = sel_frame(c, frames[j], cam, J[j].img, need, "make_new_traces"); if (rc) return rc; J[j].w = c->cam_w[cam]; J[j].h = c->cam_h[cam];
-    J[j].cloud_host = cloud3 ? cloud3 + 3*(size_t)cloud_begin[j] : nullptr; J[j].n = cloud_begin[j+1] - cloud_begin[j]; J[j].slot = &s->slots[slots[j]]; J[j].densityLidar = density_lidar[j];
+    J[j].cloud_host = cloud3 ? cloud3 + 3*(size_t)cloud_begin[j] : nullptr; J[j].cloud_dev = cloud_dev ? cloud_dev[j] : nullptr; J[j].n = cloud_begin[j+1] - cloud_begin[j]; J[j].slot = &s->slots[slots[j]]; J[j].densityLidar = density_lidar[j];
     J[j].densityDense = density_dense[j]; J[j].addFeaturePoint = add_feature_point[j]; J[j].out_host = out ? (sel::NewTrace*)out + (size_t)j*cap : nullptr;
     J[j].imm_host = (out && imm_out) ? (sel::ImmPt*)imm_out + (size_t)j*cap : nullptr; J[j].cap = cap; }
   { int rc = join_ingest_upto(c, need); if (rc) return rc; }
@@ -187,6 +206,22 @@ int sdv_make_new_traces_store_batch(sdv_ctx* c, int n, const int32_t* slots, con
                                     const float* density_dense, const int32_t* add_feature_point, int cap, int32_t* n_out, int32_t* num_points2) { SDV_GUARD_TRK(c);
   if (!c || n < 0 || (n && (!slots || !frames || !cloud_begin || !density_lidar || !density_dense || !add_feature_point || !n_out || cap < 1))) return SDV_ERR_ARG;
   return make_new_traces(c, n, slots, frames, cloud_begin, cloud3, density_lidar, density_dense, add_feature_point, cap, nullptr, nullptr, n_out, num_points2);
+}
+// The same fed from the LiDAR row sets of frames[j] (sdv_lidar_handler_rows_batch): rows, box and addFeaturePoint as the handler left them for that frame.
+int sdv_make_new_traces_rows_store_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const float* desired_density, int cap, int32_t* n_out,
+                                         int32_t* num_points2) { SDV_GUARD_TRK(c);
+  if (!c || n < 0 || (n && (!slots || !frames || !desired_density || !n_out || cap < 1))) return SDV_ERR_ARG;
+  if (n == 0) return SDV_OK; SEL_STATE("make_new_traces_rows");
+  for (int j = 0; j < n; j++) if (slots[j] < 0 || slots[j] >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces_rows: slot %d of %d", slots[j], (int)s->slots.size());
+  CK(cudaSetDevice(c->device));
+  std::vector<const double*> rows(n); std::vector<LidarRowsInfo> I(n);                   // all headers in one copy: the row counts size the engine's scratch and grids
+  { int rc = lidar_rows_fetch(c, n, frames, rows.data(), I.data(), "make_new_traces_rows"); if (rc) return rc; }
+  std::vector<int32_t> cb(n + 1, 0), add(n); std::vector<float> dl(n);
+  for (int j = 0; j < n; j++) { const LidarRowsInfo& q = I[j]; const int cam = s->cam[slots[j]];
+    if (q.overflow) return ctx_fail(c, SDV_ERR_CAPACITY, "make_new_traces_rows: the sweep of frame %llu left %d pixel rows, its row set holds %d", (unsigned long long)frames[j], q.rows, q.room);
+    dl[j] = ((float)((q.lrud[1] - q.lrud[0])*(q.lrud[3] - q.lrud[2])) / (float)(c->cam_w[cam]*c->cam_h[cam])) * desired_density[j];   // FullSystem.cpp:1287-1290
+    add[j] = q.addFeaturePoint; cb[j+1] = cb[j] + q.rows; }
+  return make_new_traces(c, n, slots, frames, cb.data(), nullptr, dl.data(), desired_density, add.data(), cap, nullptr, nullptr, n_out, num_points2, rows.data());
 }
 
 }  // extern "C"

@@ -782,6 +782,7 @@ struct SelEngine {
   struct NewTracesJob {
     FrameImg img; int w = 0, h = 0; const double* cloud_host; int n; SelectorSlot* slot; float densityLidar, densityDense; int addFeaturePoint;   // w, h: the frame's size (= the slot's map)
     NewTrace* out_host; ImmPt* imm_host; int cap;                  // cap: room for the returned points (LiDAR + monocular)
+    const double* cloud_dev = nullptr;                              // device-input path: the n rows are already on the device (cloud_host unused, nothing copied)
     int n_out, numPoints[2], passes[2];                             // out: points created, {numPointLidar, numPointMonocular}, select passes of the two makeMaps calls
     const NewTrace* out_dev = nullptr; const ImmPt* imm_dev = nullptr;   // out: the n_out records on the device (engine scratch, valid until the next engine call);
                                                                     // out_host == nullptr: they stay there (device-output path)
@@ -793,14 +794,14 @@ struct SelEngine {
     std::vector<size_t> o_ths(nj + 1, 0), o_occ(nj + 1, 0);                                 // per-job ths / thsSm pairs and occupancy masks, each at the job's size
     for (int j = 0; j < nj; j++) { o_ths[j+1] = o_ths[j] + 2*ths_floats(jobs[j].w, jobs[j].h); o_occ[j+1] = o_occ[j] + (size_t)jobs[j].w*jobs[j].h; }
     size_t bytes = Scratch::need(nj, sizeof(TraceJob)) + Scratch::need(nj, sizeof(HistJob)) + Scratch::need(o_ths[nj], 4) + Scratch::need(o_occ[nj], 1) + 8192;
-    for (auto& j : jobs) bytes += Scratch::need((size_t)3*j.n, 8) + Scratch::need(std::max(j.n, 1), 1) + 3*Scratch::need(j.n, 4) + Scratch::need((size_t)j.w*j.h, 1)
+    for (auto& j : jobs) bytes += (j.cloud_dev ? 0 : Scratch::need((size_t)3*j.n, 8)) + Scratch::need(std::max(j.n, 1), 1) + 3*Scratch::need(j.n, 4) + Scratch::need((size_t)j.w*j.h, 1)
                               + Scratch::need(j.cap, 4) + Scratch::need(j.cap, sizeof(NewTrace)) + Scratch::need(j.cap, sizeof(ImmPt)) + Scratch::need(4, 4);
     if (io.reserve(bytes, st)) { err = "scratch"; return -1; }
     io.reset(); std::vector<TraceJob> T(nj); std::vector<HistJob> Hj(nj); std::vector<MapsJobHost> ML, MD;
     TraceJob* dT = io.take<TraceJob>(nj);
     // per-type arrays of all jobs back to back: one memset / one upload per call instead of one per keyframe
     float* ths_all = io.take<float>(o_ths[nj]); unsigned char* occ_all = io.take<unsigned char>(o_occ[nj]); int* counts_all = io.take<int>((size_t)4*nj);
-    size_t tot_cl = 0; for (auto& j : jobs) tot_cl += (size_t)3*std::max(j.n, 0);
+    size_t tot_cl = 0; for (auto& j : jobs) if (!j.cloud_dev) tot_cl += (size_t)3*std::max(j.n, 0);
     double* cl_all = io.take<double>(std::max(tot_cl, (size_t)1)); size_t off = 0;
     SEL_CK(cudaMemsetAsync(ths_all, 0, o_ths[nj]*sizeof(float), st)); SEL_CK(cudaMemsetAsync(occ_all, 0, o_occ[nj], st));
     std::vector<int> c0((size_t)4*nj, 0); for (int j = 0; j < nj; j++) c0[4*j+3] = float_order_bits_host(-1000.0f);
@@ -808,13 +809,13 @@ struct SelEngine {
     int maxWH = 0;
     for (int j = 0; j < nj; j++) { NewTracesJob& N = jobs[j]; TraceJob& J = T[j]; const size_t wh = (size_t)N.w*N.h, tf = ths_floats(N.w, N.h); maxWH = std::max(maxWH, (int)wh);
       if (!N.slot->mapD) { SEL_CK(cudaMalloc((void**)&N.slot->mapD, wh)); SEL_CK(cudaMemsetAsync(N.slot->mapD, 0, wh, st)); }   // FullSystem::selectionMap: persistent; zero at birth (the reference: uninitialised)
-      double* cl = cl_all + off; unsigned char* mapL = io.take<unsigned char>(std::max(N.n, 1)); float* ths = ths_all + o_ths[j]; float* thsSm = ths + tf;
-      if (N.n) {                                              // clouds that follow each other in host memory (the C-ABI's layout) travel in ONE copy
+      const double* cl = N.cloud_dev ? N.cloud_dev : cl_all + off; unsigned char* mapL = io.take<unsigned char>(std::max(N.n, 1)); float* ths = ths_all + o_ths[j]; float* thsSm = ths + tf;
+      if (N.n && !N.cloud_dev) {                              // clouds that follow each other in host memory (the C-ABI's layout) travel in ONE copy
         const bool starts_run = (j == 0) || !(jobs[j-1].n > 0 && jobs[j-1].cloud_host + 3*(size_t)jobs[j-1].n == N.cloud_host);
         if (starts_run) { int j2 = j; size_t run = (size_t)3*N.n; while (j2 + 1 < nj && jobs[j2+1].n > 0 && jobs[j2].cloud_host + 3*(size_t)jobs[j2].n == jobs[j2+1].cloud_host) { j2++; run += (size_t)3*jobs[j2].n; }
-          SEL_CK(cudaMemcpyAsync(cl, N.cloud_host, run*sizeof(double), cudaMemcpyHostToDevice, st)); }
+          SEL_CK(cudaMemcpyAsync(cl_all + off, N.cloud_host, run*sizeof(double), cudaMemcpyHostToDevice, st)); }
+        off += (size_t)3*std::max(N.n, 0);
       }
-      off += (size_t)3*std::max(N.n, 0);
       J.img = N.img; J.w = N.w; J.h = N.h; J.cloud = cl; J.n = N.n; J.mapL = mapL; J.mapD = N.slot->mapD; J.score = io.take<float>(N.n); J.flag = io.take<int>(N.n); J.pos = io.take<int>(N.n);
       J.occ = occ_all + o_occ[j]; J.state = io.take<unsigned char>(wh); J.cand = io.take<int>(N.cap); J.ncand_cap = N.cap;
       J.out = io.take<NewTrace>(N.cap); J.imm = io.take<ImmPt>(N.cap); J.cap = N.cap; J.counts = counts_all + 4*j;

@@ -17,6 +17,7 @@
 #include <vector>
 #include <algorithm>
 #include "sdv_ctx.cuh"
+#include "sdv_pool.cuh"
 
 using namespace sdv;
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return ctx_fail(c, SDV_ERR_CUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
@@ -328,59 +329,26 @@ __host__ __device__ __forceinline__ void imm_join(const ImmRO& a, const ImmRW& b
   p.idepth_min = b.idepth_min; p.idepth_max = b.idepth_max; p.quality = b.quality; p.lastTraceUV[0] = b.lastTraceUV[0]; p.lastTraceUV[1] = b.lastTraceUV[1];
   p.lastTracePixelInterval = b.lastTracePixelInterval; p.lastTraceStatus = b.status;
 }
-struct ImmBlock { ImmRO* ro = nullptr; ImmRW* rw = nullptr; sdv_immature_meta* meta = nullptr; int n = 0, cap = 0; };   // one allocation: ro | rw | meta, cap points each
-struct ImmStore { std::unordered_map<uint64_t, ImmBlock> blocks; std::vector<ImmBlock> spare; };                       // spare: blocks of dropped hosts, reused before allocating
+static size_t al16(size_t b) { return (b + 15) & ~(size_t)15; }
+struct ImmBlock {                                                                          // one allocation: ro | rw | meta, cap points each
+  ImmRO* ro = nullptr; ImmRW* rw = nullptr; sdv_immature_meta* meta = nullptr; int n = 0, cap = 0;
+  char* base() const { return (char*)ro; }
+  static size_t bytes(int cap) { return al16((size_t)cap*sizeof(ImmRO)) + al16((size_t)cap*sizeof(ImmRW)) + (size_t)cap*sizeof(sdv_immature_meta); }
+  static ImmBlock layout(char* p, int cap) {
+    ImmBlock nb; const size_t o_rw = al16((size_t)cap*sizeof(ImmRO)), o_m = o_rw + al16((size_t)cap*sizeof(ImmRW));
+    nb.ro = (ImmRO*)p; nb.rw = (ImmRW*)(p + o_rw); nb.meta = (sdv_immature_meta*)(p + o_m); nb.cap = cap; return nb;
+  }
+};
+struct ImmStore : BlockPool<ImmBlock> {};                                                 // one block per host keyframe (sdv_pool.cuh: plan / commit / abandon)
+using ImmPlan = ImmStore::Plan;
 void imm_store_destroy(sdv_ctx* c) {
   ImmStore* S = (ImmStore*)c->imm_store; if (!S) return;
-  for (auto& kv : S->blocks) cudaFree(kv.second.ro);
-  for (auto& b : S->spare) cudaFree(b.ro);
-  delete S; c->imm_store = nullptr;
+  S->release(); delete S; c->imm_store = nullptr;
 }
 static ImmStore* imm_store(sdv_ctx* c) { if (!c->imm_store) c->imm_store = new ImmStore(); return (ImmStore*)c->imm_store; }
-static size_t al16(size_t b) { return (b + 15) & ~(size_t)15; }
-// Room for hosts that are about to receive new contents, in two phases so that a refused call changes no block.  imm_store_plan picks, per host, its own block
-// if large enough, else the smallest free spare that fits, else a new allocation; before allocating it frees the spares too small for the request (a drive
-// whose point counts grow does not keep every block it outgrew).  Nothing visible changes until imm_store_commit; on failure the new allocations become spares.
-// Stream-ordered reuse: every reader and writer of a block runs on c->st.
-struct ImmPlan { uint64_t host; int n; ImmBlock b; bool own; };
-static ImmBlock imm_block_layout(char* p, int cap) {
-  ImmBlock nb; const size_t o_rw = al16((size_t)cap*sizeof(ImmRO)), o_m = o_rw + al16((size_t)cap*sizeof(ImmRW));
-  nb.ro = (ImmRO*)p; nb.rw = (ImmRW*)(p + o_rw); nb.meta = (sdv_immature_meta*)(p + o_m); nb.cap = cap; return nb;
-}
-static size_t imm_block_bytes(int cap) { return al16((size_t)cap*sizeof(ImmRO)) + al16((size_t)cap*sizeof(ImmRW)) + (size_t)cap*sizeof(sdv_immature_meta); }
-static int imm_store_plan(sdv_ctx* c, ImmStore* S, int nh, const uint64_t* hosts, const int* n, std::vector<ImmPlan>& P) {
-  P.assign(nh, ImmPlan()); std::vector<char> taken(S->spare.size(), 0); std::vector<ImmBlock> fresh;
-  auto fail = [&](int rc) { for (auto& b : fresh) S->spare.push_back(b); return rc; };
-  for (int j = 0; j < nh; j++) {
-    ImmPlan& q = P[j]; q.host = hosts[j]; q.n = n[j]; auto it = S->blocks.find(hosts[j]);
-    if (it != S->blocks.end() && it->second.cap >= n[j]) { q.b = it->second; q.own = true; continue; }
-    q.own = false; int best = -1;
-    for (int k = 0; k < (int)S->spare.size(); k++) if (!taken[k] && S->spare[k].cap >= n[j] && (best < 0 || S->spare[k].cap < S->spare[best].cap)) best = k;
-    if (best >= 0) { taken[best] = 1; q.b = S->spare[best]; continue; }
-    bool small = false; for (int k = 0; k < (int)S->spare.size(); k++) small |= !taken[k] && S->spare[k].cap < n[j];
-    if (small) {                                                                         // spares this request outgrew: give their memory back first
-      if (cudaStreamSynchronize(c->st) != cudaSuccess) return fail(ctx_fail(c, SDV_ERR_CUDA, "immature store: stream synchronise"));
-      std::vector<ImmBlock> keep; std::vector<char> kt;
-      for (int k = 0; k < (int)S->spare.size(); k++) { if (!taken[k] && S->spare[k].cap < n[j]) cudaFree(S->spare[k].ro); else { keep.push_back(S->spare[k]); kt.push_back(taken[k]); } }
-      S->spare.swap(keep); taken.swap(kt);
-    }
-    const int cap = std::max(256, n[j] + n[j]/4); char* p = nullptr;
-    if (cudaMalloc((void**)&p, imm_block_bytes(cap)) != cudaSuccess) { cudaGetLastError(); return fail(ctx_fail(c, SDV_ERR_CUDA, "immature store: cudaMalloc of %d points", cap)); }
-    q.b = imm_block_layout(p, cap); fresh.push_back(q.b);
-  }
-  for (int k = (int)taken.size() - 1; k >= 0; k--) if (taken[k]) S->spare.erase(S->spare.begin() + k);   // the spares now in a plan
-  return SDV_OK;
-}
-// the plan's blocks and counts become the hosts' blocks; a host that moved leaves its old block as a spare
-static void imm_store_commit(ImmStore* S, std::vector<ImmPlan>& P) {
-  for (ImmPlan& q : P) {
-    auto it = S->blocks.find(q.host); q.b.n = q.n;
-    if (it == S->blocks.end()) S->blocks[q.host] = q.b;
-    else { if (!q.own) S->spare.push_back(it->second); it->second = q.b; }
-  }
-}
-// a failed call after imm_store_plan: blocks it took from the spares or allocated go back to the spares
-static void imm_store_abandon(ImmStore* S, std::vector<ImmPlan>& P) { for (ImmPlan& q : P) if (!q.own) S->spare.push_back(q.b); }
+static int imm_store_plan(sdv_ctx* c, ImmStore* S, int nh, const uint64_t* hosts, const int* n, std::vector<ImmPlan>& P) { return S->plan(c, nh, hosts, n, P, "immature store", "points"); }
+static void imm_store_commit(ImmStore* S, std::vector<ImmPlan>& P) { S->commit(P); }
+static void imm_store_abandon(ImmStore* S, std::vector<ImmPlan>& P) { S->abandon(P); }
 
 // makeNewTraces into the store: the records of the selector engine (sdv_new_trace + sdv_immature_pt) with FullSystem.cpp:1313-1317 and :1080-1084 applied
 struct DepositJob { const sdv_new_trace* t; const sdv_immature_pt* p; ImmRO* ro; ImmRW* rw; sdv_immature_meta* meta; int n; };
@@ -633,8 +601,7 @@ int sdv_immature_store_drop(sdv_ctx* c, int n, const uint64_t* hosts) { SDV_GUAR
   if (!c || n < 0 || (n && !hosts)) return SDV_ERR_ARG;
   ImmStore* S = (ImmStore*)c->imm_store;
   for (int i = 0; i < n; i++) if (!S || !S->blocks.count(hosts[i])) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_store_drop: host %llu has no block", (unsigned long long)hosts[i]);
-  for (int i = 0; i < n; i++) { auto it = S->blocks.find(hosts[i]); if (it == S->blocks.end()) continue;          // named twice
-    S->spare.push_back(it->second); S->blocks.erase(it); }
+  for (int i = 0; i < n; i++) S->drop(hosts[i]);                                          // a host named twice is dropped once
   return SDV_OK;
 }
 
