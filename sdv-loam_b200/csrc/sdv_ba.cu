@@ -11,7 +11,6 @@
 #include <cmath>
 
 using namespace sdv;
-#define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return ctx_fail(c, SDV_ERR_CUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
 
 namespace sdv {
 void ba_destroy(sdv_ctx* c) {
@@ -20,7 +19,7 @@ void ba_destroy(sdv_ctx* c) {
     for (int i=0;i<b->n_pinned;i++) frame_unpin(c, b->pinned[i]);
     cudaFree(b->hdr); cudaFreeHost(b->hdr_host); cudaFree(b->pool); cudaFree(b->partials); cudaFree(b->thbuf); cudaFree(b->thcount); delete b; }
   c->ba_windows.clear(); c->ba = nullptr;
-  cudaFree(c->ba_wins_dev); cudaFreeHost(c->ba_wins_host); c->ba_wins_dev = c->ba_wins_host = nullptr;
+  c->ba_wins_dev.release(); c->ba_wins_host.release();
   if (c->ba_graph) { cudaGraphExecDestroy(c->ba_graph); c->ba_graph = nullptr; }
 }
 }
@@ -77,13 +76,13 @@ static int ba_alloc(sdv_ctx* c, BAState* b, int nP, int nR, int nF) {
 static BAWinDev win_of(const BAState* b) { BAWinDev w; w.hdr = b->hdr; w.P = b->P; w.R = b->R; w.partials = b->partials; w.thbuf = b->thbuf; w.thcount = b->thcount; return w; }
 // device array of window descriptors for one (batched) launch sequence; maxP/maxR size the grids
 static int ba_wins(sdv_ctx* c, int n, BAState* const* bs, const BAWinDev** out, int* maxP, int* maxR) {
-  if (n > c->ba_wins_cap) { cudaFree(c->ba_wins_dev); cudaFreeHost(c->ba_wins_host); c->ba_wins_cap = n + 16;
-    CK(cudaMalloc(&c->ba_wins_dev, (size_t)c->ba_wins_cap*sizeof(BAWinDev))); CK(cudaMallocHost(&c->ba_wins_host, (size_t)c->ba_wins_cap*sizeof(BAWinDev))); }
-  BAWinDev* h = (BAWinDev*)c->ba_wins_host; int mp = 1, mr = 1;
+  const size_t bytes = Scratch::need(n, sizeof(BAWinDev));
+  if (c->ba_wins_dev.reserve(bytes, c->st_ba) || c->ba_wins_host.reserve(bytes, c->st_ba)) return ctx_fail(c, SDV_ERR_CUDA, "BA: descriptors of %d windows", n);
+  c->ba_wins_dev.reset(); c->ba_wins_host.reset(); BAWinDev* d = c->ba_wins_dev.take<BAWinDev>(n); BAWinDev* h = c->ba_wins_host.take<BAWinDev>(n); int mp = 1, mr = 1;
   CK(cudaStreamSynchronize(c->st_ba));                                          // the pinned staging array may still feed a previous launch sequence
   for (int i=0;i<n;i++) { h[i] = win_of(bs[i]); if (bs[i]->nP > mp) mp = bs[i]->nP; if (bs[i]->nR > mr) mr = bs[i]->nR; }
-  CK(cudaMemcpyAsync(c->ba_wins_dev, h, (size_t)n*sizeof(BAWinDev), cudaMemcpyHostToDevice, c->st_ba));
-  *out = (const BAWinDev*)c->ba_wins_dev; if (maxP) *maxP = mp; if (maxR) *maxR = mr;
+  CK(cudaMemcpyAsync(d, h, (size_t)n*sizeof(BAWinDev), cudaMemcpyHostToDevice, c->st_ba));
+  *out = d; if (maxP) *maxP = mp; if (maxR) *maxR = mr;
   return SDV_OK;
 }
 #define WIN1() const BAWinDev* wins; int maxP, maxR; { int rcw = ba_wins(c, 1, &b, &wins, &maxP, &maxR); if (rcw) return rcw; }
@@ -104,9 +103,9 @@ int sdv_ba_set_window(sdv_ctx* c, int nF, const uint64_t* frame_ids, const doubl
   SDV_GUARD_TRK(c);                                                           // frame table, pins, level-0 texel pool and the ingest join belong to the tracker domain
   CK(cudaSetDevice(c->device));
   BAState* b; int rc = ba_get(c, &b); if (rc) return rc;
-  int cam0 = -1;                                                              // one size per window: BAHeader::w/h are the window's frames' size
-  for (int f=0; f<nF; f++) { auto it = c->frame_index.find(frame_ids[f]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "BA frame %d: unknown frame handle", f);
-    const int cam = c->frames[it->second].cam; if (cam0 < 0) cam0 = cam;
+  FrameDev* Fr[SDV_MAX_FRAMES_WINDOW]; int cam0 = -1;                         // one size per window: BAHeader::w/h are the window's frames' size
+  for (int f=0; f<nF; f++) { int rcf = job_frame(c, "sdv_ba_set_window", f, frame_ids[f], -1, -1, nullptr, &Fr[f]); if (rcf) return rcf;
+    const int cam = Fr[f]->cam; if (cam0 < 0) cam0 = cam;
     if (!same_size(c, cam, cam0)) return ctx_fail(c, SDV_ERR_ARG, "BA frame %d is %dx%d but frame 0 is %dx%d: one window holds frames of one size", f, c->cam_w[cam], c->cam_h[cam], c->cam_w[cam0], c->cam_h[cam0]); }
   for (int i=0;i<b->n_pinned;i++) frame_unpin(c, b->pinned[i]);          // the window is being replaced: drop its references, take the new ones
   b->n_pinned = nF; for (int f=0; f<nF; f++) { b->pinned[f] = frame_ids[f]; frame_pin(c, frame_ids[f]); }
@@ -123,13 +122,12 @@ int sdv_ba_set_window(sdv_ctx* c, int nF, const uint64_t* frame_ids, const doubl
     cal.value_zero[i] = cal.value[i]; cal.vmvz[i] = 0; cal.step[i] = 0; cal.value_backup[i] = cal.value[i]; }
   cal.si[0] = 1.0f/cal.sf[0]; cal.si[1] = 1.0f/cal.sf[1]; cal.si[2] = -cal.sf[2]/cal.sf[0]; cal.si[3] = -cal.sf[3]/cal.sf[1];
   for (int f=0; f<nF; f++) {
-    auto it = c->frame_index.find(frame_ids[f]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "BA frame %d: unknown frame handle", f);
     BAFrameDev& F = H->frames[f];
     F.evalPT = se3_from7(T_evalPT7 + 7*f);
     for (int i=0;i<10;i++) { F.state[i] = state10[10*f+i]; F.state_zero[i] = state_zero10[10*f+i]; F.state_backup[i] = F.state[i]; F.step[i] = 0; }
     F.ab_exposure = ab_exposure ? ab_exposure[f] : 1.0f; F.frameID = frameID ? frameID[f] : f; F.frameEnergyTH = frameEnergyTH ? frameEnergyTH[f] : 8*8*8;
-    { int rc0 = ensure_lvl0(c, c->frames[it->second]); if (rc0) return rc0; }
-    F.img0 = c->frames[it->second].lvl[0];
+    { int rc0 = ensure_lvl0(c, *Fr[f]); if (rc0) return rc0; }
+    F.img0 = Fr[f]->lvl[0];
   }
   const int N = H->dim;
   if (HM) memcpy(H->HM, HM, (size_t)N*N*sizeof(double));

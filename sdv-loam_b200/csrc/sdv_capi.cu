@@ -18,7 +18,6 @@ int ctx_fail(sdv_ctx* c, int code, const char* fmt, ...) {
   return code;
 }
 }
-#define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return ctx_fail(c, SDV_ERR_CUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
 
 extern "C" {
 
@@ -71,12 +70,12 @@ int sdv_set_calib(sdv_ctx* c, const sdv_calib* K) { SDV_GUARD_TRK(c);
 // again when K is NULL (camera 0 only: row 0 has the context size).  Everything is checked before anything changes.
 int sdv_set_calib_slots_cams(sdv_ctx* c, int n, const int32_t* slots, const sdv_calib* K, const int32_t* cams) { SDV_GUARD_TRK(c);
   if (!c || n < 0 || (n > 0 && !slots)) return SDV_ERR_ARG;
+  { int rc = check_cams(c, n, cams, "sdv_set_calib_slots", "entry"); if (rc) return rc; }
   for (int i=0;i<n;i++) {
     if (slots[i] < 0 || slots[i] >= (int)c->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib_slots: entry %d names slot %d of %d", i, slots[i], (int)c->slots.size());
     if (K && !(K[i].fx > 0 && K[i].fy > 0 && std::isfinite(K[i].fx) && std::isfinite(K[i].fy) && std::isfinite(K[i].cx) && std::isfinite(K[i].cy)))
       return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib_slots: entry %d (slot %d): fx, fy must be positive and finite, cx, cy finite", i, slots[i]);
     const int cam = cams ? cams[i] : 0;
-    if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib_slots: entry %d names camera %d (valid: 0..%d)", i, cam, SDV_MAX_CAMERAS - 1);
     if (!K && cam != 0) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_calib_slots: entry %d binds camera %d without a K (the context calibration is camera 0's)", i, cam);
   }
   for (int i=0;i<n;i++) {                                                // a slot's reference cloud and resident map hold frames of its current size, built at its current depth
@@ -118,7 +117,7 @@ int sdv_set_camera_size(sdv_ctx* c, int cam, int w, int h) { SDV_GUARD_TRK(c);
 // camera holds clouds or a map built at the old depth, and below the selector's 3 levels while a selector slot is bound to it.
 int sdv_set_camera_levels(sdv_ctx* c, int cam, int levels) { SDV_GUARD_TRK(c);
   if (!c) return SDV_ERR_ARG;
-  if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_camera_levels: camera %d outside 0..%d", cam, SDV_MAX_CAMERAS - 1);
+  { int rc = check_cams(c, 1, &cam, "sdv_set_camera_levels", nullptr); if (rc) return rc; }
   if (levels < 1 || levels > c->levels) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_camera_levels: %d levels outside 1..%d (the context's storage depth)", levels, c->levels);
   if (levels == c->cam_levels[cam]) return SDV_OK;
   for (size_t s=0;s<c->slots.size();s++) if (c->slots[s].cam == cam && (c->slots[s].ref_frame != ~0ull || rp_slot_set(c, (int)s)))
@@ -155,7 +154,6 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
   CK(cudaStreamCreateWithFlags(&c->st_in, cudaStreamNonBlocking)); CK(cudaStreamCreateWithFlags(&c->st_cp, cudaStreamNonBlocking));
   for (int i=0;i<sdv_ctx::kIngRing;i++) CK(cudaEventCreateWithFlags(&c->ev_ing[i], cudaEventDisableTiming)); for (int i=0;i<2;i++) CK(cudaEventCreateWithFlags(&c->ev_cp[i], cudaEventDisableTiming));
   CK(cudaEventCreateWithFlags(&c->ev_in, cudaEventDisableTiming)); c->ingest_pending = false; c->launches = 0;
-  for (int i=0;i<2;i++) { c->pyr_batch_dev[i] = nullptr; c->pyr_batch_host[i] = nullptr; }
   CK(cudaEventCreate(&c->ev0)); CK(cudaEventCreate(&c->ev1)); CK(cudaEventCreate(&c->ba_ev0)); CK(cudaEventCreate(&c->ba_ev1)); CK(cudaEventCreateWithFlags(&c->ev_xdom, cudaEventDisableTiming));
   memset(&c->tc, 0, sizeof(c->tc));
   c->tc.levels = levels; c->tc.huberTH = s.huberTH; c->tc.coarseCutoffTH = s.coarseCutoffTH;
@@ -203,9 +201,7 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
   CK(cudaMalloc(&c->cd_counts, (size_t)(cd_num_blocks(w,h)+1)*sizeof(int)));
   CK(cudaMalloc(&c->cd_scalars, 8*sizeof(int)));
   CK(cudaMallocHost(&c->cd_scalars_host, 8*sizeof(int)));
-  c->cd_cap = 0; c->cd_pts4 = nullptr; c->cd_round = nullptr; c->cd_splats = nullptr; c->cd_done = nullptr;
-  c->jobs_cap = 0; c->jobs_dev = nullptr; c->jobs_host = nullptr;
-  c->desc_cap = 0; c->last_ms = 0;
+  c->last_ms = 0;
   return SDV_OK;
 }
 
@@ -218,14 +214,10 @@ void sdv_destroy(sdv_ctx* c) {
   for (auto& t : c->slots) for (int l=0;l<c->levels;l++) cudaFree(t.pts[l]);
   for (int l=0;l<c->levels;l++) { cudaFree(c->cd_id[l]); cudaFree(c->cd_ws[l]); cudaFree(c->cd_id2[l]); cudaFree(c->cd_ws2[l]); }
   cudaFree(c->cd_owner); cudaFree(c->cd_counts); cudaFree(c->cd_scalars); cudaFreeHost(c->cd_scalars_host);
-  cudaFree(c->cd_pts4); cudaFree(c->cd_round); cudaFree(c->cd_splats); cudaFree(c->cd_done);
-  for (int i=0;i<2;i++) { cudaFree(c->pyr_batch_dev[i]); cudaFreeHost(c->pyr_batch_host[i]); } cudaFree(c->partials); cudaFree(c->ticket); cudaFree(c->totals_dev); cudaFreeHost(c->totals_host);
-  cudaFree(c->tc_dev); cudaFree(c->geom_dev); cudaFree(c->jobs_dev); cudaFreeHost(c->jobs_host);
-  for (int i=0;i<2;i++) cudaFree(c->stage_u8[i]);
+  for (int i=0;i<2;i++) { c->ing_dev[i].release(); c->ing_host[i].release(); } cudaFree(c->partials); cudaFree(c->ticket); cudaFree(c->totals_dev); cudaFreeHost(c->totals_host);
+  cudaFree(c->tc_dev); cudaFree(c->geom_dev); c->scr.release(); c->scr_host.release();
   for (float* u : c->und_buf) cudaFree(u);
-  cudaFree(c->trace_dev);
   for (int i=0;i<sdv_ctx::kIngRing;i++) if (c->ev_ing[i]) cudaEventDestroy(c->ev_ing[i]); for (int i=0;i<2;i++) if (c->ev_cp[i]) cudaEventDestroy(c->ev_cp[i]); if (c->st_cp) cudaStreamDestroy(c->st_cp);
-  cudaFree(c->refine_dev); cudaFreeHost(c->refine_host);
   rp_destroy(c);
   sel_destroy(c);
   lidar_destroy(c);
@@ -246,18 +238,6 @@ int sdv_debug_gs_entry_rc(int k) { int r, c; if (k < 0 || k >= kNH) return -1; g
 float sdv_last_kernel_ms(sdv_ctx* c) { return c ? c->last_ms : 0.f; }
 
 // ------------------------------------------------------------------------------------------------ frames
-static FrameDev* find_frame(sdv_ctx* c, uint64_t id) { auto it = c->frame_index.find(id); return it == c->frame_index.end() ? nullptr : &c->frames[it->second]; }
-
-static int ensure_desc(sdv_ctx* c, int n) {
-  if (n > c->desc_cap) {
-    CK(cudaStreamSynchronize(c->st_in));
-    for (int i=0;i<2;i++) { cudaFree(c->pyr_batch_dev[i]); cudaFreeHost(c->pyr_batch_host[i]);
-      CK(cudaMalloc(&c->pyr_batch_dev[i], (size_t)n*sizeof(PyrBatchHost) + 16)); CK(cudaMallocHost(&c->pyr_batch_host[i], (size_t)n*sizeof(PyrBatchHost) + 16)); }
-    c->desc_cap = n;
-  }
-  return SDV_OK;
-}
-
 static void frame_drop_texels(sdv_ctx* c, FrameDev& f) { if (f.lvl0_slot >= 0) { c->lvl0_free.push_back(f.lvl0_slot); f.lvl0_slot = -1; } f.lvl[0] = nullptr; f.hi_tex = false; }
 
 // kind bit0: mono8 input, bit1: input already in device memory, bit2: adopt the (device, float) buffer as the frame's level-0 plane,
@@ -271,8 +251,7 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
   if (!c || n < 0 || !frames || !imgs) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK;
   const bool raw = (kind & 8), u8 = (kind & 1) || raw, dev = (kind & 2), adopt = (kind & 4) && dev && !u8;
-  if (cams) for (int k=0;k<n;k++)                                         // before any frame handle is claimed or anything is enqueued: a refused call changes no frame
-    if (cams[k] < 0 || cams[k] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "image %d names camera %d (valid: 0..%d)", k, cams[k], SDV_MAX_CAMERAS - 1);
+  { int rc = check_cams(c, n, cams, "frame upload", "image"); if (rc) return rc; }   // before any frame handle is claimed or anything is enqueued: a refused call changes no frame
   auto cam_of = [&](int k) { return cams ? cams[k] : 0; };
   if (raw) for (int k=0;k<n;k++)
     if (!c->und.cam[cam_of(k)].remapX) return ctx_fail(c, SDV_ERR_STATE, "raw upload before sdv_set_undistort (camera %d has no tables)", cam_of(k));
@@ -281,15 +260,16 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
   // staging buffers + descriptors of this parity were last used by ingest seq-2: it must have drained before the host rewrites the pinned
   // descriptors (the device-side order copy(seq) after pyramid(seq-2) is enforced on the copy stream below)
   if (seq > 2) CK(cudaEventSynchronize(c->ev_ing[(seq-2) % sdv_ctx::kIngRing]));
-  int rc = ensure_desc(c, n); if (rc) return rc;
   auto px = [&](int k) { return (size_t)c->cam_w[cam_of(k)]*c->cam_h[cam_of(k)]; };                  // rectified pixels of frame k
   auto px_in = [&](int k) { const sdv::UndistortDev& u = c->und.cam[cam_of(k)]; return raw ? (size_t)u.wOrg*u.hOrg : px(k); };   // bytes of mono8 input image k
-  if (u8 && !dev) { size_t total = 0; for (int k=0;k<n;k++) total += px_in(k);
-    if (total > c->stage_u8_cap[par]) { CK(cudaStreamSynchronize(c->st_in)); cudaFree(c->stage_u8[par]); c->stage_u8[par] = nullptr;
-      c->stage_u8_cap[par] = total; CK(cudaMalloc(&c->stage_u8[par], c->stage_u8_cap[par])); } }
+  size_t stage = 0; if (u8 && !dev) for (int k=0;k<n;k++) stage += px_in(k);
+  Scratch& sd = c->ing_dev[par]; PinnedScratch& sh = c->ing_host[par];      // need() leaves the descriptors the 16 B of slack launch_h2d_words reads past them
+  if (sd.reserve(Scratch::need(n, sizeof(PyrBatchHost)) + Scratch::need(stage, 1), c->st_in) || sh.reserve(Scratch::need(n, sizeof(PyrBatchHost)), c->st_in))
+    return ctx_fail(c, SDV_ERR_CUDA, "frame upload: staging of %d images", n);
+  sd.reset(); sh.reset(); PyrBatchHost* desc_dev = sd.take<PyrBatchHost>(n); PyrBatchHost* desc = sh.take<PyrBatchHost>(n); unsigned char* stage_u8 = sd.take<unsigned char>(stage);
   c->cp_dst.clear(); c->cp_src.clear(); c->cp_sz.clear();
   if (c->levels > 1 && ((c->w | c->h) & 1)) return ctx_fail(c, SDV_ERR_ARG, "pyramid needs even image sizes");
-  PyrBatchHost* desc = c->pyr_batch_host[par]; bool vec = true; size_t stage_off = 0; int max_w = 0, max_h = 0;
+  bool vec = true; size_t stage_off = 0; int max_w = 0, max_h = 0;
   for (int k=0;k<n;k++) {
     int idx = -1;
     auto it = c->frame_index.find(frames[k]);
@@ -305,7 +285,7 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
     b.pyr = f.pyr; b.I0 = f.I0; b.flags = (f.exposure > 0.f) ? 1 : 0; b.cam = f.cam; b.w = c->cam_w[f.cam]; b.h = c->cam_h[f.cam];
     max_w = std::max(max_w, b.w); max_h = std::max(max_h, b.h);
     if (dev) b.src = imgs[k];
-    else if (u8) { const size_t sz = px_in(k); unsigned char* d8 = c->stage_u8[par] + stage_off; stage_off += sz; b.src = d8;
+    else if (u8) { const size_t sz = px_in(k); unsigned char* d8 = stage_u8 + stage_off; stage_off += sz; b.src = d8;
       if (!c->cp_dst.empty() && (unsigned char*)c->cp_src.back() + c->cp_sz.back() == (const unsigned char*)imgs[k] && (unsigned char*)c->cp_dst.back() + c->cp_sz.back() == d8) c->cp_sz.back() += sz;   // adjacent in host memory: one copy, whatever the cameras
       else { c->cp_dst.push_back(d8); c->cp_src.push_back(const_cast<void*>(imgs[k])); c->cp_sz.push_back(sz); } }
     else { b.src = f.I0; c->cp_dst.push_back(f.I0); c->cp_src.push_back(const_cast<void*>(imgs[k])); c->cp_sz.push_back(px(k)*sizeof(float)); }
@@ -324,11 +304,11 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
     c->cp_dst.clear(); c->cp_src.clear(); c->cp_sz.clear();
     CK(cudaEventRecord(c->ev_cp[par], c->st_cp)); CK(cudaStreamWaitEvent(c->st_in, c->ev_cp[par], 0));
   }
-  launch_h2d_words(c->pyr_batch_dev[par], desc, (size_t)n*sizeof(PyrBatchHost), c->st_in);   // kernel copy: a cudaMemcpyAsync here becomes ready only after this batch's bulk copy and
+  launch_h2d_words(desc_dev, desc, (size_t)n*sizeof(PyrBatchHost), c->st_in);   // kernel copy: a cudaMemcpyAsync here becomes ready only after this batch's bulk copy and
   c->launches += 1;                                                                              // would queue behind the NEXT batch's bulk copy on the H2D engine
   const UndistortCams* und = raw ? &c->und : nullptr;
-  if (c->levels > 1) { launch_pyramid_batch(c->pyr_batch_dev[par], n, u8, vec, c->w, c->h, max_w, max_h, c->levels, c->st_in, und); c->launches += 1; }
-  else if (u8 || (dev && !adopt)) { launch_pyramid_copy0(c->pyr_batch_dev[par], n, u8, max_w, max_h, c->st_in, und); c->launches += 1; }
+  if (c->levels > 1) { launch_pyramid_batch(desc_dev, n, u8, vec, c->w, c->h, max_w, max_h, c->levels, c->st_in, und); c->launches += 1; }
+  else if (u8 || (dev && !adopt)) { launch_pyramid_copy0(desc_dev, n, u8, max_w, max_h, c->st_in, und); c->launches += 1; }
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev_ing[seq % sdv_ctx::kIngRing], c->st_in)); c->ingest_seq = seq; c->ingest_pending = true;
   return SDV_OK;
@@ -381,6 +361,19 @@ int check_frame_cam(sdv_ctx* c, const FrameDev& f, int cam, const char* who) {
   return ctx_fail(c, SDV_ERR_ARG, "%s: frame %llu is %dx%d (camera %d) but the job names camera %d, %dx%d", who, (unsigned long long)f.id,
                   c->cam_w[f.cam], c->cam_h[f.cam], f.cam, cam, c->cam_w[cam], c->cam_h[cam]);
 }
+int job_frame(sdv_ctx* c, const char* who, int k, uint64_t id, int cam, int slot, long long* need_seq, FrameDev** out) {
+  FrameDev* f = find_frame(c, id); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "%s: entry %d names unknown frame %llu", who, k, (unsigned long long)id);
+  const int rc = slot >= 0 ? check_frame_slot(c, *f, slot, who) : cam >= 0 ? check_frame_cam(c, *f, cam, who) : SDV_OK; if (rc) return rc;
+  if (need_seq && f->ingest_seq > *need_seq) *need_seq = f->ingest_seq;
+  *out = f; return SDV_OK;
+}
+int check_cams(sdv_ctx* c, int n, const int32_t* cams, const char* who, const char* what) {
+  if (cams) for (int k=0;k<n;k++) if (cams[k] < 0 || cams[k] >= SDV_MAX_CAMERAS) {
+    if (!what) return ctx_fail(c, SDV_ERR_ARG, "%s: camera %d outside 0..%d", who, cams[k], SDV_MAX_CAMERAS - 1);
+    return ctx_fail(c, SDV_ERR_ARG, "%s: %s %d names camera %d (valid: 0..%d)", who, what, k, cams[k], SDV_MAX_CAMERAS - 1);
+  }
+  return SDV_OK;
+}
 }
 extern "C" {
 
@@ -393,7 +386,7 @@ int sdv_frame_upload_batch_u8(sdv_ctx* c, int n, const uint64_t* frames, const u
 // Undistort (util/Undistort.cpp) as data: the tables the reference builds once per calibration file, kept on the device for the raw-image ingest, one entry per camera
 int sdv_set_undistort_cam(sdv_ctx* c, int cam, int w_org, int h_org, const float* remapX, const float* remapY, float factor, const float* G256, const float* vignette_inv) { SDV_GUARD_TRK(c);
   if (!c || w_org < 2 || h_org < 2 || !remapX || !remapY) return SDV_ERR_ARG;
-  if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "camera %d outside 0..%d", cam, SDV_MAX_CAMERAS - 1);
+  { int rc = check_cams(c, 1, &cam, "sdv_set_undistort_cam", nullptr); if (rc) return rc; }
   if (vignette_inv && !G256) return ctx_fail(c, SDV_ERR_ARG, "a vignette map needs a response function (PhotometricUndistorter::processFrame applies it to G[v] only)");
   CK(cudaSetDevice(c->device));
   const size_t px = (size_t)c->cam_w[cam]*c->cam_h[cam], po = (size_t)w_org*h_org;   // tables of the camera's rectified size
@@ -448,7 +441,7 @@ int sdv_frame_release(sdv_ctx* c, uint64_t frame) { SDV_GUARD_TRK(c);
 int sdv_frame_download(sdv_ctx* c, uint64_t frame, int lvl, float* dI3_out, float* abs_out) { SDV_GUARD_TRK(c);
   if (!c || lvl < 0 || lvl >= c->levels) return SDV_ERR_ARG;
   CK(cudaSetDevice(c->device));
-  FrameDev* f = find_frame(c, frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown frame %llu", (unsigned long long)frame);
+  FrameDev* f; { int rc = job_frame(c, "sdv_frame_download", 0, frame, -1, -1, nullptr, &f); if (rc) return rc; }
   if (lvl >= c->cam_levels[f->cam]) return ctx_fail(c, SDV_ERR_ARG, "sdv_frame_download: level %d of frame %llu, whose camera %d has %d levels", lvl, (unsigned long long)frame, f->cam, c->cam_levels[f->cam]);
   { int rcj = join_ingest(c); if (rcj) return rcj; }
   { int rct = ensure_texels(c, *f, lvl); if (rct) return rct; }
@@ -471,8 +464,7 @@ int sdv_tracker_set_cloud(sdv_ctx* c, int slot, uint64_t ref_frame, int lvl, int
   CK(cudaSetDevice(c->device));
   TrackerSlot& t = c->slots[slot];
   if (n > t.cap[lvl]) return ctx_fail(c, SDV_ERR_CAPACITY, "cloud of %d points exceeds capacity %d", n, t.cap[lvl]);
-  FrameDev* f = find_frame(c, ref_frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown ref frame");
-  { int rcs = check_frame_slot(c, *f, slot, "sdv_tracker_set_cloud"); if (rcs) return rcs; }
+  FrameDev* f; { int rc = job_frame(c, "sdv_tracker_set_cloud", 0, ref_frame, -1, slot, nullptr, &f); if (rc) return rc; }
   { int rcj = join_ingest(c); if (rcj) return rcj; }
   float* tmp = nullptr; CK(cudaMalloc(&tmp, (size_t)4*(n+1)*sizeof(float)));
   const float* src[4] = {u, v, idepth, color};
@@ -500,29 +492,26 @@ int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const f
   if (!c || slot < 0 || slot >= (int)c->slots.size() || n < 0 || (n > 0 && (!pts4 || !round_half))) return SDV_ERR_ARG;
   CK(cudaSetDevice(c->device));
   TrackerSlot& t = c->slots[slot];
-  FrameDev* f = find_frame(c, ref_frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown ref frame");
-  { int rcs = check_frame_slot(c, *f, slot, "sdv_tracker_set_ref"); if (rcs) return rcs; }
+  FrameDev* f; { int rc = job_frame(c, "sdv_tracker_set_ref", 0, ref_frame, -1, slot, nullptr, &f); if (rc) return rc; }
   const int w = c->cam_w[t.cam], h = c->cam_h[t.cam], L = c->cam_levels[t.cam];   // makeCoarseDepthL0 at the slot's size, for its camera's pyrLevelsUsed levels
   for (int i=0;i<n;i++) {                                   // the reference would write out of bounds here; we refuse instead
     int u = round_half[i] ? (int)(pts4[4*i]+0.5f) : (int)pts4[4*i], v = round_half[i] ? (int)(pts4[4*i+1]+0.5f) : (int)pts4[4*i+1];
     if (u < 0 || v < 0 || u >= w || v >= h) return ctx_fail(c, SDV_ERR_ARG, "splat %d (%d,%d) outside the image", i, u, v);
   }
-  if (n > c->cd_cap) {
-    cudaFree(c->cd_pts4); cudaFree(c->cd_round); cudaFree(c->cd_splats); cudaFree(c->cd_done);
-    c->cd_cap = n + n/2 + 1024;
-    CK(cudaMalloc(&c->cd_pts4, (size_t)4*c->cd_cap*sizeof(float))); CK(cudaMalloc(&c->cd_round, (size_t)c->cd_cap*sizeof(int)));
-    CK(cudaMalloc(&c->cd_splats, (size_t)c->cd_cap*sizeof(float4))); CK(cudaMalloc(&c->cd_done, (size_t)c->cd_cap*sizeof(int)));
-  }
+  Scratch& S = c->scr;
+  if (S.reserve(Scratch::need(4*(size_t)n, sizeof(float)) + 2*Scratch::need(n, sizeof(int)) + Scratch::need(n, sizeof(float4)), c->st))
+    return ctx_fail(c, SDV_ERR_CUDA, "sdv_tracker_set_ref: scratch of %d splats", n);
+  S.reset(); float* pts4_d = S.take<float>(4*(size_t)n); int* round_d = S.take<int>(n); float4* splats = S.take<float4>(n); int* done = S.take<int>(n);
   { int rcj = join_ingest(c); if (rcj) return rcj; }
   CK(cudaMemsetAsync(c->cd_id[0], 0, (size_t)w*h*sizeof(float), c->st));
   CK(cudaMemsetAsync(c->cd_ws[0], 0, (size_t)w*h*sizeof(float), c->st));
   if (n > 0) {
-    CK(cudaMemcpyAsync(c->cd_pts4, pts4, (size_t)4*n*sizeof(float), cudaMemcpyHostToDevice, c->st));
-    CK(cudaMemcpyAsync(c->cd_round, round_half, (size_t)n*sizeof(int), cudaMemcpyHostToDevice, c->st));
-    launch_cd_prep(c->cd_pts4, c->cd_round, n, w, c->cd_splats, c->cd_done, c->st);
+    CK(cudaMemcpyAsync(pts4_d, pts4, (size_t)4*n*sizeof(float), cudaMemcpyHostToDevice, c->st));
+    CK(cudaMemcpyAsync(round_d, round_half, (size_t)n*sizeof(int), cudaMemcpyHostToDevice, c->st));
+    launch_cd_prep(pts4_d, round_d, n, w, splats, done, c->st);
     for (int round = 0; round < n; round++) {               // usually 1-3 rounds: one per multiplicity of colliding splats; at most n (every splat on one pixel)
       CK(cudaMemsetAsync(c->cd_scalars, 0, sizeof(int), c->st));
-      launch_cd_round(c->cd_splats, n, c->cd_done, c->cd_owner, c->cd_id[0], c->cd_ws[0], c->cd_scalars, c->st);
+      launch_cd_round(splats, n, done, c->cd_owner, c->cd_id[0], c->cd_ws[0], c->cd_scalars, c->st);
       CK(cudaMemcpyAsync(c->cd_scalars_host, c->cd_scalars, sizeof(int), cudaMemcpyDeviceToHost, c->st));
       CK(cudaStreamSynchronize(c->st));
       if (c->cd_scalars_host[0] == 0) break;
@@ -552,7 +541,7 @@ int sdv_tracker_calc_res(sdv_ctx* c, int slot, uint64_t new_frame, int lvl, cons
   if (lvl >= slot_levels(c, slot)) return ctx_fail(c, SDV_ERR_ARG, "sdv_tracker_calc_res: level %d, but slot %d's camera has %d levels", lvl, slot, slot_levels(c, slot));
   CK(cudaSetDevice(c->device));
   TrackerSlot& t = c->slots[slot];
-  FrameDev* f = find_frame(c, new_frame); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown new frame");
+  FrameDev* f; { int rc = job_frame(c, "sdv_tracker_calc_res", 0, new_frame, -1, -1, nullptr, &f); if (rc) return rc; }
   if (t.ref_frame == ~0ull) return ctx_fail(c, SDV_ERR_STATE, "tracker slot %d has no reference", slot);
   { int rcs = check_frame_slot(c, *f, slot, "sdv_tracker_calc_res"); if (rcs) return rcs; }
   const LevelGeom& g = slot_geom(c, slot).g[lvl];
@@ -584,22 +573,20 @@ static int track_batch_impl(sdv_ctx* c, int n, const int32_t* slots, const uint6
                             const double* minRes, double* lastRes, double* flow, int32_t* good, sdv_track_stats* stats) {
   if (!c || n <= 0 || !slots || !new_frames || !T_io || !ab_io) return SDV_ERR_ARG;
   CK(cudaSetDevice(c->device));
-  if (n > c->jobs_cap) {
-    cudaFree(c->jobs_dev); cudaFreeHost(c->jobs_host); c->jobs_cap = n;
-    CK(cudaMalloc(&c->jobs_dev, (size_t)n*sizeof(TrackJob) + 16)); CK(cudaMallocHost(&c->jobs_host, (size_t)n*sizeof(TrackJob) + 16));
-  }
+  const size_t bytes = Scratch::need(n, sizeof(TrackJob));                // need(): the 16 B of slack launch_h2d_words reads past the jobs
+  if (c->scr.reserve(bytes, c->st) || c->scr_host.reserve(bytes, c->st)) return ctx_fail(c, SDV_ERR_CUDA, "sdv_tracker_track_batch: staging of %d jobs", n);
+  c->scr.reset(); c->scr_host.reset(); TrackJob* jobs_dev = c->scr.take<TrackJob>(n); TrackJob* jobs_host = c->scr_host.take<TrackJob>(n);
   long long need_seq = 0;
   for (int k=0;k<n;k++) {
     if (slots[k] < 0 || slots[k] >= (int)c->slots.size()) return SDV_ERR_ARG;
     TrackerSlot& t = c->slots[slots[k]];
-    FrameDev* f = find_frame(c, new_frames[k]); if (!f) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown new frame (job %d)", k);
-    if (f->ingest_seq > need_seq) need_seq = f->ingest_seq;
+    FrameDev* f; { int rc = job_frame(c, "sdv_tracker_track_batch", k, new_frames[k], -1, -1, &need_seq, &f); if (rc) return rc; }
     if (t.ref_frame == ~0ull) return ctx_fail(c, SDV_ERR_STATE, "tracker slot %d has no reference", slots[k]);
     { int rcs = check_frame_slot(c, *f, slots[k], "sdv_tracker_track_batch"); if (rcs) return rcs; }
     const int L = slot_levels(c, slots[k]), co = all_coarsest >= 0 ? all_coarsest : (coarsest ? coarsest[k] : L - 1);
     if (co < 0 || co >= L || co >= 5)                                   // CoarseTracker.cpp:672: assert(coarsestLvl < 5 && coarsestLvl < pyrLevelsUsed)
       return ctx_fail(c, SDV_ERR_ARG, "sdv_tracker_track_batch: job %d starts at level %d, but slot %d's camera has %d levels (and the tracker at most 5)", k, co, slots[k], L);
-    TrackJob& J = c->jobs_host[k]; memset(&J, 0, sizeof(J));
+    TrackJob& J = jobs_host[k]; memset(&J, 0, sizeof(J));
     for (int l=0;l<c->levels;l++) { J.img[l] = f->img[l]; J.pts[l] = t.pts[l]; J.npts[l] = t.npts[l]; }
     J.refExposure = t.refExposure; J.newExposure = f->exposure; J.ref_a = t.ref_a; J.ref_b = t.ref_b;
     for (int i=0;i<7;i++) J.T[i] = T_io[7*k+i];
@@ -609,15 +596,15 @@ static int track_batch_impl(sdv_ctx* c, int n, const int32_t* slots, const uint6
   }
   { int rcj = join_ingest_upto(c, need_seq); if (rcj) return rcj; }     // only the uploads that built THESE frames: batch k+1's upload keeps streaming
   c->launches += 2;                                                    // descriptor copy kernel + track_cluster_kernel
-  launch_h2d_words(c->jobs_dev, c->jobs_host, (size_t)n*sizeof(TrackJob), c->st);      // kernel copy: not queued behind the next batch's image upload
+  launch_h2d_words(jobs_dev, jobs_host, (size_t)n*sizeof(TrackJob), c->st);      // kernel copy: not queued behind the next batch's image upload
   CK(cudaEventRecord(c->ev0, c->st));
-  CK(launch_track_cluster(c->jobs_dev, n, c->tc_dev, c->geom_dev, c->set.cluster_size, c->set.track_threads, c->st));
+  CK(launch_track_cluster(jobs_dev, n, c->tc_dev, c->geom_dev, c->set.cluster_size, c->set.track_threads, c->st));
   CK(cudaEventRecord(c->ev1, c->st));
-  CK(cudaMemcpyAsync(c->jobs_host, c->jobs_dev, (size_t)n*sizeof(TrackJob), cudaMemcpyDeviceToHost, c->st));
+  CK(cudaMemcpyAsync(jobs_host, jobs_dev, (size_t)n*sizeof(TrackJob), cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st)); CK(cudaGetLastError());
   CK(cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   for (int k=0;k<n;k++) {
-    const TrackJob& J = c->jobs_host[k];
+    const TrackJob& J = jobs_host[k];
     for (int i=0;i<7;i++) T_io[7*k+i] = J.T[i];
     ab_io[2*k] = J.ab[0]; ab_io[2*k+1] = J.ab[1];
     if (lastRes) for (int i=0;i<5;i++) lastRes[5*k+i] = J.lastRes[i];

@@ -32,14 +32,20 @@ __device__ __forceinline__ int block_excl_scan(int v, int* sm /* 2*blockDim */, 
 
 #define SEL_CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { err = std::string(#call) + " -> " + cudaGetErrorString(e_); return -1; } } while (0)
 
-struct Scratch {                                             // grow-only device buffer carved into aligned pieces
+}  // namespace sel
+
+// Grow-only buffer carved into 256-byte aligned pieces: reserve(sum of need()), reset, then take the pieces in order.  One instance serves one stream:
+// reserve waits for that stream before it frees a buffer that is too small, and keeps 25 % headroom, so the steady state allocates nothing.
+// need() includes 256 bytes of slack past the piece.  Mem: alloc / dealloc of the memory kind (DeviceMem here; sdv_ctx.cuh adds pinned host memory).
+template <class Mem> struct ScratchOf {
   char* p = nullptr; size_t cap = 0, used = 0;
-  int reserve(size_t bytes, cudaStream_t st) { if (bytes <= cap) return 0; cudaStreamSynchronize(st); if (p) cudaFree(p); p = nullptr; cap = 0; if (cudaMalloc((void**)&p, bytes + bytes/4) != cudaSuccess) return -1; cap = bytes + bytes/4; return 0; }
+  int reserve(size_t bytes, cudaStream_t st) { if (bytes <= cap) return 0; cudaStreamSynchronize(st); release(); if (Mem::alloc((void**)&p, bytes + bytes/4) != cudaSuccess) { p = nullptr; return -1; } cap = bytes + bytes/4; return 0; }
   void reset() { used = 0; }
   template <class T> T* take(size_t n) { used = (used + 255) & ~(size_t)255; T* r = (T*)(p + used); used += n*sizeof(T); return r; }
   static size_t need(size_t n, size_t sz) { return ((n*sz + 255) & ~(size_t)255) + 256; }
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+  void release() { if (p) Mem::dealloc(p); p = nullptr; cap = 0; }
 };
+struct DeviceMem { static cudaError_t alloc(void** p, size_t n) { return cudaMalloc(p, n); } static void dealloc(void* p) { cudaFree(p); } };
+using Scratch = ScratchOf<DeviceMem>;
 
-
-}}  // namespace sdv::sel
+}  // namespace sdv

@@ -5,9 +5,14 @@
 #include <mutex>
 #include <atomic>
 #include "sdv_kernels.cuh"
+#include "sdv_core_common.cuh"
 #include "../../include/sdv_b200.h"
 
 namespace sdv {
+
+// pinned host twin of Scratch: taken in the same order as its device instance, a staged layout moves in one copy (or one launch_h2d_words)
+struct PinnedMem { static cudaError_t alloc(void** p, size_t n) { return cudaMallocHost(p, n); } static void dealloc(void* p) { cudaFreeHost(p); } };
+using PinnedScratch = ScratchOf<PinnedMem>;
 
 struct FrameDev {                         // one FrameHessian's images on the device
   uint64_t id; float exposure; bool used;
@@ -56,8 +61,8 @@ struct sdv_ctx {
   // frames whose device images are referenced by a resident BA window (BAHeader::frames[].img0) or map slot (MapDev::hostI0): refcount per handle.
   // A pinned frame can be neither released nor re-uploaded (SDV_ERR_STATE) — its pool storage would be handed to another frame under the reader.
   std::unordered_map<uint64_t,int> pins;
-  unsigned char* stage_u8[2] = {nullptr, nullptr}; size_t stage_u8_cap[2] = {0, 0};   // contiguous mono8 staging per parity (adjacent host images coalesce into one copy)
-  int desc_cap; sdv::PyrBatchHost* pyr_batch_dev[2]; sdv::PyrBatchHost* pyr_batch_host[2];     // double-buffered by ingest parity
+  // ingest staging, double-buffered by ingest parity (serves st_in): pyramid descriptors, then the contiguous mono8 images (adjacent host images coalesce into one copy)
+  sdv::Scratch ing_dev[2]; sdv::PinnedScratch ing_host[2];
   sdv::UndistortCams und = {}; float* und_buf[SDV_MAX_CAMERAS] = {};                 // sdv_set_undistort_cam: per camera, remap tables (+ response / vignette) of the raw-image ingest
                                                                                     // in one allocation und_buf[k]; a camera is set iff und.cam[k].remapX != nullptr
   std::vector<float4*> lvl0_pool; std::vector<int> lvl0_free;
@@ -66,11 +71,9 @@ struct sdv_ctx {
   double* partials; unsigned int* ticket; double* totals_dev; double* totals_host;
   float *cd_id[sdv::kLevels], *cd_ws[sdv::kLevels], *cd_id2[sdv::kLevels], *cd_ws2[sdv::kLevels];
   int* cd_owner; int* cd_counts; int* cd_scalars; int* cd_scalars_host;
-  int cd_cap; float* cd_pts4; int* cd_round; float4* cd_splats; int* cd_done;
-  int jobs_cap; sdv::TrackJob* jobs_dev; sdv::TrackJob* jobs_host;
   float last_ms;
-  void* refine_dev = nullptr; void* refine_host = nullptr; size_t refine_cap = 0;      // staging of sdv_tracker_struct_pose_batch
-  void* trace_dev = nullptr; size_t trace_cap = 0;                                  // scratch of the immature-point calls (sdv_trace.cu)
+  // per-call scratch of the tracker stream st (splats, tracker jobs, refine, Reprojector, immature points); valid until the next call that takes from it
+  sdv::Scratch scr; sdv::PinnedScratch scr_host;
   cudaEvent_t ev_trk_async = nullptr;           // recorded on st after the last call that returned with a kernel still reading frames (FrameDev::trk_async)
   void* imm_store = nullptr;                    // sdv::ImmStore: device-resident immature points, one block per host keyframe (sdv_trace.cu)
   void* lidar = nullptr;                        // sdv::LidarState: engine of the LiDAR front-end (sdv_lidar.cu)
@@ -78,7 +81,8 @@ struct sdv_ctx {
   void* sel = nullptr;                          // sdv::SelState: PixelSelector slots + engine of the candidate management (sdv_select.cu)
   sdv::RpState* rp = nullptr;                   // map slots + scratch of the Reprojector path (sdv_reproject.cu)
   sdv::BAState* ba = nullptr;                   // selected back-end window
-  std::vector<sdv::BAState*> ba_windows; void* ba_wins_dev = nullptr; void* ba_wins_host = nullptr; int ba_wins_cap = 0;
+  // ba_wins_dev serves st_ba and holds only the window descriptors, at offset 0: its address keys ba_graph
+  std::vector<sdv::BAState*> ba_windows; sdv::Scratch ba_wins_dev; sdv::PinnedScratch ba_wins_host;
   // the fixed Gauss-Newton launch schedule of sdv_ba_optimize_batch as a CUDA graph, keyed by what the launches depend on
   cudaGraphExec_t ba_graph = nullptr; const void* bag_wins = nullptr; int bag_n = 0, bag_maxP = 0, bag_maxR = 0, bag_its = 0;
   char err[512];
@@ -122,9 +126,17 @@ inline bool same_size_depth(const sdv_ctx* c, int cam_a, int cam_b) { return sam
 inline int slot_levels(const sdv_ctx* c, int slot) { return c->cam_levels[c->slots[slot].cam]; }   // pyrLevelsUsed of a tracker / map slot
 int  check_frame_slot(sdv_ctx* c, const FrameDev& f, int slot, const char* who);   // SDV_ERR_ARG (with a message) when frame f's size differs from slot's
 int  check_frame_cam(sdv_ctx* c, const FrameDev& f, int cam, const char* who);     // ... from camera cam's (keyframe-rate stages: the job names its camera)
+inline FrameDev* find_frame(sdv_ctx* c, uint64_t id) { auto it = c->frame_index.find(id); return it == c->frame_index.end() ? nullptr : &c->frames[it->second]; }
+// *out = the frame entry k of `who` names: SDV_ERR_NOFRAME for an unknown handle, SDV_ERR_ARG when its size is not that of tracker / map slot `slot` (slot >= 0) or
+// of camera cam (cam >= 0; neither: any size).  *need_seq (if given) rises to the ingest that built it: join_ingest_upto(need_seq) once after the caller's loop.
+int  job_frame(sdv_ctx* c, const char* who, int k, uint64_t id, int cam, int slot, long long* need_seq, FrameDev** out);
+// SDV_ERR_ARG (with a message) unless every cams[k] of the n is a camera; cams == NULL: every entry is camera 0
+int  check_cams(sdv_ctx* c, int n, const int32_t* cams, const char* who, const char* what);
 bool sel_cam_bound(const sdv_ctx* c, int cam, int* slot);                          // a selector slot (*slot) is bound to camera cam (sdv_selector_set_slot_cams)
 bool rp_slot_set(const sdv_ctx* c, int slot);                                     // map slot `slot` holds a resident map (sdv_map_set, not cleared)
 }
 // entry-point guards (a NULL context falls through to the entry's own argument check)
 #define SDV_GUARD_TRK(c) std::unique_lock<std::recursive_mutex> lk_trk_; if (c) lk_trk_ = std::unique_lock<std::recursive_mutex>((c)->mu_trk)
 #define SDV_GUARD_BA(c)  std::unique_lock<std::recursive_mutex> lk_ba_;  if (c) lk_ba_  = std::unique_lock<std::recursive_mutex>((c)->mu_ba)
+// a failed CUDA call returns SDV_ERR_CUDA from the enclosing function, with the call and the place in the context's message (needs `c` in scope)
+#define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return sdv::ctx_fail(c, SDV_ERR_CUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)

@@ -12,7 +12,6 @@
 #include "sdv_lidar_core.cuh"
 
 using namespace sdv;
-#define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return ctx_fail(c, SDV_ERR_CUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
 
 namespace sdv {
 struct LidarState { lidar::LidarEngine eng; };
@@ -28,9 +27,9 @@ struct RowBlock {
   static RowBlock layout(char* p, int cap) { RowBlock b; b.p = p; b.cap = cap; return b; }
 };
 static_assert(sizeof(lidar::RowsHdr) == 64, "row-set header");
-struct RowStore : BlockPool<RowBlock> { sel::Scratch io; };                                // io: the header gather of lidar_rows_fetch
+struct RowStore : BlockPool<RowBlock> {};
 static RowStore* rows_store(sdv_ctx* c) { if (!c->lidar_rows) c->lidar_rows = new RowStore(); return (RowStore*)c->lidar_rows; }
-void lidar_rows_destroy(sdv_ctx* c) { RowStore* R = (RowStore*)c->lidar_rows; if (!R) return; R->release(); R->io.release(); delete R; c->lidar_rows = nullptr; }
+void lidar_rows_destroy(sdv_ctx* c) { RowStore* R = (RowStore*)c->lidar_rows; if (!R) return; R->release(); delete R; c->lidar_rows = nullptr; }
 __global__ void __launch_bounds__(128) lf_rows_hdr_gather_kernel(const lidar::RowsHdr* const* __restrict__ src, int n, lidar::RowsHdr* __restrict__ dst) {
   const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i < n) dst[i] = *src[i];
 }
@@ -40,8 +39,8 @@ int lidar_rows_fetch(sdv_ctx* c, int n, const uint64_t* frames, const double** r
     if (!R || it == R->blocks.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "%s: frame %llu has no LiDAR row set", who, (unsigned long long)frames[j]);
     src[j] = it->second.hdr(); rows_dev[j] = it->second.rows(); info[j].room = it->second.n; }
   if (n == 0) return SDV_OK;
-  if (R->io.reserve(sel::Scratch::need(n, sizeof(void*)) + sel::Scratch::need(n, sizeof(lidar::RowsHdr)), c->st)) return ctx_fail(c, SDV_ERR_CUDA, "%s: scratch", who);
-  R->io.reset(); const lidar::RowsHdr** dsrc = R->io.take<const lidar::RowsHdr*>(n); lidar::RowsHdr* dh = R->io.take<lidar::RowsHdr>(n); std::vector<lidar::RowsHdr> h(n);
+  if (c->scr.reserve(Scratch::need(n, sizeof(void*)) + Scratch::need(n, sizeof(lidar::RowsHdr)), c->st)) return ctx_fail(c, SDV_ERR_CUDA, "%s: scratch", who);
+  c->scr.reset(); const lidar::RowsHdr** dsrc = c->scr.take<const lidar::RowsHdr*>(n); lidar::RowsHdr* dh = c->scr.take<lidar::RowsHdr>(n); std::vector<lidar::RowsHdr> h(n);
   CK(cudaMemcpyAsync(dsrc, src.data(), n*sizeof(void*), cudaMemcpyHostToDevice, c->st));
   lf_rows_hdr_gather_kernel<<<(n + 127)/128, 128, 0, c->st>>>(dsrc, n, dh); c->launches += 1; CK(cudaGetLastError());
   CK(cudaMemcpyAsync(h.data(), dh, n*sizeof(lidar::RowsHdr), cudaMemcpyDeviceToHost, c->st)); CK(cudaStreamSynchronize(c->st));
@@ -70,8 +69,8 @@ int sdv_lidar_handler_batch_cams(sdv_ctx* c, int n, const int32_t* sweep_begin, 
   LidarState* s = (LidarState*)c->lidar; if (!s) return ctx_fail(c, SDV_ERR_STATE, "lidar_handler: sdv_lidar_init has not been called");
   if (sweep_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler: sweep_begin[0] must be 0");
   for (int j = 0; j < n; j++) { if (sweep_begin[j+1] < sweep_begin[j]) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler: sweep_begin is not ascending at sweep %d", j);
-    if (sweep_begin[j+1] > sweep_begin[j] && !xyzi) return SDV_ERR_ARG;
-    if (cams && (cams[j] < 0 || cams[j] >= SDV_MAX_CAMERAS)) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler: sweep %d names camera %d (valid: 0..%d)", j, cams[j], SDV_MAX_CAMERAS - 1); }
+    if (sweep_begin[j+1] > sweep_begin[j] && !xyzi) return SDV_ERR_ARG; }
+  { int rc = check_cams(c, n, cams, "lidar_handler", "sweep"); if (rc) return rc; }
   CK(cudaSetDevice(c->device));
   std::vector<lidar::LidarEngine::Sweep> S(n);
   for (int j = 0; j < n; j++) { auto& w = S[j]; w.xyzi_host = xyzi ? xyzi + 4*(size_t)sweep_begin[j] : nullptr; w.n = sweep_begin[j+1] - sweep_begin[j];

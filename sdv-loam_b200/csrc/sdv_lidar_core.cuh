@@ -21,7 +21,6 @@
 #include <float.h>
 
 namespace sdv { namespace lidar {
-using sel::Scratch;
 
 struct LidarSet { int N, H; float ang_res_x, ang_res_y, ang_bottom; int groundScanInd; float sensorMountAngle, segmentTheta, sinX, cosX, sinY, cosY; int validPointNum, validLineNum; };
 struct LidarJob {

@@ -205,15 +205,6 @@ void launch_struct_pose(RefineJob* jobs, int n_jobs, const sdv_overlap_pt* pts, 
 } // namespace sdv
 
 using namespace sdv;
-#define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return ctx_fail(c, SDV_ERR_CUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
-
-static int refine_reserve(sdv_ctx* c, size_t bytes) {
-  if (bytes <= c->refine_cap) return SDV_OK;
-  cudaFree(c->refine_dev); cudaFreeHost(c->refine_host); c->refine_dev = c->refine_host = nullptr; c->refine_cap = 0;
-  size_t cap = bytes + bytes/2 + 4096;
-  CK(cudaMalloc(&c->refine_dev, cap)); CK(cudaMallocHost(&c->refine_host, cap)); c->refine_cap = cap;
-  return SDV_OK;
-}
 
 extern "C" {
 
@@ -230,23 +221,24 @@ int sdv_tracker_struct_pose_batch_slots(sdv_ctx* c, int n_jobs, const int32_t* s
     for (int i=pt_begin[k]; i<pt_begin[k+1]; i++) if (pts[i].host < 0 || pts[i].host >= hs) return ctx_fail(c, SDV_ERR_ARG, "struct_pose job %d: point %d names host %d of %d", k, i, pts[i].host, hs);
   }
   CK(cudaSetDevice(c->device));
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  size_t o_jobs = 0, o_pts = al(o_jobs + (size_t)n_jobs*sizeof(RefineJob)), o_host = al(o_pts + (size_t)nP*sizeof(sdv_overlap_pt)), total = al(o_host + (size_t)nH*7*sizeof(double));
-  { int rc = refine_reserve(c, total); if (rc) return rc; }
-  unsigned char* hb = (unsigned char*)c->refine_host; unsigned char* db = (unsigned char*)c->refine_dev;
-  RefineJob* J = (RefineJob*)(hb + o_jobs);
+  Scratch& D = c->scr; PinnedScratch& Hs = c->scr_host;                  // the same layout on both sides: one copy stages jobs, points and host poses
+  const size_t bytes = Scratch::need(n_jobs, sizeof(RefineJob)) + Scratch::need(nP, sizeof(sdv_overlap_pt)) + Scratch::need((size_t)nH*7, sizeof(double));
+  if (D.reserve(bytes, c->st) || Hs.reserve(bytes, c->st)) return ctx_fail(c, SDV_ERR_CUDA, "struct_pose: staging of %d jobs", n_jobs);
+  D.reset(); Hs.reset();
+  RefineJob* J = Hs.take<RefineJob>(n_jobs); sdv_overlap_pt* hpts = Hs.take<sdv_overlap_pt>(nP); double* hT = Hs.take<double>((size_t)nH*7);
+  RefineJob* dJ = D.take<RefineJob>(n_jobs); const sdv_overlap_pt* dpts = D.take<sdv_overlap_pt>(nP); const double* dT = D.take<double>((size_t)nH*7);
   for (int k=0;k<n_jobs;k++) { memset(&J[k], 0, sizeof(RefineJob)); for (int i=0;i<7;i++) J[k].T[i] = curToWorld_io[7*k+i];
     J[k].pt_begin = pt_begin[k]; J[k].pt_end = pt_begin[k+1]; J[k].host_begin = host_begin[k]; J[k].nH = host_begin[k+1]-host_begin[k];
     J[k].geom_row = slots ? c->slots[slots[k]].geom_row : 0; }
-  if (nP) memcpy(hb + o_pts, pts, (size_t)nP*sizeof(sdv_overlap_pt));
-  memcpy(hb + o_host, host_T7, (size_t)nH*7*sizeof(double));
+  if (nP) memcpy(hpts, pts, (size_t)nP*sizeof(sdv_overlap_pt));
+  memcpy(hT, host_T7, (size_t)nH*7*sizeof(double));
   c->launches += 1;
-  CK(cudaMemcpyAsync(db, hb, total, cudaMemcpyHostToDevice, c->st));
+  CK(cudaMemcpyAsync(D.p, Hs.p, Hs.used, cudaMemcpyHostToDevice, c->st));
   CK(cudaEventRecord(c->ev0, c->st));
-  launch_struct_pose((RefineJob*)(db + o_jobs), n_jobs, (const sdv_overlap_pt*)(db + o_pts), (const double*)(db + o_host), c->geom_dev, c->st);
+  launch_struct_pose(dJ, n_jobs, dpts, dT, c->geom_dev, c->st);
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev1, c->st));
-  CK(cudaMemcpyAsync(hb + o_jobs, db + o_jobs, (size_t)n_jobs*sizeof(RefineJob), cudaMemcpyDeviceToHost, c->st));
+  CK(cudaMemcpyAsync(J, dJ, (size_t)n_jobs*sizeof(RefineJob), cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st));
   CK(cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   for (int k=0;k<n_jobs;k++) { for (int i=0;i<7;i++) curToWorld_io[7*k+i] = J[k].T[i];

@@ -316,11 +316,10 @@ __global__ void __launch_bounds__(1024) rp_emit_kernel(const RpJob* __restrict__
 } // namespace sdv
 
 using namespace sdv;
-#define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return ctx_fail(c, SDV_ERR_CUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
 
 namespace sdv {
 struct MapSlot { long long ingest_seq = 0; MapDev host_copy; MapDev* dev = nullptr; sdv_map_pt* pts = nullptr; int cap = 0; int nH = 0, nP = 0; uint64_t host_ids[kRpMaxHosts]; double host_ab[kRpMaxHosts][2]; float host_exposure[kRpMaxHosts]; bool set = false; };
-struct RpState { std::vector<MapSlot> maps; void* dev = nullptr; void* host = nullptr; size_t cap = 0, host_cap = 0; RpConst C; };
+struct RpState { std::vector<MapSlot> maps; RpConst C; };
 static void rp_job_K(const LevelGeom& g, double* K, double* Ki);
 static RpState* rp_state(sdv_ctx* c) {
   if (!c->rp) { c->rp = new RpState(); c->rp->maps.resize(c->slots.size()); RpConst& C = c->rp->C;
@@ -328,7 +327,7 @@ static RpState* rp_state(sdv_ctx* c) {
   return c->rp;
 }
 bool rp_slot_set(const sdv_ctx* c, int slot) { return c->rp && slot < (int)c->rp->maps.size() && c->rp->maps[slot].set; }
-void rp_destroy(sdv_ctx* c) { if (!c->rp) return; for (auto& m : c->rp->maps) { if (m.set) for (int k=0;k<m.nH;k++) frame_unpin(c, m.host_ids[k]); cudaFree(m.dev); cudaFree(m.pts); } cudaFree(c->rp->dev); cudaFreeHost(c->rp->host); delete c->rp; c->rp = nullptr; }
+void rp_destroy(sdv_ctx* c) { if (!c->rp) return; for (auto& m : c->rp->maps) { if (m.set) for (int k=0;k<m.nH;k++) frame_unpin(c, m.host_ids[k]); cudaFree(m.dev); cudaFree(m.pts); } delete c->rp; c->rp = nullptr; }
 static void rp_job_K(const LevelGeom& g, double* K, double* Ki) {        // the Reprojector's K_ and K_.inverse() (Reprojector.cpp:565) from level 0 of a geometry row
   for (int i=0;i<9;i++) K[i] = 0; K[0] = (double)g.fx; K[2] = (double)g.cx; K[4] = (double)g.fy; K[5] = (double)g.cy; K[8] = 1.0;
   { const double* A = K; double* R = Ki;                                       // Eigen fixed 3x3 inverse: cofactors / determinant
@@ -354,13 +353,13 @@ int sdv_map_set(sdv_ctx* c, int slot, int nH, const uint64_t* host_frames, const
   if (!m.dev) CK(cudaMalloc(&m.dev, sizeof(MapDev)));
   if (nP > m.cap) { cudaFree(m.pts); m.pts = nullptr; m.cap = nP + nP/4 + 256; CK(cudaMalloc(&m.pts, (size_t)m.cap*sizeof(sdv_map_pt))); }
   { int rcj = join_ingest(c); if (rcj) return rcj; }
-  for (int k=0;k<nH;k++) { auto it = c->frame_index.find(host_frames[k]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "map_set: unknown keyframe handle (host %d)", k);
-    int rcs = check_frame_slot(c, c->frames[it->second], slot, "sdv_map_set"); if (rcs) return rcs; }
+  FrameDev* F[kRpMaxHosts]; long long need_seq = 0;
+  for (int k=0;k<nH;k++) { int rcs = job_frame(c, "sdv_map_set", k, host_frames[k], -1, slot, &need_seq, &F[k]); if (rcs) return rcs; }
   if (m.set) for (int k=0;k<m.nH;k++) frame_unpin(c, m.host_ids[k]);       // the slot's previous keyframes are no longer referenced by it
   for (int k=0;k<nH;k++) frame_pin(c, host_frames[k]);
-  MapDev& h = m.host_copy; memset(&h, 0, sizeof(h)); h.nH = nH; h.nP = nP; h.pts = m.pts; m.ingest_seq = 0;
-  for (int k=0;k<nH;k++) { auto it = c->frame_index.find(host_frames[k]);
-    const FrameDev& f = c->frames[it->second]; h.hostI0[k] = f.I0; m.host_exposure[k] = f.exposure; m.host_ids[k] = host_frames[k]; if (f.ingest_seq > m.ingest_seq) m.ingest_seq = f.ingest_seq;
+  MapDev& h = m.host_copy; memset(&h, 0, sizeof(h)); h.nH = nH; h.nP = nP; h.pts = m.pts; m.ingest_seq = need_seq;
+  for (int k=0;k<nH;k++) {
+    const FrameDev& f = *F[k]; h.hostI0[k] = f.I0; m.host_exposure[k] = f.exposure; m.host_ids[k] = host_frames[k];
     for (int i=0;i<7;i++) h.hostT[k][i] = host_T7[7*k+i]; m.host_ab[k][0] = host_ab ? host_ab[2*k] : 0.0; m.host_ab[k][1] = host_ab ? host_ab[2*k+1] : 0.0; }
   m.nH = nH; m.nP = nP; m.set = true;
   CK(cudaStreamSynchronize(c->st));                                            // a previous launch may still read the slot
@@ -389,28 +388,22 @@ static int rp_launch(sdv_ctx* c, int n_jobs, const int32_t* slots, const uint64_
   for (int k=0;k<n_jobs;k++) { if (slots[k] < 0 || slots[k] >= (int)st->maps.size() || !st->maps[slots[k]].set) return ctx_fail(c, SDV_ERR_STATE, "reproject job %d: map slot %d not set", k, slots[k]);
     totalP += st->maps[slots[k]].nP; maxP = std::max(maxP, st->maps[slots[k]].nP); }
   const long long nc = (long long)n_jobs*C.ncells; R.nc = nc;
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  size_t o_jobs = 0, o_px = al(o_jobs + (size_t)n_jobs*sizeof(RpJob)), o_key = al(o_px + (size_t)totalP*sizeof(double2)), o_cell = al(o_key + (size_t)totalP*4), o_list = al(o_cell + (size_t)totalP*4),
-         o_count = al(o_list + (size_t)totalP*8), o_begin = al(o_count + (size_t)nc*4), o_cur = al(o_begin + (size_t)nc*4), o_opt = al(o_cur + (size_t)nc*4), o_opx = al(o_opt + (size_t)nc*4),
-         o_xf = al(o_opx + (size_t)nc*sizeof(double2)), o_ov = al(o_xf + (size_t)n_jobs*kRpMaxHosts*14*sizeof(double)), o_rj = al(o_ov + (size_t)nc*sizeof(sdv_overlap_pt)), o_no = al(o_rj + (size_t)n_jobs*sizeof(RefineJob)), o_co = al(o_no + (size_t)n_jobs*4),
-         total = al(o_co + (size_t)C.ncells*4);
-  size_t h_jobs = 0, h_opt = al(h_jobs + (size_t)n_jobs*sizeof(RpJob)), h_opx = al(h_opt + (size_t)nc*4), h_rj = al(h_opx + (size_t)nc*sizeof(double2)), h_no = al(h_rj + (size_t)n_jobs*sizeof(RefineJob)),
-         h_co = al(h_no + (size_t)n_jobs*4), host_total = al(h_co + (size_t)C.ncells*4);
-  if (total > st->cap || host_total > st->host_cap) { cudaFree(st->dev); cudaFreeHost(st->host); st->dev = st->host = nullptr; st->cap = st->host_cap = 0;
-    const size_t cap = total + total/4, hcap = host_total + host_total/4;
-    CK(cudaMalloc(&st->dev, cap)); CK(cudaMallocHost(&st->host, hcap)); st->cap = cap; st->host_cap = hcap; }
-  unsigned char* db = (unsigned char*)st->dev; unsigned char* hb = (unsigned char*)st->host;
-  RpJob* J = (RpJob*)(hb + h_jobs); R.jobs_host = J; R.h_opt = (int32_t*)(hb + h_opt); R.h_opx = (double2*)(hb + h_opx); R.rj_host = (RefineJob*)(hb + h_rj); R.n_out_host = (int*)(hb + h_no);
-  long long need_seq = 0;
-  for (int k=0;k<n_jobs;k++) { auto it = c->frame_index.find(cur_frames[k]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "reproject job %d: unknown target frame", k);
-    { int rcs = check_frame_slot(c, c->frames[it->second], slots[k], "reproject / refine"); if (rcs) return rcs; }
-    need_seq = std::max(need_seq, std::max(c->frames[it->second].ingest_seq, st->maps[slots[k]].ingest_seq)); }
+  Scratch& D = c->scr; PinnedScratch& H = c->scr_host;
+  const size_t d_bytes = Scratch::need(n_jobs, sizeof(RpJob)) + Scratch::need(totalP, sizeof(double2)) + 2*Scratch::need(totalP, 4) + Scratch::need(totalP, 8) + 4*Scratch::need(nc, 4)
+                       + Scratch::need(nc, sizeof(double2)) + Scratch::need((size_t)n_jobs*kRpMaxHosts*14, sizeof(double)) + Scratch::need(nc, sizeof(sdv_overlap_pt))
+                       + Scratch::need(n_jobs, sizeof(RefineJob)) + Scratch::need(n_jobs, 4) + Scratch::need(C.ncells, 4),
+               h_bytes = Scratch::need(n_jobs, sizeof(RpJob)) + Scratch::need(nc, 4) + Scratch::need(nc, sizeof(double2)) + Scratch::need(n_jobs, sizeof(RefineJob)) + Scratch::need(n_jobs, 4);
+  if (D.reserve(d_bytes, c->st) || H.reserve(h_bytes, c->st)) return ctx_fail(c, SDV_ERR_CUDA, "reproject / refine: scratch of %d jobs", n_jobs);
+  D.reset(); H.reset();
+  RpJob* J = H.take<RpJob>(n_jobs); R.jobs_host = J; R.h_opt = H.take<int32_t>(nc); R.h_opx = H.take<double2>(nc); R.rj_host = H.take<RefineJob>(n_jobs); R.n_out_host = H.take<int>(n_jobs);
+  long long need_seq = 0; std::vector<FrameDev*> F(n_jobs);
+  for (int k=0;k<n_jobs;k++) { int rcs = job_frame(c, "reproject / refine", k, cur_frames[k], -1, slots[k], &need_seq, &F[k]); if (rcs) return rcs;
+    need_seq = std::max(need_seq, st->maps[slots[k]].ingest_seq); }
   { int rcj = join_ingest_upto(c, need_seq); if (rcj) return rcj; }     // only the uploads these frames came from (a later batch may still be streaming in)
   long long off = 0;
   for (int k=0;k<n_jobs;k++) {
     const MapSlot& m = st->maps[slots[k]]; RpJob& j = J[k]; memset(&j, 0, sizeof(j));
-    auto it = c->frame_index.find(cur_frames[k]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "reproject job %d: unknown target frame", k);
-    const FrameDev& f = c->frames[it->second];
+    const FrameDev& f = *F[k];
     j.map = m.dev; for (int l=0;l<c->levels;l++) j.cur[l] = f.img[l];
     rp_job_K(slot_geom(c, slots[k]).g[0], j.K, j.Ki); j.geom_row = c->slots[slots[k]].geom_row; j.cam = (unsigned char)c->slots[slots[k]].cam;
     for (int i=0;i<7;i++) j.curT[i] = cur_T7[7*k+i];
@@ -427,14 +420,14 @@ static int rp_launch(sdv_ctx* c, int n_jobs, const int32_t* slots, const uint64_
     const double ca = cur_ab ? cur_ab[2*k] : 0.0, cbb = cur_ab ? cur_ab[2*k+1] : 0.0;
     for (int i=0;i<m.nH;i++) { double o2[2]; aff_from_to(m.host_exposure[i], f.exposure, m.host_ab[i][0], m.host_ab[i][1], ca, cbb, o2); j.affLL[i][0] = (float)o2[0]; j.affLL[i][1] = (float)o2[1]; }
   }
-  RpScratch& S = R.S; S.cand_px = (double2*)(db + o_px); S.cand_key = (float*)(db + o_key); S.cand_cell = (int*)(db + o_cell); S.list = (unsigned long long*)(db + o_list);
-  S.count = (int*)(db + o_count); S.begin = (int*)(db + o_begin); S.cursor = (int*)(db + o_cur); S.out_pt = (int*)(db + o_opt); S.out_px = (double2*)(db + o_opx); S.xf = (double*)(db + o_xf);
-  R.ov = (sdv_overlap_pt*)(db + o_ov); R.rj = (RefineJob*)(db + o_rj); R.n_out_dev = (int*)(db + o_no); R.cell_order_dev = (int*)(db + o_co);
+  RpJob* jd = D.take<RpJob>(n_jobs); R.jobs_dev = jd;
+  RpScratch& S = R.S; S.cand_px = D.take<double2>(totalP); S.cand_key = D.take<float>(totalP); S.cand_cell = D.take<int>(totalP); S.list = D.take<unsigned long long>(totalP);
+  S.count = D.take<int>(nc); S.begin = D.take<int>(nc); S.cursor = D.take<int>(nc); S.out_pt = D.take<int>(nc); S.out_px = D.take<double2>(nc); S.xf = D.take<double>((size_t)n_jobs*kRpMaxHosts*14);
+  R.ov = D.take<sdv_overlap_pt>(nc); R.rj = D.take<RefineJob>(n_jobs); R.n_out_dev = D.take<int>(n_jobs); R.cell_order_dev = D.take<int>(C.ncells);
   cudaStream_t s = c->st;
-  launch_h2d_words(db + o_jobs, J, (size_t)n_jobs*sizeof(RpJob), s);               // kernel copy (see launch_h2d_words)
+  launch_h2d_words(jd, J, (size_t)n_jobs*sizeof(RpJob), s);                      // kernel copy (see launch_h2d_words); need() leaves it its 16 B of slack
   CK(cudaMemsetAsync(S.count, 0, (size_t)nc*4, s));
   CK(cudaEventRecord(c->ev0, s));
-  RpJob* jd = (RpJob*)(db + o_jobs); R.jobs_dev = jd;
   rp_project_kernel<<<dim3((maxP + 255)/256, n_jobs), 256, 0, s>>>(jd, C, S);
   rp_scan_kernel<<<n_jobs, 1024, 0, s>>>(C, S);
   rp_scatter_kernel<<<dim3((maxP + 255)/256, n_jobs), 256, 0, s>>>(jd, C, S);

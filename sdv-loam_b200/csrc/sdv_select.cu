@@ -14,30 +14,27 @@
 #include "sdv_select_core.cuh"
 
 using namespace sdv;
-#define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return ctx_fail(c, SDV_ERR_CUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
 static_assert(sizeof(sel::NewTrace) == sizeof(sdv_new_trace) && sizeof(sel::ImmPt) == sizeof(sdv_immature_pt), "engine records mirror the C-ABI structs");
 
 namespace sdv {
-struct SelState { sel::SelEngine eng; std::vector<sel::SelectorSlot> slots; std::vector<int> cam; sel::Scratch aux;   // cam[s]: camera of slot s
+struct SelState { sel::SelEngine eng; std::vector<sel::SelectorSlot> slots; std::vector<int> cam;   // cam[s]: camera of slot s
                   int* boxD = nullptr; };                                                // FullSystem::left/right/up/down of every slot (4 ints each, device), FullSystem.h:191-194
 static const int32_t kBox0[4] = {10000, -1, 10000, -1};                                   // their initial values
 void sel_destroy(sdv_ctx* c) {
   SelState* s = (SelState*)c->sel; if (!s) return;
   for (auto& sl : s->slots) if (sl.mapD) cudaFree(sl.mapD);
   cudaFree(s->boxD);
-  s->eng.io.release(); s->aux.release(); s->eng.destroy(); delete s; c->sel = nullptr;
+  s->eng.io.release(); s->eng.destroy(); delete s; c->sel = nullptr;
 }
 bool sel_cam_bound(const sdv_ctx* c, int cam, int* slot) {
   const SelState* s = (const SelState*)c->sel; if (!s) return false;
   for (size_t k = 0; k < s->cam.size(); k++) if (s->cam[k] == cam) { *slot = (int)k; return true; }
   return false;
 }
-static int sel_frame(sdv_ctx* c, uint64_t id, int cam, sel::FrameImg& F, long long& need_seq, const char* who, bool texels = true) {
-  auto it = c->frame_index.find(id); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "%s: unknown frame %llu", who, (unsigned long long)id);
-  FrameDev& f = c->frames[it->second]; { int rcs = check_frame_cam(c, f, cam, who); if (rcs) return rcs; }
-  if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
-  F.I0 = f.I0; F.L1 = nullptr; F.L2 = nullptr;
-  if (texels) { int rc = ensure_texels(c, f, 1); if (rc) return rc; F.L1 = f.lvl[1]; F.L2 = f.lvl[2]; }   // |grad|^2 of levels 1 and 2 (makeMaps / makeNewTraces read the packed texels)
+static int sel_frame(sdv_ctx* c, int k, uint64_t id, int cam, sel::FrameImg& F, long long& need_seq, const char* who, bool texels = true) {
+  FrameDev* f; { int rc = job_frame(c, who, k, id, cam, -1, &need_seq, &f); if (rc) return rc; }
+  F.I0 = f->I0; F.L1 = nullptr; F.L2 = nullptr;
+  if (texels) { int rc = ensure_texels(c, *f, 1); if (rc) return rc; F.L1 = f->lvl[1]; F.L2 = f->lvl[2]; }   // |grad|^2 of levels 1 and 2 (makeMaps / makeNewTraces read the packed texels)
   return SDV_OK;
 }
 int sel_n_slots(const sdv_ctx* c) { const SelState* s = (const SelState*)c->sel; return s ? (int)s->slots.size() : -1; }
@@ -70,9 +67,9 @@ int sdv_selector_init(sdv_ctx* c, const uint8_t* random_pattern, int n_slots) { 
 // selectionMap / sequence); the same size keeps its state.
 int sdv_selector_set_slot_cams(sdv_ctx* c, int n, const int32_t* slots, const int32_t* cams) { SDV_GUARD_TRK(c);
   if (!c || n < 0 || (n && (!slots || !cams))) return SDV_ERR_ARG; SEL_STATE("selector_set_slot_cams");
+  { int rc = check_cams(c, n, cams, "selector_set_slot_cams", "entry"); if (rc) return rc; }
   for (int i = 0; i < n; i++) {
     if (slots[i] < 0 || slots[i] >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "selector_set_slot_cams: entry %d names slot %d of %d", i, slots[i], (int)s->slots.size());
-    if (cams[i] < 0 || cams[i] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "selector_set_slot_cams: entry %d names camera %d (valid: 0..%d)", i, cams[i], SDV_MAX_CAMERAS - 1);
     if (c->cam_levels[cams[i]] < 3) return ctx_fail(c, SDV_ERR_ARG, "selector_set_slot_cams: entry %d names camera %d of %d levels (the selector reads levels 0..2)", i, cams[i], c->cam_levels[cams[i]]);
   }
   CK(cudaSetDevice(c->device));
@@ -108,13 +105,13 @@ int sdv_selector_get_map(sdv_ctx* c, int slot, uint8_t* out) { SDV_GUARD_TRK(c);
 }
 int sdv_selector_make_hists_cam(sdv_ctx* c, int cam, uint64_t frame, float* ths_out, float* thsSmoothed_out) { SDV_GUARD_TRK(c);
   if (!c) return SDV_ERR_ARG; SEL_STATE("selector_make_hists");
-  if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "selector_make_hists: camera %d (valid: 0..%d)", cam, SDV_MAX_CAMERAS - 1);
+  { int rc = check_cams(c, 1, &cam, "selector_make_hists", nullptr); if (rc) return rc; }
   CK(cudaSetDevice(c->device));
-  sel::FrameImg F; long long need = 0; { int rc = sel_frame(c, frame, cam, F, need, "selector_make_hists", false); if (rc) return rc; }
+  sel::FrameImg F; long long need = 0; { int rc = sel_frame(c, 0, frame, cam, F, need, "selector_make_hists", false); if (rc) return rc; }
   { int rc = join_ingest_upto(c, need); if (rc) return rc; }
   const int w = c->cam_w[cam], h = c->cam_h[cam];
-  const size_t tf = sel::SelEngine::ths_floats(w, h); if (s->aux.reserve(2*sel::Scratch::need(tf, 4), c->st)) return ctx_fail(c, SDV_ERR_CUDA, "selector_make_hists: scratch");
-  s->aux.reset(); float* a = s->aux.take<float>(tf); float* b = s->aux.take<float>(tf);
+  const size_t tf = sel::SelEngine::ths_floats(w, h); if (c->scr.reserve(2*Scratch::need(tf, 4), c->st)) return ctx_fail(c, SDV_ERR_CUDA, "selector_make_hists: scratch");
+  c->scr.reset(); float* a = c->scr.take<float>(tf); float* b = c->scr.take<float>(tf);
   CK(cudaMemsetAsync(a, 0, tf*4, c->st)); CK(cudaMemsetAsync(b, 0, tf*4, c->st));
   sel::HistJob J{F.I0, a, b, w, h}; const long long l0 = s->eng.launches;
   if (s->eng.make_hists(1, &J)) return sel_fail(c, s, -1, "selector_make_hists");
@@ -139,19 +136,19 @@ int sdv_selector_make_maps_batch(sdv_ctx* c, int n, const int32_t* slots, const 
   CK(cudaSetDevice(c->device));
   long long need = 0; std::vector<int> jw(n), jh(n);                                   // job j works at its slot's camera size
   for (int j = 0; j < n; j++) { const int cam = s->cam[slots[j]]; jw[j] = c->cam_w[cam]; jh[j] = c->cam_h[cam]; }
-  std::vector<sel::FrameImg> F(n); for (int j = 0; j < n; j++) { int rc = sel_frame(c, frames[j], s->cam[slots[j]], F[j], need, "selector_make_maps"); if (rc) return rc; }
+  std::vector<sel::FrameImg> F(n); for (int j = 0; j < n; j++) { int rc = sel_frame(c, j, frames[j], s->cam[slots[j]], F[j], need, "selector_make_maps"); if (rc) return rc; }
   { int rc = join_ingest_upto(c, need); if (rc) return rc; }
   size_t bytes = 1024; for (int j = 0; j < n; j++) { const int m = lidar ? cloud_begin[j+1] - cloud_begin[j] : 0;
-    bytes += 2*sel::Scratch::need(sel::SelEngine::ths_floats(jw[j], jh[j]), 4) + sel::Scratch::need(3*(size_t)m, 8) + sel::Scratch::need(lidar ? (size_t)std::max(m, 1) : (size_t)jw[j]*jh[j], 1); }
-  if (s->aux.reserve(bytes, c->st)) return ctx_fail(c, SDV_ERR_CUDA, "selector_make_maps: scratch");
-  s->aux.reset(); std::vector<sel::MapsJobHost> M(n); std::vector<sel::HistJob> Hj(n);
+    bytes += 2*Scratch::need(sel::SelEngine::ths_floats(jw[j], jh[j]), 4) + Scratch::need(3*(size_t)m, 8) + Scratch::need(lidar ? (size_t)std::max(m, 1) : (size_t)jw[j]*jh[j], 1); }
+  if (c->scr.reserve(bytes, c->st)) return ctx_fail(c, SDV_ERR_CUDA, "selector_make_maps: scratch");
+  c->scr.reset(); std::vector<sel::MapsJobHost> M(n); std::vector<sel::HistJob> Hj(n);
   for (int j = 0; j < n; j++) { const int m = lidar ? cloud_begin[j+1] - cloud_begin[j] : 0; const size_t wh = (size_t)jw[j]*jh[j], tf = sel::SelEngine::ths_floats(jw[j], jh[j]);
-    float* a = s->aux.take<float>(tf); float* b = s->aux.take<float>(tf); CK(cudaMemsetAsync(a, 0, tf*4, c->st)); CK(cudaMemsetAsync(b, 0, tf*4, c->st));
-    double* cl = nullptr; if (lidar) { cl = s->aux.take<double>(3*(size_t)std::max(m, 1)); if (m) CK(cudaMemcpyAsync(cl, cloud3 + 3*(size_t)cloud_begin[j], 3*(size_t)m*sizeof(double), cudaMemcpyHostToDevice, c->st)); }
+    float* a = c->scr.take<float>(tf); float* b = c->scr.take<float>(tf); CK(cudaMemsetAsync(a, 0, tf*4, c->st)); CK(cudaMemsetAsync(b, 0, tf*4, c->st));
+    double* cl = nullptr; if (lidar) { cl = c->scr.take<double>(3*(size_t)std::max(m, 1)); if (m) CK(cudaMemcpyAsync(cl, cloud3 + 3*(size_t)cloud_begin[j], 3*(size_t)m*sizeof(double), cudaMemcpyHostToDevice, c->st)); }
     sel::SelectorSlot& sl = s->slots[slots[j]];
     if (!lidar && !sl.mapD) { CK(cudaMalloc((void**)&sl.mapD, wh)); CK(cudaMemsetAsync(sl.mapD, 0, wh, c->st)); }
     Hj[j] = sel::HistJob{F[j].I0, a, b, jw[j], jh[j]};
-    M[j].img = F[j]; M[j].w = jw[j]; M[j].h = jh[j]; M[j].thsSm = b; M[j].cloud_dev = cl; M[j].n = m; M[j].map = lidar ? s->aux.take<unsigned char>(std::max(m, 1)) : sl.mapD; M[j].density = density[j];
+    M[j].img = F[j]; M[j].w = jw[j]; M[j].h = jh[j]; M[j].thsSm = b; M[j].cloud_dev = cl; M[j].n = m; M[j].map = lidar ? c->scr.take<unsigned char>(std::max(m, 1)) : sl.mapD; M[j].density = density[j];
     M[j].recursionsLeft = recursions_left[j]; M[j].thFactor = th_factor[j]; M[j].currentPotential = &sl.currentPotential; M[j].numHaveSub = 0; M[j].passes = 0; }
   const long long l0 = s->eng.launches;
   if (s->eng.make_hists(n, Hj.data())) return sel_fail(c, s, -1, "selector_make_maps");
@@ -178,7 +175,7 @@ static int make_new_traces(sdv_ctx* c, int n, const int32_t* slots, const uint64
     if (!out) for (int k = 0; k < j; k++) if (frames[k] == frames[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces_store: frame %llu appears twice in one batch", (unsigned long long)frames[j]); }
   CK(cudaSetDevice(c->device));
   long long need = 0; std::vector<sel::SelEngine::NewTracesJob> J(n);
-  for (int j = 0; j < n; j++) { const int cam = s->cam[slots[j]]; int rc = sel_frame(c, frames[j], cam, J[j].img, need, "make_new_traces"); if (rc) return rc; J[j].w = c->cam_w[cam]; J[j].h = c->cam_h[cam];
+  for (int j = 0; j < n; j++) { const int cam = s->cam[slots[j]]; int rc = sel_frame(c, j, frames[j], cam, J[j].img, need, "make_new_traces"); if (rc) return rc; J[j].w = c->cam_w[cam]; J[j].h = c->cam_h[cam];
     J[j].cloud_host = cloud3 ? cloud3 + 3*(size_t)cloud_begin[j] : nullptr; J[j].cloud_dev = cloud_dev ? cloud_dev[j] : nullptr; J[j].n = cloud_begin[j+1] - cloud_begin[j]; J[j].slot = &s->slots[slots[j]]; J[j].densityLidar = density_lidar[j];
     J[j].densityDense = density_dense[j]; J[j].addFeaturePoint = add_feature_point[j]; J[j].out_host = out ? (sel::NewTrace*)out + (size_t)j*cap : nullptr;
     J[j].imm_host = (out && imm_out) ? (sel::ImmPt*)imm_out + (size_t)j*cap : nullptr; J[j].cap = cap; }
@@ -233,7 +230,7 @@ int sel_activate_select(sdv_ctx* c, int n, const int32_t* host_begin, const int3
   if (!c || n < 0 || (n && (!host_begin || !pt_begin || !cand_host_begin || !cand_begin || !min_act_dist))) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK; SEL_STATE("activate_select");
   if (host_begin[0] != 0 || cand_host_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "activate_select: host_begin[0] and cand_host_begin[0] must be 0");
-  if (cams) for (int j = 0; j < n; j++) if (cams[j] < 0 || cams[j] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "activate_select: sequence %d names camera %d (valid: 0..%d)", j, cams[j], SDV_MAX_CAMERAS - 1);
+  { int rc = check_cams(c, n, cams, "activate_select", "sequence"); if (rc) return rc; }
   // the engine wants, per sequence, CSR offsets that start at 0: rebase the global ones
   std::vector<std::vector<int>> pb(n), cb(n); std::vector<sel::SelEngine::ActJob> J(n); size_t map_off = 0;     // distance maps back to back, each at its camera's level-1 size
   for (int j = 0; j < n; j++) {

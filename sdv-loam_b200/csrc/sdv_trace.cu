@@ -20,7 +20,6 @@
 #include "sdv_pool.cuh"
 
 using namespace sdv;
-#define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return ctx_fail(c, SDV_ERR_CUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
 
 namespace sdv {
 
@@ -307,11 +306,9 @@ static TraceSet trace_settings(const sdv_ctx* c) {
   S.minImprovementFactor = 2;                                                                   // util/settings.cpp:111,130-139
   return S;
 }
-static int trace_scratch(sdv_ctx* c, size_t bytes) {
-  if (bytes <= c->trace_cap) return SDV_OK;
-  CK(cudaStreamSynchronize(c->st)); cudaFree(c->trace_dev); c->trace_dev = nullptr; c->trace_cap = 0;
-  CK(cudaMalloc(&c->trace_dev, bytes + bytes/2)); c->trace_cap = bytes + bytes/2; return SDV_OK;
-}
+// The immature-point calls carve their device arrays from the tracker-stream scratch c->scr and upload from pageable vectors, whose copies are staged before
+// the call returns.  Not from pinned memory: sdv_immature_trace_store_batch without counts returns with its kernel still queued, and the next call rewrites c->scr_host.
+#define TRACE_SCRATCH(bytes, who) do { if (c->scr.reserve(bytes, c->st)) return ctx_fail(c, SDV_ERR_CUDA, "%s: scratch of %zu bytes", who, (size_t)(bytes)); c->scr.reset(); } while (0)
 
 // ---- the immature-point store: host->immaturePoints of every keyframe kept on the device (sdv_immature_store_*, sdv_immature_trace_store_batch)
 // A block keeps each record in two arrays split by what traceOn does with the fields: ImmRO (92 B) it only reads, ImmRW (28 B) it writes.  A per-frame trace
@@ -364,9 +361,10 @@ int imm_store_deposit(sdv_ctx* c, int nj, const uint64_t* hosts, const int* n, c
   std::vector<DepositJob> D(nj); int maxN = 0;
   for (int j = 0; j < nj; j++) { D[j] = DepositJob{(const sdv_new_trace*)nt_dev[j], (const sdv_immature_pt*)imm_dev[j], P[j].b.ro, P[j].b.rw, P[j].b.meta, n[j]}; maxN = std::max(maxN, n[j]); }
   if (maxN > 0) {
-    { int rc = trace_scratch(c, nj*sizeof(DepositJob)); if (rc) { imm_store_abandon(S, P); return rc; } }
-    if (cudaMemcpyAsync(c->trace_dev, D.data(), nj*sizeof(DepositJob), cudaMemcpyHostToDevice, c->st) != cudaSuccess) { imm_store_abandon(S, P); CK(cudaGetLastError()); }
-    imm_deposit_kernel<<<dim3((maxN + 127)/128, nj), 128, 0, c->st>>>((const DepositJob*)c->trace_dev); c->launches += 1;
+    if (c->scr.reserve(Scratch::need(nj, sizeof(DepositJob)), c->st)) { imm_store_abandon(S, P); return ctx_fail(c, SDV_ERR_CUDA, "immature store: deposit scratch"); }
+    c->scr.reset(); DepositJob* dD = c->scr.take<DepositJob>(nj);
+    if (cudaMemcpyAsync(dD, D.data(), nj*sizeof(DepositJob), cudaMemcpyHostToDevice, c->st) != cudaSuccess) { imm_store_abandon(S, P); CK(cudaGetLastError()); }
+    imm_deposit_kernel<<<dim3((maxN + 127)/128, nj), 128, 0, c->st>>>(dD); c->launches += 1;
     if (cudaGetLastError() != cudaSuccess) { imm_store_abandon(S, P); return ctx_fail(c, SDV_ERR_CUDA, "immature store: deposit launch"); }
   }
   imm_store_commit(S, P);
@@ -440,23 +438,20 @@ extern "C" {
 
 int sdv_immature_init_cam(sdv_ctx* c, int cam, uint64_t host_frame, int n, const int32_t* uv, sdv_immature_pt* out) { SDV_GUARD_TRK(c);
   if (!c || n < 0 || (n && (!uv || !out))) return SDV_ERR_ARG;
-  if (cam < 0 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "immature_init: camera %d (valid: 0..%d)", cam, SDV_MAX_CAMERAS - 1);
+  { int rc = check_cams(c, 1, &cam, "immature_init", nullptr); if (rc) return rc; }
   if (n == 0) return SDV_OK;
   CK(cudaSetDevice(c->device));
-  auto it = c->frame_index.find(host_frame); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_init: unknown host frame %llu", (unsigned long long)host_frame);
-  { int rcs = check_frame_cam(c, c->frames[it->second], cam, "immature_init"); if (rcs) return rcs; }
+  long long need_seq = 0; FrameDev* f; { int rc = job_frame(c, "immature_init", 0, host_frame, cam, -1, &need_seq, &f); if (rc) return rc; }
   const int w = c->cam_w[cam], h = c->cam_h[cam];
   for (int i = 0; i < n; i++) if (uv[2*i] < 2 || uv[2*i+1] < 2 || uv[2*i] >= w-3 || uv[2*i+1] >= h-3)     // the 8-pattern (+-2) and the +1 bilinear neighbour must stay inside the image
     return ctx_fail(c, SDV_ERR_ARG, "immature_init: candidate %d at (%d,%d) is closer than 3 px to the border", i, uv[2*i], uv[2*i+1]);
-  FrameDev& f = c->frames[it->second];
-  { int rc = join_ingest_upto(c, f.ingest_seq); if (rc) return rc; }
-  const size_t o_pts = (size_t)n*2*sizeof(int), bytes = o_pts + (size_t)n*sizeof(sdv_immature_pt);
-  { int rc = trace_scratch(c, bytes); if (rc) return rc; }
-  char* d = (char*)c->trace_dev;
-  CK(cudaMemcpyAsync(d, uv, o_pts, cudaMemcpyHostToDevice, c->st));
-  imm_init_kernel<<<(n + 127)/128, 128, 0, c->st>>>(f.I0, w, h, n, (const int*)d, (sdv_immature_pt*)(d + o_pts), trace_settings(c)); c->launches += 1;
+  { int rc = join_ingest_upto(c, need_seq); if (rc) return rc; }
+  TRACE_SCRATCH(Scratch::need(2*(size_t)n, sizeof(int)) + Scratch::need(n, sizeof(sdv_immature_pt)), "immature_init");
+  int* d_uv = c->scr.take<int>(2*(size_t)n); sdv_immature_pt* d_pts = c->scr.take<sdv_immature_pt>(n);
+  CK(cudaMemcpyAsync(d_uv, uv, (size_t)n*2*sizeof(int), cudaMemcpyHostToDevice, c->st));
+  imm_init_kernel<<<(n + 127)/128, 128, 0, c->st>>>(f->I0, w, h, n, d_uv, d_pts, trace_settings(c)); c->launches += 1;
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out, d + o_pts, (size_t)n*sizeof(sdv_immature_pt), cudaMemcpyDeviceToHost, c->st));
+  CK(cudaMemcpyAsync(out, d_pts, (size_t)n*sizeof(sdv_immature_pt), cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st));
   return SDV_OK;
 }
@@ -466,7 +461,7 @@ int sdv_immature_trace_batch_cams(sdv_ctx* c, int n_groups, const uint64_t* fram
                                   sdv_immature_pt* pts_io, int32_t* status_out) { SDV_GUARD_TRK(c);
   if (!c || n_groups < 0 || (n_groups && (!frames || !pt_begin || !KRKi9 || !Kt3 || !aff2))) return SDV_ERR_ARG;
   if (n_groups == 0) return SDV_OK;
-  if (cams) for (int g = 0; g < n_groups; g++) if (cams[g] < 0 || cams[g] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "immature_trace: group %d names camera %d (valid: 0..%d)", g, cams[g], SDV_MAX_CAMERAS - 1);
+  { int rc = check_cams(c, n_groups, cams, "immature_trace", "group"); if (rc) return rc; }
   if (pt_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "immature_trace: pt_begin[0] must be 0");
   for (int g = 0; g < n_groups; g++) if (pt_begin[g+1] < pt_begin[g]) return ctx_fail(c, SDV_ERR_ARG, "immature_trace: pt_begin is not ascending at group %d", g);
   const int n = pt_begin[n_groups];
@@ -475,28 +470,24 @@ int sdv_immature_trace_batch_cams(sdv_ctx* c, int n_groups, const uint64_t* fram
   CK(cudaSetDevice(c->device));
   std::vector<TraceGroupDev> G(n_groups); std::vector<int> gof(n); long long need_seq = 0;
   for (int g = 0; g < n_groups; g++) {
-    auto it = c->frame_index.find(frames[g]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_trace: unknown frame %llu (group %d)", (unsigned long long)frames[g], g);
-    const int cam = cams ? cams[g] : 0; const FrameDev& f = c->frames[it->second]; { int rcs = check_frame_cam(c, f, cam, "immature_trace"); if (rcs) return rcs; }
-    if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
-    G[g].w = c->cam_w[cam]; G[g].h = c->cam_h[cam]; G[g].I0 = f.I0; for (int k = 0; k < 9; k++) G[g].KRKi[k] = KRKi9[9*g+k]; for (int k = 0; k < 3; k++) G[g].Kt[k] = Kt3[3*g+k]; G[g].aff[0] = aff2[2*g]; G[g].aff[1] = aff2[2*g+1];
+    const int cam = cams ? cams[g] : 0; FrameDev* f; { int rc = job_frame(c, "immature_trace", g, frames[g], cam, -1, &need_seq, &f); if (rc) return rc; }
+    G[g].w = c->cam_w[cam]; G[g].h = c->cam_h[cam]; G[g].I0 = f->I0; for (int k = 0; k < 9; k++) G[g].KRKi[k] = KRKi9[9*g+k]; for (int k = 0; k < 3; k++) G[g].Kt[k] = Kt3[3*g+k]; G[g].aff[0] = aff2[2*g]; G[g].aff[1] = aff2[2*g+1];
     G[g].pt_begin = pt_begin[g]; G[g].pt_end = pt_begin[g+1];
     for (int i = pt_begin[g]; i < pt_begin[g+1]; i++) gof[i] = g;
   }
   { int rc = join_ingest_upto(c, need_seq); if (rc) return rc; }
-  const size_t o_g = 0, o_of = (n_groups*sizeof(TraceGroupDev) + 15) & ~(size_t)15, o_st = o_of + (((size_t)n*sizeof(int) + 15) & ~(size_t)15),
-               o_pts = o_st + (((size_t)n*sizeof(int) + 15) & ~(size_t)15), bytes = o_pts + (size_t)n*sizeof(sdv_immature_pt);
-  { int rc = trace_scratch(c, bytes); if (rc) return rc; }
-  char* d = (char*)c->trace_dev;
-  CK(cudaMemcpyAsync(d + o_g, G.data(), n_groups*sizeof(TraceGroupDev), cudaMemcpyHostToDevice, c->st));       // pageable sources: staged before the calls return
-  CK(cudaMemcpyAsync(d + o_of, gof.data(), (size_t)n*sizeof(int), cudaMemcpyHostToDevice, c->st));
-  CK(cudaMemcpyAsync(d + o_pts, pts_io, (size_t)n*sizeof(sdv_immature_pt), cudaMemcpyHostToDevice, c->st));
+  TRACE_SCRATCH(Scratch::need(n_groups, sizeof(TraceGroupDev)) + 2*Scratch::need(n, sizeof(int)) + Scratch::need(n, sizeof(sdv_immature_pt)), "immature_trace");
+  TraceGroupDev* dG = c->scr.take<TraceGroupDev>(n_groups); int* dof = c->scr.take<int>(n); int* dst = c->scr.take<int>(n); sdv_immature_pt* dpts = c->scr.take<sdv_immature_pt>(n);
+  CK(cudaMemcpyAsync(dG, G.data(), n_groups*sizeof(TraceGroupDev), cudaMemcpyHostToDevice, c->st));       // pageable sources: staged before the calls return
+  CK(cudaMemcpyAsync(dof, gof.data(), (size_t)n*sizeof(int), cudaMemcpyHostToDevice, c->st));
+  CK(cudaMemcpyAsync(dpts, pts_io, (size_t)n*sizeof(sdv_immature_pt), cudaMemcpyHostToDevice, c->st));
   CK(cudaEventRecord(c->ev0, c->st));
-  imm_trace_kernel<<<(n + 127)/128, 128, 0, c->st>>>((const TraceGroupDev*)(d + o_g), (const int*)(d + o_of), n, (sdv_immature_pt*)(d + o_pts), (int*)(d + o_st), trace_settings(c));
+  imm_trace_kernel<<<(n + 127)/128, 128, 0, c->st>>>(dG, dof, n, dpts, dst, trace_settings(c));
   c->launches += 1;
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev1, c->st));
-  CK(cudaMemcpyAsync(pts_io, d + o_pts, (size_t)n*sizeof(sdv_immature_pt), cudaMemcpyDeviceToHost, c->st));
-  if (status_out) CK(cudaMemcpyAsync(status_out, d + o_st, (size_t)n*sizeof(int), cudaMemcpyDeviceToHost, c->st));
+  CK(cudaMemcpyAsync(pts_io, dpts, (size_t)n*sizeof(sdv_immature_pt), cudaMemcpyDeviceToHost, c->st));
+  if (status_out) CK(cudaMemcpyAsync(status_out, dst, (size_t)n*sizeof(int), cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st));
   CK(cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   return SDV_OK;
@@ -509,7 +500,7 @@ int sdv_immature_optimize_batch_cams(sdv_ctx* c, int n_groups, const int32_t* pt
                                      int32_t* res_state_out) { SDV_GUARD_TRK(c);
   if (!c || n_groups < 0 || (n_groups && (!pt_begin || !tgt_begin || !target_frames || !pre14 || !calib6))) return SDV_ERR_ARG;
   if (n_groups == 0) return SDV_OK;
-  if (cams) for (int g = 0; g < n_groups; g++) if (cams[g] < 0 || cams[g] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "immature_optimize: group %d names camera %d (valid: 0..%d)", g, cams[g], SDV_MAX_CAMERAS - 1);
+  { int rc = check_cams(c, n_groups, cams, "immature_optimize", "group"); if (rc) return rc; }
   if (pt_begin[0] != 0 || tgt_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "immature_optimize: pt_begin[0] and tgt_begin[0] must be 0");
   for (int g = 0; g < n_groups; g++) { if (pt_begin[g+1] < pt_begin[g] || tgt_begin[g+1] < tgt_begin[g]) return ctx_fail(c, SDV_ERR_ARG, "immature_optimize: offsets not ascending at group %d", g);
     const int nres = tgt_begin[g+1] - tgt_begin[g]; if (nres > kOptMaxRes || nres > res_stride) return ctx_fail(c, SDV_ERR_ARG, "immature_optimize: group %d has %d targets (max %d, res_stride %d)", g, nres, kOptMaxRes, res_stride); }
@@ -520,34 +511,30 @@ int sdv_immature_optimize_batch_cams(sdv_ctx* c, int n_groups, const int32_t* pt
   std::vector<OptGroupDev> G(n_groups); std::vector<OptTargetDev> T(nt); std::vector<int> gof(n); long long need_seq = 0;
   std::vector<int> cam_of(nt, 0); if (cams) for (int g = 0; g < n_groups; g++) for (int t = tgt_begin[g]; t < tgt_begin[g+1]; t++) cam_of[t] = cams[g];
   for (int t = 0; t < nt; t++) {
-    auto it = c->frame_index.find(target_frames[t]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_optimize: unknown target frame %llu", (unsigned long long)target_frames[t]);
-    const FrameDev& f = c->frames[it->second]; { int rcs = check_frame_cam(c, f, cam_of[t], "immature_optimize"); if (rcs) return rcs; }
-    if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
-    T[t].I0 = f.I0; for (int k = 0; k < 9; k++) T[t].R[k] = pre14[14*t+k]; for (int k = 0; k < 3; k++) T[t].t[k] = pre14[14*t+9+k]; T[t].aff[0] = pre14[14*t+12]; T[t].aff[1] = pre14[14*t+13];
+    FrameDev* f; { int rc = job_frame(c, "immature_optimize", t, target_frames[t], cam_of[t], -1, &need_seq, &f); if (rc) return rc; }
+    T[t].I0 = f->I0; for (int k = 0; k < 9; k++) T[t].R[k] = pre14[14*t+k]; for (int k = 0; k < 3; k++) T[t].t[k] = pre14[14*t+9+k]; T[t].aff[0] = pre14[14*t+12]; T[t].aff[1] = pre14[14*t+13];
   }
   for (int g = 0; g < n_groups; g++) { G[g].tgt_begin = tgt_begin[g]; G[g].nres = tgt_begin[g+1] - tgt_begin[g]; const float* q = calib6 + 6*g;
     G[g].fxl = q[0]; G[g].fyl = q[1]; G[g].cxl = q[2]; G[g].cyl = q[3]; G[g].fxli = q[4]; G[g].fyli = q[5]; const int cam = cams ? cams[g] : 0; G[g].w = c->cam_w[cam]; G[g].h = c->cam_h[cam];
     for (int i = pt_begin[g]; i < pt_begin[g+1]; i++) gof[i] = g; }
   { int rc = join_ingest_upto(c, need_seq); if (rc) return rc; }
-  auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
-  const size_t o_g = 0, o_t = al(n_groups*sizeof(OptGroupDev)), o_of = o_t + al(nt*sizeof(OptTargetDev)), o_fs = o_of + al((size_t)n*sizeof(int)), o_st = o_fs + al((size_t)n),
-               o_id = o_st + al((size_t)n*sizeof(int)), o_rs = o_id + al((size_t)n*sizeof(float)), o_pts = o_rs + al((size_t)n*res_stride*sizeof(int)), bytes = o_pts + (size_t)n*sizeof(sdv_immature_pt);
-  { int rc = trace_scratch(c, bytes); if (rc) return rc; }
-  char* d = (char*)c->trace_dev;
-  CK(cudaMemcpyAsync(d + o_g, G.data(), n_groups*sizeof(OptGroupDev), cudaMemcpyHostToDevice, c->st));
-  CK(cudaMemcpyAsync(d + o_t, T.data(), nt*sizeof(OptTargetDev), cudaMemcpyHostToDevice, c->st));
-  CK(cudaMemcpyAsync(d + o_of, gof.data(), (size_t)n*sizeof(int), cudaMemcpyHostToDevice, c->st));
-  if (is_from_sensor) CK(cudaMemcpyAsync(d + o_fs, is_from_sensor, (size_t)n, cudaMemcpyHostToDevice, c->st));
-  CK(cudaMemcpyAsync(d + o_pts, pts, (size_t)n*sizeof(sdv_immature_pt), cudaMemcpyHostToDevice, c->st));
+  TRACE_SCRATCH(Scratch::need(n_groups, sizeof(OptGroupDev)) + Scratch::need(nt, sizeof(OptTargetDev)) + 3*Scratch::need(n, sizeof(int)) + Scratch::need(n, 1)
+                + Scratch::need((size_t)n*res_stride, sizeof(int)) + Scratch::need(n, sizeof(sdv_immature_pt)), "immature_optimize");
+  OptGroupDev* dG = c->scr.take<OptGroupDev>(n_groups); OptTargetDev* dT = c->scr.take<OptTargetDev>(nt); int* dof = c->scr.take<int>(n); unsigned char* dfs = c->scr.take<unsigned char>(n);
+  int* dst = c->scr.take<int>(n); float* did = c->scr.take<float>(n); int* drs = c->scr.take<int>((size_t)n*res_stride); sdv_immature_pt* dpts = c->scr.take<sdv_immature_pt>(n);
+  CK(cudaMemcpyAsync(dG, G.data(), n_groups*sizeof(OptGroupDev), cudaMemcpyHostToDevice, c->st));
+  CK(cudaMemcpyAsync(dT, T.data(), nt*sizeof(OptTargetDev), cudaMemcpyHostToDevice, c->st));
+  CK(cudaMemcpyAsync(dof, gof.data(), (size_t)n*sizeof(int), cudaMemcpyHostToDevice, c->st));
+  if (is_from_sensor) CK(cudaMemcpyAsync(dfs, is_from_sensor, (size_t)n, cudaMemcpyHostToDevice, c->st));
+  CK(cudaMemcpyAsync(dpts, pts, (size_t)n*sizeof(sdv_immature_pt), cudaMemcpyHostToDevice, c->st));
   CK(cudaEventRecord(c->ev0, c->st));
-  imm_optimize_kernel<<<(n + 63)/64, 64, 0, c->st>>>((const OptGroupDev*)(d + o_g), (const OptTargetDev*)(d + o_t), (const int*)(d + o_of), n, (const sdv_immature_pt*)(d + o_pts),
-      is_from_sensor ? (const unsigned char*)(d + o_fs) : nullptr, min_obs, res_stride, (int*)(d + o_st), (float*)(d + o_id), (int*)(d + o_rs), c->set.huberTH);
+  imm_optimize_kernel<<<(n + 63)/64, 64, 0, c->st>>>(dG, dT, dof, n, dpts, is_from_sensor ? dfs : nullptr, min_obs, res_stride, dst, did, drs, c->set.huberTH);
   c->launches += 1;
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev1, c->st));
-  CK(cudaMemcpyAsync(status_out, d + o_st, (size_t)n*sizeof(int), cudaMemcpyDeviceToHost, c->st));
-  CK(cudaMemcpyAsync(idepth_out, d + o_id, (size_t)n*sizeof(float), cudaMemcpyDeviceToHost, c->st));
-  CK(cudaMemcpyAsync(res_state_out, d + o_rs, (size_t)n*res_stride*sizeof(int), cudaMemcpyDeviceToHost, c->st));
+  CK(cudaMemcpyAsync(status_out, dst, (size_t)n*sizeof(int), cudaMemcpyDeviceToHost, c->st));
+  CK(cudaMemcpyAsync(idepth_out, did, (size_t)n*sizeof(float), cudaMemcpyDeviceToHost, c->st));
+  CK(cudaMemcpyAsync(res_state_out, drs, (size_t)n*res_stride*sizeof(int), cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st));
   CK(cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   return SDV_OK;
@@ -609,19 +596,17 @@ int sdv_immature_trace_store_batch(sdv_ctx* c, int n_groups, const uint64_t* hos
                                    const float* aff2, int32_t* counts_out) { SDV_GUARD_TRK(c);
   if (!c || n_groups < 0 || (n_groups && (!hosts || !frames || !KRKi9 || !Kt3 || !aff2))) return SDV_ERR_ARG;
   if (n_groups == 0) return SDV_OK;
-  if (cams) for (int g = 0; g < n_groups; g++) if (cams[g] < 0 || cams[g] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "immature_trace_store: group %d names camera %d (valid: 0..%d)", g, cams[g], SDV_MAX_CAMERAS - 1);
+  { int rc = check_cams(c, n_groups, cams, "immature_trace_store", "group"); if (rc) return rc; }
   const ImmStore* S = (const ImmStore*)c->imm_store;
-  std::vector<TraceStoreGroupDev> G(n_groups); std::vector<int> gbeg(n_groups + 1, 0); long long need_seq = 0;
+  std::vector<TraceStoreGroupDev> G(n_groups); std::vector<int> gbeg(n_groups + 1, 0); std::vector<FrameDev*> F(n_groups); long long need_seq = 0;
   std::unordered_map<uint64_t, int> seen; seen.reserve(2*n_groups);
   for (int g = 0; g < n_groups; g++) {
     auto bt = S ? S->blocks.find(hosts[g]) : decltype(S->blocks.end())();
     if (!S || bt == S->blocks.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_trace_store: host %llu has no block (group %d)", (unsigned long long)hosts[g], g);
     if (!seen.emplace(hosts[g], g).second) return ctx_fail(c, SDV_ERR_ARG, "immature_trace_store: host %llu in groups %d and %d", (unsigned long long)hosts[g], seen[hosts[g]], g);
-    auto it = c->frame_index.find(frames[g]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_trace_store: unknown frame %llu (group %d)", (unsigned long long)frames[g], g);
-    const int cam = cams ? cams[g] : 0; const FrameDev& f = c->frames[it->second]; { int rcs = check_frame_cam(c, f, cam, "immature_trace_store"); if (rcs) return rcs; }
-    if (f.ingest_seq > need_seq) need_seq = f.ingest_seq;
+    const int cam = cams ? cams[g] : 0; { int rc = job_frame(c, "immature_trace_store", g, frames[g], cam, -1, &need_seq, &F[g]); if (rc) return rc; }
     const ImmBlock& blk = bt->second; TraceStoreGroupDev& D = G[g];
-    D.I0 = f.I0; D.w = c->cam_w[cam]; D.h = c->cam_h[cam]; D.ro = blk.ro; D.rw = blk.rw;
+    D.I0 = F[g]->I0; D.w = c->cam_w[cam]; D.h = c->cam_h[cam]; D.ro = blk.ro; D.rw = blk.rw;
     for (int k = 0; k < 9; k++) D.KRKi[k] = KRKi9[9*g+k]; for (int k = 0; k < 3; k++) D.Kt[k] = Kt3[3*g+k]; D.aff[0] = aff2[2*g]; D.aff[1] = aff2[2*g+1];
     gbeg[g+1] = gbeg[g] + blk.n;
   }
@@ -629,24 +614,23 @@ int sdv_immature_trace_store_batch(sdv_ctx* c, int n_groups, const uint64_t* hos
   if (n == 0) { if (counts_out) memset(counts_out, 0, (size_t)6*n_groups*sizeof(int32_t)); return SDV_OK; }
   CK(cudaSetDevice(c->device));
   { int rc = join_ingest_upto(c, need_seq); if (rc) return rc; }
-  const size_t o_b = al16(n_groups*sizeof(TraceStoreGroupDev)), o_c = o_b + al16((n_groups + 1)*sizeof(int)), bytes = o_c + (size_t)6*n_groups*sizeof(int);
-  { int rc = trace_scratch(c, bytes); if (rc) return rc; }
-  char* d = (char*)c->trace_dev;
-  CK(cudaMemcpyAsync(d, G.data(), n_groups*sizeof(TraceStoreGroupDev), cudaMemcpyHostToDevice, c->st));       // pageable sources: staged before the calls return
-  CK(cudaMemcpyAsync(d + o_b, gbeg.data(), (n_groups + 1)*sizeof(int), cudaMemcpyHostToDevice, c->st));
-  if (counts_out) CK(cudaMemsetAsync(d + o_c, 0, (size_t)6*n_groups*sizeof(int), c->st));
+  TRACE_SCRATCH(Scratch::need(n_groups, sizeof(TraceStoreGroupDev)) + Scratch::need(n_groups + 1, sizeof(int)) + Scratch::need((size_t)6*n_groups, sizeof(int)), "immature_trace_store");
+  TraceStoreGroupDev* dG = c->scr.take<TraceStoreGroupDev>(n_groups); int* dgb = c->scr.take<int>(n_groups + 1); int* dcnt = c->scr.take<int>((size_t)6*n_groups);
+  CK(cudaMemcpyAsync(dG, G.data(), n_groups*sizeof(TraceStoreGroupDev), cudaMemcpyHostToDevice, c->st));       // pageable sources: staged before the calls return
+  CK(cudaMemcpyAsync(dgb, gbeg.data(), (n_groups + 1)*sizeof(int), cudaMemcpyHostToDevice, c->st));
+  if (counts_out) CK(cudaMemsetAsync(dcnt, 0, (size_t)6*n_groups*sizeof(int), c->st));
   CK(cudaEventRecord(c->ev0, c->st));
-  imm_trace_store_kernel<<<(n + 127)/128, 128, 0, c->st>>>((const TraceStoreGroupDev*)d, (const int*)(d + o_b), n_groups, n, trace_settings(c), counts_out ? (int*)(d + o_c) : nullptr);
+  imm_trace_store_kernel<<<(n + 127)/128, 128, 0, c->st>>>(dG, dgb, n_groups, n, trace_settings(c), counts_out ? dcnt : nullptr);
   c->launches += 1;
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev1, c->st));
   if (counts_out) {
-    CK(cudaMemcpyAsync(counts_out, d + o_c, (size_t)6*n_groups*sizeof(int), cudaMemcpyDeviceToHost, c->st));
+    CK(cudaMemcpyAsync(counts_out, dcnt, (size_t)6*n_groups*sizeof(int), cudaMemcpyDeviceToHost, c->st));
     CK(cudaStreamSynchronize(c->st)); CK(cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   } else {                                                                               // returns with the kernel pending: a re-ingest or release of a traced frame waits for it
     if (!c->ev_trk_async) CK(cudaEventCreateWithFlags(&c->ev_trk_async, cudaEventDisableTiming));
     CK(cudaEventRecord(c->ev_trk_async, c->st));
-    for (int g = 0; g < n_groups; g++) c->frames[c->frame_index[frames[g]]].trk_async = true;
+    for (FrameDev* f : F) f->trk_async = true;
   }
   return SDV_OK;
 }
@@ -663,49 +647,49 @@ int sdv_activate_points_store_batch(sdv_ctx* c, int n, const int32_t* host_begin
   if (n == 0) return SDV_OK;
   if (cap > 0 && (!act_host || !act_idx || !act_pts || !act_meta || !act_idepth || !act_res_state)) return SDV_ERR_ARG;
   if (!c->sel) return ctx_fail(c, SDV_ERR_STATE, "activate_points_store: sdv_selector_init has not been called");
-  if (cams) for (int j = 0; j < n; j++) if (cams[j] < 0 || cams[j] >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "activate_points_store: sequence %d names camera %d (valid: 0..%d)", j, cams[j], SDV_MAX_CAMERAS - 1);
+  { int rc = check_cams(c, n, cams, "activate_points_store", "sequence"); if (rc) return rc; }
   if (host_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "activate_points_store: host_begin[0] must be 0");
   for (int j = 0; j < n; j++) { const int nH = host_begin[j+1] - host_begin[j];
     if (nH < 1 || nH > 16 || nH - 1 > SDV_MAX_FRAMES_WINDOW) return ctx_fail(c, SDV_ERR_ARG, "activate_points_store: sequence %d has %d keyframes (1..16, at most %d targets)", j, nH, SDV_MAX_FRAMES_WINDOW); }
   const int NH = host_begin[n]; const ImmStore* S = (const ImmStore*)c->imm_store;
-  std::vector<int> seq_of(NH), gbeg(NH + 1, 0), pre_begin(n + 1, 0); std::vector<const FrameDev*> F(NH); std::vector<ActHostDev> HD(NH); long long need_seq = 0;
+  std::vector<int> seq_of(NH), gbeg(NH + 1, 0), pre_begin(n + 1, 0); std::vector<FrameDev*> F(NH); std::vector<ActHostDev> HD(NH); long long need_seq = 0;
   std::unordered_map<uint64_t, int> seen; seen.reserve(2*NH);
   for (int j = 0; j < n; j++) { const int nH = host_begin[j+1] - host_begin[j]; pre_begin[j+1] = pre_begin[j] + nH*(nH - 1);
     for (int g = host_begin[j]; g < host_begin[j+1]; g++) { seq_of[g] = j;
       auto bt = S ? S->blocks.find(hosts[g]) : decltype(S->blocks.end())();
       if (!S || bt == S->blocks.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "activate_points_store: host %llu has no block", (unsigned long long)hosts[g]);
       if (!seen.emplace(hosts[g], g).second) return ctx_fail(c, SDV_ERR_ARG, "activate_points_store: host %llu appears twice", (unsigned long long)hosts[g]);
-      auto it = c->frame_index.find(hosts[g]); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "activate_points_store: keyframe %llu is not resident", (unsigned long long)hosts[g]);
-      const FrameDev& f = c->frames[it->second]; { int rcs = check_frame_cam(c, f, cams ? cams[j] : 0, "activate_points_store"); if (rcs) return rcs; }
-      if (f.ingest_seq > need_seq) need_seq = f.ingest_seq; F[g] = &f;
+      { int rc = job_frame(c, "activate_points_store", g, hosts[g], cams ? cams[j] : 0, -1, &need_seq, &F[g]); if (rc) return rc; }
       const ImmBlock& blk = bt->second; HD[g] = ActHostDev{blk.ro, blk.rw, blk.meta, g == host_begin[j+1] - 1 ? 1 : 0, flagged[g] ? 1 : 0}; gbeg[g+1] = gbeg[g] + blk.n; } }
   const int N = gbeg[NH];
   CK(cudaSetDevice(c->device));
   { int rc = join_ingest_upto(c, need_seq); if (rc) return rc; }
   // scratch, sized once for every phase
-  const size_t nN = (size_t)std::max(N, 1), R = SDV_MAX_FRAMES_WINDOW; size_t off = 0;
-  auto take = [&](size_t b) { const size_t o = off; off += al16(b); return o; };
-  const size_t o_hd = take(NH*sizeof(ActHostDev)), o_gb = take((NH + 1)*sizeof(int)), o_code = take(nN*4), o_rows = take(nN*16), o_c4 = take(nN*16), o_idx = take(nN*4),
-               o_og = take(NH*sizeof(OptGroupDev)), o_ot = take((size_t)pre_begin[n]*sizeof(OptTargetDev) + 16), o_gof = take(nN*4), o_pts = take(nN*sizeof(sdv_immature_pt)),
-               o_meta = take(nN*16), o_fs = take(nN), o_st = take(nN*4), o_id = take(nN*4), o_rs = take(nN*R*4), o_perm = take(nN*4), o_nb = take((NH + 1)*sizeof(int)),
-               o_bd = take(NH*sizeof(ActBlockDev)), o_sro = take(nN*sizeof(ImmRO)), o_srw = take(nN*sizeof(ImmRW)), o_sme = take(nN*16), bytes = off;
-  { int rc = trace_scratch(c, bytes); if (rc) return rc; }
-  char* d = (char*)c->trace_dev;
+  const size_t nN = (size_t)std::max(N, 1), R = SDV_MAX_FRAMES_WINDOW;
+  TRACE_SCRATCH(Scratch::need(NH, sizeof(ActHostDev)) + 2*Scratch::need(NH + 1, sizeof(int)) + 6*Scratch::need(nN, sizeof(int)) + 2*Scratch::need(nN, sizeof(float4))
+                + Scratch::need(NH, sizeof(OptGroupDev)) + Scratch::need(pre_begin[n], sizeof(OptTargetDev)) + Scratch::need(nN, sizeof(sdv_immature_pt)) + 2*Scratch::need(nN, sizeof(sdv_immature_meta))
+                + Scratch::need(nN, 1) + Scratch::need(nN*R, sizeof(int)) + Scratch::need(NH, sizeof(ActBlockDev)) + Scratch::need(nN, sizeof(ImmRO)) + Scratch::need(nN, sizeof(ImmRW)), "activate_points_store");
+  Scratch& D = c->scr;
+  ActHostDev* dHD = D.take<ActHostDev>(NH); int* dGB = D.take<int>(NH + 1); int* dcode = D.take<int>(nN); float4* drows = D.take<float4>(nN); float4* dc4 = D.take<float4>(nN);
+  int* didx = D.take<int>(nN); OptGroupDev* dOG = D.take<OptGroupDev>(NH); OptTargetDev* dOT = D.take<OptTargetDev>(pre_begin[n]); int* dgof = D.take<int>(nN);
+  sdv_immature_pt* dpts = D.take<sdv_immature_pt>(nN); sdv_immature_meta* dmeta = D.take<sdv_immature_meta>(nN); unsigned char* dfs = D.take<unsigned char>(nN); int* dst = D.take<int>(nN);
+  float* did = D.take<float>(nN); int* drs = D.take<int>(nN*R); int* dperm = D.take<int>(nN); int* dnb = D.take<int>(NH + 1); ActBlockDev* dBD = D.take<ActBlockDev>(NH);
+  ImmRO* dsro = D.take<ImmRO>(nN); ImmRW* dsrw = D.take<ImmRW>(nN); sdv_immature_meta* dsme = D.take<sdv_immature_meta>(nN);
   // (1) the filter of :612-645 on the device; the host reads one code per point back (class and status, 4 bytes), no record
   std::vector<int> code(nN, 0);
-  CK(cudaMemcpyAsync(d + o_hd, HD.data(), NH*sizeof(ActHostDev), cudaMemcpyHostToDevice, c->st));
-  CK(cudaMemcpyAsync(d + o_gb, gbeg.data(), (NH + 1)*sizeof(int), cudaMemcpyHostToDevice, c->st));
-  if (N) { imm_act_filter_kernel<<<(N + 127)/128, 128, 0, c->st>>>((const ActHostDev*)(d + o_hd), (const int*)(d + o_gb), NH, N, 3.0f /* setting_minTraceQuality, settings.cpp:131 */,
-                                                                 (int*)(d + o_code), (float4*)(d + o_rows)); c->launches += 1; CK(cudaGetLastError());
-           CK(cudaMemcpyAsync(code.data(), d + o_code, (size_t)N*4, cudaMemcpyDeviceToHost, c->st)); }
+  CK(cudaMemcpyAsync(dHD, HD.data(), NH*sizeof(ActHostDev), cudaMemcpyHostToDevice, c->st));
+  CK(cudaMemcpyAsync(dGB, gbeg.data(), (NH + 1)*sizeof(int), cudaMemcpyHostToDevice, c->st));
+  if (N) { imm_act_filter_kernel<<<(N + 127)/128, 128, 0, c->st>>>(dHD, dGB, NH, N, 3.0f /* setting_minTraceQuality, settings.cpp:131 */, dcode, drows);
+           c->launches += 1; CK(cudaGetLastError());
+           CK(cudaMemcpyAsync(code.data(), dcode, (size_t)N*4, cudaMemcpyDeviceToHost, c->st)); }
   CK(cudaStreamSynchronize(c->st));
   // (2) makeDistanceMap + the walk (:597-671) over the candidates, rows gathered on the device in host-then-point order
   std::vector<int> cidx, cand_begin(NH + 1, 0);
   for (int g = 0; g < NH; g++) { for (int i = gbeg[g]; i < gbeg[g+1]; i++) if ((code[i] & 3) == ACT_CAND) cidx.push_back(i); cand_begin[g+1] = (int)cidx.size(); }
   const int NC = (int)cidx.size(); std::vector<int32_t> decision(std::max(NC, 1), 0);
-  if (NC) { CK(cudaMemcpyAsync(d + o_idx, cidx.data(), (size_t)NC*4, cudaMemcpyHostToDevice, c->st));
-            imm_act_rows_kernel<<<(NC + 127)/128, 128, 0, c->st>>>((const float4*)(d + o_rows), (const int*)(d + o_idx), NC, (float4*)(d + o_c4)); c->launches += 1; CK(cudaGetLastError()); }
-  { int rc = sel_activate_select(c, n, src_host_begin, src_pt_begin, KRKi9, Kt3, uvid, host_begin, cand_begin.data(), cKRKi9, cKt3, nullptr, (const float*)(d + o_c4), min_act_dist, cams,
+  if (NC) { CK(cudaMemcpyAsync(didx, cidx.data(), (size_t)NC*4, cudaMemcpyHostToDevice, c->st));
+            imm_act_rows_kernel<<<(NC + 127)/128, 128, 0, c->st>>>(drows, didx, NC, dc4); c->launches += 1; CK(cudaGetLastError()); }
+  { int rc = sel_activate_select(c, n, src_host_begin, src_pt_begin, KRKi9, Kt3, uvid, host_begin, cand_begin.data(), cKRKi9, cKt3, nullptr, (const float*)dc4, min_act_dist, cams,
                                  decision.data(), nullptr); if (rc) return rc; }
   // (3) optimizeImmaturePoint (min_obs 1) on the accepted candidates, toOptimize order, read from the store
   std::vector<int> oidx, ohost; std::vector<int> opt_of(NC, -1);
@@ -718,19 +702,17 @@ int sdv_activate_points_store_batch(sdv_ctx* c, int n, const int32_t* host_begin
       T.I0 = F[tg]->I0; for (int e = 0; e < 9; e++) T.R[e] = r[e]; for (int e = 0; e < 3; e++) T.t[e] = r[9+e]; T.aff[0] = r[12]; T.aff[1] = r[13]; } }
   std::vector<sdv_immature_pt> opts(NO); std::vector<sdv_immature_meta> ometa(NO); std::vector<int> ost(NO); std::vector<float> oid(NO); std::vector<int> ors((size_t)NO*R);
   if (NO) {
-    CK(cudaMemcpyAsync(d + o_idx, oidx.data(), (size_t)NO*4, cudaMemcpyHostToDevice, c->st));
-    CK(cudaMemcpyAsync(d + o_og, OG.data(), NH*sizeof(OptGroupDev), cudaMemcpyHostToDevice, c->st));
-    if (!OT.empty()) CK(cudaMemcpyAsync(d + o_ot, OT.data(), OT.size()*sizeof(OptTargetDev), cudaMemcpyHostToDevice, c->st));
-    CK(cudaMemcpyAsync(d + o_gof, gof.data(), (size_t)NO*4, cudaMemcpyHostToDevice, c->st));
-    imm_act_gather_kernel<<<(NO + 127)/128, 128, 0, c->st>>>((const ActHostDev*)(d + o_hd), (const int*)(d + o_gb), NH, (const int*)(d + o_idx), NO, (sdv_immature_pt*)(d + o_pts),
-                                                            (sdv_immature_meta*)(d + o_meta), (unsigned char*)(d + o_fs));
-    imm_optimize_kernel<<<(NO + 63)/64, 64, 0, c->st>>>((const OptGroupDev*)(d + o_og), (const OptTargetDev*)(d + o_ot), (const int*)(d + o_gof), NO, (const sdv_immature_pt*)(d + o_pts),
-                                                        (const unsigned char*)(d + o_fs), 1, (int)R, (int*)(d + o_st), (float*)(d + o_id), (int*)(d + o_rs), c->set.huberTH);
+    CK(cudaMemcpyAsync(didx, oidx.data(), (size_t)NO*4, cudaMemcpyHostToDevice, c->st));
+    CK(cudaMemcpyAsync(dOG, OG.data(), NH*sizeof(OptGroupDev), cudaMemcpyHostToDevice, c->st));
+    if (!OT.empty()) CK(cudaMemcpyAsync(dOT, OT.data(), OT.size()*sizeof(OptTargetDev), cudaMemcpyHostToDevice, c->st));
+    CK(cudaMemcpyAsync(dgof, gof.data(), (size_t)NO*4, cudaMemcpyHostToDevice, c->st));
+    imm_act_gather_kernel<<<(NO + 127)/128, 128, 0, c->st>>>(dHD, dGB, NH, didx, NO, dpts, dmeta, dfs);
+    imm_optimize_kernel<<<(NO + 63)/64, 64, 0, c->st>>>(dOG, dOT, dgof, NO, dpts, dfs, 1, (int)R, dst, did, drs, c->set.huberTH);
     c->launches += 2; CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(ost.data(), d + o_st, (size_t)NO*4, cudaMemcpyDeviceToHost, c->st)); CK(cudaMemcpyAsync(oid.data(), d + o_id, (size_t)NO*4, cudaMemcpyDeviceToHost, c->st));
-    CK(cudaMemcpyAsync(ors.data(), d + o_rs, (size_t)NO*R*4, cudaMemcpyDeviceToHost, c->st));
-    CK(cudaMemcpyAsync(opts.data(), d + o_pts, (size_t)NO*sizeof(sdv_immature_pt), cudaMemcpyDeviceToHost, c->st));
-    CK(cudaMemcpyAsync(ometa.data(), d + o_meta, (size_t)NO*16, cudaMemcpyDeviceToHost, c->st));
+    CK(cudaMemcpyAsync(ost.data(), dst, (size_t)NO*4, cudaMemcpyDeviceToHost, c->st)); CK(cudaMemcpyAsync(oid.data(), did, (size_t)NO*4, cudaMemcpyDeviceToHost, c->st));
+    CK(cudaMemcpyAsync(ors.data(), drs, (size_t)NO*R*4, cudaMemcpyDeviceToHost, c->st));
+    CK(cudaMemcpyAsync(opts.data(), dpts, (size_t)NO*sizeof(sdv_immature_pt), cudaMemcpyDeviceToHost, c->st));
+    CK(cudaMemcpyAsync(ometa.data(), dmeta, (size_t)NO*16, cudaMemcpyDeviceToHost, c->st));
     CK(cudaStreamSynchronize(c->st));
   }
   std::vector<int> nact(n, 0); int total = 0; for (int k = 0; k < NO; k++) if (ost[k] == 1) { nact[seq_of[gof[k]]]++; total++; }
@@ -746,11 +728,10 @@ int sdv_activate_points_store_batch(sdv_ctx* c, int n, const int32_t* host_begin
     perm.insert(perm.end(), v.begin(), v.end()); nbeg[g+1] = (int)perm.size(); BD[g] = ActBlockDev{const_cast<ImmRO*>(HD[g].ro), const_cast<ImmRW*>(HD[g].rw), const_cast<sdv_immature_meta*>(HD[g].meta)}; }
   const int NP = (int)perm.size();
   if (NP) {
-    CK(cudaMemcpyAsync(d + o_perm, perm.data(), (size_t)NP*4, cudaMemcpyHostToDevice, c->st)); CK(cudaMemcpyAsync(d + o_nb, nbeg.data(), (NH + 1)*sizeof(int), cudaMemcpyHostToDevice, c->st));
-    CK(cudaMemcpyAsync(d + o_bd, BD.data(), NH*sizeof(ActBlockDev), cudaMemcpyHostToDevice, c->st));
+    CK(cudaMemcpyAsync(dperm, perm.data(), (size_t)NP*4, cudaMemcpyHostToDevice, c->st)); CK(cudaMemcpyAsync(dnb, nbeg.data(), (NH + 1)*sizeof(int), cudaMemcpyHostToDevice, c->st));
+    CK(cudaMemcpyAsync(dBD, BD.data(), NH*sizeof(ActBlockDev), cudaMemcpyHostToDevice, c->st));
     for (int pass = 0; pass < 2; pass++)
-      imm_act_permute_kernel<<<(NP + 127)/128, 128, 0, c->st>>>((const ActBlockDev*)(d + o_bd), (const int*)(d + o_nb), NH, (const int*)(d + o_perm), NP, (ImmRO*)(d + o_sro),
-                                                                (ImmRW*)(d + o_srw), (sdv_immature_meta*)(d + o_sme), pass);
+      imm_act_permute_kernel<<<(NP + 127)/128, 128, 0, c->st>>>(dBD, dnb, NH, dperm, NP, dsro, dsrw, dsme, pass);
     c->launches += 2; CK(cudaGetLastError());
   }
   ImmStore* SW = (ImmStore*)c->imm_store;
