@@ -492,6 +492,34 @@ int  sdv_make_new_traces_store_batch(sdv_ctx* c, int n, const int32_t* slots, co
  * the host-row path gives. */
 int  sdv_make_new_traces_rows_store_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const float* desired_density, int cap, int32_t* n_out,
                                           int32_t* num_points2);
+/* The start of a sequence (FullSystem::addActiveFrame for frames 0 and 1 of a LiDAR run, FullSystem.cpp:842-850 and :299-338), for n sequences in one call.  Job j
+ * bootstraps keyframe frames[j] on tracker slot slots[j], at the size and depth of that slot's camera (sdv_set_calib_slots_cams):
+ *   CoarseInitializer::setFirstFromLidar, level 0 (CoarseInitializer.cpp:766-888): a FRESH PixelSelector (currentPotential 3, makeHists, the camera's prefix of the
+ *     random pattern) runs makeMapsFromLidar(frame, statusMap, 0.03f*lidarArea, 1, false, 2, rows), lidarArea = (right-left)*(down-up) of the box; the Pnt list
+ *     is the rows with status != 0 and (float)depth > 0 in cloud order.  No selector slot is read or written (potential, map and box stay as they are).
+ *   FullSystem::initializeFromInitializer's point loop (FullSystem.cpp:1176-1225): Pnt k is dropped when rand_draws[draw_begin[j] + k] / (float)RAND_MAX >
+ *     desired_point_density[j] / numPoints[0] (rand_draws: the C library's rand() values, glibc RAND_MAX), else it becomes ImmaturePoint((int)(u+0.5f),
+ *     (int)(v+0.5f)) with idepth_min = idepth_max = 1/depth and, when its energyTH is finite, a PointHessian with idepth = idepth_zero = 1/depth, hasDepthPrior,
+ *     ACTIVE and isFromSensor.  n_selected_out[j] = numPoints[0]: the caller's rand() stream moves on by that much.  n_out[j] = the points kept; for each, in Pnt
+ *     order, the sdv_immature_pt record pts_out[j*cap + i], sdv_immature_meta meta_out[j*cap + i] = {my_type = status byte, type 0 CORNER, isFromSensor 1,
+ *     idepth_fromSensor = 1/depth} and idepth_out[j*cap + i] = the PointHessian's idepth and idepth_zero (each of the three may be NULL).
+ *   CoarseTracker::setCTRefForFirstFrame (CoarseTracker.cpp:636-647, :108-256): tracker slot slots[j] gets the reference of sdv_tracker_set_ref with the splat rows
+ *     {u, v, idepth, HdiF 0}, round_half 1, ref_frame = frames[j], ref_a = ref_b = 0; and map slot slots[j] gets sdv_map_set of one keyframe frames[j] with identity
+ *     camToWorld, aff_g2l {0, 0} and the kept points {u, v, idepth, host 0, CORNER}.  No record crosses PCIe for this.
+ * Reference behaviour restated: EFPoint::HdiF is read uninitialised by makeCoarseDepthForFirstFrame (taken as 0, a zeroed block) and PointHessian::type is never set
+ * for these points (taken as CORNER).  A point whose 8-pattern would read outside the frame's plane is not kept (the reference reads past its image there).
+ * job j has rows cloud3[3*cloud_begin[j] ..] (host, cloud_begin[0] = 0) and box lrud[4j..] = FullSystem::left, right, up, down after its sweep; the _rows form takes
+ * both from frames[j]'s row set (sdv_lidar_handler_rows_batch).  Refused before anything is enqueued, changing no slot: sdv_selector_init missing (SDV_ERR_STATE);
+ * a frame without a row set (SDV_ERR_NOFRAME) or with an overflowed one (SDV_ERR_CAPACITY); fewer draws than rows, a slot out of range or named twice, a frame
+ * named twice, a slot camera of fewer than 3 levels (SDV_ERR_ARG); a frame of another size than its slot's camera (as sdv_tracker_set_ref).  More than cap kept
+ * points in a job return SDV_ERR_CAPACITY with n_out and n_selected_out filled and no slot changed.  A reference cloud over max_ref_points behaves as in
+ * sdv_tracker_set_ref.  An empty cloud keeps no point: the slot's reference has 0 points at every level.  The call waits for the device. */
+int  sdv_init_from_lidar_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const int32_t* lrud,
+                               const float* desired_point_density, const int32_t* draw_begin, const int32_t* rand_draws, int cap, int32_t* n_out, int32_t* n_selected_out,
+                               sdv_immature_pt* pts_out, sdv_immature_meta* meta_out, float* idepth_out);
+int  sdv_init_from_lidar_rows_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const float* desired_point_density, const int32_t* draw_begin,
+                                    const int32_t* rand_draws, int cap, int32_t* n_out, int32_t* n_selected_out, sdv_immature_pt* pts_out, sdv_immature_meta* meta_out,
+                                    float* idepth_out);
 /* The selection half of void FullSystem::activatePointsMT() for n sequences: CoarseDistanceMap::makeDistanceMap from the ACTIVE points of the other keyframes, then the
  * candidate walk :600-671 with addIntoDistFinal after every accept.  Sequence j owns source keyframes host_begin[j] .. host_begin[j+1] (their points: uvid rows
  * pt_begin[k] .. pt_begin[k+1] = {u, v, idepth_scaled}; KRKi9 / Kt3 per keyframe = K[1] R K[0]^-1, K[1] t of host -> newest, FullSystem.cpp:606-608) and candidate

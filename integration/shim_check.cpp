@@ -368,6 +368,44 @@ int shim_process_pop(RowsQueue& fsys) {
   const uint64_t id = fsys.qCloudPixel.front(); fsys.qCloudPixel.erase(fsys.qCloudPixel.begin()); return sdv_lidar_rows_drop(gpu, 1, &id);
 }
 
+// ------------------------------------------------------------------------------------------------ the initializer branch (FullSystem.cpp:842-850, :299-338)
+// Frame 0 (coarseInitializer->setFirstFromLidar): nothing runs on the host; the frame's handle keys its row set, where frame 1 finds the rows and the box.
+// Frame 1 (trackNewCoarse with allFrameHistory.size() == 2): initializeFromInitializer + setCTRefForFirstFrame in one call, the PointHessians from its records,
+// then the 53-hypothesis track of frame 1.
+extern float setting_desiredPointDensity;
+struct InitBranch { FrameHessian* firstFrame; int32_t slot; };
+void shim_setFirstFromLidar(InitBranch& ib, FrameHessian* fh) { ib.firstFrame = fh; }
+Vec4 shim_initializer_frame1(FullSystem& fs, InitBranch& ib, FrameHessian* newFrame, int& rc) {
+  const uint64_t id0 = (uint64_t)ib.firstFrame->shell->id; int32_t rows = 0;
+  rc = sdv_lidar_rows_get(gpu, id0, 0, nullptr, &rows, nullptr, nullptr); if (rc) return Vec4{};
+  // the C library's stream here is srand(3141592) and w*h draws by frame 0's PixelSelector (PixelSelector2.cpp:14-16); nothing else draws in between
+  const long skip = (long)wG[0]*hG[0];
+  srand(3141592); for (long k = 0; k < skip; k++) rand();
+  std::vector<int32_t> draws(rows > 0 ? rows : 1); for (int k = 0; k < rows; k++) draws[k] = rand();
+  const int32_t draw_begin[2] = {0, rows}; const float dens = setting_desiredPointDensity; const int cap = 1 << 14; int32_t n = 0, n_sel = 0;
+  std::vector<sdv_immature_pt> pts(cap); std::vector<sdv_immature_meta> meta(cap); std::vector<float> idepth(cap);
+  rc = sdv_init_from_lidar_rows_batch(gpu, 1, &ib.slot, &id0, &dens, draw_begin, draws.data(), cap, &n, &n_sel, pts.data(), meta.data(), idepth.data());
+  if (rc) return Vec4{};
+  srand(3141592); for (long k = 0; k < skip + n_sel; k++) rand();        // the stream as initializeFromInitializer leaves it (:1203): numPoints[0] draws on
+  for (int i = 0; i < n; i++) {                                           // :1205-1231: PointHessian(pt), setIdepthScaled / setIdepthZero(midepth), prior, ACTIVE
+    PointHessian* ph = new PointHessian(); ph->u = pts[i].u; ph->v = pts[i].v; ph->idepth = ph->idepth_zero = idepth[i];
+    for (int k = 0; k < 8; k++) { ph->color[k] = pts[i].color[k]; ph->weights[k] = pts[i].weights[k]; }
+    ph->hasDepthPrior = true; ph->isFromSensor = meta[i].isFromSensor != 0; ph->type = meta[i].type; ph->host = ib.firstFrame; ph->efPoint = nullptr;
+    ib.firstFrame->pointHessians.push_back(ph);                           // + ef->insertPoint(ph), as in the reference
+  }
+  ib.firstFrame->shell->camToWorld = SE3(); ib.firstFrame->shell->aff_g2l = AffLight(0, 0);   // :1235-1256
+  // the tracker slot holds setCTRefForFirstFrame's reference and the map slot the first keyframe: frame 1 is tracked with the 53 hypotheses of :299-331
+  // (the Reprojector behind fs.cell_order shuffles with the stream as it stands now)
+  sdv_track_new_coarse_io io{}; io.slot = ib.slot; io.frame = (uint64_t)newFrame->shell->id; io.poses_valid = 2;
+  se3_to7(SE3(), io.sprelast_c2w); se3_to7(SE3(), io.slast_c2w); se3_to7(SE3(), io.lastF_c2w);
+  for (int i = 0; i < 5; i++) io.lastCoarseRMSE[i] = fs.lastCoarseRMSE[i];
+  rc = sdv_track_new_coarse_batch(gpu, 1, &io, fs.cell_order.data(), (int)(0.8f*setting_desiredImmatureDensity));
+  newFrame->shell->camToWorld = se3_from7(io.camToWorld); newFrame->shell->camToTrackingRef = se3_from7(io.camToTrackingRef); newFrame->shell->trackingRef = ib.firstFrame->shell;
+  newFrame->shell->aff_g2l = AffLight(io.aff_g2l[0], io.aff_g2l[1]);
+  for (int i = 0; i < 5; i++) fs.lastCoarseRMSE[i] = io.lastCoarseRMSE[i];
+  return Vec4{{io.lastCoarseRMSE[0], io.flow[0], io.flow[1], io.flow[2]}};
+}
+
 // referenced so that -Wunused does not hide a missing call path
 int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const Undistort* u, const uint8_t* raw) {
   std::vector<int32_t> sel, st; Vec5 mr{}; SE3 T; AffLight a;
@@ -386,6 +424,7 @@ int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const 
     std::vector<float> idp2; std::vector<int32_t> rs2, cn2; const float cal6[6] = {1, 1, 0, 0, 1, 1};
     rc |= shim_activatePoints_store({(uint64_t)fh->shell->id}, {0}, ai, {}, cal6, rc2, idp2, rs2, cn2); }
   { RowsQueue q{{}, 0}; int32_t ni = 0; rc |= shim_lidarCloudHandler_rows(q, rig, (uint64_t)fh->shell->id, nullptr, 0) | shim_makeNewTraces_rows(fh, q, ni) | shim_process_pop(q); }
+  { InitBranch ib{nullptr, 0}; int rci = 0; shim_setFirstFromLidar(ib, fh); shim_initializer_frame1(fs, ib, fh, rci); rc |= rci; }
   fs.optimize(6); fs.set_map(0); fs.handover(sel, st); fs.trackNewCoarse(fh); fs.refine_only(fh); shim_frame_destructor(fh);
   return rc;
 }

@@ -121,6 +121,8 @@ def _load():
     L.sdv_lidar_rows_get.argtypes = [_vp, C.c_uint64, C.c_int, _vp, C.POINTER(C.c_int32), _vp, C.POINTER(C.c_int32)]
     L.sdv_lidar_rows_drop.argtypes = [_vp, C.c_int, _u64p]
     L.sdv_make_new_traces_rows_store_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _f32p, C.c_int, _i32p, _i32p]
+    L.sdv_init_from_lidar_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _i32p, _vp, _i32p, _f32p, _i32p, _i32p, C.c_int, _i32p, _i32p, _vp, _vp, _vp]
+    L.sdv_init_from_lidar_rows_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _f32p, _i32p, _i32p, C.c_int, _i32p, _i32p, _vp, _vp, _vp]
     return L
 
 
@@ -771,6 +773,36 @@ def random_pattern(w: int, h: int):
     NB: re-seeds the process-wide rand() stream exactly as constructing a PixelSelector does."""
     libc = C.CDLL(None); libc.srand(3141592)
     return np.array([libc.rand() & 0xFF for _ in range(w * h)], np.uint8)
+
+
+def initializer_draws(w: int, h: int, n: int, seed: int = 3141592):
+    """the n rand() values FullSystem::initializeFromInitializer draws in a running reference (FullSystem.cpp:1203): the frame-0 PixelSelector re-seeds the C library
+    (srand(3141592)) and draws w*h values for its pattern, nothing else calls rand() before.  NB: re-seeds the process-wide rand() stream, like random_pattern."""
+    libc = C.CDLL(None); libc.srand(seed)
+    for _ in range(w * h):
+        libc.rand()
+    return np.array([libc.rand() for _ in range(n)], np.int32)
+
+
+def initializeFromLidarBatch(ctx: "Context", slots, frame_ids, clouds, lruds, desired_point_density, draws, cap: int = 1 << 14):
+    """The start of n sequences (sdv_init_from_lidar_batch / _rows_batch): CoarseInitializer::setFirstFromLidar at level 0 on keyframe frame_ids[j], the point loop of
+    FullSystem::initializeFromInitializer with job j's rand() values draws[j] (at least one per row), and setCTRefForFirstFrame + the one-keyframe map installed on
+    tracker / map slot slots[j].  clouds (n arrays of rows {Ku, Kv, depth}) and lruds (n boxes) given: the host form; None: the rows and box of each frame's LiDAR row
+    set.  -> dict(pts, meta, idepth: per-job record arrays of the kept points, n_selected = numPoints[0] per job (the rand() draws consumed), n = points kept)"""
+    n = len(slots); sl = np.ascontiguousarray(slots, np.int32); fr = np.ascontiguousarray(frame_ids, np.uint64)
+    dens = np.ascontiguousarray(np.broadcast_to(desired_point_density, n), np.float32)
+    dr = [np.ascontiguousarray(d, np.int32).reshape(-1) for d in draws]; db = np.ascontiguousarray(np.concatenate([[0], np.cumsum([len(d) for d in dr])]), np.int32)
+    da = np.ascontiguousarray(np.concatenate(dr) if sum(len(d) for d in dr) else np.zeros(1), np.int32)
+    n_out = np.zeros(n, np.int32); n_sel = np.zeros(n, np.int32)
+    P = np.zeros((n, max(cap, 1)), IMMATURE_PT_DTYPE); M = np.zeros((n, max(cap, 1)), IMMATURE_META_DTYPE); D = np.zeros((n, max(cap, 1)), np.float32)
+    if clouds is None:
+        ctx._ck(LIB.sdv_init_from_lidar_rows_batch(ctx.p, n, sl, fr, dens, db, da, cap, n_out, n_sel, P.ctypes.data, M.ctypes.data, D.ctypes.data))
+    else:
+        cl = [np.ascontiguousarray(c, np.float64).reshape(-1, 3) for c in clouds]; cb = np.ascontiguousarray(np.concatenate([[0], np.cumsum([len(c) for c in cl])]), np.int32)
+        c3 = np.ascontiguousarray(np.concatenate(cl) if cb[-1] else np.zeros((1, 3)), np.float64); box = np.ascontiguousarray(lruds, np.int32).reshape(n * 4)
+        ctx._ck(LIB.sdv_init_from_lidar_batch(ctx.p, n, sl, fr, cb, c3.ctypes.data, box, dens, db, da, cap, n_out, n_sel, P.ctypes.data, M.ctypes.data, D.ctypes.data))
+    return dict(pts=[P[j, :n_out[j]].copy() for j in range(n)], meta=[M[j, :n_out[j]].copy() for j in range(n)], idepth=[D[j, :n_out[j]].copy() for j in range(n)],
+                n_selected=n_sel, n=n_out)
 
 
 def lidar_density(lrud, wh, desiredImmatureDensity):

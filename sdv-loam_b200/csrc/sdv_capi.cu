@@ -493,7 +493,7 @@ int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const f
   CK(cudaSetDevice(c->device));
   TrackerSlot& t = c->slots[slot];
   FrameDev* f; { int rc = job_frame(c, "sdv_tracker_set_ref", 0, ref_frame, -1, slot, nullptr, &f); if (rc) return rc; }
-  const int w = c->cam_w[t.cam], h = c->cam_h[t.cam], L = c->cam_levels[t.cam];   // makeCoarseDepthL0 at the slot's size, for its camera's pyrLevelsUsed levels
+  const int w = c->cam_w[t.cam], h = c->cam_h[t.cam];               // makeCoarseDepthL0 at the slot's size, for its camera's pyrLevelsUsed levels
   for (int i=0;i<n;i++) {                                   // the reference would write out of bounds here; we refuse instead
     int u = round_half[i] ? (int)(pts4[4*i]+0.5f) : (int)pts4[4*i], v = round_half[i] ? (int)(pts4[4*i+1]+0.5f) : (int)pts4[4*i+1];
     if (u < 0 || v < 0 || u >= w || v >= h) return ctx_fail(c, SDV_ERR_ARG, "splat %d (%d,%d) outside the image", i, u, v);
@@ -503,15 +503,26 @@ int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const f
     return ctx_fail(c, SDV_ERR_CUDA, "sdv_tracker_set_ref: scratch of %d splats", n);
   S.reset(); float* pts4_d = S.take<float>(4*(size_t)n); int* round_d = S.take<int>(n); float4* splats = S.take<float4>(n); int* done = S.take<int>(n);
   { int rcj = join_ingest(c); if (rcj) return rcj; }
-  CK(cudaMemsetAsync(c->cd_id[0], 0, (size_t)w*h*sizeof(float), c->st));
-  CK(cudaMemsetAsync(c->cd_ws[0], 0, (size_t)w*h*sizeof(float), c->st));
   if (n > 0) {
     CK(cudaMemcpyAsync(pts4_d, pts4, (size_t)4*n*sizeof(float), cudaMemcpyHostToDevice, c->st));
     CK(cudaMemcpyAsync(round_d, round_half, (size_t)n*sizeof(int), cudaMemcpyHostToDevice, c->st));
-    launch_cd_prep(pts4_d, round_d, n, w, splats, done, c->st);
+  }
+  return tracker_set_ref_dev(c, slot, f, ref_frame, n, pts4_d, round_d, splats, done, ref_a, ref_b, nullptr);
+}
+}  // extern "C"
+
+namespace sdv {
+int tracker_set_ref_dev(sdv_ctx* c, int slot, FrameDev* f, uint64_t ref_frame, int n, const float* pts4_d, const int* round_d, float4* splats, int* done, double ref_a, double ref_b,
+                        int* launches) {
+  TrackerSlot& t = c->slots[slot];
+  const int w = c->cam_w[t.cam], h = c->cam_h[t.cam], L = c->cam_levels[t.cam];
+  CK(cudaMemsetAsync(c->cd_id[0], 0, (size_t)w*h*sizeof(float), c->st));
+  CK(cudaMemsetAsync(c->cd_ws[0], 0, (size_t)w*h*sizeof(float), c->st));
+  if (n > 0) {
+    launch_cd_prep(pts4_d, round_d, n, w, splats, done, c->st); if (launches) *launches += 1;
     for (int round = 0; round < n; round++) {               // usually 1-3 rounds: one per multiplicity of colliding splats; at most n (every splat on one pixel)
       CK(cudaMemsetAsync(c->cd_scalars, 0, sizeof(int), c->st));
-      launch_cd_round(splats, n, done, c->cd_owner, c->cd_id[0], c->cd_ws[0], c->cd_scalars, c->st);
+      launch_cd_round(splats, n, done, c->cd_owner, c->cd_id[0], c->cd_ws[0], c->cd_scalars, c->st); if (launches) *launches += 1;
       CK(cudaMemcpyAsync(c->cd_scalars_host, c->cd_scalars, sizeof(int), cudaMemcpyDeviceToHost, c->st));
       CK(cudaStreamSynchronize(c->st));
       if (c->cd_scalars_host[0] == 0) break;
@@ -522,6 +533,7 @@ int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const f
     launch_cd_dilate(c->cd_id[l], c->cd_ws[l], c->cd_id2[l], c->cd_ws2[l], w>>l, h>>l, l < 2 ? 1 : 0, c->st);
     launch_cd_compact(c->cd_id2[l], c->cd_ws2[l], f->img[l], w>>l, h>>l, c->cd_counts, c->cd_scalars + 1 + l, t.pts[l], t.cap[l], c->st);
   }
+  if (launches) *launches += 3*L - 1;
   CK(cudaMemcpyAsync(c->cd_scalars_host, c->cd_scalars, 8*sizeof(int), cudaMemcpyDeviceToHost, c->st));
   CK(cudaStreamSynchronize(c->st));
   CK(cudaGetLastError());
@@ -534,6 +546,8 @@ int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const f
   t.ref_frame = ref_frame; t.ref_a = ref_a; t.ref_b = ref_b; t.refExposure = f->exposure; t.has_totals = false;
   return SDV_OK;
 }
+}  // namespace sdv
+extern "C" {
 
 // ------------------------------------------------------------------------------------------------ calcRes / calcGSSSE
 int sdv_tracker_calc_res(sdv_ctx* c, int slot, uint64_t new_frame, int lvl, const double T[7], double a, double b, float cutoffTH, double rs_out[6]) { SDV_GUARD_TRK(c);

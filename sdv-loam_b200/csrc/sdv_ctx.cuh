@@ -103,6 +103,18 @@ int  sel_n_slots(const sdv_ctx* c);                                             
 void sel_slot_box(const sdv_ctx* c, int slot, int* cam, int** box_dev);
 // makeNewTraces into the store: job j's n[j] records (sel::NewTrace / sel::ImmPt device arrays, stream-ordered on c->st) replace the block of hosts[j]
 int  imm_store_deposit(sdv_ctx* c, int nj, const uint64_t* hosts, const int* n, const void* const* new_trace_dev, const void* const* imm_dev);
+// one job of the initialiser's point construction (launch_init_points, sdv_trace.cu): n cloud rows {Ku, Kv, depth} with their level-0 status bytes, the job's
+// rand() draws, its keyframe's level-0 plane (w x h); out, up to n points each: records, idepth, splat rows {u, v, idepth, HdiF} + round_half, map rows; counts[2] =
+// {numPoints[0], points kept}.  All device pointers.
+struct InitPointsJob { const double* cloud; const unsigned char* map; const int32_t* draws; const float* I0; int n, w, h; float desired;
+                       sdv_immature_pt* pts; sdv_immature_meta* meta; float* idepth; float* splat4; int* round; sdv_map_pt* mp; int* counts; };
+int  launch_init_points(sdv_ctx* c, int nj, const InitPointsJob* jobs_dev);
+// the half of sdv_tracker_set_ref after the upload: splat rounds, pool, dilate, compact and the capacity rule from n device splat rows pts4_d / round_d
+// (splats / done: device scratch of n float4 / ints); f is the reference frame, already checked against the slot.  *launches (may be NULL) grows by the kernels it ran.
+int  tracker_set_ref_dev(sdv_ctx* c, int slot, FrameDev* f, uint64_t ref_frame, int n, const float* pts4_d, const int* round_d, float4* splats, int* done, double ref_a, double ref_b,
+                         int* launches);
+// sdv_map_set with its points already in memory of kind `kind` (cudaMemcpyHostToDevice: host rows, cudaMemcpyDeviceToDevice: device rows)
+int  map_set_impl(sdv_ctx* c, int slot, int nH, const uint64_t* host_frames, const double* host_T7, const double* host_ab, int nP, const sdv_map_pt* pts, cudaMemcpyKind kind);
 int  sel_activate_select(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,
                          const int32_t* cand_host_begin, const int32_t* cand_begin, const float* cKRKi9, const float* cKt3, const float* cand4, const float* cand4_dev,
                          const float* min_act_dist, const int32_t* cams, int32_t* decision_out, float* dist_map_out);

@@ -346,6 +346,10 @@ int sdv_reproject_grid(sdv_ctx* c, int* n_cols, int* n_rows) { SDV_GUARD_TRK(c);
 }
 
 int sdv_map_set(sdv_ctx* c, int slot, int nH, const uint64_t* host_frames, const double* host_T7, const double* host_ab, int nP, const sdv_map_pt* pts) { SDV_GUARD_TRK(c);
+  return map_set_impl(c, slot, nH, host_frames, host_T7, host_ab, nP, pts, cudaMemcpyHostToDevice);
+}
+}  // extern "C"
+int sdv::map_set_impl(sdv_ctx* c, int slot, int nH, const uint64_t* host_frames, const double* host_T7, const double* host_ab, int nP, const sdv_map_pt* pts, cudaMemcpyKind kind) {
   if (!c || nH < 1 || nH > kRpMaxHosts || !host_frames || !host_T7 || nP < 0 || nP >= (1 << 27) || (nP > 0 && !pts)) return SDV_ERR_ARG;   // point index packs into 27 bits of the sort key
   CK(cudaSetDevice(c->device)); RpState* st = rp_state(c);
   if (slot < 0 || slot >= (int)st->maps.size()) return SDV_ERR_ARG;
@@ -364,10 +368,11 @@ int sdv_map_set(sdv_ctx* c, int slot, int nH, const uint64_t* host_frames, const
   m.nH = nH; m.nP = nP; m.set = true;
   CK(cudaStreamSynchronize(c->st));                                            // a previous launch may still read the slot
   CK(cudaMemcpyAsync(m.dev, &h, sizeof(MapDev), cudaMemcpyHostToDevice, c->st));
-  if (nP) CK(cudaMemcpyAsync(m.pts, pts, (size_t)nP*sizeof(sdv_map_pt), cudaMemcpyHostToDevice, c->st));
+  if (nP) CK(cudaMemcpyAsync(m.pts, pts, (size_t)nP*sizeof(sdv_map_pt), kind, c->st));
   CK(cudaStreamSynchronize(c->st));
   return SDV_OK;
 }
+extern "C" {
 
 int sdv_map_clear(sdv_ctx* c, int slot) { SDV_GUARD_TRK(c);
   if (!c) return SDV_ERR_ARG; CK(cudaSetDevice(c->device)); RpState* st = rp_state(c);

@@ -222,6 +222,107 @@ int sdv_make_new_traces_rows_store_batch(sdv_ctx* c, int n, const int32_t* slots
 }
 
 }  // extern "C"
+// The start of a sequence for n jobs: CoarseInitializer::setFirstFromLidar at level 0 (CoarseInitializer.cpp:766-888), the point loop of
+// FullSystem::initializeFromInitializer (FullSystem.cpp:1176-1225) and CoarseTracker::setCTRefForFirstFrame (CoarseTracker.cpp:636-647, :108-256).  Job j's rows are
+// cloud3 + 3*cloud_begin[j] (host) or cloud_dev[j] (a row set), its box lrud[4j..].  Every check runs before anything is enqueued; the tracker and map slots
+// are written only once every job's points are known to fit `cap`.
+static int init_from_lidar(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const double* const* cloud_dev,
+                           const int32_t* lrud, const float* desired, const int32_t* draw_begin, const int32_t* rand_draws, int cap, int32_t* n_out, int32_t* n_sel_out,
+                           sdv_immature_pt* pts_out, sdv_immature_meta* meta_out, float* idepth_out) {
+  const char* who = "init_from_lidar";
+  if (n == 0) return SDV_OK; SEL_STATE("init_from_lidar");
+  const int ns = (int)c->slots.size();
+  if (cloud_begin[0] != 0 || draw_begin[0] < 0) return ctx_fail(c, SDV_ERR_ARG, "%s: cloud_begin[0] must be 0 and draw_begin[0] >= 0", who);
+  for (int j = 0; j < n; j++) { const int m = cloud_begin[j+1] - cloud_begin[j];
+    if (m < 0) return ctx_fail(c, SDV_ERR_ARG, "%s: cloud_begin is not ascending at job %d", who, j);
+    if (m > 0 && !cloud3 && !cloud_dev) return SDV_ERR_ARG;
+    if (draw_begin[j+1] - draw_begin[j] < m) return ctx_fail(c, SDV_ERR_ARG, "%s: job %d has %d rows and %d rand() draws", who, j, m, draw_begin[j+1] - draw_begin[j]);
+    if (slots[j] < 0 || slots[j] >= ns) return ctx_fail(c, SDV_ERR_ARG, "%s: slot %d of %d", who, slots[j], ns);
+    for (int k = 0; k < j; k++) { if (slots[k] == slots[j]) return ctx_fail(c, SDV_ERR_ARG, "%s: slot %d appears twice in one batch", who, slots[j]);
+      if (frames[k] == frames[j]) return ctx_fail(c, SDV_ERR_ARG, "%s: frame %llu appears twice in one batch", who, (unsigned long long)frames[j]); } }
+  CK(cudaSetDevice(c->device));
+  long long need = 0; std::vector<FrameDev*> F(n); std::vector<int> cam(n);
+  for (int j = 0; j < n; j++) { cam[j] = c->slots[slots[j]].cam;
+    if (c->cam_levels[cam[j]] < 3) return ctx_fail(c, SDV_ERR_ARG, "%s: slot %d's camera has %d levels (the selector reads levels 0..2)", who, slots[j], c->cam_levels[cam[j]]);
+    int rc = job_frame(c, who, j, frames[j], -1, slots[j], &need, &F[j]); if (rc) return rc; }
+  std::vector<sel::FrameImg> img(n);
+  for (int j = 0; j < n; j++) { int rc = ensure_texels(c, *F[j], 1); if (rc) return rc; img[j] = sel::FrameImg{F[j]->I0, F[j]->lvl[1], F[j]->lvl[2]}; }
+  { int rc = join_ingest_upto(c, need); if (rc) return rc; }
+  // every device array of the call in the engine's io scratch: the selection uses scr / scr2, the tracker reference c->scr
+  const size_t nrows = (size_t)cloud_begin[n], ndraw = (size_t)(draw_begin[n] - draw_begin[0]);
+  size_t bytes = Scratch::need(n, sizeof(InitPointsJob)) + Scratch::need(2*(size_t)n, 4) + Scratch::need(std::max(ndraw, (size_t)1), 4) + Scratch::need(cloud3 ? 3*std::max(nrows, (size_t)1) : 1, 8);
+  for (int j = 0; j < n; j++) { const size_t m = std::max(cloud_begin[j+1] - cloud_begin[j], 1);
+    bytes += 2*Scratch::need(sel::SelEngine::ths_floats(c->cam_w[cam[j]], c->cam_h[cam[j]]), 4) + Scratch::need(m, 1) + Scratch::need(m, sizeof(sdv_immature_pt)) + Scratch::need(m, sizeof(sdv_immature_meta))
+           + Scratch::need(m, 4) + Scratch::need(4*m, 4) + Scratch::need(m, 4) + Scratch::need(m, sizeof(sdv_map_pt)); }
+  Scratch& io = s->eng.io;
+  if (io.reserve(bytes, c->st)) return ctx_fail(c, SDV_ERR_CUDA, "%s: scratch of %zu bytes", who, bytes);
+  const long long l0 = s->eng.launches; int cd_launches = 0;
+  CK(cudaEventRecord(c->ev0, c->st));
+  io.reset(); InitPointsJob* dJ = io.take<InitPointsJob>(n); int* counts = io.take<int>(2*(size_t)n); int32_t* draws = io.take<int32_t>(std::max(ndraw, (size_t)1));
+  double* cl = cloud3 ? io.take<double>(3*std::max(nrows, (size_t)1)) : nullptr;
+  if (ndraw) CK(cudaMemcpyAsync(draws, rand_draws + draw_begin[0], ndraw*sizeof(int32_t), cudaMemcpyHostToDevice, c->st));
+  if (cloud3 && nrows) CK(cudaMemcpyAsync(cl, cloud3, 3*nrows*sizeof(double), cudaMemcpyHostToDevice, c->st));
+  std::vector<int> pot(n, 3); std::vector<sel::HistJob> Hj(n); std::vector<sel::MapsJobHost> M(n); std::vector<InitPointsJob> J(n);
+  for (int j = 0; j < n; j++) { const int m = cloud_begin[j+1] - cloud_begin[j], w = c->cam_w[cam[j]], h = c->cam_h[cam[j]]; const size_t tf = sel::SelEngine::ths_floats(w, h), mm = std::max(m, 1);
+    float* a = io.take<float>(tf); float* b = io.take<float>(tf); CK(cudaMemsetAsync(a, 0, tf*4, c->st)); CK(cudaMemsetAsync(b, 0, tf*4, c->st));
+    const double* rows = cloud3 ? cl + 3*(size_t)cloud_begin[j] : cloud_dev[j];
+    const int area = (lrud[4*j+1] - lrud[4*j])*(lrud[4*j+3] - lrud[4*j+2]);                      // lidarArea of the FullSystem box
+    Hj[j] = sel::HistJob{F[j]->I0, a, b, w, h};                                                  // a fresh PixelSelector: makeHists runs
+    sel::MapsJobHost& q = M[j]; q.img = img[j]; q.w = w; q.h = h; q.thsSm = b; q.cloud_dev = rows; q.n = m; q.map = io.take<unsigned char>(mm);
+    q.density = 0.03f*area; q.recursionsLeft = 1; q.thFactor = 2; q.currentPotential = &pot[j]; q.numHaveSub = 0; q.passes = 0;   // makeMapsFromLidar(.., 0.03*lidarArea, 1, false, 2, ..)
+    InitPointsJob& P = J[j]; P.cloud = rows; P.map = q.map; P.draws = draws + (draw_begin[j] - draw_begin[0]); P.I0 = F[j]->I0; P.n = m; P.w = w; P.h = h; P.desired = desired[j];
+    P.pts = io.take<sdv_immature_pt>(mm); P.meta = io.take<sdv_immature_meta>(mm); P.idepth = io.take<float>(mm); P.splat4 = io.take<float>(4*mm); P.round = io.take<int>(mm);
+    P.mp = io.take<sdv_map_pt>(mm); P.counts = counts + 2*j; }
+  if (s->eng.make_hists(n, Hj.data())) return sel_fail(c, s, -1, who);
+  if (s->eng.make_maps(M, true)) return sel_fail(c, s, -1, who);
+  CK(cudaMemcpyAsync(dJ, J.data(), n*sizeof(InitPointsJob), cudaMemcpyHostToDevice, c->st));
+  { int rc = launch_init_points(c, n, dJ); if (rc) return rc; }
+  std::vector<int> cnt(2*(size_t)n);
+  CK(cudaMemcpyAsync(cnt.data(), counts, cnt.size()*sizeof(int), cudaMemcpyDeviceToHost, c->st)); CK(cudaStreamSynchronize(c->st));
+  int over = -1, maxk = 0;
+  for (int j = 0; j < n; j++) { n_sel_out[j] = cnt[2*j]; n_out[j] = cnt[2*j+1]; maxk = std::max(maxk, cnt[2*j+1]); if (cnt[2*j+1] > cap && over < 0) over = j; }
+  c->launches += s->eng.launches - l0;
+  if (over >= 0) return ctx_fail(c, SDV_ERR_CAPACITY, "%s: job %d keeps %d points, cap is %d", who, over, n_out[over], cap);
+  for (int j = 0; j < n; j++) { const size_t k = (size_t)n_out[j]; if (!k) continue;
+    if (pts_out) CK(cudaMemcpyAsync(pts_out + (size_t)j*cap, J[j].pts, k*sizeof(sdv_immature_pt), cudaMemcpyDeviceToHost, c->st));
+    if (meta_out) CK(cudaMemcpyAsync(meta_out + (size_t)j*cap, J[j].meta, k*sizeof(sdv_immature_meta), cudaMemcpyDeviceToHost, c->st));
+    if (idepth_out) CK(cudaMemcpyAsync(idepth_out + (size_t)j*cap, J[j].idepth, k*sizeof(float), cudaMemcpyDeviceToHost, c->st)); }
+  // install: setCTRefForFirstFrame from the splat rows (round_half 1, HdiF 0, lastRef_aff_g2l = (0,0)), and the map of one keyframe at camToWorld = SE3(), aff_g2l = (0,0)
+  if (c->scr.reserve(Scratch::need(std::max(maxk, 1), sizeof(float4)) + Scratch::need(std::max(maxk, 1), sizeof(int)), c->st)) return ctx_fail(c, SDV_ERR_CUDA, "%s: splat scratch", who);
+  static const double kT0[7] = {1, 0, 0, 0, 0, 0, 0}, kAb0[2] = {0, 0};
+  for (int j = 0; j < n; j++) {
+    c->scr.reset(); float4* splats = c->scr.take<float4>(std::max(maxk, 1)); int* done = c->scr.take<int>(std::max(maxk, 1));
+    { int rc = tracker_set_ref_dev(c, slots[j], F[j], frames[j], n_out[j], J[j].splat4, J[j].round, splats, done, 0.0, 0.0, &cd_launches); if (rc) return rc; }
+    { int rc = map_set_impl(c, slots[j], 1, &frames[j], kT0, kAb0, n_out[j], J[j].mp, cudaMemcpyDeviceToDevice); if (rc) return rc; }
+  }
+  CK(cudaEventRecord(c->ev1, c->st)); CK(cudaStreamSynchronize(c->st)); CK(cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
+  c->launches += cd_launches;
+  return SDV_OK;
+}
+extern "C" {
+int sdv_init_from_lidar_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const int32_t* cloud_begin, const double* cloud3, const int32_t* lrud,
+                              const float* desired_point_density, const int32_t* draw_begin, const int32_t* rand_draws, int cap, int32_t* n_out, int32_t* n_selected_out,
+                              sdv_immature_pt* pts_out, sdv_immature_meta* meta_out, float* idepth_out) { SDV_GUARD_TRK(c);
+  if (!c || n < 0 || (n && (!slots || !frames || !cloud_begin || !lrud || !desired_point_density || !draw_begin || !rand_draws || !n_out || !n_selected_out || cap < 0))) return SDV_ERR_ARG;
+  return init_from_lidar(c, n, slots, frames, cloud_begin, cloud3, nullptr, lrud, desired_point_density, draw_begin, rand_draws, cap, n_out, n_selected_out, pts_out, meta_out, idepth_out);
+}
+// The same fed from the LiDAR row sets of frames[j]: rows and box as the handler left them for that frame (sdv_make_new_traces_rows_store_batch reads them the same way).
+int sdv_init_from_lidar_rows_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* frames, const float* desired_point_density, const int32_t* draw_begin,
+                                   const int32_t* rand_draws, int cap, int32_t* n_out, int32_t* n_selected_out, sdv_immature_pt* pts_out, sdv_immature_meta* meta_out,
+                                   float* idepth_out) { SDV_GUARD_TRK(c);
+  if (!c || n < 0 || (n && (!slots || !frames || !desired_point_density || !draw_begin || !rand_draws || !n_out || !n_selected_out || cap < 0))) return SDV_ERR_ARG;
+  if (n == 0) return SDV_OK; SEL_STATE("init_from_lidar_rows");
+  CK(cudaSetDevice(c->device));
+  std::vector<const double*> rows(n); std::vector<LidarRowsInfo> I(n);                   // all headers in one copy
+  { int rc = lidar_rows_fetch(c, n, frames, rows.data(), I.data(), "init_from_lidar_rows"); if (rc) return rc; }
+  std::vector<int32_t> cb(n + 1, 0), box(4*(size_t)n);
+  for (int j = 0; j < n; j++) { const LidarRowsInfo& q = I[j];
+    if (q.overflow) return ctx_fail(c, SDV_ERR_CAPACITY, "init_from_lidar_rows: the sweep of frame %llu left %d pixel rows, its row set holds %d", (unsigned long long)frames[j], q.rows, q.room);
+    for (int k = 0; k < 4; k++) box[4*j+k] = q.lrud[k];
+    cb[j+1] = cb[j] + q.rows; }
+  return init_from_lidar(c, n, slots, frames, cb.data(), nullptr, rows.data(), box.data(), desired_point_density, draw_begin, rand_draws, cap, n_out, n_selected_out, pts_out, meta_out, idepth_out);
+}
+}  // extern "C"
 namespace sdv {
 // makeDistanceMap + the candidate walk; cand4_dev != nullptr: the cand4 rows are device memory (the activation on the immature-point store)
 int sel_activate_select(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,

@@ -53,11 +53,9 @@ __device__ __forceinline__ void interp33(const float* __restrict__ I, float x, f
   for (int k = 0; k < 3; k++) out[k] = w11*c11[k] + w01*c01[k] + w10*c10[k] + w00*c00[k];
 }
 
-// ---- ImmaturePoint::ImmaturePoint (ImmaturePoint.cpp:8-36): one thread per candidate
-__global__ void __launch_bounds__(128) imm_init_kernel(const float* __restrict__ I0, int w, int h, int n, const int* __restrict__ uv, sdv_immature_pt* __restrict__ out, TraceSet S) {
-  const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= n) return;
-  sdv_immature_pt p;
-  p.u = (float)uv[2*i]; p.v = (float)uv[2*i+1]; p.idepth_min = 0; p.idepth_max = NAN; p.lastTraceStatus = IPS_UNINITIALIZED;
+// ---- ImmaturePoint::ImmaturePoint (ImmaturePoint.cpp:8-36) at integer pixel (u, v) of the level-0 plane I0 (row stride w)
+__device__ __forceinline__ void imm_construct(const float* __restrict__ I0, int w, int u, int v, sdv_immature_pt& p, const TraceSet& S) {
+  p.u = (float)u; p.v = (float)v; p.idepth_min = 0; p.idepth_max = NAN; p.lastTraceStatus = IPS_UNINITIALIZED;
   for (int k = 0; k < 4; k++) p.gradH[k] = 0;
   p.lastTraceUV[0] = p.lastTraceUV[1] = 0; p.quality = 10000; p.lastTracePixelInterval = 0; p.energyTH = NAN;
   for (int k = 0; k < 8; k++) { p.color[k] = 0; p.weights[k] = 0; }
@@ -75,6 +73,11 @@ __global__ void __launch_bounds__(128) imm_init_kernel(const float* __restrict__
     p.weights[idx] = sqrtf(S.outlierTHSumComponent / (S.outlierTHSumComponent + (gx*gx + gy*gy)));
   }
   if (finite) { p.energyTH = 8*S.outlierTH; p.energyTH *= S.overallEnergyTHWeight*S.overallEnergyTHWeight; }
+}
+// one thread per candidate
+__global__ void __launch_bounds__(128) imm_init_kernel(const float* __restrict__ I0, int w, int h, int n, const int* __restrict__ uv, sdv_immature_pt* __restrict__ out, TraceSet S) {
+  const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= n) return;
+  sdv_immature_pt p; imm_construct(I0, w, uv[2*i], uv[2*i+1], p, S);
   out[i] = p;
 }
 
@@ -431,6 +434,55 @@ __global__ void __launch_bounds__(128) imm_act_permute_kernel(const ActBlockDev*
   const int g = group_of_point(nbeg, n_hosts, k); const ActBlockDev& B = blocks[g]; const int j = k - __ldg(nbeg + g);
   if (pass == 0) { const int o = perm[k]; sro[k] = B.ro[o]; srw[k] = B.rw[o]; smeta[k] = B.meta[o]; }
   else { B.ro[j] = sro[k]; B.rw[j] = srw[k]; B.meta[j] = smeta[k]; }
+}
+
+// ---- the point loop of FullSystem::initializeFromInitializer (FullSystem.cpp:1176-1225) over the level-0 Pnt list of CoarseInitializer::setFirstFromLidar
+// (CoarseInitializer.cpp:766-888): one CTA per job, the rows in chunks of blockDim in cloud order.  A Pnt is a row with status != 0 and (float)depth > 0 (the
+// first block scan numbers them: draw k belongs to Pnt k); it is kept unless rand()/(float)RAND_MAX > keepPercentage, and if its ImmaturePoint at
+// (int)(u+0.5f), (int)(v+0.5f) has a finite energyTH (the second scan numbers the kept points).  A point whose 8-pattern would read outside the frame's
+// plane is not kept: the reference reads past its image there.
+__device__ __forceinline__ int block_excl_scan(bool pred, int* wt /* 33 ints of shared memory */, int& total) {
+  const unsigned b = __ballot_sync(0xffffffffu, pred); const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (lane == 0) wt[wid] = __popc(b);
+  __syncthreads();
+  if (threadIdx.x == 0) { int a = 0; for (int k = 0; k < (int)(blockDim.x >> 5); k++) { const int t = wt[k]; wt[k] = a; a += t; } wt[32] = a; }
+  __syncthreads();
+  const int r = wt[wid] + __popc(b & ((1u << lane) - 1u)); total = wt[32];
+  __syncthreads();
+  return r;
+}
+__global__ void __launch_bounds__(256) init_points_kernel(const InitPointsJob* __restrict__ jobs, TraceSet S) {
+  const InitPointsJob& J = jobs[blockIdx.x]; __shared__ int wt[33];
+  const int n = J.n, w = J.w, h = J.h;
+  int nsel = 0;
+  for (int base = 0; base < n; base += blockDim.x) { const int i = base + threadIdx.x;
+    nsel += __syncthreads_count(i < n && J.map[i] != 0 && (float)J.cloud[3*i+2] > 0.f); }
+  const float keepPercentage = J.desired / nsel;                                                  // setting_desiredPointDensity / numPoints[0]
+  int kbase = 0, obase = 0;
+  for (int base = 0; base < n; base += blockDim.x) { const int i = base + threadIdx.x;
+    const bool sel = i < n && J.map[i] != 0 && (float)J.cloud[3*i+2] > 0.f;
+    int tot; const int k = kbase + block_excl_scan(sel, wt, tot); kbase += tot;
+    bool keep = false; sdv_immature_pt p; int pu = 0, pv = 0;
+    if (sel && !((float)J.draws[k] / (float)2147483647 > keepPercentage)) {                      // glibc RAND_MAX
+      pu = (int)((float)J.cloud[3*i] + 0.5f); pv = (int)((float)J.cloud[3*i+1] + 0.5f);
+      keep = pu >= 0 && pu < w && pv >= 0 && pv < h && pu + (pv-2)*w >= 0 && pu + 1 + (pv+3)*w < w*h;
+      if (keep) { imm_construct(J.I0, w, pu, pv, p, S); keep = isfinite(p.energyTH); }
+    }
+    const int o = obase + block_excl_scan(keep, wt, tot); obase += tot;
+    if (keep) {
+      const float mdepth = (float)J.cloud[3*i+2], midepth = 1 / mdepth;
+      p.idepth_min = p.idepth_max = midepth; J.pts[o] = p;
+      sdv_immature_meta m; m.my_type = (float)J.map[i]; m.type = 0; m.isFromSensor = 1; m.idepth_fromSensor = midepth; J.meta[o] = m;
+      J.idepth[o] = midepth;
+      J.splat4[4*o] = (float)pu; J.splat4[4*o+1] = (float)pv; J.splat4[4*o+2] = midepth; J.splat4[4*o+3] = 0.f; J.round[o] = 1;   // HdiF = 0, int(u + 0.5f)
+      sdv_map_pt q; q.u = (float)pu; q.v = (float)pv; q.idepth = midepth; q.host = 0; q.type = 0; J.mp[o] = q;
+    }
+  }
+  if (threadIdx.x == 0) { J.counts[0] = nsel; J.counts[1] = obase; }
+}
+int launch_init_points(sdv_ctx* c, int nj, const InitPointsJob* jobs_dev) {
+  init_points_kernel<<<nj, 256, 0, c->st>>>(jobs_dev, trace_settings(c)); c->launches += 1;
+  CK(cudaGetLastError()); return SDV_OK;
 }
 }  // namespace sdv
 
