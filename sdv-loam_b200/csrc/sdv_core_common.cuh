@@ -1,5 +1,5 @@
 // sdv_core_common.cuh — what the self-contained device cores (sdv_select_core.cuh, sdv_lidar_core.cuh) share: launch macros (CUDA, or the host emulation of tests/emu),
-// a block-wide exclusive scan, a grow-only scratch allocator.  Depends on nothing but the CUDA runtime.
+// a block-wide exclusive scan, a grow-only scratch allocator, makeImages' gradient of a planar plane.  Depends on nothing but the CUDA runtime.
 #pragma once
 #include <stdint.h>
 #include <math.h>
@@ -18,7 +18,25 @@
 #define SDV_LAUNCH_SYNC_SMEM(kern, grid, block, smem, st, ...) kern<<<grid, block, smem, st>>>(__VA_ARGS__)
 #endif
 
-namespace sdv { namespace sel {
+namespace sdv {
+
+__device__ __forceinline__ float grad_guard(float d) { return isfinite(d) ? d : 0.0f; }     // if(!std::isfinite(dx)) dx=0;
+// gradient of texel idx of a planar intensity plane as FrameHessian::makeImages forms it (HessianBlocks.cpp:147-156): central differences of flat-index
+// neighbours (at x = 0 / x = w-1 the reference reads across the row boundary, and so does this), zero on the first and last row
+// (returns false there), non-finite -> 0.
+__device__ __forceinline__ bool planar_grad(const float* __restrict__ I, int idx, int w, int h, float& dx, float& dy) {
+  dx = 0.f; dy = 0.f;
+  if (idx >= w && idx < w*(h-1)) {
+    dx = 0.5f*(__ldg(I + idx+1) - __ldg(I + idx-1));
+    dy = 0.5f*(__ldg(I + idx+w) - __ldg(I + idx-w));
+    if (!isfinite(dx)) dx = 0;
+    if (!isfinite(dy)) dy = 0;
+    return true;
+  }
+  return false;
+}
+
+namespace sel {
 
 __device__ __forceinline__ int imin_(int a, int b) { return a < b ? a : b; }
 // exclusive prefix sum of a block's values through shared memory (Hillis-Steele); every thread of the CTA must call it

@@ -10,6 +10,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "sdv_math.cuh"
+#include "sdv_core_common.cuh"
 
 namespace sdv {
 
@@ -95,51 +96,61 @@ __device__ __forceinline__ void finalize_gs_warp(const double* tot, double* H /*
 
 #if defined(__CUDACC__)
 // One reference point through calcRes (CoarseTracker.cpp:525-601) and, if it lands in buf_warped_*, through the
-// Jacobian/outer-product of calcGSSSE + Accumulator9::updateSSE_eighted (CoarseTracker.cpp:442-466, MatrixAccumulators.h:1040-1115).
-// Arithmetic order follows the reference expression trees; the TU is compiled with --fmad=false so only the explicit
+// Jacobian/outer-product of calcGSSSE + Accumulator9::updateSSE_eighted (CoarseTracker.cpp:442-466, MatrixAccumulators.h:1040-1115), in pieces that
+// both tracker kernels compose: eval_point (coarse_res_gs_kernel) and stage_project / stage_accumulate (track_cluster_kernel, which gathers the taps
+// asynchronously between the two).  Arithmetic order follows the reference expression trees; the TU is compiled with --fmad=false so only the explicit
 // fmaf() of the accumulation contracts.
-__device__ __forceinline__ float grad_guard(float d) { return isfinite(d) ? d : 0.0f; }     // if(!std::isfinite(dx)) dx=0;
-__device__ __forceinline__ void eval_point(const float4 p, int i, const LevelGeom& g, const EvalParams& ep,
-                                           const float* __restrict__ I, float (&acc)[kNAcc]) {
-  const float x = p.x, y = p.y, id = p.z, refColor = p.w;
+struct ProjPt { float u, v, Ku, Kv, nid; };               // normalised and pixel coordinates, new inverse depth
+__device__ __forceinline__ ProjPt project_point(const float4 p, const LevelGeom& g, const EvalParams& ep) {
+  const float x = p.x, y = p.y, id = p.z;
   float pt0 = ((ep.RKi[0]*x + ep.RKi[1]*y) + ep.RKi[2]*1.0f) + ep.t[0]*id;
   float pt1 = ((ep.RKi[3]*x + ep.RKi[4]*y) + ep.RKi[5]*1.0f) + ep.t[1]*id;
   float pt2 = ((ep.RKi[6]*x + ep.RKi[7]*y) + ep.RKi[8]*1.0f) + ep.t[2]*id;
-  float u = pt0 / pt2, v = pt1 / pt2;
-  float Ku = g.fx*u + g.cx, Kv = g.fy*v + g.cy;
-  float new_idepth = id / pt2;
+  ProjPt q;
+  q.u = pt0 / pt2; q.v = pt1 / pt2;
+  q.Ku = g.fx*q.u + g.cx; q.Kv = g.fy*q.v + g.cy;
+  q.nid = id / pt2;
+  return q;
+}
+__device__ __forceinline__ bool proj_inside(const ProjPt& q, const LevelGeom& g) {
+  return q.Ku > 2 && q.Kv > 2 && q.Ku < (float)(g.w-3) && q.Kv < (float)(g.h-3) && q.nid > 0;
+}
 
-  if (ep.lvl == 0 && (i & 31) == 0) {                       // flow indicators, CoarseTracker.cpp:538-566
-    float k0 = (g.Ki[0]*x + g.Ki[1]*y) + g.Ki[2]*1.0f, k1 = (g.Ki[3]*x + g.Ki[4]*y) + g.Ki[5]*1.0f, k2 = (g.Ki[6]*x + g.Ki[7]*y) + g.Ki[8]*1.0f;
-    float r0 = (ep.RKi[0]*x + ep.RKi[1]*y) + ep.RKi[2]*1.0f, r1 = (ep.RKi[3]*x + ep.RKi[4]*y) + ep.RKi[5]*1.0f, r2 = (ep.RKi[6]*x + ep.RKi[7]*y) + ep.RKi[8]*1.0f;
-    float a0 = k0 + ep.t[0]*id, a1 = k1 + ep.t[1]*id, a2 = k2 + ep.t[2]*id;
-    float KuT = g.fx*(a0/a2) + g.cx, KvT = g.fy*(a1/a2) + g.cy;
-    float b0_ = k0 - ep.t[0]*id, b1_ = k1 - ep.t[1]*id, b2_ = k2 - ep.t[2]*id;
-    float KuT2 = g.fx*(b0_/b2_) + g.cx, KvT2 = g.fy*(b1_/b2_) + g.cy;
-    float c0 = r0 - ep.t[0]*id, c1 = r1 - ep.t[1]*id, c2 = r2 - ep.t[2]*id;
-    float Ku3 = g.fx*(c0/c2) + g.cx, Kv3 = g.fy*(c1/c2) + g.cy;
-    acc[kIdxFlowT]  += (KuT-x)*(KuT-x) + (KvT-y)*(KvT-y);
-    acc[kIdxFlowT]  += (KuT2-x)*(KuT2-x) + (KvT2-y)*(KvT2-y);
-    acc[kIdxFlowRT] += (Ku-x)*(Ku-x) + (Kv-y)*(Kv-y);
-    acc[kIdxFlowRT] += (Ku3-x)*(Ku3-x) + (Kv3-y)*(Kv3-y);
-    acc[kIdxFlowN]  += 2.0f;
-  }
+// flow indicators of one level-0 point with index % 32 == 0 (CoarseTracker.cpp:538-566)
+__device__ __forceinline__ void flow_point(const float4 p, const LevelGeom& g, const EvalParams& ep, float (&acc)[kNAcc]) {
+  const float x = p.x, y = p.y, id = p.z;
+  const ProjPt q = project_point(p, g, ep);
+  float k0 = (g.Ki[0]*x + g.Ki[1]*y) + g.Ki[2]*1.0f, k1 = (g.Ki[3]*x + g.Ki[4]*y) + g.Ki[5]*1.0f, k2 = (g.Ki[6]*x + g.Ki[7]*y) + g.Ki[8]*1.0f;
+  float r0 = (ep.RKi[0]*x + ep.RKi[1]*y) + ep.RKi[2]*1.0f, r1 = (ep.RKi[3]*x + ep.RKi[4]*y) + ep.RKi[5]*1.0f, r2 = (ep.RKi[6]*x + ep.RKi[7]*y) + ep.RKi[8]*1.0f;
+  float a0 = k0 + ep.t[0]*id, a1 = k1 + ep.t[1]*id, a2 = k2 + ep.t[2]*id;
+  float KuT = g.fx*(a0/a2) + g.cx, KvT = g.fy*(a1/a2) + g.cy;
+  float b0_ = k0 - ep.t[0]*id, b1_ = k1 - ep.t[1]*id, b2_ = k2 - ep.t[2]*id;
+  float KuT2 = g.fx*(b0_/b2_) + g.cx, KvT2 = g.fy*(b1_/b2_) + g.cy;
+  float c0 = r0 - ep.t[0]*id, c1 = r1 - ep.t[1]*id, c2 = r2 - ep.t[2]*id;
+  float Ku3 = g.fx*(c0/c2) + g.cx, Kv3 = g.fy*(c1/c2) + g.cy;
+  acc[kIdxFlowT]  += (KuT-x)*(KuT-x) + (KvT-y)*(KvT-y);
+  acc[kIdxFlowT]  += (KuT2-x)*(KuT2-x) + (KvT2-y)*(KvT2-y);
+  acc[kIdxFlowRT] += (q.Ku-x)*(q.Ku-x) + (q.Kv-y)*(q.Kv-y);
+  acc[kIdxFlowRT] += (Ku3-x)*(Ku3-x) + (Kv3-y)*(Kv3-y);
+  acc[kIdxFlowN]  += 2.0f;
+}
 
-  if (!(Ku > 2 && Kv > 2 && Ku < (float)(g.w-3) && Kv < (float)(g.h-3) && new_idepth > 0)) return;
-
-  // getInterpolatedElement33, util/globalFuncs.h:51-65
-  int ix = (int)Ku, iy = (int)Kv;
-  float dx = Ku - ix, dy = Kv - iy, dxdy = dx*dy;
-  float4 p00, p10, p01, p11;                                // planar intensity, gradients formed on the fly exactly like makeImages does
-  const float* b = I + ix + iy*g.w; const int w = g.w;      // (HessianBlocks.cpp:147-156; taps never touch rows 0 / h-1)
-  float a_m1_0 = __ldg(b - w),     a_m1_1 = __ldg(b - w + 1);
-  float a_0_m1 = __ldg(b - 1),     a_0_0 = __ldg(b),         a_0_1 = __ldg(b + 1),         a_0_2 = __ldg(b + 2);
-  float a_1_m1 = __ldg(b + w - 1), a_1_0 = __ldg(b + w),     a_1_1 = __ldg(b + w + 1),     a_1_2 = __ldg(b + w + 2);
-  float a_2_0 = __ldg(b + 2*w),    a_2_1 = __ldg(b + 2*w + 1);
+// getInterpolatedElement33 (util/globalFuncs.h:51-65) at fractional offset (dx, dy) of the inside point q, residual, Huber weight and outer product.
+// tap(k), k = 0..11: the 12-tap planar footprint rows -1..2 around the integer pixel — row -1: 0,1; row 0: -1..2; row 1: -1..2; row 2: 0,1 — from which the
+// gradients are formed exactly like makeImages does (HessianBlocks.cpp:147-156; the taps never touch rows 0 / h-1).
+template <class Tap>
+__device__ __forceinline__ void accumulate_point(const Tap& tap, float dx, float dy, const ProjPt& q, float refColor, const LevelGeom& g, const EvalParams& ep,
+                                                 float (&acc)[kNAcc]) {
+  float4 p00, p10, p01, p11;
+  float a_m1_0 = tap(0), a_m1_1 = tap(1);
+  float a_0_m1 = tap(2), a_0_0 = tap(3), a_0_1 = tap(4), a_0_2 = tap(5);
+  float a_1_m1 = tap(6), a_1_0 = tap(7), a_1_1 = tap(8), a_1_2 = tap(9);
+  float a_2_0 = tap(10), a_2_1 = tap(11);
   p00.x = a_0_0; p00.y = grad_guard(0.5f*(a_0_1 - a_0_m1)); p00.z = grad_guard(0.5f*(a_1_0 - a_m1_0));
   p10.x = a_0_1; p10.y = grad_guard(0.5f*(a_0_2 - a_0_0));  p10.z = grad_guard(0.5f*(a_1_1 - a_m1_1));
   p01.x = a_1_0; p01.y = grad_guard(0.5f*(a_1_1 - a_1_m1)); p01.z = grad_guard(0.5f*(a_2_0 - a_0_0));
   p11.x = a_1_1; p11.y = grad_guard(0.5f*(a_1_2 - a_1_0));  p11.z = grad_guard(0.5f*(a_2_1 - a_0_1));
+  const float dxdy = dx*dy, u = q.u, v = q.v, new_idepth = q.nid;
   float w11 = dxdy, w01 = dy-dxdy, w10 = dx-dxdy, w00 = 1-dx-dy+dxdy;
   float hit0 = ((w11*p11.x + w01*p01.x) + w10*p10.x) + w00*p00.x;
   float hit1 = ((w11*p11.y + w01*p01.y) + w10*p10.y) + w00*p00.y;
@@ -171,6 +182,21 @@ __device__ __forceinline__ void eval_point(const float4 p, int i, const LevelGeo
 #pragma unroll
     for (int c = r; c < 9; c++) { acc[k] = fmaf(Jw, J[c], acc[k]); k++; }
   }
+}
+
+// point i of the reference cloud, taps read straight from the planar level I
+__device__ __forceinline__ void eval_point(const float4 p, int i, const LevelGeom& g, const EvalParams& ep,
+                                           const float* __restrict__ I, float (&acc)[kNAcc]) {
+  const ProjPt q = project_point(p, g, ep);
+  if (ep.lvl == 0 && (i & 31) == 0) flow_point(p, g, ep, acc);
+  if (!proj_inside(q, g)) return;
+  const int ix = (int)q.Ku, iy = (int)q.Kv, w = g.w;
+  const float* b = I + ix + iy*w;
+  const auto tap = [&](int k) {
+    const float* r = k < 2 ? b - w : (k < 6 ? b : (k < 10 ? b + w : b + 2*w));
+    return __ldg(r + (k < 2 ? k : (k < 6 ? k - 3 : (k < 10 ? k - 7 : k - 10))));
+  };
+  accumulate_point(tap, q.Ku - ix, q.Kv - iy, q, p.w, g, ep, acc);
 }
 #endif
 

@@ -42,17 +42,10 @@ template <> __device__ __forceinline__ float4 px_load4<unsigned char>(const unsi
   const uchar4 v = __ldg(reinterpret_cast<const uchar4*>(p + i)); return make_float4((float)v.x, (float)v.y, (float)v.z, (float)v.w);
 }
 
-// gradient + pack of one texel of a planar intensity image (HessianBlocks.cpp:147-165).  Flat-index neighbours on purpose: at x=0 / x=w-1 the
-// reference reads across the row boundary (idx±1), and so do we.
+// gradient + pack of one texel of a planar intensity image (HessianBlocks.cpp:147-165)
 __device__ __forceinline__ float4 grad_texel(const float* __restrict__ I, int idx, int w, int h) {
-  float c = __ldg(I + idx); float dx = 0.f, dy = 0.f, ab = 0.f;
-  if (idx >= w && idx < w*(h-1)) {
-    dx = 0.5f*(__ldg(I + idx+1) - __ldg(I + idx-1));
-    dy = 0.5f*(__ldg(I + idx+w) - __ldg(I + idx-w));
-    if (!isfinite(dx)) dx = 0;
-    if (!isfinite(dy)) dy = 0;
-    ab = dx*dx + dy*dy;
-  }
+  const float c = __ldg(I + idx); float dx, dy, ab = 0.f;
+  if (planar_grad(I, idx, w, h, dx, dy)) ab = dx*dx + dy*dy;
   return make_float4(c, dx, dy, ab);
 }
 // packed texels of one level from its planar intensity, on demand (keyframes entering the BA window or the selector, debugging read-back)
@@ -327,25 +320,20 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 __device__ __forceinline__ void cp_async_wait1()  { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait0()  { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-struct PtState { float u, v, nid, dx, dy, col; bool ok; };     // what the accumulate stage needs of a projected point (its taps are in the thread's smem slot)
+struct PtState { ProjPt q; float dx, dy, col; bool ok; };    // what the accumulate stage needs of a projected point (its taps are in the thread's smem slot)
 
 // calcRes, first half (CoarseTracker.cpp:525-575): projection + bounds, then launch the gather of the 12-tap planar footprint into `slot`.
 constexpr int kTaps = 12;
 template <int THREADS>
 __device__ __forceinline__ PtState stage_project(const float4 p, const LevelGeom& g, const EvalParams& ep, const float* __restrict__ I, uint32_t slot) {
-  PtState s; const float x = p.x, y = p.y, id = p.z; s.col = p.w;
-  float pt0 = ((ep.RKi[0]*x + ep.RKi[1]*y) + ep.RKi[2]*1.0f) + ep.t[0]*id;
-  float pt1 = ((ep.RKi[3]*x + ep.RKi[4]*y) + ep.RKi[5]*1.0f) + ep.t[1]*id;
-  float pt2 = ((ep.RKi[6]*x + ep.RKi[7]*y) + ep.RKi[8]*1.0f) + ep.t[2]*id;
-  s.u = pt0 / pt2; s.v = pt1 / pt2;
-  const float Ku = g.fx*s.u + g.cx, Kv = g.fy*s.v + g.cy;
-  s.nid = id / pt2;
-  s.ok = (Ku > 2 && Kv > 2 && Ku < (float)(g.w-3) && Kv < (float)(g.h-3) && s.nid > 0);
+  PtState s; s.col = p.w;
+  s.q = project_point(p, g, ep);
+  s.ok = proj_inside(s.q, g);
   s.dx = 0.f; s.dy = 0.f;
   if (s.ok) {
-    const int ix = (int)Ku, iy = (int)Kv, w = g.w;
-    s.dx = Ku - ix; s.dy = Kv - iy;
-    const float* b = I + ix + iy*w;                         // rows -1..2 (gradients are formed in stage_accumulate exactly like makeImages does)
+    const int ix = (int)s.q.Ku, iy = (int)s.q.Kv, w = g.w;
+    s.dx = s.q.Ku - ix; s.dy = s.q.Kv - iy;
+    const float* b = I + ix + iy*w;                         // rows -1..2 in accumulate_point's tap order
     cp_async4(slot + 0*THREADS*4, b - w);       cp_async4(slot + 1*THREADS*4, b - w + 1);
     cp_async4(slot + 2*THREADS*4, b - 1);       cp_async4(slot + 3*THREADS*4, b);         cp_async4(slot + 4*THREADS*4, b + 1);     cp_async4(slot + 5*THREADS*4, b + 2);
     cp_async4(slot + 6*THREADS*4, b + w - 1);   cp_async4(slot + 7*THREADS*4, b + w);     cp_async4(slot + 8*THREADS*4, b + w + 1); cp_async4(slot + 9*THREADS*4, b + w + 2);
@@ -353,72 +341,11 @@ __device__ __forceinline__ PtState stage_project(const float4 p, const LevelGeom
   }
   return s;
 }
-// calcRes second half + calcGSSSE for one point whose taps have landed (CoarseTracker.cpp:576-601, 442-466).  Expression trees identical to eval_point.
+// calcRes second half + calcGSSSE for one point whose taps have landed (CoarseTracker.cpp:576-601, 442-466)
 template <int THREADS>
 __device__ __forceinline__ void stage_accumulate(const PtState s, const LevelGeom& g, const EvalParams& ep, const float* slot, float (&acc)[kNAcc]) {
   if (!s.ok) return;
-  float4 p00, p10, p01, p11;
-  const float* t = slot;
-  float a_m1_0 = t[0*THREADS], a_m1_1 = t[1*THREADS];
-  float a_0_m1 = t[2*THREADS], a_0_0 = t[3*THREADS], a_0_1 = t[4*THREADS], a_0_2 = t[5*THREADS];
-  float a_1_m1 = t[6*THREADS], a_1_0 = t[7*THREADS], a_1_1 = t[8*THREADS], a_1_2 = t[9*THREADS];
-  float a_2_0 = t[10*THREADS], a_2_1 = t[11*THREADS];
-  p00.x = a_0_0; p00.y = grad_guard(0.5f*(a_0_1 - a_0_m1)); p00.z = grad_guard(0.5f*(a_1_0 - a_m1_0));
-  p10.x = a_0_1; p10.y = grad_guard(0.5f*(a_0_2 - a_0_0));  p10.z = grad_guard(0.5f*(a_1_1 - a_m1_1));
-  p01.x = a_1_0; p01.y = grad_guard(0.5f*(a_1_1 - a_1_m1)); p01.z = grad_guard(0.5f*(a_2_0 - a_0_0));
-  p11.x = a_1_1; p11.y = grad_guard(0.5f*(a_1_2 - a_1_0));  p11.z = grad_guard(0.5f*(a_2_1 - a_0_1));
-  const float dx = s.dx, dy = s.dy, dxdy = dx*dy, u = s.u, v = s.v, new_idepth = s.nid, refColor = s.col;
-  float w11 = dxdy, w01 = dy-dxdy, w10 = dx-dxdy, w00 = 1-dx-dy+dxdy;
-  float hit0 = ((w11*p11.x + w01*p01.x) + w10*p10.x) + w00*p00.x;
-  float hit1 = ((w11*p11.y + w01*p01.y) + w10*p10.y) + w00*p00.y;
-  float hit2 = ((w11*p11.z + w01*p01.z) + w10*p10.z) + w00*p00.z;
-  if (!isfinite(hit0)) return;
-  float residual = hit0 - (ep.aLL*refColor + ep.bLL);
-  float ar = fabsf(residual);
-  float hw = ar < ep.huber ? 1.0f : ep.huber / ar;
-  acc[kIdxNE] += 1.0f;
-  if (ar > ep.cutoff) { acc[kIdxE] += ep.maxEnergy; acc[kIdxNSat] += 1.0f; return; }
-  acc[kIdxE] += hw*residual*residual*(2-hw);
-  float dxf = hit1*g.fx, dyf = hit2*g.fy;
-  float J[9];
-  J[0] = new_idepth*dxf;
-  J[1] = new_idepth*dyf;
-  J[2] = 0.0f - new_idepth*(u*dxf + v*dyf);
-  J[3] = 0.0f - ((u*v)*dxf + dyf*(1.0f + v*v));
-  J[4] = (u*v)*dyf + dxf*(1.0f + u*u);
-  J[5] = u*dyf - v*dxf;
-  J[6] = ep.aLL*(ep.b0 - refColor);
-  J[7] = -1.0f;
-  J[8] = residual;
-  int k = 0;
-#pragma unroll
-  for (int r = 0; r < 9; r++) {
-    float Jw = J[r]*hw;
-#pragma unroll
-    for (int c = r; c < 9; c++) { acc[k] = fmaf(Jw, J[c], acc[k]); k++; }
-  }
-}
-// flow indicators of one level-0 point with index % 32 == 0 (CoarseTracker.cpp:538-566); same expressions as eval_point
-__device__ __forceinline__ void flow_point(const float4 p, const LevelGeom& g, const EvalParams& ep, float (&acc)[kNAcc]) {
-  const float x = p.x, y = p.y, id = p.z;
-  float pt0 = ((ep.RKi[0]*x + ep.RKi[1]*y) + ep.RKi[2]*1.0f) + ep.t[0]*id;
-  float pt1 = ((ep.RKi[3]*x + ep.RKi[4]*y) + ep.RKi[5]*1.0f) + ep.t[1]*id;
-  float pt2 = ((ep.RKi[6]*x + ep.RKi[7]*y) + ep.RKi[8]*1.0f) + ep.t[2]*id;
-  float u = pt0 / pt2, v = pt1 / pt2;
-  float Ku = g.fx*u + g.cx, Kv = g.fy*v + g.cy;
-  float k0 = (g.Ki[0]*x + g.Ki[1]*y) + g.Ki[2]*1.0f, k1 = (g.Ki[3]*x + g.Ki[4]*y) + g.Ki[5]*1.0f, k2 = (g.Ki[6]*x + g.Ki[7]*y) + g.Ki[8]*1.0f;
-  float r0 = (ep.RKi[0]*x + ep.RKi[1]*y) + ep.RKi[2]*1.0f, r1 = (ep.RKi[3]*x + ep.RKi[4]*y) + ep.RKi[5]*1.0f, r2 = (ep.RKi[6]*x + ep.RKi[7]*y) + ep.RKi[8]*1.0f;
-  float a0 = k0 + ep.t[0]*id, a1 = k1 + ep.t[1]*id, a2 = k2 + ep.t[2]*id;
-  float KuT = g.fx*(a0/a2) + g.cx, KvT = g.fy*(a1/a2) + g.cy;
-  float b0_ = k0 - ep.t[0]*id, b1_ = k1 - ep.t[1]*id, b2_ = k2 - ep.t[2]*id;
-  float KuT2 = g.fx*(b0_/b2_) + g.cx, KvT2 = g.fy*(b1_/b2_) + g.cy;
-  float c0 = r0 - ep.t[0]*id, c1 = r1 - ep.t[1]*id, c2 = r2 - ep.t[2]*id;
-  float Ku3 = g.fx*(c0/c2) + g.cx, Kv3 = g.fy*(c1/c2) + g.cy;
-  acc[kIdxFlowT]  += (KuT-x)*(KuT-x) + (KvT-y)*(KvT-y);
-  acc[kIdxFlowT]  += (KuT2-x)*(KuT2-x) + (KvT2-y)*(KvT2-y);
-  acc[kIdxFlowRT] += (Ku-x)*(Ku-x) + (Kv-y)*(Kv-y);
-  acc[kIdxFlowRT] += (Ku3-x)*(Ku3-x) + (Kv3-y)*(Kv3-y);
-  acc[kIdxFlowN]  += 2.0f;
+  accumulate_point([&](int k) { return slot[k*THREADS]; }, s.dx, s.dy, s.q, s.col, g, ep, acc);
 }
 
 #ifdef SDV_TRACK_PROFILE
@@ -541,10 +468,10 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
       if (lvl == 0) {                                       // dense flow-indicator pre-pass: point indices 0, 32, 64, ...
         for (int j = rank*THREADS + tid; 32*j < n; j += stride) flow_point(__ldg(pts + 32*j), g, ctl.ep, acc);
       }
-      PtState sN; sN.ok = false; sN.u = sN.v = sN.nid = sN.dx = sN.dy = sN.col = 0.f;
+      PtState sN; sN.ok = false; sN.q.u = sN.q.v = sN.q.nid = sN.dx = sN.dy = sN.col = 0.f;
       auto project = [&](int m) {                           // stage A for sweep iteration m (its chunk has landed)
         const int i = m*stride + rank*THREADS + tid;
-        PtState s; s.ok = false; s.u = s.v = s.nid = s.dx = s.dy = s.col = 0.f;
+        PtState s; s.ok = false; s.q.u = s.q.v = s.q.nid = s.dx = s.dy = s.col = 0.f;
         if (i < n) {
 #ifdef SDV_PTS_LDG
           const float4 p = __ldg(pts + i);

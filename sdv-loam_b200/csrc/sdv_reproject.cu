@@ -69,7 +69,6 @@ __device__ __forceinline__ float interp_plane(const float* __restrict__ I, float
   const float* bp = I + ix + iy*width;
   return ((dxdy*__ldg(bp+1+width) + (dy-dxdy)*__ldg(bp+width)) + (dx-dxdy)*__ldg(bp+1)) + (1-dx-dy+dxdy)*__ldg(bp);
 }
-__device__ __forceinline__ float grad_g(float d) { return isfinite(d) ? d : 0.0f; }
 
 template <bool OWN_K>                                                          // OWN_K: as in find_match_direct
 __device__ __forceinline__ void project_point(const RpJob& jb, const RpConst& C, const MapDev* __restrict__ m, const sdv_map_pt& p, double* px) {
@@ -94,8 +93,8 @@ __global__ void __launch_bounds__(256) rp_project_kernel(RpJob* __restrict__ job
   if (!in_frame(w, h, px[0], px[1], 8)) return;
   const int k = (int)(px[1]/kRpCell)*((w + kRpCell - 1)/kRpCell) + (int)(px[0]/kRpCell);      // the job's own grid
   const float* __restrict__ I = m->hostI0[p.host]; const int idx = (int)(p.v*w + p.u);
-  float key = 0.f;
-  if (idx >= w && idx < w*(h-1)) { const float gx = grad_g(0.5f*(__ldg(I+idx+1) - __ldg(I+idx-1))), gy = grad_g(0.5f*(__ldg(I+idx+w) - __ldg(I+idx-w))); key = sqrtf(gx*gx + gy*gy); }
+  float gx, gy, key = 0.f;
+  if (planar_grad(I, idx, w, h, gx, gy)) key = sqrtf(gx*gx + gy*gy);
   S.cand_px[gi] = make_double2(px[0], px[1]); S.cand_key[gi] = key; S.cand_cell[gi] = k;
   atomicAdd(&S.count[(long long)blockIdx.y*C.ncells + k], 1);
 }
@@ -188,7 +187,7 @@ __device__ bool find_match_direct(const RpJob& jb, const RpConst& C, const sdv_m
   bool early_false = false;
   if (pt.type == 1) {                                                          // EDGELET: align1D :346-455
     const float* __restrict__ I = m->hostI0[ref]; const int idx = (int)(px[0] + px[1]*w0);
-    double g0 = (double)grad_g(0.5f*(__ldg(I+idx+1) - __ldg(I+idx-1))), g1 = (double)grad_g(0.5f*(__ldg(I+idx+w0) - __ldg(I+idx-w0)));
+    double g0 = (double)grad_guard(0.5f*(__ldg(I+idx+1) - __ldg(I+idx-1))), g1 = (double)grad_guard(0.5f*(__ldg(I+idx+w0) - __ldg(I+idx-w0)));
     { const double n = sqrt(g0*g0 + g1*g1); g0 /= n; g1 /= n; }
     double d0 = A[0]*g0 + A[1]*g1, d1 = A[2]*g0 + A[3]*g1; { const double n2 = sqrt(d0*d0 + d1*d1); d0 /= n2; d1 /= n2; }
     const float dir0 = (float)d0, dir1 = (float)d1;

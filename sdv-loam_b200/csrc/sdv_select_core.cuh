@@ -45,15 +45,6 @@ SDV_DEVCONST float kSelDirs[16][2] = {{0,1.0000f},{0.3827f,0.9239f},{0.1951f,0.9
                                       {0.5556f,-0.8315f},{0.9808f,0.1951f},{0.9239f,-0.3827f},{0.7071f,-0.7071f},{0.5556f,0.8315f},{0.9808f,-0.1951f},{1.0000f,0.0000f},{0.1951f,-0.9808f}};
 SDV_DEVCONST int kSelPat[8][2] = {{0,-2},{-1,-1},{1,-1},{-2,0},{0,0},{2,0},{-1,1},{0,2}};
 
-// level-0 gradient of FrameHessian::makeImages (HessianBlocks.cpp:147-156) from the planar plane: flat-index neighbours, first / last row zero
-__device__ __forceinline__ void grad0(const float* __restrict__ I, int idx, int w, int h, float& dx, float& dy) {
-  dx = 0.f; dy = 0.f;
-  if (idx >= w && idx < w*(h-1)) {
-    dx = 0.5f*(__ldg(I + idx+1) - __ldg(I + idx-1)); dy = 0.5f*(__ldg(I + idx+w) - __ldg(I + idx-w));
-    if (!isfinite(dx)) dx = 0;
-    if (!isfinite(dy)) dy = 0;
-  }
-}
 __device__ __forceinline__ int slot_of_cell(int cx, int cy, int nbx4) {                 // position of cell (cx,cy) in the reference's visiting order (4x4 block, 2x2 sub-block, cell)
   return (((cy>>2)*nbx4 + (cx>>2)) << 4) | (((cy>>1)&1) << 3) | (((cx>>1)&1) << 2) | ((cy&1) << 1) | (cx&1);
 }
@@ -62,7 +53,7 @@ __device__ __forceinline__ PtRec make_rec(const FrameImg& F, const float* __rest
   PtRec r; r.valid = 1; r.out = out;
   const int w32 = w/32, w1 = w>>1, w2 = w>>2;
   r.th0 = __ldg(thsSm + ((int)xf>>5) + ((int)yf>>5)*w32);
-  grad0(F.I0, idx, w, h, r.dx, r.dy); r.ag0 = r.dx*r.dx + r.dy*r.dy;
+  planar_grad(F.I0, idx, w, h, r.dx, r.dy); r.ag0 = r.dx*r.dx + r.dy*r.dy;
   r.ag1 = __ldg(&F.L1[(int)(xf*0.5f+0.25f) + (int)(yf*0.5f+0.25f)*w1].w);
   r.ag2 = __ldg(&F.L2[(int)((double)(xf*0.25f)+0.125) + (int)((double)(yf*0.25f)+0.125)*w2].w);
   return r;
@@ -97,7 +88,7 @@ __global__ void __launch_bounds__(128) sel_hist_kernel(const HistJob* __restrict
   for (int k = threadIdx.x; k < 1024; k += blockDim.x) {
     const int it = (k&31) + 32*bx, jt = (k>>5) + 32*by;
     if (it > w-2 || jt > h-2 || it < 1 || jt < 1) continue;
-    float dx, dy; grad0(J.I0, it + jt*w, w, h, dx, dy);
+    float dx, dy; planar_grad(J.I0, it + jt*w, w, h, dx, dy);
     int g = (int)sqrtf(dx*dx + dy*dy); if (g > 48) g = 48;
     atomicAdd(&hist[g+1], 1); atomicAdd(&hist[0], 1);
   }

@@ -30,15 +30,9 @@ struct TraceGroupDev { const float* I0; float KRKi[9], Kt[3], aff[2]; int pt_beg
 struct TraceSet { float outlierTH, outlierTHSumComponent, overallEnergyTHWeight, huberTH, maxPixSearch; int minTraceTestRadius; float stepsize; int GNIterations;
                   float GNThreshold, extraSlackOnTH, slackInterval, minImprovementFactor; };
 
-// dIp[0][idx] = {I, dx, dy} from the planar level-0 plane: central differences, zero on the first / last image row (flat-index rule), non-finite -> 0
+// dIp[0][idx] = {I, dx, dy} from the planar level-0 plane
 __device__ __forceinline__ void texel0(const float* __restrict__ I, int idx, int w, int h, float& c, float& dx, float& dy) {
-  c = __ldg(I + idx); dx = 0.f; dy = 0.f;
-  if (idx >= w && idx < w*(h-1)) {
-    dx = 0.5f*(__ldg(I + idx+1) - __ldg(I + idx-1));
-    dy = 0.5f*(__ldg(I + idx+w) - __ldg(I + idx-w));
-    if (!isfinite(dx)) dx = 0;
-    if (!isfinite(dy)) dy = 0;
-  }
+  c = __ldg(I + idx); planar_grad(I, idx, w, h, dx, dy);
 }
 __device__ __forceinline__ float interp31(const float* __restrict__ I, float x, float y, int w) {   // getInterpolatedElement31, util/globalFuncs.h:102-116
   const int ix = (int)x, iy = (int)y; const float dx = x - ix, dy = y - iy, dxdy = dx*dy; const float* bp = I + ix + iy*w;
