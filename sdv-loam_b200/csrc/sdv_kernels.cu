@@ -445,7 +445,9 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
     {
       const float4* __restrict__ pts = J.pts[lvl]; const int n = J.npts[lvl];
       const float* __restrict__ I = J.img[lvl];
-      const LevelGeom& g = geom.g[lvl];
+      // the sweep's operands as register copies: the cp.async / mbarrier asm below clobbers "memory", which would reload them from shared memory for every point
+      const LevelGeom g = geom.g[lvl];
+      const EvalParams ep = ctl.ep;
       const int K = (n + stride - 1)/stride;                // sweep iterations (uniform over the CTA)
       const int NC = (K + kPtChunk - 1)/kPtChunk;           // point chunks
       auto issue_chunk = [&](int c) {                       // thread 0: TMA bulk copies of chunk c's (<= kPtChunk) blocks into buffer c&1
@@ -466,7 +468,7 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
 #endif
       SDV_PROF_T(tp1); SDV_PROF_ADD(0, tp0, tp1);
       if (lvl == 0) {                                       // dense flow-indicator pre-pass: point indices 0, 32, 64, ...
-        for (int j = rank*THREADS + tid; 32*j < n; j += stride) flow_point(__ldg(pts + 32*j), g, ctl.ep, acc);
+        for (int j = rank*THREADS + tid; 32*j < n; j += stride) flow_point(__ldg(pts + 32*j), g, ep, acc);
       }
       PtState sN; sN.ok = false; sN.q.u = sN.q.v = sN.q.nid = sN.dx = sN.dy = sN.col = 0.f;
       auto project = [&](int m) {                           // stage A for sweep iteration m (its chunk has landed)
@@ -479,7 +481,7 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
           const float4 p = pbuf[(((m/kPtChunk) & 1)*kPtChunk + (m % kPtChunk))*THREADS + tid];
 #endif
           const uint32_t so = (uint32_t)(m & 1)*kSlotStride;
-          s = stage_project<THREADS>(p, g, ctl.ep, I, slot_base + so);
+          s = stage_project<THREADS>(p, g, ep, I, slot_base + so);
         }
         return s;
       };
@@ -507,7 +509,7 @@ __global__ void __launch_bounds__(THREADS, MINB) track_cluster_kernel(TrackJob* 
         }
         cp_async_commit();
         cp_async_wait1();                                   // the gather of iteration k (committed one iteration ago) has landed in this thread's slot
-        stage_accumulate<THREADS>(sC, g, ctl.ep, reinterpret_cast<const float*>(ring + (size_t)(k & 1)*kSlotStride) + tid, acc);
+        stage_accumulate<THREADS>(sC, g, ep, reinterpret_cast<const float*>(ring + (size_t)(k & 1)*kSlotStride) + tid, acc);
       }
       SDV_PROF_T(tp4); SDV_PROF_ADD(3, tp3, tp4);
       cp_async_wait0();
