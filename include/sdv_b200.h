@@ -158,6 +158,18 @@ int  sdv_frame_download(sdv_ctx* c, uint64_t frame, int lvl, float* dI3_out, flo
  * with round_half[i]=0 for `int(u)` (newest-KF sensor points, :270-271) or 1 for `int(u+0.5f)` (:116-117, :285-286). */
 int  sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const float* pts4, const int32_t* round_half,
                          float ref_exposure_unused, double ref_a, double ref_b);
+/* setCoarseTrackingRef for n tracker slots in one launch sequence (makeKeyFrame of many sequences).  Job j is sdv_tracker_set_ref(slots[j], ref_frames[j],
+ * rows pt_begin[j] .. pt_begin[j+1] of pts4 / round_half, ref_ab[2j], ref_ab[2j+1]) at its slot camera's size and depth; ref_ab == NULL is (0, 0) for every
+ * job.  Two jobs may share a reference frame.  npts_out[j*SDV_PYR_LEVELS + l] (may be NULL) = job j's true cloud size at level l, 0 past its camera's depth.
+ * The clouds are bit-identical to n single calls; sdv_tracker_set_ref is this call with n = 1.  n == 0 returns SDV_OK.
+ * Refused before anything is enqueued, changing no slot: a NULL array, pt_begin[0] != 0 or decreasing, a slot out of range or named twice (SDV_ERR_ARG);
+ * an unknown frame (SDV_ERR_NOFRAME); a frame of another size than its slot's camera, or a splat outside its slot camera's image (SDV_ERR_ARG).
+ * Over capacity (max_ref_points): every job whose clouds fit is installed; every job with a level over its slot's capacity is left with NO reference (as
+ * sdv_tracker_set_ref leaves its slot), and the call returns SDV_ERR_CAPACITY naming the first such job, with npts_out filled.
+ * Launches: a fixed number per chunk of jobs whose planes fit the build's plane budget (DESIGN.md Round 13), whatever the splat count or multiplicity;
+ * one host wait per call.  Counted by sdv_launch_count, timed by sdv_last_kernel_ms. */
+int  sdv_tracker_set_ref_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* ref_frames, const int32_t* pt_begin, const float* pts4,
+                               const int32_t* round_half, const double* ref_ab, int32_t* npts_out);
 /* direct injection / readback of one level's reference cloud pc_u,pc_v,pc_idepth,pc_color (tests, stress config) */
 int  sdv_tracker_set_cloud(sdv_ctx* c, int slot, uint64_t ref_frame, int lvl, int n, const float* u, const float* v,
                            const float* idepth, const float* color, double ref_a, double ref_b);
@@ -219,6 +231,12 @@ int  sdv_tracker_track_batch_levels(sdv_ctx* c, int n, const int32_t* slots, con
 typedef struct { float u, v, idepth; int32_t host; int32_t type; } sdv_map_pt;
 int  sdv_reproject_grid(sdv_ctx* c, int* n_cols, int* n_rows);
 int  sdv_map_set(sdv_ctx* c, int slot, int nH, const uint64_t* host_frames, const double* host_T7, const double* host_ab, int nP, const sdv_map_pt* pts);
+/* sdv_map_set for n slots: job j has the keyframes host_begin[j] .. host_begin[j+1] of host_frames / host_T7 / host_ab (may be NULL: every ab = (0, 0)) and
+ * the points pt_begin[j] .. pt_begin[j+1] of pts, whose `host` field indexes the job's own keyframes.  All-or-nothing: every check of sdv_map_set runs for
+ * every job, and a slot named twice or host_begin[0] / pt_begin[0] != 0 returns SDV_ERR_ARG, before any slot, pin or buffer changes.  Pins follow
+ * sdv_map_set.  The call waits for the device twice whatever n is: before it overwrites slots an earlier launch may read, and after its one upload. */
+int  sdv_map_set_batch(sdv_ctx* c, int n, const int32_t* slots, const int32_t* host_begin, const uint64_t* host_frames, const double* host_T7,
+                       const double* host_ab, const int32_t* pt_begin, const sdv_map_pt* pts);
 /* A resident map slot (and a resident BA window, below) REFERENCES the device images of its keyframes: while it does, sdv_frame_release /
  * re-uploading one of those handles returns SDV_ERR_STATE instead of handing the storage to another frame under the reader.  sdv_map_set on
  * the same slot replaces the references; sdv_map_clear drops them (the FrameHessian destructor path of a marginalised keyframe). */

@@ -130,9 +130,8 @@ int shim_makeK(int slot, CalibHessian* HCalib) { sdv_calib K{HCalib->fxl(), HCal
 // ------------------------------------------------------------------------------------------------ CoarseTracker (CoarseTracker.cpp:649-660, 662-838)
 struct CoarseTracker {
   int slot; FrameHessian* lastRef; int refFrameID; AffLight lastRef_aff_g2l; double firstCoarseRMSE; Vec5 lastResiduals; double lastFlowIndicators[3];
-  void setCoarseTrackingRef(std::vector<FrameHessian*> frameHessians) {
-    lastRef = frameHessians.back();
-    std::vector<float> pts; std::vector<int32_t> round_half;                  // the graph walk of makeCoarseDepthL0 :264-294 stays on the host
+  // the graph walk of makeCoarseDepthL0 :264-294 stays on the host: one row per splat, appended to pts / round_half
+  static void splat_rows(const std::vector<FrameHessian*>& frameHessians, std::vector<float>& pts, std::vector<int32_t>& round_half) {
     for (FrameHessian* fh : frameHessians) for (PointHessian* ph : fh->pointHessians) {
       if (fh == frameHessians.back() && ph->isFromSensor) {
         pts.insert(pts.end(), {ph->u, ph->v, ph->idepth, ph->efPoint->HdiF}); round_half.push_back(0);
@@ -141,6 +140,10 @@ struct CoarseTracker {
         pts.insert(pts.end(), {r->centerProjectedTo[0], r->centerProjectedTo[1], r->centerProjectedTo[2], ph->efPoint->HdiF}); round_half.push_back(1);
       }
     }
+  }
+  void setCoarseTrackingRef(std::vector<FrameHessian*> frameHessians) {
+    lastRef = frameHessians.back();
+    std::vector<float> pts; std::vector<int32_t> round_half; splat_rows(frameHessians, pts, round_half);
     sdv_tracker_set_ref(gpu, slot, (uint64_t)lastRef->shell->id, (int)round_half.size(), pts.data(), round_half.data(), 0.f, lastRef->aff_g2l().a, lastRef->aff_g2l().b);
     refFrameID = lastRef->shell->id; lastRef_aff_g2l = lastRef->aff_g2l(); firstCoarseRMSE = -1;
   }
@@ -192,12 +195,14 @@ struct FullSystem {
   }
 
   // FullSystem::makeKeyFrame: keep the map resident for the Reprojector (Reprojector.cpp:117-156) ...
-  int set_map(int slot) {
-    std::vector<sdv_map_pt> pts; std::vector<uint64_t> ids; std::vector<double> c2w, ab;
+  void map_rows(std::vector<uint64_t>& ids, std::vector<double>& c2w, std::vector<double>& ab, std::vector<sdv_map_pt>& pts) const {   // appended, host index job-local
     for (FrameHessian* fh : frameHessians) {
       ids.push_back((uint64_t)fh->shell->id); double T[7]; se3_to7(fh->shell->camToWorld, T); c2w.insert(c2w.end(), T, T + 7); ab.push_back(fh->aff_g2l().a); ab.push_back(fh->aff_g2l().b);
       for (PointHessian* ph : fh->pointHessians) pts.push_back(sdv_map_pt{ph->u, ph->v, ph->idepth, fh->idx, ph->type == PointHessian::EDGELET});
     }
+  }
+  int set_map(int slot) {
+    std::vector<sdv_map_pt> pts; std::vector<uint64_t> ids; std::vector<double> c2w, ab; map_rows(ids, c2w, ab, pts);
     return sdv_map_set(gpu, slot, (int)ids.size(), ids.data(), c2w.data(), ab.data(), (int)pts.size(), pts.data());
   }
   // ... and the hand-over after optimize(): flagPointsForRemoval / marginalizePointsF / marginalizeFrame (FullSystem.cpp:1152-1171)
@@ -406,6 +411,24 @@ Vec4 shim_initializer_frame1(FullSystem& fs, InitBranch& ib, FrameHessian* newFr
   return Vec4{{io.lastCoarseRMSE[0], io.flow[0], io.flow[1], io.flow[2]}};
 }
 
+// ------------------------------------------------------------------------------------------------ batched makeKeyFrame (INTEGRATION.md §4)
+// one context serving many FullSystems: each sequence that made a keyframe walks its own graph, then ONE call installs every tracker reference
+// (setCoarseTrackingRef of coarseTracker_forNewKF, slot ref_slot[i]) and ONE call every resident map (slot map_slot[i])
+int shim_makeKeyFrame_batch(const std::vector<FullSystem*>& fss, const std::vector<int32_t>& ref_slot, const std::vector<int32_t>& map_slot, std::vector<int32_t>& npts) {
+  const int n = (int)fss.size();
+  std::vector<float> pts; std::vector<int32_t> rh, pb{0}, hb{0}, mb{0}; std::vector<uint64_t> ref_ids, ids; std::vector<double> ref_ab, c2w, ab; std::vector<sdv_map_pt> mp;
+  for (FullSystem* fs : fss) {
+    CoarseTracker::splat_rows(fs->frameHessians, pts, rh); pb.push_back((int32_t)rh.size());
+    FrameHessian* ref = fs->frameHessians.back(); ref_ids.push_back((uint64_t)ref->shell->id); ref_ab.push_back(ref->aff_g2l().a); ref_ab.push_back(ref->aff_g2l().b);
+    fs->map_rows(ids, c2w, ab, mp); hb.push_back((int32_t)ids.size()); mb.push_back((int32_t)mp.size());
+  }
+  npts.assign((size_t)n*SDV_PYR_LEVELS, 0);
+  int rc = sdv_tracker_set_ref_batch(gpu, n, ref_slot.data(), ref_ids.data(), pb.data(), pts.data(), rh.data(), ref_ab.data(), npts.data());
+  if (rc == SDV_OK) rc = sdv_map_set_batch(gpu, n, map_slot.data(), hb.data(), ids.data(), c2w.data(), ab.data(), mb.data(), mp.data());
+  for (FullSystem* fs : fss) { FrameHessian* ref = fs->frameHessians.back(); CoarseTracker* t = fs->coarseTracker; t->lastRef = ref; t->refFrameID = ref->shell->id; t->lastRef_aff_g2l = ref->aff_g2l(); t->firstCoarseRMSE = -1; }
+  return rc;
+}
+
 // referenced so that -Wunused does not hide a missing call path
 int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const Undistort* u, const uint8_t* raw) {
   std::vector<int32_t> sel, st; Vec5 mr{}; SE3 T; AffLight a;
@@ -425,6 +448,7 @@ int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const 
     rc |= shim_activatePoints_store({(uint64_t)fh->shell->id}, {0}, ai, {}, cal6, rc2, idp2, rs2, cn2); }
   { RowsQueue q{{}, 0}; int32_t ni = 0; rc |= shim_lidarCloudHandler_rows(q, rig, (uint64_t)fh->shell->id, nullptr, 0) | shim_makeNewTraces_rows(fh, q, ni) | shim_process_pop(q); }
   { InitBranch ib{nullptr, 0}; int rci = 0; shim_setFirstFromLidar(ib, fh); shim_initializer_frame1(fs, ib, fh, rci); rc |= rci; }
+  { std::vector<FullSystem*> fss{&fs}; std::vector<int32_t> np; rc |= shim_makeKeyFrame_batch(fss, {0}, {0}, np); }
   fs.optimize(6); fs.set_map(0); fs.handover(sel, st); fs.trackNewCoarse(fh); fs.refine_only(fh); shim_frame_destructor(fh);
   return rc;
 }

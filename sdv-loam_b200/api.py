@@ -80,6 +80,8 @@ def _load():
     L.sdv_tracker_calc_gs.argtypes = [_vp, C.c_int, C.c_int, _f64p, _f64p]
     L.sdv_reproject_grid.argtypes = [_vp, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.sdv_map_set.argtypes = [_vp, C.c_int, C.c_int, _u64p, _f64p, _f64p, C.c_int, _vp]
+    L.sdv_tracker_set_ref_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _i32p, _f32p, _i32p, _vp, _i32p]
+    L.sdv_map_set_batch.argtypes = [_vp, C.c_int, _i32p, _i32p, _u64p, _f64p, _f64p, _i32p, _vp]
     L.sdv_reproject_map_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _f64p, _f64p, _i32p, _i32p, _i32p, _vp, C.c_int, _i32p, _i32p, _f64p]
     L.sdv_tracker_refine_batch.argtypes = [_vp, C.c_int, _i32p, _u64p, _f64p, _f64p, _vp, C.c_int, _i32p, _f32p, _i32p, _i32p]
     L.sdv_tracker_struct_pose_batch.argtypes = [_vp, C.c_int, _i32p, _vp, _i32p, _f64p, _f64p, _f32p, _i32p, _i32p]
@@ -355,6 +357,21 @@ class Context:
             self._ck(LIB.sdv_tracker_track_batch_levels(self.p, n, slots, ids, T, ab, None if co is None else co.ctypes.data, mr, lastRes, flow, good, sp))
         return dict(good=good.astype(bool), lastResiduals=lastRes, flow=flow, evals=stats["point_evals"], iterations=stats["iterations"], accepts=stats["accepts"])
 
+    def setCoarseTrackingRefBatch(self, slots, frame_ids, pts_list, round_half_list, ref_ab=None):
+        """CoarseTracker::setCoarseTrackingRef for n tracker slots in one call (sdv_tracker_set_ref_batch): slot slots[j] gets the reference frame frame_ids[j]
+        and the splat rows pts_list[j] ({u, v, idepth, HdiF}) with round_half_list[j]; ref_ab (n, 2) or None = (0, 0).  Returns the (n, levels) cloud sizes.
+        Over max_ref_points raises SdvError after installing every job that fits (see sdv_b200.h)."""
+        n = len(slots); sl = np.ascontiguousarray(slots, np.int32).reshape(-1); fr = np.ascontiguousarray(frame_ids, np.uint64).reshape(-1)
+        P = [np.ascontiguousarray(p, np.float32).reshape(-1, 4) for p in pts_list]; R = [np.ascontiguousarray(r, np.int32).reshape(-1) for r in round_half_list]
+        if not (len(sl) == len(fr) == len(P) == len(R) == n) or any(len(p) != len(r) for p, r in zip(P, R)):
+            raise ValueError("setCoarseTrackingRefBatch: one frame, one row array and one round_half array per slot, of equal lengths")
+        pb = np.ascontiguousarray(np.concatenate([[0], np.cumsum([len(p) for p in P], dtype=np.int64)]), np.int32)
+        p4 = np.ascontiguousarray(np.concatenate(P) if pb[-1] else np.zeros((1, 4)), np.float32); rh = np.ascontiguousarray(np.concatenate(R) if pb[-1] else np.zeros(1), np.int32)
+        ab = None if ref_ab is None else np.ascontiguousarray(ref_ab, np.float64).reshape(n, 2)
+        out = np.zeros((max(n, 1), PYR_LEVELS), np.int32)
+        self._ck(LIB.sdv_tracker_set_ref_batch(self.p, n, sl, fr, pb, p4, rh, None if ab is None else ab.ctypes.data, out))
+        return out[:n, :self.levels]
+
 
 class CoarseTracker:
     """Mirror of sdv_loam::CoarseTracker (FullSystem/CoarseTracker.h:16-133) bound to one tracker slot of a Context."""
@@ -468,6 +485,22 @@ class Reprojector:
         pts = np.ascontiguousarray(pts, MAP_PT_DTYPE); hT = np.ascontiguousarray(host_T7, np.float64).reshape(-1, 7)
         hab = np.zeros((len(hT), 2)) if host_ab is None else np.ascontiguousarray(host_ab, np.float64).reshape(-1, 2)
         self.ctx._ck(LIB.sdv_map_set(self.ctx.p, slot, len(hT), np.ascontiguousarray(host_frame_ids, np.uint64), hT, hab, len(pts), pts.ctypes.data if len(pts) else None))
+
+    def setMapBatch(self, slots, host_frame_ids_list, host_T7_list, host_ab_list, pts_list):
+        """setMap for n slots in one call (sdv_map_set_batch): job j has the keyframes host_frame_ids_list[j] with host_T7_list[j] and host_ab_list[j] (None: all
+        (0, 0); host_ab_list itself may be None) and the points pts_list[j] (MAP_PT_DTYPE, host indexing the job's keyframes).  All-or-nothing."""
+        n = len(slots); sl = np.ascontiguousarray(slots, np.int32).reshape(-1)
+        ids = [np.ascontiguousarray(f, np.uint64).reshape(-1) for f in host_frame_ids_list]; T = [np.ascontiguousarray(t, np.float64).reshape(-1, 7) for t in host_T7_list]
+        abl = [None] * n if host_ab_list is None else host_ab_list
+        AB = [np.zeros((len(t), 2)) if a is None else np.ascontiguousarray(a, np.float64).reshape(-1, 2) for a, t in zip(abl, T)]
+        P = [np.ascontiguousarray(p, MAP_PT_DTYPE).reshape(-1) for p in pts_list]
+        if not (len(sl) == len(ids) == len(T) == len(AB) == len(P) == n):
+            raise ValueError("setMapBatch: one keyframe list, pose list, ab list and point array per slot")
+        cum = lambda a: np.ascontiguousarray(np.concatenate([[0], np.cumsum([len(x) for x in a], dtype=np.int64)]), np.int32)
+        hb, pb = cum(ids), cum(P)
+        cat = lambda a, empty: np.ascontiguousarray(np.concatenate(a) if sum(len(x) for x in a) else empty)
+        pts = cat(P, np.zeros(1, MAP_PT_DTYPE))
+        self.ctx._ck(LIB.sdv_map_set_batch(self.ctx.p, n, sl, hb, cat(ids, np.zeros(1, np.uint64)), cat(T, np.zeros((1, 7))), cat(AB, np.zeros((1, 2))), pb, pts.ctypes.data))
 
     def reprojectMapBatch(self, slots, cur_frame_ids, cur_T7, cur_ab=None, cur_kf_index=None, only_host=None, backup=None, cell_order=None, max_matches=400):
         n = len(slots); i32 = lambda a, d: np.full(n, d, np.int32) if a is None else np.ascontiguousarray(a, np.int32)

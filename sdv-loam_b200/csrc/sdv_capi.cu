@@ -191,16 +191,6 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
   CK(cudaMalloc(&c->ticket, sizeof(unsigned int))); CK(cudaMemset(c->ticket, 0, sizeof(unsigned int)));
   CK(cudaMalloc(&c->totals_dev, kNAcc*sizeof(double)));
   CK(cudaMallocHost(&c->totals_host, kNAcc*sizeof(double)));
-  // coarse-depth work buffers
-  for (int l=0;l<levels;l++) {
-    size_t n = (size_t)(w>>l)*(h>>l);
-    CK(cudaMalloc(&c->cd_id[l], n*sizeof(float))); CK(cudaMalloc(&c->cd_ws[l], n*sizeof(float)));
-    CK(cudaMalloc(&c->cd_id2[l], n*sizeof(float))); CK(cudaMalloc(&c->cd_ws2[l], n*sizeof(float)));
-  }
-  CK(cudaMalloc(&c->cd_owner, (size_t)w*h*sizeof(int)));
-  CK(cudaMalloc(&c->cd_counts, (size_t)(cd_num_blocks(w,h)+1)*sizeof(int)));
-  CK(cudaMalloc(&c->cd_scalars, 8*sizeof(int)));
-  CK(cudaMallocHost(&c->cd_scalars_host, 8*sizeof(int)));
   c->last_ms = 0;
   return SDV_OK;
 }
@@ -212,8 +202,6 @@ void sdv_destroy(sdv_ctx* c) {
   for (auto& f : c->frames) { cudaFree(f.base); cudaFree(f.pyr); cudaFree(f.I0_own); }
   for (auto p : c->lvl0_pool) cudaFree(p);
   for (auto& t : c->slots) for (int l=0;l<c->levels;l++) cudaFree(t.pts[l]);
-  for (int l=0;l<c->levels;l++) { cudaFree(c->cd_id[l]); cudaFree(c->cd_ws[l]); cudaFree(c->cd_id2[l]); cudaFree(c->cd_ws2[l]); }
-  cudaFree(c->cd_owner); cudaFree(c->cd_counts); cudaFree(c->cd_scalars); cudaFreeHost(c->cd_scalars_host);
   for (int i=0;i<2;i++) { c->ing_dev[i].release(); c->ing_host[i].release(); } cudaFree(c->partials); cudaFree(c->ticket); cudaFree(c->totals_dev); cudaFreeHost(c->totals_host);
   cudaFree(c->tc_dev); cudaFree(c->geom_dev); c->scr.release(); c->scr_host.release();
   for (float* u : c->und_buf) cudaFree(u);
@@ -487,66 +475,43 @@ int sdv_tracker_get_cloud(sdv_ctx* c, int slot, int lvl, int* n_out, float* u, f
   return SDV_OK;
 }
 
-int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const float* pts4, const int32_t* round_half,
-                        float /*unused*/, double ref_a, double ref_b) { SDV_GUARD_TRK(c);
-  if (!c || slot < 0 || slot >= (int)c->slots.size() || n < 0 || (n > 0 && (!pts4 || !round_half))) return SDV_ERR_ARG;
-  CK(cudaSetDevice(c->device));
-  TrackerSlot& t = c->slots[slot];
-  FrameDev* f; { int rc = job_frame(c, "sdv_tracker_set_ref", 0, ref_frame, -1, slot, nullptr, &f); if (rc) return rc; }
-  const int w = c->cam_w[t.cam], h = c->cam_h[t.cam];               // makeCoarseDepthL0 at the slot's size, for its camera's pyrLevelsUsed levels
-  for (int i=0;i<n;i++) {                                   // the reference would write out of bounds here; we refuse instead
-    int u = round_half[i] ? (int)(pts4[4*i]+0.5f) : (int)pts4[4*i], v = round_half[i] ? (int)(pts4[4*i+1]+0.5f) : (int)pts4[4*i+1];
-    if (u < 0 || v < 0 || u >= w || v >= h) return ctx_fail(c, SDV_ERR_ARG, "splat %d (%d,%d) outside the image", i, u, v);
-  }
-  Scratch& S = c->scr;
-  if (S.reserve(Scratch::need(4*(size_t)n, sizeof(float)) + 2*Scratch::need(n, sizeof(int)) + Scratch::need(n, sizeof(float4)), c->st))
-    return ctx_fail(c, SDV_ERR_CUDA, "sdv_tracker_set_ref: scratch of %d splats", n);
-  S.reset(); float* pts4_d = S.take<float>(4*(size_t)n); int* round_d = S.take<int>(n); float4* splats = S.take<float4>(n); int* done = S.take<int>(n);
-  { int rcj = join_ingest(c); if (rcj) return rcj; }
-  if (n > 0) {
-    CK(cudaMemcpyAsync(pts4_d, pts4, (size_t)4*n*sizeof(float), cudaMemcpyHostToDevice, c->st));
-    CK(cudaMemcpyAsync(round_d, round_half, (size_t)n*sizeof(int), cudaMemcpyHostToDevice, c->st));
-  }
-  return tracker_set_ref_dev(c, slot, f, ref_frame, n, pts4_d, round_d, splats, done, ref_a, ref_b, nullptr);
-}
-}  // extern "C"
-
-namespace sdv {
-int tracker_set_ref_dev(sdv_ctx* c, int slot, FrameDev* f, uint64_t ref_frame, int n, const float* pts4_d, const int* round_d, float4* splats, int* done, double ref_a, double ref_b,
-                        int* launches) {
-  TrackerSlot& t = c->slots[slot];
-  const int w = c->cam_w[t.cam], h = c->cam_h[t.cam], L = c->cam_levels[t.cam];
-  CK(cudaMemsetAsync(c->cd_id[0], 0, (size_t)w*h*sizeof(float), c->st));
-  CK(cudaMemsetAsync(c->cd_ws[0], 0, (size_t)w*h*sizeof(float), c->st));
-  if (n > 0) {
-    launch_cd_prep(pts4_d, round_d, n, w, splats, done, c->st); if (launches) *launches += 1;
-    for (int round = 0; round < n; round++) {               // usually 1-3 rounds: one per multiplicity of colliding splats; at most n (every splat on one pixel)
-      CK(cudaMemsetAsync(c->cd_scalars, 0, sizeof(int), c->st));
-      launch_cd_round(splats, n, done, c->cd_owner, c->cd_id[0], c->cd_ws[0], c->cd_scalars, c->st); if (launches) *launches += 1;
-      CK(cudaMemcpyAsync(c->cd_scalars_host, c->cd_scalars, sizeof(int), cudaMemcpyDeviceToHost, c->st));
-      CK(cudaStreamSynchronize(c->st));
-      if (c->cd_scalars_host[0] == 0) break;
+// CoarseTracker::setCoarseTrackingRef for n slots: every check runs before anything is enqueued, then one build (set_ref_build) serves all jobs
+int sdv_tracker_set_ref_batch(sdv_ctx* c, int n, const int32_t* slots, const uint64_t* ref_frames, const int32_t* pt_begin, const float* pts4, const int32_t* round_half,
+                              const double* ref_ab, int32_t* npts_out) { SDV_GUARD_TRK(c);
+  const char* who = "sdv_tracker_set_ref_batch";
+  if (!c || n < 0 || (n > 0 && (!slots || !ref_frames || !pt_begin))) return SDV_ERR_ARG;
+  if (n == 0) return SDV_OK;
+  if (pt_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "%s: pt_begin[0] must be 0", who);
+  for (int j = 0; j < n; j++) if (pt_begin[j+1] < pt_begin[j]) return ctx_fail(c, SDV_ERR_ARG, "%s: pt_begin decreases at job %d", who, j);
+  if (pt_begin[n] > 0 && (!pts4 || !round_half)) return SDV_ERR_ARG;
+  const int ns = (int)c->slots.size(); std::vector<char> seen(ns, 0); std::vector<FrameDev*> F(n);
+  for (int j = 0; j < n; j++) {
+    if (slots[j] < 0 || slots[j] >= ns) return ctx_fail(c, SDV_ERR_ARG, "%s: job %d names slot %d of %d", who, j, slots[j], ns);
+    if (seen[slots[j]]) return ctx_fail(c, SDV_ERR_ARG, "%s: slot %d appears twice in one batch", who, slots[j]);
+    seen[slots[j]] = 1;
+    { int rc = job_frame(c, who, j, ref_frames[j], -1, slots[j], nullptr, &F[j]); if (rc) return rc; }
+    const int cam = c->slots[slots[j]].cam, w = c->cam_w[cam], h = c->cam_h[cam];        // makeCoarseDepthL0 at the slot's size
+    for (int i = pt_begin[j]; i < pt_begin[j+1]; i++) {                                   // the reference would write out of bounds here; we refuse instead
+      const int u = round_half[i] ? (int)(pts4[4*i]+0.5f) : (int)pts4[4*i], v = round_half[i] ? (int)(pts4[4*i+1]+0.5f) : (int)pts4[4*i+1];
+      if (u < 0 || v < 0 || u >= w || v >= h) return ctx_fail(c, SDV_ERR_ARG, "%s: job %d, row %d: splat (%d,%d) outside the %dx%d image", who, j, i - pt_begin[j], u, v, w, h);
     }
   }
-  for (int l=1;l<L;l++) launch_cd_pool(c->cd_id[l-1], c->cd_ws[l-1], c->cd_id[l], c->cd_ws[l], w>>l, h>>l, w>>(l-1), c->st);
-  for (int l=0;l<L;l++) {
-    launch_cd_dilate(c->cd_id[l], c->cd_ws[l], c->cd_id2[l], c->cd_ws2[l], w>>l, h>>l, l < 2 ? 1 : 0, c->st);
-    launch_cd_compact(c->cd_id2[l], c->cd_ws2[l], f->img[l], w>>l, h>>l, c->cd_counts, c->cd_scalars + 1 + l, t.pts[l], t.cap[l], c->st);
-  }
-  if (launches) *launches += 3*L - 1;
-  CK(cudaMemcpyAsync(c->cd_scalars_host, c->cd_scalars, 8*sizeof(int), cudaMemcpyDeviceToHost, c->st));
-  CK(cudaStreamSynchronize(c->st));
-  CK(cudaGetLastError());
-  for (int l=0;l<L;l++) if (c->cd_scalars_host[1+l] > t.cap[l]) {
-    // the emit kernel never wrote past cap[l], but the slot's clouds are now a truncated mix: invalidate the slot instead of leaving it half-updated
-    t.ref_frame = ~0ull; t.has_totals = false; for (int k=0;k<c->levels;k++) t.npts[k] = 0;
-    return ctx_fail(c, SDV_ERR_CAPACITY, "level %d cloud (%d) exceeds capacity %d (max_ref_points); slot %d has no reference now", l, c->cd_scalars_host[1+l], t.cap[l], slot);
-  }
-  for (int l=0;l<c->levels;l++) t.npts[l] = l < L ? c->cd_scalars_host[1+l] : 0;       // levels past the camera's depth are never read
-  t.ref_frame = ref_frame; t.ref_a = ref_a; t.ref_b = ref_b; t.refExposure = f->exposure; t.has_totals = false;
-  return SDV_OK;
+  CK(cudaSetDevice(c->device));
+  int launches = 0;
+  CK(cudaEventRecord(c->ev0, c->st));
+  const int rc = set_ref_build(c, n, slots, F.data(), ref_frames, pt_begin, pts4, round_half, cudaMemcpyHostToDevice, ref_ab, npts_out, &launches);
+  c->launches += launches;
+  if (rc && rc != SDV_ERR_CAPACITY) return rc;
+  CK(cudaEventRecord(c->ev1, c->st)); CK(cudaEventSynchronize(c->ev1)); CK(cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
+  return rc;
 }
-}  // namespace sdv
+int sdv_tracker_set_ref(sdv_ctx* c, int slot, uint64_t ref_frame, int n, const float* pts4, const int32_t* round_half,
+                        float /*unused*/, double ref_a, double ref_b) {
+  if (!c || n < 0 || (n > 0 && (!pts4 || !round_half))) return SDV_ERR_ARG;
+  const int32_t s = slot, pb[2] = {0, n}; const double ab[2] = {ref_a, ref_b};
+  return sdv_tracker_set_ref_batch(c, 1, &s, &ref_frame, pb, pts4, round_half, ab, nullptr);
+}
+}  // extern "C"
 extern "C" {
 
 // ------------------------------------------------------------------------------------------------ calcRes / calcGSSSE

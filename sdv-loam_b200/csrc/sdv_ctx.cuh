@@ -69,8 +69,6 @@ struct sdv_ctx {
   std::vector<void*> cp_dst, cp_src; std::vector<size_t> cp_sz; bool no_batch_copy = false;
   std::vector<sdv::TrackerSlot> slots;
   double* partials; unsigned int* ticket; double* totals_dev; double* totals_host;
-  float *cd_id[sdv::kLevels], *cd_ws[sdv::kLevels], *cd_id2[sdv::kLevels], *cd_ws2[sdv::kLevels];
-  int* cd_owner; int* cd_counts; int* cd_scalars; int* cd_scalars_host;
   float last_ms;
   // per-call scratch of the tracker stream st (splats, tracker jobs, refine, Reprojector, immature points); valid until the next call that takes from it
   sdv::Scratch scr; sdv::PinnedScratch scr_host;
@@ -109,12 +107,15 @@ int  imm_store_deposit(sdv_ctx* c, int nj, const uint64_t* hosts, const int* n, 
 struct InitPointsJob { const double* cloud; const unsigned char* map; const int32_t* draws; const float* I0; int n, w, h; float desired;
                        sdv_immature_pt* pts; sdv_immature_meta* meta; float* idepth; float* splat4; int* round; sdv_map_pt* mp; int* counts; };
 int  launch_init_points(sdv_ctx* c, int nj, const InitPointsJob* jobs_dev);
-// the half of sdv_tracker_set_ref after the upload: splat rounds, pool, dilate, compact and the capacity rule from n device splat rows pts4_d / round_d
-// (splats / done: device scratch of n float4 / ints); f is the reference frame, already checked against the slot.  *launches (may be NULL) grows by the kernels it ran.
-int  tracker_set_ref_dev(sdv_ctx* c, int slot, FrameDev* f, uint64_t ref_frame, int n, const float* pts4_d, const int* round_d, float4* splats, int* done, double ref_a, double ref_b,
-                         int* launches);
-// sdv_map_set with its points already in memory of kind `kind` (cudaMemcpyHostToDevice: host rows, cudaMemcpyDeviceToDevice: device rows)
-int  map_set_impl(sdv_ctx* c, int slot, int nH, const uint64_t* host_frames, const double* host_T7, const double* host_ab, int nP, const sdv_map_pt* pts, cudaMemcpyKind kind);
+// sdv_tracker_set_ref_batch after its checks (sdv_coarse_depth.cu): makeCoarseDepthL0 of nj jobs and the install with the capacity rule.  Job j is slot
+// slots[j] (distinct, in range) with reference frame F[j] = ref_frames[j] (checked against the slot) and the splat rows pt_begin[j] .. pt_begin[j+1] of
+// pts4 / round_half, in memory of kind `kind` (cudaMemcpyHostToDevice: host rows inside their slot camera's image, cudaMemcpyDeviceToDevice: device rows).
+// ref_ab (2 nj) and npts_out (nj x SDV_PYR_LEVELS) may be NULL.  Waits for the device once; *launches (may be NULL) grows by the kernels it ran.
+int  set_ref_build(sdv_ctx* c, int nj, const int32_t* slots, FrameDev* const* F, const uint64_t* ref_frames, const int32_t* pt_begin, const float* pts4,
+                   const int32_t* round_half, cudaMemcpyKind kind, const double* ref_ab, int32_t* npts_out, int* launches);
+// sdv_map_set_batch with its points already in memory of kind `kind` (cudaMemcpyHostToDevice: host rows, cudaMemcpyDeviceToDevice: device rows)
+int  map_set_impl(sdv_ctx* c, int n, const int32_t* slots, const int32_t* host_begin, const uint64_t* host_frames, const double* host_T7, const double* host_ab,
+                  const int32_t* pt_begin, const sdv_map_pt* pts, cudaMemcpyKind kind);
 int  sel_activate_select(sdv_ctx* c, int n, const int32_t* host_begin, const int32_t* pt_begin, const float* KRKi9, const float* Kt3, const float* uvid,
                          const int32_t* cand_host_begin, const int32_t* cand_begin, const float* cKRKi9, const float* cKt3, const float* cand4, const float* cand4_dev,
                          const float* min_act_dist, const int32_t* cams, int32_t* decision_out, float* dist_map_out);

@@ -4,7 +4,7 @@
 //   coarse_res_gs_kernel                   CoarseTracker::calcRes + calcGSSSE  CoarseTracker.cpp:486-634, 427-484 (one fused pass)
 //   track_cluster_kernel                   CoarseTracker::trackNewestCoarse    CoarseTracker.cpp:662-838 (whole coarse-to-fine LM
 //                                          device-resident: one thread-block cluster per call, DSMEM all-reduce, per-CTA redundant solve)
-//   cd_* kernels                           CoarseTracker::makeCoarseDepthL0    CoarseTracker.cpp:258-425
+//   (CoarseTracker::makeCoarseDepthL0, CoarseTracker.cpp:258-425, is sdv_coarse_depth.cu)
 #include "sdv_kernels.cuh"
 #include "sdv_warp_solve.cuh"
 #include <cooperative_groups.h>
@@ -751,134 +751,6 @@ void launch_h2d_words(void* dst_dev, const void* src_pinned, size_t bytes, cudaS
   const size_t n16 = (bytes + 15)/16; if (!n16) return;
   int blocks = (int)((n16 + 255)/256); if (blocks > num_sms()*2) blocks = num_sms()*2;
   h2d_words_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<uint4*>(dst_dev), reinterpret_cast<const uint4*>(src_pinned), n16);
-}
-
-// ================================================================================================ makeCoarseDepthL0
-// (a) splat in POINT ORDER per pixel: round r adds, for every pixel, the not-yet-added point of lowest index, which
-//     reproduces the reference's sequential float `+=` order bit-for-bit even for colliding points (CoarseTracker.cpp:264-294).
-__global__ void cd_owner_kernel(const float4* __restrict__ splats /*{pix as int bits, idepth*w, w, 0}*/, int n, const int* __restrict__ done, int* owner) {
-  int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= n || done[i]) return;
-  atomicMin(owner + __float_as_int(splats[i].x), i);
-}
-__global__ void cd_apply_kernel(const float4* __restrict__ splats, int n, int* done, int* owner, float* idepth, float* weightSums, int* remaining) {
-  int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= n || done[i]) return;
-  int pix = __float_as_int(splats[i].x);
-  if (owner[pix] == i) { idepth[pix] += splats[i].y; weightSums[pix] += splats[i].z; done[i] = 1; }
-  else atomicAdd(remaining, 1);
-}
-__global__ void cd_reset_owner_kernel(const float4* __restrict__ splats, int n, int* owner) {
-  int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= n) return;
-  owner[__float_as_int(splats[i].x)] = 0x7fffffff;
-}
-__global__ void cd_prep_kernel(const float* __restrict__ pts4, const int* __restrict__ round_half, int n, int w, float4* splats, int* done) {
-  int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= n) return;
-  float pu = pts4[4*i], pv = pts4[4*i+1], id = pts4[4*i+2], HdiF = pts4[4*i+3];
-  int u = round_half[i] ? (int)(pu + 0.5f) : (int)pu;
-  int v = round_half[i] ? (int)(pv + 0.5f) : (int)pv;
-  float weight = sqrtf((float)(1e-3 / ((double)HdiF + 1e-12)));      // sqrtf(1e-3 / (HdiF+1e-12)) — double division, float sqrt (:273)
-  splats[i] = make_float4(__int_as_float(u + w*v), id*weight, weight, 0.f);
-  done[i] = 0;
-}
-// (b) sum-pool to the next level (:296-322)
-__global__ void cd_pool_kernel(const float* __restrict__ id_lm, const float* __restrict__ ws_lm, float* id_l, float* ws_l, int wl, int hl, int wlm1) {
-  int idx = blockIdx.x*blockDim.x + threadIdx.x; if (idx >= wl*hl) return;
-  int y = idx / wl, x = idx - y*wl; int bidx = 2*x + 2*y*wlm1;
-  id_l[idx] = ((id_lm[bidx] + id_lm[bidx+1]) + id_lm[bidx+wlm1]) + id_lm[bidx+wlm1+1];
-  ws_l[idx] = ((ws_lm[bidx] + ws_lm[bidx+1]) + ws_lm[bidx+wlm1]) + ws_lm[bidx+wlm1+1];
-}
-// (c) 1-px dilation into empty cells, reading the pre-dilation weights (:324-375).  diag=1: 4 diagonal neighbours (levels 0,1),
-//     diag=0: 4 axis neighbours.  The reference updates idepth in place but only ever reads cells with bak>0 and writes cells
-//     with bak<=0, so reading the un-dilated idepth array is equivalent.
-__global__ void cd_dilate_kernel(const float* __restrict__ id_in, const float* __restrict__ bak, float* id_out, float* ws_out, int w, int h, int diag) {
-  int i = blockIdx.x*blockDim.x + threadIdx.x; int n = w*h; if (i >= n) return;
-  float idv = id_in[i], wsv = bak[i];
-  if (i >= w && i < n - w && bak[i] <= 0) {
-    int o0, o1, o2, o3;
-    if (diag) { o0 = 1+w; o1 = -1-w; o2 = w-1; o3 = -w+1; } else { o0 = 1; o1 = -1; o2 = w; o3 = -w; }
-    float sum = 0, num = 0, numn = 0;
-    // The reference reads one element past either end of the array for the first / last pixel of the loop (i = w: i-1-w = -1; i = n-w-1: i+1+w = n) —
-    // undefined there; here such a neighbour counts as empty.  Both pixels lie in the 2 px border that the cloud emission drops, so no output depends on it.
-#define CD_NB(o) { const int j = i + (o); if (j >= 0 && j < n && bak[j] > 0) { sum += id_in[j]; num += bak[j]; numn++; } }
-    CD_NB(o0) CD_NB(o1) CD_NB(o2) CD_NB(o3)
-#undef CD_NB
-    if (numn > 0) { idv = sum/numn; wsv = num/numn; }
-  }
-  id_out[i] = idv; ws_out[i] = wsv;
-}
-// (d) normalise + raster-order compaction (:378-423): block counts -> exclusive scan -> scatter
-constexpr int kScanThreads = 256, kScanItems = 4;            // 1024 pixels per block, contiguous per thread
-__device__ __forceinline__ bool cd_valid(const float* id, const float* ws, const float* ref, int i, int w, int h, float& idn, float& col) {
-  int y = i / w, x = i - y*w;
-  if (x < 2 || x >= w-2 || y < 2 || y >= h-2) return false;
-  if (!(ws[i] > 0)) return false;
-  idn = id[i] / ws[i]; col = ref[i];
-  return isfinite(col) && (idn > 0);
-}
-__global__ void __launch_bounds__(kScanThreads) cd_count_kernel(const float* __restrict__ id, const float* __restrict__ ws, const float* __restrict__ ref, int w, int h, int* blockCounts) {
-  __shared__ int s[kScanThreads/32];
-  int base = (blockIdx.x*kScanThreads + threadIdx.x)*kScanItems; int c = 0, n = w*h;
-  for (int j = 0; j < kScanItems; j++) { int i = base + j; float a, b; if (i < n && cd_valid(id, ws, ref, i, w, h, a, b)) c++; }
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) { int t = 0; for (int k = 0; k < kScanThreads/32; k++) t += s[k]; blockCounts[blockIdx.x] = t; }
-}
-__global__ void cd_scan_kernel(int* blockCounts, int nblocks, int* total) {   // single block exclusive scan (nblocks <= a few thousand)
-  __shared__ int carry;
-  __shared__ int sh[1024];
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (int base = 0; base < nblocks; base += 1024) {
-    int i = base + threadIdx.x; int v = (i < nblocks) ? blockCounts[i] : 0;
-    sh[threadIdx.x] = v; __syncthreads();
-    for (int o = 1; o < 1024; o <<= 1) { int t = (threadIdx.x >= o) ? sh[threadIdx.x - o] : 0; __syncthreads(); sh[threadIdx.x] += t; __syncthreads(); }
-    int incl = sh[threadIdx.x]; int c = carry;
-    if (i < nblocks) blockCounts[i] = c + incl - v;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry = c + incl;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *total = carry;
-}
-__global__ void __launch_bounds__(kScanThreads) cd_emit_kernel(const float* __restrict__ id, const float* __restrict__ ws, const float* __restrict__ ref, int w, int h,
-                                                              const int* __restrict__ blockOffsets, float4* out, int cap) {
-  __shared__ int s[kScanThreads/32];
-  int base = (blockIdx.x*kScanThreads + threadIdx.x)*kScanItems; int n = w*h;
-  float idn[kScanItems], col[kScanItems]; bool ok[kScanItems]; int c = 0;
-  for (int j = 0; j < kScanItems; j++) { int i = base + j; ok[j] = (i < n) && cd_valid(id, ws, ref, i, w, h, idn[j], col[j]); c += ok[j]; }
-  int lane = threadIdx.x & 31, warp = threadIdx.x >> 5; int incl = c;
-  for (int o = 1; o < 32; o <<= 1) { int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-  if (lane == 31) s[warp] = incl;
-  __syncthreads();
-  int woff = 0; for (int k = 0; k < warp; k++) woff += s[k];
-  int pos = blockOffsets[blockIdx.x] + woff + incl - c;
-  // cap = capacity of `out` (max_ref_points may make it smaller than the cloud): never write past it — the host compares the scanned total with cap afterwards
-  for (int j = 0; j < kScanItems; j++) if (ok[j]) { int i = base + j; int y = i / w, x = i - y*w; if (pos < cap) out[pos] = make_float4((float)x, (float)y, idn[j], col[j]); pos++; }
-}
-
-int cd_num_blocks(int w, int h) { return (w*h + kScanThreads*kScanItems - 1)/(kScanThreads*kScanItems); }
-
-void launch_cd_prep(const float* pts4, const int* round_half, int n, int w, float4* splats, int* done, cudaStream_t st) {
-  if (n > 0) cd_prep_kernel<<<(n+255)/256, 256, 0, st>>>(pts4, round_half, n, w, splats, done);
-}
-void launch_cd_round(const float4* splats, int n, int* done, int* owner, float* idepth, float* ws, int* remaining, cudaStream_t st) {
-  if (n <= 0) return;
-  int g = (n+255)/256;
-  cd_reset_owner_kernel<<<g, 256, 0, st>>>(splats, n, owner);
-  cd_owner_kernel<<<g, 256, 0, st>>>(splats, n, done, owner);
-  cd_apply_kernel<<<g, 256, 0, st>>>(splats, n, done, owner, idepth, ws, remaining);
-}
-void launch_cd_pool(const float* id_lm, const float* ws_lm, float* id_l, float* ws_l, int wl, int hl, int wlm1, cudaStream_t st) {
-  cd_pool_kernel<<<(wl*hl+255)/256, 256, 0, st>>>(id_lm, ws_lm, id_l, ws_l, wl, hl, wlm1);
-}
-void launch_cd_dilate(const float* id_in, const float* bak, float* id_out, float* ws_out, int w, int h, int diag, cudaStream_t st) {
-  cd_dilate_kernel<<<(w*h+255)/256, 256, 0, st>>>(id_in, bak, id_out, ws_out, w, h, diag);
-}
-void launch_cd_compact(const float* id, const float* ws, const float* ref, int w, int h, int* blockCounts, int* total, float4* out, int cap, cudaStream_t st) {
-  int nb = cd_num_blocks(w, h);
-  cd_count_kernel<<<nb, kScanThreads, 0, st>>>(id, ws, ref, w, h, blockCounts);
-  cd_scan_kernel<<<1, 1024, 0, st>>>(blockCounts, nb, total);
-  cd_emit_kernel<<<nb, kScanThreads, 0, st>>>(id, ws, ref, w, h, blockCounts, out, cap);
 }
 
 __global__ void pack_cloud_kernel(const float* u, const float* v, const float* id, const float* col, int n, float4* out) {

@@ -31,13 +31,6 @@ void launch_coarse_res_gs(const float4* pts, int n, const float* I, const LevelG
 void launch_h2d_words(void* dst_dev, const void* src_pinned, size_t bytes, cudaStream_t st);
 cudaError_t launch_track_cluster(TrackJob* jobs_dev, int njobs, const TrackConst* tc_dev, const GeomRow* geom_dev, int cluster_size, int threads, cudaStream_t st);
 
-// makeCoarseDepthL0 (CoarseTracker.cpp:258-425)
-int  cd_num_blocks(int w, int h);
-void launch_cd_prep(const float* pts4, const int* round_half, int n, int w, float4* splats, int* done, cudaStream_t st);
-void launch_cd_round(const float4* splats, int n, int* done, int* owner, float* idepth, float* ws, int* remaining, cudaStream_t st);
-void launch_cd_pool(const float* id_lm, const float* ws_lm, float* id_l, float* ws_l, int wl, int hl, int wlm1, cudaStream_t st);
-void launch_cd_dilate(const float* id_in, const float* bak, float* id_out, float* ws_out, int w, int h, int diag, cudaStream_t st);
-void launch_cd_compact(const float* id, const float* ws, const float* ref, int w, int h, int* blockCounts, int* total, float4* out, int cap, cudaStream_t st);
 void launch_pack_cloud(const float* u, const float* v, const float* id, const float* col, int n, float4* out, cudaStream_t st);
 
 } // namespace sdv

@@ -345,30 +345,79 @@ int sdv_reproject_grid(sdv_ctx* c, int* n_cols, int* n_rows) { SDV_GUARD_TRK(c);
 }
 
 int sdv_map_set(sdv_ctx* c, int slot, int nH, const uint64_t* host_frames, const double* host_T7, const double* host_ab, int nP, const sdv_map_pt* pts) { SDV_GUARD_TRK(c);
-  return map_set_impl(c, slot, nH, host_frames, host_T7, host_ab, nP, pts, cudaMemcpyHostToDevice);
+  if (nH < 0 || nP < 0) return SDV_ERR_ARG;
+  const int32_t hb[2] = {0, nH}, pb[2] = {0, nP};
+  return map_set_impl(c, 1, &slot, hb, host_frames, host_T7, host_ab, pb, pts, cudaMemcpyHostToDevice);
+}
+int sdv_map_set_batch(sdv_ctx* c, int n, const int32_t* slots, const int32_t* host_begin, const uint64_t* host_frames, const double* host_T7,
+                      const double* host_ab, const int32_t* pt_begin, const sdv_map_pt* pts) { SDV_GUARD_TRK(c);
+  if (!c || n < 0 || (n > 0 && (!slots || !host_begin || !pt_begin))) return SDV_ERR_ARG;
+  if (n == 0) return SDV_OK;
+  if (host_begin[0] != 0 || pt_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "sdv_map_set_batch: host_begin[0] and pt_begin[0] must be 0");
+  return map_set_impl(c, n, slots, host_begin, host_frames, host_T7, host_ab, pt_begin, pts, cudaMemcpyHostToDevice);
 }
 }  // extern "C"
-int sdv::map_set_impl(sdv_ctx* c, int slot, int nH, const uint64_t* host_frames, const double* host_T7, const double* host_ab, int nP, const sdv_map_pt* pts, cudaMemcpyKind kind) {
-  if (!c || nH < 1 || nH > kRpMaxHosts || !host_frames || !host_T7 || nP < 0 || nP >= (1 << 27) || (nP > 0 && !pts)) return SDV_ERR_ARG;   // point index packs into 27 bits of the sort key
+namespace sdv {
+// the single staged upload of sdv_map_set_batch: segment k copies words[k] 4-byte words from src[k] to dst[k]; blockIdx.y strides over the segments
+struct MapCopySeg { const uint32_t* src; uint32_t* dst; size_t words; };
+__global__ void map_copy_kernel(const MapCopySeg* __restrict__ seg, int nseg) {
+  for (int k = blockIdx.y; k < nseg; k += gridDim.y) { const MapCopySeg q = seg[k];
+    for (size_t i = (size_t)blockIdx.x*blockDim.x + threadIdx.x; i < q.words; i += (size_t)gridDim.x*blockDim.x) q.dst[i] = q.src[i]; }
+}
+}
+int sdv::map_set_impl(sdv_ctx* c, int n, const int32_t* slots, const int32_t* host_begin, const uint64_t* host_frames, const double* host_T7, const double* host_ab,
+                      const int32_t* pt_begin, const sdv_map_pt* pts, cudaMemcpyKind kind) {
+  if (!c) return SDV_ERR_ARG;
   CK(cudaSetDevice(c->device)); RpState* st = rp_state(c);
-  if (slot < 0 || slot >= (int)st->maps.size()) return SDV_ERR_ARG;
-  MapSlot& m = st->maps[slot];
-  if (!m.dev) CK(cudaMalloc(&m.dev, sizeof(MapDev)));
-  if (nP > m.cap) { cudaFree(m.pts); m.pts = nullptr; m.cap = nP + nP/4 + 256; CK(cudaMalloc(&m.pts, (size_t)m.cap*sizeof(sdv_map_pt))); }
+  // every check of every job before any slot, pin or buffer changes
+  for (int j = 0; j < n; j++) if (host_begin[j+1] <= host_begin[j] || pt_begin[j+1] < pt_begin[j]) return SDV_ERR_ARG;
+  std::vector<char> seen(st->maps.size(), 0); std::vector<FrameDev*> F((size_t)host_begin[n]); long long need_seq = 0; size_t maxP = 0, totP = 0;
+  for (int j = 0; j < n; j++) {
+    const int nH = host_begin[j+1] - host_begin[j], nP = pt_begin[j+1] - pt_begin[j];
+    if (nH < 1 || nH > kRpMaxHosts || !host_frames || !host_T7 || nP < 0 || nP >= (1 << 27) || (nP > 0 && !pts)) return SDV_ERR_ARG;   // point index packs into 27 bits of the sort key
+    if (slots[j] < 0 || slots[j] >= (int)st->maps.size()) return SDV_ERR_ARG;
+    if (seen[slots[j]]) return ctx_fail(c, SDV_ERR_ARG, "sdv_map_set_batch: slot %d appears twice in one batch", slots[j]);
+    seen[slots[j]] = 1;
+    for (int k = host_begin[j]; k < host_begin[j+1]; k++) { int rcs = job_frame(c, "sdv_map_set", k - host_begin[j], host_frames[k], -1, slots[j], &need_seq, &F[k]); if (rcs) return rcs; }
+    maxP = std::max(maxP, (size_t)nP); totP += nP;
+  }
   { int rcj = join_ingest(c); if (rcj) return rcj; }
-  FrameDev* F[kRpMaxHosts]; long long need_seq = 0;
-  for (int k=0;k<nH;k++) { int rcs = job_frame(c, "sdv_map_set", k, host_frames[k], -1, slot, &need_seq, &F[k]); if (rcs) return rcs; }
-  if (m.set) for (int k=0;k<m.nH;k++) frame_unpin(c, m.host_ids[k]);       // the slot's previous keyframes are no longer referenced by it
-  for (int k=0;k<nH;k++) frame_pin(c, host_frames[k]);
-  MapDev& h = m.host_copy; memset(&h, 0, sizeof(h)); h.nH = nH; h.nP = nP; h.pts = m.pts; m.ingest_seq = need_seq;
-  for (int k=0;k<nH;k++) {
-    const FrameDev& f = *F[k]; h.hostI0[k] = f.I0; m.host_exposure[k] = f.exposure; m.host_ids[k] = host_frames[k];
-    for (int i=0;i<7;i++) h.hostT[k][i] = host_T7[7*k+i]; m.host_ab[k][0] = host_ab ? host_ab[2*k] : 0.0; m.host_ab[k][1] = host_ab ? host_ab[2*k+1] : 0.0; }
-  m.nH = nH; m.nP = nP; m.set = true;
-  CK(cudaStreamSynchronize(c->st));                                            // a previous launch may still read the slot
-  CK(cudaMemcpyAsync(m.dev, &h, sizeof(MapDev), cudaMemcpyHostToDevice, c->st));
-  if (nP) CK(cudaMemcpyAsync(m.pts, pts, (size_t)nP*sizeof(sdv_map_pt), kind, c->st));
-  CK(cudaStreamSynchronize(c->st));
+  CK(cudaStreamSynchronize(c->st));                                            // host wait 1: a previous launch may still read the slots
+  const bool staged = kind == cudaMemcpyHostToDevice;
+  const size_t seg_bytes = Scratch::need(2*(size_t)n, sizeof(MapCopySeg)), dev_bytes = Scratch::need(n, sizeof(MapDev)) + (staged ? Scratch::need(totP, sizeof(sdv_map_pt)) : 0);
+  if (c->scr.reserve(seg_bytes + dev_bytes, c->st) || c->scr_host.reserve(seg_bytes + dev_bytes, c->st)) return ctx_fail(c, SDV_ERR_CUDA, "sdv_map_set_batch: staging of %d maps", n);
+  for (int j = 0; j < n; j++) {                                                  // room for the points (not visible until the slot is rewritten below)
+    MapSlot& m = st->maps[slots[j]]; const int nP = pt_begin[j+1] - pt_begin[j];
+    if (!m.dev) CK(cudaMalloc(&m.dev, sizeof(MapDev)));
+    if (nP > m.cap) { cudaFree(m.pts); m.pts = nullptr; m.cap = nP + nP/4 + 256; CK(cudaMalloc(&m.pts, (size_t)m.cap*sizeof(sdv_map_pt))); }
+  }
+  // one pinned image of the upload, laid out as its device twin: segment table, the MapDev of every job, the points of every job
+  c->scr.reset(); c->scr_host.reset();
+  MapCopySeg* seg_d = c->scr.take<MapCopySeg>(2*(size_t)n); MapDev* md_d = c->scr.take<MapDev>(n); sdv_map_pt* pts_d = staged ? c->scr.take<sdv_map_pt>(totP) : nullptr;
+  MapCopySeg* seg = c->scr_host.take<MapCopySeg>(2*(size_t)n); MapDev* md = c->scr_host.take<MapDev>(n); sdv_map_pt* pts_h = staged ? c->scr_host.take<sdv_map_pt>(totP) : nullptr;
+  const size_t up_bytes = staged ? (size_t)((char*)(pts_h + totP) - (char*)seg) : (size_t)((char*)(md + n) - (char*)seg);
+  int nseg = 0;
+  for (int j = 0; j < n; j++) {
+    MapSlot& m = st->maps[slots[j]]; const int h0 = host_begin[j], nH = host_begin[j+1] - h0, nP = pt_begin[j+1] - pt_begin[j];
+    if (m.set) for (int k=0;k<m.nH;k++) frame_unpin(c, m.host_ids[k]);       // the slot's previous keyframes are no longer referenced by it
+    for (int k=0;k<nH;k++) frame_pin(c, host_frames[h0+k]);
+    MapDev& h = m.host_copy; memset(&h, 0, sizeof(h)); h.nH = nH; h.nP = nP; h.pts = m.pts; m.ingest_seq = need_seq;
+    for (int k=0;k<nH;k++) {
+      const FrameDev& f = *F[h0+k]; h.hostI0[k] = f.I0; m.host_exposure[k] = f.exposure; m.host_ids[k] = host_frames[h0+k];
+      for (int i=0;i<7;i++) h.hostT[k][i] = host_T7[7*(h0+k)+i]; m.host_ab[k][0] = host_ab ? host_ab[2*(h0+k)] : 0.0; m.host_ab[k][1] = host_ab ? host_ab[2*(h0+k)+1] : 0.0; }
+    m.nH = nH; m.nP = nP; m.set = true;
+    md[j] = h; seg[nseg++] = MapCopySeg{(const uint32_t*)(md_d + j), (uint32_t*)m.dev, sizeof(MapDev)/4};
+    if (nP) {
+      const sdv_map_pt* src = pts + pt_begin[j];
+      if (staged) { memcpy(pts_h + pt_begin[j], src, (size_t)nP*sizeof(sdv_map_pt)); src = pts_d + pt_begin[j]; }
+      seg[nseg++] = MapCopySeg{(const uint32_t*)src, (uint32_t*)m.pts, (size_t)nP*sizeof(sdv_map_pt)/4};
+    }
+  }
+  CK(cudaMemcpyAsync(seg_d, seg, up_bytes, cudaMemcpyHostToDevice, c->st));
+  map_copy_kernel<<<dim3((unsigned)std::min<size_t>((maxP*sizeof(sdv_map_pt)/4 + 255)/256 + 1, 64), (unsigned)std::min(nseg, 65535)), 256, 0, c->st>>>(seg_d, nseg);
+  c->launches += 1;
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(c->st));                                            // host wait 2: the upload has landed (the caller may reuse its rows)
   return SDV_OK;
 }
 extern "C" {

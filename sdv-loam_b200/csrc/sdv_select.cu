@@ -279,8 +279,8 @@ static int init_from_lidar(sdv_ctx* c, int n, const int32_t* slots, const uint64
   { int rc = launch_init_points(c, n, dJ); if (rc) return rc; }
   std::vector<int> cnt(2*(size_t)n);
   CK(cudaMemcpyAsync(cnt.data(), counts, cnt.size()*sizeof(int), cudaMemcpyDeviceToHost, c->st)); CK(cudaStreamSynchronize(c->st));
-  int over = -1, maxk = 0;
-  for (int j = 0; j < n; j++) { n_sel_out[j] = cnt[2*j]; n_out[j] = cnt[2*j+1]; maxk = std::max(maxk, cnt[2*j+1]); if (cnt[2*j+1] > cap && over < 0) over = j; }
+  int over = -1;
+  for (int j = 0; j < n; j++) { n_sel_out[j] = cnt[2*j]; n_out[j] = cnt[2*j+1]; if (cnt[2*j+1] > cap && over < 0) over = j; }
   c->launches += s->eng.launches - l0;
   if (over >= 0) return ctx_fail(c, SDV_ERR_CAPACITY, "%s: job %d keeps %d points, cap is %d", who, over, n_out[over], cap);
   for (int j = 0; j < n; j++) { const size_t k = (size_t)n_out[j]; if (!k) continue;
@@ -288,12 +288,12 @@ static int init_from_lidar(sdv_ctx* c, int n, const int32_t* slots, const uint64
     if (meta_out) CK(cudaMemcpyAsync(meta_out + (size_t)j*cap, J[j].meta, k*sizeof(sdv_immature_meta), cudaMemcpyDeviceToHost, c->st));
     if (idepth_out) CK(cudaMemcpyAsync(idepth_out + (size_t)j*cap, J[j].idepth, k*sizeof(float), cudaMemcpyDeviceToHost, c->st)); }
   // install: setCTRefForFirstFrame from the splat rows (round_half 1, HdiF 0, lastRef_aff_g2l = (0,0)), and the map of one keyframe at camToWorld = SE3(), aff_g2l = (0,0)
-  if (c->scr.reserve(Scratch::need(std::max(maxk, 1), sizeof(float4)) + Scratch::need(std::max(maxk, 1), sizeof(int)), c->st)) return ctx_fail(c, SDV_ERR_CUDA, "%s: splat scratch", who);
+  // one job per build: a job over max_ref_points stops the loop with the jobs before it installed
   static const double kT0[7] = {1, 0, 0, 0, 0, 0, 0}, kAb0[2] = {0, 0};
   for (int j = 0; j < n; j++) {
-    c->scr.reset(); float4* splats = c->scr.take<float4>(std::max(maxk, 1)); int* done = c->scr.take<int>(std::max(maxk, 1));
-    { int rc = tracker_set_ref_dev(c, slots[j], F[j], frames[j], n_out[j], J[j].splat4, J[j].round, splats, done, 0.0, 0.0, &cd_launches); if (rc) return rc; }
-    { int rc = map_set_impl(c, slots[j], 1, &frames[j], kT0, kAb0, n_out[j], J[j].mp, cudaMemcpyDeviceToDevice); if (rc) return rc; }
+    const int32_t pb[2] = {0, n_out[j]}, hb[2] = {0, 1};
+    { int rc = set_ref_build(c, 1, &slots[j], &F[j], &frames[j], pb, J[j].splat4, J[j].round, cudaMemcpyDeviceToDevice, nullptr, nullptr, &cd_launches); if (rc) return rc; }
+    { int rc = map_set_impl(c, 1, &slots[j], hb, &frames[j], kT0, kAb0, pb, J[j].mp, cudaMemcpyDeviceToDevice); if (rc) return rc; }
   }
   CK(cudaEventRecord(c->ev1, c->st)); CK(cudaStreamSynchronize(c->st)); CK(cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   c->launches += cd_launches;
