@@ -448,6 +448,37 @@ int  sdv_ba_flag_points(sdv_ctx* c, const int32_t* selected, int32_t* status_out
 int  sdv_ba_marginalize_points(sdv_ctx* c, const int32_t* status);
 int  sdv_ba_marginalize_frame(sdv_ctx* c, int idx);
 int  sdv_ba_get_prior(sdv_ctx* c, int* dim, double* HM, double* bM);
+/* ---- batched install and hand-over: the per-window entries above for n windows of one context in one call each (FullSystem::makeKeyFrame around
+ * optimize, FullSystem.cpp:1152-1171, for every resident sequence).  Windows are named by index (sdv_ba_select numbering), each at most once; every
+ * per-window array is the call's arrays concatenated in the order the windows are listed.  The number of launches and host waits of a call does not
+ * grow with n (sdv_launch_count, sdv_ba_host_wait_count).  A refused call (SDV_ERR_ARG, the message names the window and the point or residual) leaves
+ * every listed window as it was, and so does a failed allocation; a CUDA error in the launches themselves leaves the listed windows undefined.
+ * sdv_ba_set_window_batch        insertFrame + setAdjointsF + the HM/bM carry-over (sdv_ba_set_window) and CalibHessian::value_zero (sdv_ba_set_calib_zero)
+ *                                for n windows.  Window i holds frames f_begin[i] .. f_begin[i+1] (1..SDV_MAX_FRAMES_WINDOW, one size); the per-frame
+ *                                arrays are indexed by that frame range; calib_value_scaled[4n], calib_value_zero[4n] (NULL: value_zero = value);
+ *                                HM / bM (NULL: zero) concatenated per window with dim = 4 + 6 nF_i.  A window not set before is created.
+ *                                A window gets its point storage at its first sdv_ba_set_points(_batch), zero points included.
+ * sdv_ba_set_points_batch        makeIDX + setPrecalcValues (sdv_ba_set_points) for n windows: window i's points are p_begin[i] .. p_begin[i+1], its
+ *                                residuals r_begin[i] .. r_begin[i+1]; res_begin and r_point are window-local, window i's res_begin block has nP_i + 1
+ *                                entries and starts at p_begin[i] + i.  The checks run on the device before any window changes.
+ * sdv_ba_flag_points_batch       sdv_ba_flag_points for n windows; selected / status_out concatenated by the windows' point counts.
+ * sdv_ba_marginalize_points_batch sdv_ba_marginalize_points for n windows; status NULL: each window's device-resident status of the flag call.
+ * sdv_ba_marginalize_frames_batch EnergyFunctional::marginalizeFrame, repeated: window i eliminates frames idx[k_begin[i] .. k_begin[i+1]) in that order,
+ *                                each index into the window as the previous eliminations left it (the reference's `i = 0` restart); zero frames is
+ *                                allowed, elimination down to zero frames is refused.  HM_out / bM_out (may be NULL) receive every window's prior
+ *                                afterwards, concatenated, dim = 4 + 6 nF_i.  Unpinning and the stale-points rule are those of sdv_ba_marginalize_frame. */
+int  sdv_ba_set_window_batch(sdv_ctx* c, int n, const int32_t* windows, const int32_t* f_begin, const uint64_t* frame_ids, const double* T_evalPT7,
+                             const double* state10, const double* state_zero10, const float* ab_exposure, const int32_t* frameID, const float* frameEnergyTH,
+                             const double* calib_value_scaled, const double* calib_value_zero, const double* HM, const double* bM);
+int  sdv_ba_set_points_batch(sdv_ctx* c, int n, const int32_t* windows, const int32_t* p_begin, const int32_t* r_begin, const float* uv, const float* idepth,
+                             const float* idepth_zero, const float* color8, const float* weights8, const int32_t* host, const int32_t* hasDepthPrior,
+                             const int32_t* isFromSensor, const int32_t* res_begin, const int32_t* r_point, const int32_t* r_host, const int32_t* r_target,
+                             const int32_t* r_hasMatcher, const float* r_matcher, const int32_t* r_isNew);
+/* host waits on the back-end stream so far (each synchronise of an sdv_ba_* entry, and the wait of a staging buffer that grows) */
+long long sdv_ba_host_wait_count(sdv_ctx* c);
+int  sdv_ba_flag_points_batch(sdv_ctx* c, int n, const int32_t* windows, const int32_t* selected, int32_t* status_out);
+int  sdv_ba_marginalize_points_batch(sdv_ctx* c, int n, const int32_t* windows, const int32_t* status);
+int  sdv_ba_marginalize_frames_batch(sdv_ctx* c, int n, const int32_t* windows, const int32_t* k_begin, const int32_t* idx, double* HM_out, double* bM_out);
 int  sdv_ba_get_linearized(sdv_ctx* c, float* res_toZero2, int32_t* isLinearized);
 int  sdv_ba_get_system(sdv_ctx* c, double* HA, double* bA, double* Hsc, double* bsc, double* lastHS, double* lastbS);
 int  sdv_ba_get_precalc(sdv_ctx* c, int host, int target, float out27[27], double adHost36[36], double adTarget36[36], float adHTdelta6[6]);

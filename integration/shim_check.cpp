@@ -164,27 +164,41 @@ struct FullSystem {
   std::vector<double> HM, bM;                                                   // ef->HM / ef->bM, row-major copies
   std::vector<int32_t> cell_order;                                              // Reprojector grid_.cell_order (Reprojector.cpp:107)
 
-  // FullSystem::optimize (FullSystemOptimize.cpp:344-502): flatten in ef->frames / allPoints / residualsAll order (EnergyFunctional::makeIDX, EnergyFunctional.cpp:761-782)
-  float optimize(int mnumOptIts) {
-    const int nF = (int)frameHessians.size();
-    std::vector<uint64_t> ids(nF); std::vector<double> T_eval(7*nF), state(10*nF), state_zero(10*nF); std::vector<float> exposure(nF), energyTH(nF); std::vector<int32_t> frameID(nF);
-    for (int i = 0; i < nF; i++) { FrameHessian* fh = frameHessians[i];
-      ids[i] = (uint64_t)fh->shell->id; se3_to7(fh->worldToCam_evalPT, &T_eval[7*i]); exposure[i] = fh->ab_exposure; frameID[i] = fh->frameID; energyTH[i] = fh->frameEnergyTH;
-      for (int k = 0; k < 10; k++) { state[10*i+k] = fh->state.data()[k]; state_zero[10*i+k] = fh->state_zero.data()[k]; } }
-    std::vector<float> uv, idepth, idepth_zero, color, weights, r_matcher; std::vector<int32_t> host, hasPrior, fromSensor, res_begin{0}, r_point, r_host, r_target, r_hasM, r_isNew;
+  // a window flattened in ef->frames / allPoints / residualsAll order (EnergyFunctional::makeIDX, EnergyFunctional.cpp:761-782); append() adds one window to the
+  // concatenated arrays of a batched install (res_begin block of nP + 1 window-local entries, per-window begins)
+  struct WindowRows {
+    std::vector<uint64_t> ids; std::vector<double> T_eval, state, state_zero, calib, calib_zero, HM, bM; std::vector<float> exposure, energyTH; std::vector<int32_t> frameID;
+    std::vector<float> uv, idepth, idepth_zero, color, weights, r_matcher; std::vector<int32_t> host, hasPrior, fromSensor, res_begin, r_point, r_host, r_target, r_hasM, r_isNew;
+    std::vector<int32_t> f_begin{0}, p_begin{0}, r_begin{0};
+  };
+  void append(WindowRows& w) const {
+    const int nF = (int)frameHessians.size(), p0 = (int)w.host.size(), r0 = (int)w.r_point.size();
+    for (int i = 0; i < nF; i++) { FrameHessian* fh = frameHessians[i]; double T[7]; se3_to7(fh->worldToCam_evalPT, T);
+      w.ids.push_back((uint64_t)fh->shell->id); w.T_eval.insert(w.T_eval.end(), T, T + 7); w.exposure.push_back(fh->ab_exposure); w.frameID.push_back(fh->frameID); w.energyTH.push_back(fh->frameEnergyTH);
+      for (int k = 0; k < 10; k++) { w.state.push_back(fh->state.data()[k]); w.state_zero.push_back(fh->state_zero.data()[k]); } }
+    w.calib.insert(w.calib.end(), Hcalib.value_scaled.data(), Hcalib.value_scaled.data() + 4); w.calib_zero.insert(w.calib_zero.end(), Hcalib.value_zero.data(), Hcalib.value_zero.data() + 4);
+    w.HM.insert(w.HM.end(), HM.begin(), HM.begin() + (size_t)(4 + 6*nF)*(4 + 6*nF)); w.bM.insert(w.bM.end(), bM.begin(), bM.begin() + 4 + 6*nF);
+    w.res_begin.push_back(0);
     for (FrameHessian* fh : frameHessians) for (PointHessian* ph : fh->pointHessians) {
-      const int p = (int)host.size();
-      uv.push_back(ph->u); uv.push_back(ph->v); idepth.push_back(ph->idepth); idepth_zero.push_back(ph->idepth_zero);
-      color.insert(color.end(), ph->color, ph->color + 8); weights.insert(weights.end(), ph->weights, ph->weights + 8);
-      host.push_back(fh->idx); hasPrior.push_back(ph->hasDepthPrior); fromSensor.push_back(ph->isFromSensor);
-      for (PointFrameResidual* r : ph->residuals) { r_point.push_back(p); r_host.push_back(r->host->idx); r_target.push_back(r->target->idx); r_hasM.push_back(r->hasMatcher);
-        r_matcher.push_back(r->matcher[0]); r_matcher.push_back(r->matcher[1]); r_isNew.push_back(r->isNew); }
-      res_begin.push_back((int32_t)r_point.size());
+      const int p = (int)w.host.size() - p0;
+      w.uv.push_back(ph->u); w.uv.push_back(ph->v); w.idepth.push_back(ph->idepth); w.idepth_zero.push_back(ph->idepth_zero);
+      w.color.insert(w.color.end(), ph->color, ph->color + 8); w.weights.insert(w.weights.end(), ph->weights, ph->weights + 8);
+      w.host.push_back(fh->idx); w.hasPrior.push_back(ph->hasDepthPrior); w.fromSensor.push_back(ph->isFromSensor);
+      for (PointFrameResidual* r : ph->residuals) { w.r_point.push_back(p); w.r_host.push_back(r->host->idx); w.r_target.push_back(r->target->idx); w.r_hasM.push_back(r->hasMatcher);
+        w.r_matcher.push_back(r->matcher[0]); w.r_matcher.push_back(r->matcher[1]); w.r_isNew.push_back(r->isNew); }
+      w.res_begin.push_back((int32_t)w.r_point.size() - r0);
     }
-    int rc = sdv_ba_set_window(gpu, nF, ids.data(), T_eval.data(), state.data(), state_zero.data(), exposure.data(), frameID.data(), energyTH.data(), Hcalib.value_scaled.data(), HM.data(), bM.data());
+    w.f_begin.push_back((int32_t)w.ids.size()); w.p_begin.push_back((int32_t)w.host.size()); w.r_begin.push_back((int32_t)w.r_point.size());
+  }
+
+  // FullSystem::optimize (FullSystemOptimize.cpp:344-502) on this system's window alone
+  float optimize(int mnumOptIts) {
+    const int nF = (int)frameHessians.size(); WindowRows w; append(w);
+    const std::vector<int32_t>& host = w.host;
+    int rc = sdv_ba_set_window(gpu, nF, w.ids.data(), w.T_eval.data(), w.state.data(), w.state_zero.data(), w.exposure.data(), w.frameID.data(), w.energyTH.data(), Hcalib.value_scaled.data(), HM.data(), bM.data());
     if (rc == SDV_OK) rc = sdv_ba_set_calib_zero(gpu, Hcalib.value_zero.data());                   // the linearisation point of the intrinsics stays at the initial K (HessianBlocks.h:287)
-    if (rc == SDV_OK) rc = sdv_ba_set_points(gpu, (int)host.size(), uv.data(), idepth.data(), idepth_zero.data(), color.data(), weights.data(), host.data(), hasPrior.data(), fromSensor.data(),
-                                             res_begin.data(), (int)r_point.size(), r_point.data(), r_host.data(), r_target.data(), r_hasM.data(), r_matcher.data(), r_isNew.data());
+    if (rc == SDV_OK) rc = sdv_ba_set_points(gpu, (int)host.size(), w.uv.data(), w.idepth.data(), w.idepth_zero.data(), w.color.data(), w.weights.data(), host.data(), w.hasPrior.data(), w.fromSensor.data(),
+                                             w.res_begin.data(), (int)w.r_point.size(), w.r_point.data(), w.r_host.data(), w.r_target.data(), w.r_hasM.data(), w.r_matcher.data(), w.r_isNew.data());
     float rmse = 0; int32_t its = 0, acc = 0;
     if (rc == SDV_OK) rc = sdv_ba_optimize(gpu, mnumOptIts, &rmse, &its, &acc);
     std::vector<double> Tn(7*nF), st(10*nF), step(10*nF), pre(7*nF); std::vector<float> th(nF); double cv[4], cs[4];
@@ -429,6 +443,40 @@ int shim_makeKeyFrame_batch(const std::vector<FullSystem*>& fss, const std::vect
   return rc;
 }
 
+// ------------------------------------------------------------------------------------------------ batched back-end makeKeyFrame (INTEGRATION.md §4)
+// the back-end part of makeKeyFrame for every sequence that made a keyframe: each flattens its own window (window[i] of the context), then one call per step
+// serves them all: install, optimize, flagPointsForRemoval, marginalizePointsF, marginalizeFrame (frames flagged for marginalisation, in the reference's
+// restart order) with the priors back into ef->HM / ef->bM
+int shim_backend_keyframe_batch(const std::vector<FullSystem*>& fss, const std::vector<int32_t>& windows, const std::vector<std::vector<int32_t>>& selected,
+                                std::vector<float>& rmse) {
+  const int n = (int)fss.size(); FullSystem::WindowRows w;
+  for (FullSystem* fs : fss) fs->append(w);
+  int rc = sdv_ba_set_window_batch(gpu, n, windows.data(), w.f_begin.data(), w.ids.data(), w.T_eval.data(), w.state.data(), w.state_zero.data(), w.exposure.data(),
+                                   w.frameID.data(), w.energyTH.data(), w.calib.data(), w.calib_zero.data(), w.HM.data(), w.bM.data());
+  if (rc == SDV_OK) rc = sdv_ba_set_points_batch(gpu, n, windows.data(), w.p_begin.data(), w.r_begin.data(), w.uv.data(), w.idepth.data(), w.idepth_zero.data(), w.color.data(),
+                                                 w.weights.data(), w.host.data(), w.hasPrior.data(), w.fromSensor.data(), w.res_begin.data(), w.r_point.data(), w.r_host.data(),
+                                                 w.r_target.data(), w.r_hasM.data(), w.r_matcher.data(), w.r_isNew.data());
+  rmse.assign(n, 0.f); std::vector<int32_t> its(n), acc(n);
+  if (rc == SDV_OK) rc = sdv_ba_optimize_batch(gpu, n, windows.data(), 6, rmse.data(), its.data(), acc.data());
+  std::vector<int32_t> sel, status, kb{0}, idx;
+  for (const std::vector<int32_t>& s : selected) sel.insert(sel.end(), s.begin(), s.end());
+  status.resize(sel.size());
+  if (rc == SDV_OK) rc = sdv_ba_flag_points_batch(gpu, n, windows.data(), sel.data(), status.data());
+  if (rc == SDV_OK) rc = sdv_ba_marginalize_points_batch(gpu, n, windows.data(), nullptr);
+  for (FullSystem* fs : fss) {                                                   // for (i ...) if (flaggedForMarginalization) { marginalizeFrame; i = 0; }
+    int removed = 0;
+    for (FrameHessian* fh : fs->frameHessians) if (fh->flaggedForMarginalization) idx.push_back(fh->idx - removed++);
+    kb.push_back((int32_t)idx.size());
+  }
+  std::vector<double> HM, bM;
+  for (int i = 0; i < n; i++) { const int nF = (int)fss[i]->frameHessians.size() - (kb[i+1] - kb[i]), N = 4 + 6*nF; HM.resize(HM.size() + (size_t)N*N); bM.resize(bM.size() + N); }
+  if (rc == SDV_OK) rc = sdv_ba_marginalize_frames_batch(gpu, n, windows.data(), kb.data(), idx.data(), HM.data(), bM.data());
+  size_t h = 0, b = 0;
+  for (int i = 0; i < n && rc == SDV_OK; i++) { FullSystem* fs = fss[i]; const int N = 4 + 6*((int)fs->frameHessians.size() - (kb[i+1] - kb[i]));
+    fs->HM.assign(HM.begin() + h, HM.begin() + h + (size_t)N*N); fs->bM.assign(bM.begin() + b, bM.begin() + b + N); h += (size_t)N*N; b += N; }
+  return rc;
+}
+
 // referenced so that -Wunused does not hide a missing call path
 int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const Undistort* u, const uint8_t* raw) {
   std::vector<int32_t> sel, st; Vec5 mr{}; SE3 T; AffLight a;
@@ -449,6 +497,7 @@ int shim_check_anchor(FullSystem& fs, FrameHessian* fh, CalibHessian& hc, const 
   { RowsQueue q{{}, 0}; int32_t ni = 0; rc |= shim_lidarCloudHandler_rows(q, rig, (uint64_t)fh->shell->id, nullptr, 0) | shim_makeNewTraces_rows(fh, q, ni) | shim_process_pop(q); }
   { InitBranch ib{nullptr, 0}; int rci = 0; shim_setFirstFromLidar(ib, fh); shim_initializer_frame1(fs, ib, fh, rci); rc |= rci; }
   { std::vector<FullSystem*> fss{&fs}; std::vector<int32_t> np; rc |= shim_makeKeyFrame_batch(fss, {0}, {0}, np); }
+  { std::vector<FullSystem*> fss{&fs}; std::vector<float> rm; rc |= shim_backend_keyframe_batch(fss, {0}, {sel}, rm); }
   fs.optimize(6); fs.set_map(0); fs.handover(sel, st); fs.trackNewCoarse(fh); fs.refine_only(fh); shim_frame_destructor(fh);
   return rc;
 }

@@ -322,6 +322,11 @@ class Context:
     def launch_count(self) -> int:
         return int(LIB.sdv_launch_count(self.p))
 
+    def ba_host_wait_count(self) -> int:
+        """host waits on the back-end stream so far (sdv_ba_host_wait_count)"""
+        LIB.sdv_ba_host_wait_count.argtypes = [_vp]; LIB.sdv_ba_host_wait_count.restype = C.c_longlong
+        return int(LIB.sdv_ba_host_wait_count(self.p))
+
     def releaseFrame(self, frame_id: int):
         self._ck(LIB.sdv_frame_release(self.p, frame_id)); self.frame_cam.pop(frame_id, None)
 
@@ -567,7 +572,43 @@ def _ba_protos():
     L.sdv_ba_marginalize_frame.argtypes = [_vp, C.c_int]
     L.sdv_ba_get_prior.argtypes = [_vp, C.POINTER(C.c_int), _vp, _vp]
     L.sdv_ba_get_linearized.argtypes = [_vp, _f32p, _i32p]
+    L.sdv_ba_set_window_batch.argtypes = [_vp, C.c_int, _i32p, _i32p, _u64p, _f64p, _f64p, _f64p, _f32p, _i32p, _f32p, _f64p, _vp, _vp, _vp]
+    L.sdv_ba_set_points_batch.argtypes = [_vp, C.c_int, _i32p, _i32p, _i32p] + [_f32p] * 5 + [_i32p] * 4 + [_i32p] * 4 + [_f32p, _i32p]
+    L.sdv_ba_flag_points_batch.argtypes = [_vp, C.c_int, _i32p, _i32p, _vp]
+    L.sdv_ba_marginalize_points_batch.argtypes = [_vp, C.c_int, _i32p, _vp]
+    L.sdv_ba_marginalize_frames_batch.argtypes = [_vp, C.c_int, _i32p, _i32p, _i32p, _vp, _vp]
     L._ba_done = True
+
+
+def _cat(arrs, dtype):
+    a = [np.ascontiguousarray(x, dtype).reshape(-1) for x in arrs]
+    return np.concatenate(a) if a else np.zeros(0, dtype)
+
+
+def pack_ba_windows(wins, frame_ids_list):
+    """The window dicts (synth.make_ba_window's layout) of one sdv_ba_set_window_batch / sdv_ba_set_points_batch call, concatenated in list order:
+    f_begin / p_begin / r_begin (n + 1 each), the per-frame, per-point and per-residual arrays, res_begin blocks of nP_i + 1 entries each, calib_value_scaled
+    and calib_value_zero (4 per window; the latter None unless some window has "K_zero", and for the others value_zero = value = value_scaled * (1.0f/50.0f) as the library forms it) and HM / bM (None unless some
+    window has a prior; zero for the others, dim = 4 + 6 nF_i)."""
+    n = len(wins); assert len(frame_ids_list) == n
+    nF = np.array([int(w["nF"]) for w in wins], np.int64); nP = np.array([len(w["uv"]) for w in wins], np.int64); nR = np.array([len(w["r_point"]) for w in wins], np.int64)
+    beg = lambda v: np.concatenate([[0], np.cumsum(v)]).astype(np.int32)
+    for w, f in zip(wins, frame_ids_list):
+        assert len(f) == int(w["nF"])
+    o = dict(n=n, f_begin=beg(nF), p_begin=beg(nP), r_begin=beg(nR), frame_ids=_cat(frame_ids_list, np.uint64))
+    for k, t in (("T_eval", np.float64), ("state", np.float64), ("state_zero", np.float64), ("ab_exposure", np.float32), ("frameID", np.int32), ("frameEnergyTH", np.float32),
+                 ("uv", np.float32), ("idepth", np.float32), ("idepth_zero", np.float32), ("color", np.float32), ("weights", np.float32), ("host", np.int32),
+                 ("hasDepthPrior", np.int32), ("isFromSensor", np.int32), ("res_begin", np.int32), ("r_point", np.int32), ("r_host", np.int32), ("r_target", np.int32),
+                 ("r_hasMatcher", np.int32), ("r_matcher", np.float32), ("r_isNew", np.int32)):
+        o[k] = _cat([w[k] for w in wins], t)
+    o["K"] = _cat([w["K"] for w in wins], np.float64)
+    zero = any("K_zero" in w for w in wins)
+    o["K_zero"] = _cat([w["K_zero"] if "K_zero" in w else np.asarray(w["K"], np.float64) * np.float64(np.float32(1) / np.float32(50)) for w in wins], np.float64) if zero else None
+    prior = any(w.get("HM") is not None for w in wins)
+    dims = [4 + 6 * int(w["nF"]) for w in wins]
+    o["HM"] = _cat([w["HM"] if w.get("HM") is not None else np.zeros((d, d)) for w, d in zip(wins, dims)], np.float64) if prior else None
+    o["bM"] = _cat([w["bM"] if w.get("bM") is not None else np.zeros(d) for w, d in zip(wins, dims)], np.float64) if prior else None
+    return o
 
 
 class EnergyFunctional:
@@ -588,6 +629,23 @@ class EnergyFunctional:
                                       c("weights", np.float32), c("host", np.int32), c("hasDepthPrior", np.int32), c("isFromSensor", np.int32), c("res_begin", np.int32),
                                       self.nR, c("r_point", np.int32), c("r_host", np.int32), c("r_target", np.int32), c("r_hasMatcher", np.int32),
                                       c("r_matcher", np.float32), c("r_isNew", np.int32)))
+
+    @staticmethod
+    def install_batch(ctx: "Context", windows, wins, frame_ids_list):
+        """EnergyFunctional(ctx, wins[i], frame_ids_list[i], window=windows[i]) for every i, in two calls (sdv_ba_set_window_batch, sdv_ba_set_points_batch)."""
+        _ba_protos(); w = np.ascontiguousarray(windows, np.int32); n = len(w); k = pack_ba_windows(wins, frame_ids_list)
+        ptr = lambda a: None if a is None else a.ctypes.data
+        ctx._ck(LIB.sdv_ba_set_window_batch(ctx.p, n, w, k["f_begin"], k["frame_ids"], k["T_eval"], k["state"], k["state_zero"], k["ab_exposure"], k["frameID"],
+                                            k["frameEnergyTH"], k["K"], ptr(k["K_zero"]), ptr(k["HM"]), ptr(k["bM"])))
+        ctx._ck(LIB.sdv_ba_set_points_batch(ctx.p, n, w, k["p_begin"], k["r_begin"], k["uv"], k["idepth"], k["idepth_zero"], k["color"], k["weights"], k["host"],
+                                            k["hasDepthPrior"], k["isFromSensor"], k["res_begin"], k["r_point"], k["r_host"], k["r_target"], k["r_hasMatcher"],
+                                            k["r_matcher"], k["r_isNew"]))
+        out = []
+        for i, win in enumerate(wins):
+            e = EnergyFunctional.__new__(EnergyFunctional); e.ctx = ctx; e.win = win; e.window = int(w[i])
+            e.nF = int(win["nF"]); e.nP = len(win["uv"]); e.nR = len(win["r_point"]); e.n = 4 + 6 * e.nF
+            out.append(e)
+        return out
 
     def _sel(self): self.ctx._ck(LIB.sdv_ba_select(self.ctx.p, self.window))
     def reset_oob(self): self._sel(); self.ctx._ck(LIB.sdv_ba_reset_oob(self.ctx.p))
@@ -665,6 +723,43 @@ class EnergyFunctional:
         self._sel(); o = np.zeros(27, np.float32); aH = np.zeros(36); aT = np.zeros(36); d = np.zeros(6, np.float32)
         self.ctx._ck(LIB.sdv_ba_get_precalc(self.ctx.p, host, target, o, aH, aT, d))
         return dict(KRKi=o[:9].reshape(3, 3), Kt=o[9:12], R0=o[12:21].reshape(3, 3), t0=o[21:24], aff=o[24:26], b0=o[26], adHost=aH.reshape(6, 6), adTarget=aT.reshape(6, 6), adHTdelta=d)
+
+
+def _ba_group(efs):
+    assert efs and all(e.ctx is efs[0].ctx for e in efs), "one context"
+    _ba_protos(); return efs[0].ctx, np.array([e.window for e in efs], np.int32)
+
+
+def flag_points_batch(efs, selected):
+    """EnergyFunctional.flagPointsForRemoval of several windows in one call: selected[i] per window -> status per window"""
+    ctx, w = _ba_group(efs); sel = _cat(selected, np.int32); st = np.zeros(len(sel), np.int32)
+    assert len(sel) == sum(e.nP for e in efs)
+    ctx._ck(LIB.sdv_ba_flag_points_batch(ctx.p, len(w), w, sel, st.ctypes.data))
+    return np.split(st, np.cumsum([e.nP for e in efs])[:-1])
+
+
+def marginalize_points_batch(efs, status=None):
+    """EnergyFunctional.marginalizePointsF of several windows in one call (status None: the device-resident result of the flag call)"""
+    ctx, w = _ba_group(efs); st = None if status is None else _cat(status, np.int32)
+    ctx._ck(LIB.sdv_ba_marginalize_points_batch(ctx.p, len(w), w, None if st is None else st.ctypes.data))
+
+
+def marginalize_frames_batch(efs, idx_lists, prior: bool = True):
+    """EnergyFunctional.marginalizeFrame of several windows in one call: window i eliminates idx_lists[i] in order (each index into the window as the previous
+    eliminations left it).  Returns each window's (HM, bM) afterwards when prior is set."""
+    ctx, w = _ba_group(efs); k = np.array([len(x) for x in idx_lists], np.int64); kb = np.concatenate([[0], np.cumsum(k)]).astype(np.int32)
+    idx = _cat(idx_lists, np.int32); dims = [e.n - 6 * int(kk) for e, kk in zip(efs, k)]
+    HM = np.zeros(sum(d * d for d in dims)) if prior else None; bM = np.zeros(sum(dims)) if prior else None
+    ctx._ck(LIB.sdv_ba_marginalize_frames_batch(ctx.p, len(w), w, kb, idx, None if HM is None else HM.ctypes.data, None if bM is None else bM.ctypes.data))
+    for e, kk in zip(efs, k):
+        if kk:
+            e.nF -= int(kk); e.n -= 6 * int(kk); e.nP = 0; e.nR = 0
+    if not prior:
+        return None
+    out, h, b = [], 0, 0
+    for d in dims:
+        out.append((HM[h:h + d * d].reshape(d, d), bM[b:b + d])); h += d * d; b += d
+    return out
 
 
 def optimize_batch(ctx: Context, windows, its: int = 6):

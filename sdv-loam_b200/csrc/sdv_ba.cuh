@@ -5,6 +5,7 @@
 // (EnergyFunctional.cpp:761-782; contiguous per host frame), residuals grouped per point in residualsAll order.
 #pragma once
 #include <cuda_runtime.h>
+#include <cstddef>
 #include "sdv_math.cuh"
 
 namespace sdv {
@@ -113,7 +114,41 @@ void launch_ba_reanchor(const BAWinDev* wins, int W, int maxP, cudaStream_t st);
 // keyframe hand-over (FullSystem::makeKeyFrame, FullSystem.cpp:1152-1171)
 void launch_ba_marg_flag(const BAWinDev* wins, int W, int maxP, cudaStream_t st);           // flagPointsForRemoval numeric part; P.marg_status in: selected, out: status
 void launch_ba_marg_points(const BAWinDev* wins, int W, int maxP, cudaStream_t st);         // marginalizePointsF
-void launch_ba_marg_frame(const BAWinDev* wins, int W, int idx, cudaStream_t st);           // marginalizeFrame (frame idx of every window)
+void launch_ba_marg_frame(const BAWinDev* wins, int W, const int* idx, cudaStream_t st);    // marginalizeFrame (frame idx[w] of window w; -1: none)
 void launch_ba_decide(const BAWinDev* wins, int W, int stage, cudaStream_t st);              // 0 init, 1 after step+linearize, 2 after reload, 3 final rmse
+
+// ---- batched window install (sdv_ba_install.cu): insertFrame / makeIDX / setPrecalcValues for n windows in fixed launches
+constexpr size_t kHdrPrefix = offsetof(BAHeader, precalc);   // what the host sets in a header besides HM / bM; the rest starts at zero
+struct BAHdrInstall { BAHeader* hdr; long long src; int hm_n, bm_n; };   // staging byte offset of the prefix, then hm_n + bm_n doubles of HM / bM
+// header w := its staged prefix, HM[0..hm_n), bM[0..bm_n), zero elsewhere (the bytes a full-header copy of a zeroed host header leaves)
+void launch_ba_hdr_install(const BAHdrInstall* d, int n, const char* stage, cudaStream_t st);
+// rows of window w in the concatenated point / residual arrays of one call: points p0 .. p0+nP, residuals r0 .. r0+nR, res_begin at p0 + w
+struct BAPtsInstall { int p0, r0, nP, nR, nF; };
+struct BAPtsStage {                      // the call's rows on the device, concatenated in window order
+  const float2* uv; const float* idepth; const float* idepth_zero; const float* color; const float* weights;
+  const int* host; const int* hasDepthPrior; const int* isFromSensor; const int* res_begin;
+  const int* r_point; const int* r_host; const int* r_target; const int* r_hasMatcher; const float2* r_matcher; const int* r_isNew;
+  int* rot;                              // [8 per point] res_of_target, written by the check
+  int* cnt;                              // [kPairCnt per window] residuals per (host + nF*target) at 0..63, points per host at 64..71
+  unsigned* key_in; unsigned* key; int* val_in; int* pair_res;   // pair sort: key = window*64 + pair, value = residual (window-local)
+};
+constexpr int kPairCnt = kMaxF*kMaxF + kMaxF;
+// refusal code of a window (low 4 bits of its err word; ~0 = none) and the point / residual it names (see ba_err_*)
+enum { BA_ERR_SPAN = 1, BA_ERR_MONO = 2, BA_ERR_HOST = 3, BA_ERR_RES = 4, BA_ERR_DUP = 5 };
+__host__ __device__ inline int ba_err_code(unsigned long long e) { return (int)(e & 15); }
+__host__ __device__ inline int ba_err_point(unsigned long long e) { return (int)((e >> 34) & ((1u << 28) - 1)); }
+__host__ __device__ inline int ba_err_res(unsigned long long e) { return (int)((e >> 4) & ((1u << 30) - 1)) - 1; }
+constexpr int kMaxPtsWin = (1 << 28) - 1, kMaxResWin = (1 << 30) - 2;   // what the err word can name
+// the makeIDX checks of every point (err[w]: the window's first failure), res_of_target and the per-pair / per-host counts; err and cnt start at ~0 / 0
+void launch_ba_pts_check(const BAPtsInstall* D, int n, int totP, const BAPtsStage& S, unsigned long long* err, cudaStream_t st);
+// after the check passed: the pair lists (stable sort, before any window is written), pair_begin / host_begin / header nP, nR, the rows into each
+// window's pool.  Returns the launches, or -1 when the sort could not be enqueued (no window written then).
+int  launch_ba_pts_install(const BAWinDev* wins, const BAPtsInstall* D, int n, int totR, int maxP, int maxR, const BAPtsStage& S, void* sort_tmp, size_t sort_bytes,
+                           cudaStream_t st);
+size_t ba_pts_sort_bytes(int n, int totR);
+// P.marg_status of window w <-> buf[off[w] .. off[w+1])  (to_window: 1 copy in, 0 copy out)
+void launch_ba_status_copy(const BAWinDev* wins, int n, int maxP, const int* off, int* buf, int to_window, cudaStream_t st);
+// (HM, bM) of window w (dim = header dim) -> out + off[2w] / out + off[2w+1]
+void launch_ba_prior_gather(const BAWinDev* wins, int n, const long long* off, double* out, cudaStream_t st);
 
 } // namespace sdv

@@ -973,9 +973,10 @@ __global__ void __launch_bounds__(kSolveThreads) ba_marg_stitch_kernel(const BAW
 
 // EnergyFunctional::marginalizeFrame (EnergyFunctional.cpp:434-512): fp64, one CTA.  The frame's 6 unknowns are moved to the end, its
 // prior added, the system is diagonally pre-scaled, the 6x6 block inverted (partial-pivot LU) and eliminated, the result un-scaled and
-// symmetrised.  Frame idx is then dropped from the header (frames[], nF, dim); points/residuals of the window are stale afterwards.
-__global__ void __launch_bounds__(kSolveThreads) ba_marg_frame_kernel(const BAWinDev* __restrict__ wins, int idx) {
+// symmetrised.  idxs[w] names window w's frame (-1: none this round).  Frame idx is then dropped from the header (frames[], nF, dim); points/residuals of the window are stale afterwards.
+__global__ void __launch_bounds__(kSolveThreads) ba_marg_frame_kernel(const BAWinDev* __restrict__ wins, const int* __restrict__ idxs) {
   BA_WIN(0)
+  const int idx = idxs[blockIdx.y];
   const int tid = threadIdx.x; const int nF = H->nF, odim = H->dim, ndim = odim - 6;
   if (idx < 0 || idx >= nF) return;
   __shared__ double sH[kMaxDim*kMaxDim]; __shared__ double sb[kMaxDim], SV[kMaxDim], SVI[kMaxDim]; __shared__ double hpi[36], bli[kMaxDim*6]; __shared__ int ord[kMaxDim];
@@ -1058,7 +1059,7 @@ void launch_ba_marg_points(const BAWinDev* wins, int W, int maxP, cudaStream_t s
   accumulate_mode(wins, W, maxP, GATE_ALWAYS, 2, st);
   ba_marg_stitch_kernel<<<dim3(1, W), kSolveThreads, 0, st>>>(wins);
 }
-void launch_ba_marg_frame(const BAWinDev* wins, int W, int idx, cudaStream_t st) { ba_marg_frame_kernel<<<dim3(1, W), kSolveThreads, 0, st>>>(wins, idx); }
+void launch_ba_marg_frame(const BAWinDev* wins, int W, const int* idx, cudaStream_t st) { ba_marg_frame_kernel<<<dim3(1, W), kSolveThreads, 0, st>>>(wins, idx); }
 void launch_ba_decide(const BAWinDev* wins, int W, int stage, cudaStream_t st) { ba_decide_kernel<<<(W + 127)/128, 128, 0, st>>>(wins, W, stage); }
 
 } // namespace sdv

@@ -81,6 +81,9 @@ struct sdv_ctx {
   sdv::BAState* ba = nullptr;                   // selected back-end window
   // ba_wins_dev serves st_ba and holds only the window descriptors, at offset 0: its address keys ba_graph
   std::vector<sdv::BAState*> ba_windows; sdv::Scratch ba_wins_dev; sdv::PinnedScratch ba_wins_host;
+  // staging of the batched install and hand-over entries (serves st_ba): a leading part taken alike from both moves in one copy, rows follow on the device
+  sdv::Scratch ba_scr; sdv::PinnedScratch ba_scr_host;
+  long long ba_waits = 0;                       // host waits on st_ba (sdv_ba_host_wait_count), under mu_ba
   // the fixed Gauss-Newton launch schedule of sdv_ba_optimize_batch as a CUDA graph, keyed by what the launches depend on
   cudaGraphExec_t ba_graph = nullptr; const void* bag_wins = nullptr; int bag_n = 0, bag_maxP = 0, bag_maxR = 0, bag_its = 0;
   char err[512];
