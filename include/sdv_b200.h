@@ -115,6 +115,14 @@ int  sdv_frame_upload_batch_raw_u8(sdv_ctx* c, int n, const uint64_t* frames, co
 #define SDV_MAX_CAMERAS 8
 int  sdv_set_undistort_cam(sdv_ctx* c, int cam, int w_org, int h_org, const float* remapX, const float* remapY, float factor, const float* G256, const float* vignette_inv);
 int  sdv_frame_upload_batch_raw_u8_cams(sdv_ctx* c, int n, const uint64_t* frames, const uint8_t* const* raw_imgs, const int32_t* cams, const float* exposures);
+/* FullSystem::setGammaFunction (FullSystem.cpp:225-249) for camera `cam`: BInv256 is the array the reference passes, PhotometricUndistorter::getG()
+ * (src/main.cpp sets it from the same calibration as the camera's Undistort).  Its inverse B weighs every absSquaredGrad the frames of this camera get:
+ * |grad|^2 * gw^2 with gw = B[c+1]-B[c], c = (int)(I+0.5f) clamped to [5, 250] (FrameHessian::makeImages, HessianBlocks.cpp:158-164, with the default
+ * setting_gammaWeightsPixelSelect = 1).  That is what the PixelSelector reads (makeHists level 0, makeMaps / makeMapsFromLidar levels 0..2: makeNewTraces
+ * and the LiDAR initialiser) and what sdv_frame_download returns as abs_out; the gradients themselves and every tracker / back-end input are unweighted.
+ * BInv256 == NULL restores the identity B[i] = i (gw = 1), which a camera has until this is called.  The reference sets the gamma before its first frame:
+ * SDV_ERR_STATE while a frame of this camera is resident; SDV_ERR_ARG for a camera outside [0, SDV_MAX_CAMERAS).  A refused call changes nothing. */
+int  sdv_set_gamma_cam(sdv_ctx* c, int cam, const float* BInv256);
 int  sdv_frame_build_batch_dev(sdv_ctx* c, int n, const uint64_t* frames, const void* const* imgs_dev, int fmt, const float* exposures);
 /* fmt: 0 float (copied into frame storage), 1 mono8, 2 float ADOPTED as the frame's level-0 plane (zero copy: the buffer must stay
  * valid and unmodified until sdv_frame_release / the handle is re-uploaded — for producers that already write into device memory). */

@@ -81,6 +81,8 @@ int shim_ingest_raw(FrameShell* shell, const uint8_t* raw_mono8, float exposure)
 int shim_set_undistort_cam(int cam, const Undistort* u) {
   return sdv_set_undistort_cam(gpu, cam, u->wOrg, u->hOrg, u->remapX, u->remapY, 1.0f, nullptr, nullptr);
 }
+// §4 one FullSystem::setGammaFunction per camera: G of that camera's PhotometricUndistorter (NULL: no calibration), before any frame of the camera is resident
+int shim_set_gamma_cam(int cam, float* G_or_null) { return sdv_set_gamma_cam(gpu, cam, G_or_null); }
 int shim_ingest_raw_cams(int n, const uint64_t* ids, const uint8_t* const* raw_mono8, const int32_t* cams, const float* exposures) {
   return sdv_frame_upload_batch_raw_u8_cams(gpu, n, ids, raw_mono8, cams, exposures);
 }
@@ -163,6 +165,11 @@ struct FullSystem {
   std::vector<FrameHessian*> frameHessians; std::vector<FrameShell*> allFrameHistory; CalibHessian Hcalib; CoarseTracker* coarseTracker; Vec5 lastCoarseRMSE;
   std::vector<double> HM, bM;                                                   // ef->HM / ef->bM, row-major copies
   std::vector<int32_t> cell_order;                                              // Reprojector grid_.cell_order (Reprojector.cpp:107)
+
+  // FullSystem::setGammaFunction (FullSystem.cpp:225-249), called by main.cpp with getPhotometricGamma() before the first frame: the body stays (Hcalib.B) and
+  // the same BInv goes to the library, which inverts it alike and weighs every absSquaredGrad of this context's camera with it.  A NULL BInv returns at once in
+  // the reference; the library takes it as the identity, which is what a fresh FullSystem has.
+  void setGammaFunction(float* BInv) { if (BInv == 0) return; sdv_set_gamma_cam(gpu, 0, BInv); }
 
   // a window flattened in ef->frames / allPoints / residualsAll order (EnergyFunctional::makeIDX, EnergyFunctional.cpp:761-782); append() adds one window to the
   // concatenated arrays of a batched install (res_begin block of nP + 1 window-local entries, per-window begins)

@@ -69,6 +69,7 @@ def _load():
     L.sdv_frame_upload_batch_raw_u8.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _f32p]
     L.sdv_set_undistort_cam.argtypes = [_vp, C.c_int, C.c_int, C.c_int, _f32p, _f32p, C.c_float, _vp, _vp]
     L.sdv_frame_upload_batch_raw_u8_cams.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _vp, _f32p]
+    L.sdv_set_gamma_cam.argtypes = [_vp, C.c_int, _vp]
     L.sdv_track_job_bytes.argtypes = []
     L.sdv_launch_count.argtypes = [_vp]; L.sdv_launch_count.restype = C.c_longlong
     L.sdv_frame_release.argtypes = [_vp, C.c_uint64]
@@ -267,6 +268,23 @@ class Context:
         assert V is None or V.size == und.wOrg * und.hOrg
         self._ck(LIB.sdv_set_undistort_cam(self.p, int(cam), int(und.wOrg), int(und.hOrg), rx, ry, float(factor), None if G is None else G.ctypes.data, None if V is None else V.ctypes.data))
         self.wh_org = getattr(self, "wh_org", {}); self.wh_org[int(cam)] = (int(und.wOrg), int(und.hOrg))
+
+    def setGammaFunction(self, BInv, cam: int = 0):
+        """FullSystem::setGammaFunction for camera `cam`: BInv = PhotometricUndistorter.getG() (at least 256 values, the first 256 are read), or None for the
+        identity.  The frames of this camera then carry makeImages' gamma-weighted absSquaredGrad (sdv_set_gamma_cam).  Call it before the camera's first frame."""
+        if BInv is None:
+            self._ck(LIB.sdv_set_gamma_cam(self.p, int(cam), None)); return
+        b = np.ascontiguousarray(np.asarray(BInv, np.float32).reshape(-1)[:256])
+        if b.size != 256:
+            raise ValueError(f"setGammaFunction reads 256 values, got {b.size}")
+        self._ck(LIB.sdv_set_gamma_cam(self.p, int(cam), b.ctypes.data))
+
+    def setCameraPhotometric(self, und, factor: float = 1.0, cam: int = 0):
+        """what src/main.cpp does for a camera: its Undistort (with the PhotometricUndistorter attached by Undistort.set_photometric, if any) for the raw
+        ingest, then FullSystem::setGammaFunction(getPhotometricGamma()), which is None (identity) without a valid photometric calibration"""
+        self.setUndistort(und, factor, cam)
+        pu = getattr(und, "photometricUndist", None)
+        self.setGammaFunction(None if pu is None else pu.getG(), cam)
 
     def makeImagesRaw(self, frame_id: int, raw, exposure: float = 1.0, cam: int = 0):
         """Undistort::undistort<unsigned char> + FrameHessian::makeImages of one native-size mono8 image of camera `cam`"""

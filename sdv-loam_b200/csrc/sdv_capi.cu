@@ -205,6 +205,7 @@ void sdv_destroy(sdv_ctx* c) {
   for (int i=0;i<2;i++) { c->ing_dev[i].release(); c->ing_host[i].release(); } cudaFree(c->partials); cudaFree(c->ticket); cudaFree(c->totals_dev); cudaFreeHost(c->totals_host);
   cudaFree(c->tc_dev); cudaFree(c->geom_dev); c->scr.release(); c->scr_host.release();
   for (float* u : c->und_buf) cudaFree(u);
+  cudaFree(c->gw2_dev);
   for (int i=0;i<sdv_ctx::kIngRing;i++) if (c->ev_ing[i]) cudaEventDestroy(c->ev_ing[i]); for (int i=0;i<2;i++) if (c->ev_cp[i]) cudaEventDestroy(c->ev_cp[i]); if (c->st_cp) cudaStreamDestroy(c->st_cp);
   rp_destroy(c);
   sel_destroy(c);
@@ -324,7 +325,7 @@ int ensure_lvl0(sdv_ctx* c, FrameDev& f) {        // FrameHessian::dI of a keyfr
   if (c->lvl0_free.empty()) return ctx_fail(c, SDV_ERR_CAPACITY, "keyframe level-0 image pool exhausted (max_kf_images=%d)", (int)c->lvl0_pool.size());
   int rc = join_ingest(c); if (rc) return rc;
   f.lvl0_slot = c->lvl0_free.back(); c->lvl0_free.pop_back(); f.lvl[0] = c->lvl0_pool[f.lvl0_slot];
-  launch_grad_texels(f.I0, f.lvl[0], c->cam_w[f.cam], c->cam_h[f.cam], c->st); c->launches += 1;
+  launch_grad_texels(f.I0, f.lvl[0], c->cam_w[f.cam], c->cam_h[f.cam], cam_gw2(c, f.cam), c->st); c->launches += 1;
   CK(cudaGetLastError());
   return SDV_OK;
 }
@@ -332,7 +333,7 @@ int ensure_texels(sdv_ctx* c, FrameDev& f, int lvl) {   // FrameHessian::dIp / a
   if (lvl == 0) return ensure_lvl0(c, f);
   if (f.hi_tex) return SDV_OK;
   int rc = join_ingest_upto(c, f.ingest_seq); if (rc) return rc;        // only the ingest that built this frame: a later batch keeps streaming
-  for (int l=1;l<c->levels;l++) launch_grad_texels(f.img[l], f.lvl[l], c->cam_w[f.cam]>>l, c->cam_h[f.cam]>>l, c->st);
+  for (int l=1;l<c->levels;l++) launch_grad_texels(f.img[l], f.lvl[l], c->cam_w[f.cam]>>l, c->cam_h[f.cam]>>l, cam_gw2(c, f.cam), c->st);
   c->launches += c->levels - 1;
   CK(cudaGetLastError());
   f.hi_tex = true;
@@ -394,6 +395,29 @@ int sdv_set_undistort_cam(sdv_ctx* c, int cam, int w_org, int h_org, const float
   if (G256) { CK(cudaMemcpy(p, G256, 256*sizeof(float), cudaMemcpyHostToDevice)); d.G = p; p += 256; }
   if (vignette_inv) { CK(cudaMemcpy(p, vignette_inv, po*sizeof(float), cudaMemcpyHostToDevice)); d.vignette = p; p += po; }
   d.wOrg = w_org; d.hOrg = h_org; d.factor = factor; u = d;                // set only once every table is on the device
+  return SDV_OK;
+}
+// FullSystem::setGammaFunction (FullSystem.cpp:225-249) for one camera: B inverts BInv on the host in the reference's float arithmetic, the device keeps
+// gw2[c] = (B[c+1]-B[c])*(B[c+1]-B[c]), the factor FrameHessian::makeImages applies to absSquaredGrad (HessianBlocks.cpp:158-164)
+int sdv_set_gamma_cam(sdv_ctx* c, int cam, const float* BInv256) { SDV_GUARD_TRK(c);
+  if (!c) return SDV_ERR_ARG;
+  { int rc = check_cams(c, 1, &cam, "sdv_set_gamma_cam", nullptr); if (rc) return rc; }
+  for (const auto& kv : c->frame_index) if (c->frames[kv.second].cam == cam)       // texels and level-0 pool entries were weighed with the camera's current table
+    return ctx_fail(c, SDV_ERR_STATE, "sdv_set_gamma_cam: frame %llu of camera %d is resident: set the gamma before the camera's first frame", (unsigned long long)kv.first, cam);
+  if (!BInv256) { c->gamma_set[cam] = false; return SDV_OK; }
+  float B[256];
+  for (int i=0;i<256;i++) B[i] = (float)i;                                  // CalibHessian(): B[i] = i (HessianBlocks.h:293); an i no bracket finds keeps it
+  for (int i=1;i<255;i++)
+    for (int s=1;s<255;s++)
+      if (BInv256[s] <= i && BInv256[s+1] >= i) { B[i] = s+(i - BInv256[s]) / (BInv256[s+1]-BInv256[s]); break; }
+  B[0] = 0; B[255] = 255;
+  float gw2[256];
+  for (int k=0;k<255;k++) { const float gw = B[k+1]-B[k]; gw2[k] = gw*gw; }
+  gw2[255] = 1.0f;                                                          // never read: gamma_w2 clamps c to [5, 250]
+  CK(cudaSetDevice(c->device));
+  if (!c->gw2_dev) CK(cudaMalloc(&c->gw2_dev, (size_t)SDV_MAX_CAMERAS*256*sizeof(float)));
+  CK(cudaMemcpy(c->gw2_dev + 256*(size_t)cam, gw2, sizeof(gw2), cudaMemcpyHostToDevice));   // no resident frame of this camera: no pending kernel reads the row
+  c->gamma_set[cam] = true;
   return SDV_OK;
 }
 int sdv_set_undistort(sdv_ctx* c, int w_org, int h_org, const float* remapX, const float* remapY, float factor, const float* G256, const float* vignette_inv) {

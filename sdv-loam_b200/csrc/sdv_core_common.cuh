@@ -35,6 +35,17 @@ __device__ __forceinline__ bool planar_grad(const float* __restrict__ I, int idx
   }
   return false;
 }
+// the factor makeImages applies to |grad|^2 of a texel of intensity I (HessianBlocks.cpp:158-164): gw*gw with gw = CalibHessian::getBGradOnly(I) = B[c+1]-B[c],
+// c = (int)(I+0.5f) clamped to [5, 250] (HessianBlocks.h:343-349).  gw2[c] holds that product per camera (sdv_set_gamma_cam); nullptr is the identity B[i] = i (gw = 1).
+// (int) of a NaN or of a value outside the int range is undefined in C++; the reference's x86 build converts with cvttss2si, which gives INT_MIN there, so c = 5.
+// The device conversion saturates instead, so that case is restated explicitly (DESIGN §0).
+__host__ __device__ __forceinline__ float gamma_w2(float I, const float* __restrict__ gw2) {
+  if (!gw2) return 1.0f;
+  const float t = I + 0.5f;
+  int c = 5;
+  if (t >= 6.0f && t < 2147483648.0f) c = t >= 250.0f ? 250 : (int)t;
+  return gw2[c];
+}
 
 namespace sel {
 

@@ -65,6 +65,9 @@ struct sdv_ctx {
   sdv::Scratch ing_dev[2]; sdv::PinnedScratch ing_host[2];
   sdv::UndistortCams und = {}; float* und_buf[SDV_MAX_CAMERAS] = {};                 // sdv_set_undistort_cam: per camera, remap tables (+ response / vignette) of the raw-image ingest
                                                                                     // in one allocation und_buf[k]; a camera is set iff und.cam[k].remapX != nullptr
+  // sdv_set_gamma_cam: per camera, the 256 factors gamma_w2 reads (FullSystem::setGammaFunction's B as makeImages weighs |grad|^2 with it), in one allocation
+  // of SDV_MAX_CAMERAS rows; a camera without gamma (B[i] = i) passes nullptr to the kernels
+  float* gw2_dev = nullptr; bool gamma_set[SDV_MAX_CAMERAS] = {};
   std::vector<float4*> lvl0_pool; std::vector<int> lvl0_free;
   std::vector<void*> cp_dst, cp_src; std::vector<size_t> cp_sz; bool no_batch_copy = false;
   std::vector<sdv::TrackerSlot> slots;
@@ -137,6 +140,7 @@ int  join_ingest_upto(sdv_ctx* c, long long seq);   // ... for ingest calls <= s
 inline const GeomRow& slot_geom(const sdv_ctx* c, int slot) { return c->geom[c->slots[slot].geom_row]; }   // the K a tracker / map slot uses, at every level
 // frames are depth-agnostic (stored at the context's depth): a frame fits a camera of the same size.  A tracker / map slot holds clouds built at its camera's
 // depth as well: it may only keep them on a camera of the same size and depth.
+inline const float* cam_gw2(const sdv_ctx* c, int cam) { return c->gamma_set[cam] ? c->gw2_dev + 256*(size_t)cam : nullptr; }   // gamma weights of camera cam, or nullptr
 inline bool same_size(const sdv_ctx* c, int cam_a, int cam_b) { return c->cam_w[cam_a] == c->cam_w[cam_b] && c->cam_h[cam_a] == c->cam_h[cam_b]; }
 inline bool same_size_depth(const sdv_ctx* c, int cam_a, int cam_b) { return same_size(c, cam_a, cam_b) && c->cam_levels[cam_a] == c->cam_levels[cam_b]; }
 inline int slot_levels(const sdv_ctx* c, int slot) { return c->cam_levels[c->slots[slot].cam]; }   // pyrLevelsUsed of a tracker / map slot

@@ -42,16 +42,16 @@ template <> __device__ __forceinline__ float4 px_load4<unsigned char>(const unsi
   const uchar4 v = __ldg(reinterpret_cast<const uchar4*>(p + i)); return make_float4((float)v.x, (float)v.y, (float)v.z, (float)v.w);
 }
 
-// gradient + pack of one texel of a planar intensity image (HessianBlocks.cpp:147-165)
-__device__ __forceinline__ float4 grad_texel(const float* __restrict__ I, int idx, int w, int h) {
+// gradient + pack of one texel of a planar intensity image (HessianBlocks.cpp:147-165); |grad|^2 carries the camera's gamma weight (gw2 == nullptr: none)
+__device__ __forceinline__ float4 grad_texel(const float* __restrict__ I, int idx, int w, int h, const float* __restrict__ gw2) {
   const float c = __ldg(I + idx); float dx, dy, ab = 0.f;
-  if (planar_grad(I, idx, w, h, dx, dy)) ab = dx*dx + dy*dy;
+  if (planar_grad(I, idx, w, h, dx, dy)) { ab = dx*dx + dy*dy; if (gw2) ab *= gamma_w2(c, gw2); }
   return make_float4(c, dx, dy, ab);
 }
-// packed texels of one level from its planar intensity, on demand (keyframes entering the BA window or the selector, debugging read-back)
-__global__ void __launch_bounds__(256) grad_texel_kernel(const float* __restrict__ I, float4* __restrict__ out, int w, int h) {
-  const int n = w*h;
-  for (int idx = blockIdx.x*blockDim.x + threadIdx.x; idx < n; idx += gridDim.x*blockDim.x) out[idx] = grad_texel(I, idx, w, h);
+// packed texels of one level from its planar intensity, on demand (keyframes entering the BA window or the selector, debugging read-back); G: gw2 is set
+template <bool G> __global__ void __launch_bounds__(256) grad_texel_kernel(const float* __restrict__ I, float4* __restrict__ out, int w, int h, const float* __restrict__ gw2_) {
+  const int n = w*h; const float* gw2 = G ? gw2_ : nullptr;
+  for (int idx = blockIdx.x*blockDim.x + threadIdx.x; idx < n; idx += gridDim.x*blockDim.x) out[idx] = grad_texel(I, idx, w, h, gw2);
 }
 
 // Undistort::undistort<unsigned char> (util/Undistort.cpp:341-435) fused with PhotometricUndistorter::processFrame (:177-214): one rectified level-0 pixel from the
@@ -194,9 +194,9 @@ void launch_pyramid_copy0(const void* batch_dev_v, int nframes, bool src_u8, int
   if (und) pyr_remap0_kernel<<<g, 256, 0, st>>>(batch_dev, *und);
   else if (src_u8) pyr_copy0_kernel<unsigned char><<<g, 256, 0, st>>>(batch_dev); else pyr_copy0_kernel<float><<<g, 256, 0, st>>>(batch_dev);
 }
-void launch_grad_texels(const float* I, float4* out, int w, int h, cudaStream_t st) {
+void launch_grad_texels(const float* I, float4* out, int w, int h, const float* gw2, cudaStream_t st) {
   int n = w*h; int grid = (n + 255)/256; if (grid > num_sms()*16) grid = num_sms()*16;
-  grad_texel_kernel<<<grid, 256, 0, st>>>(I, out, w, h);
+  if (gw2) grad_texel_kernel<true><<<grid, 256, 0, st>>>(I, out, w, h, gw2); else grad_texel_kernel<false><<<grid, 256, 0, st>>>(I, out, w, h, nullptr);
 }
 
 __global__ void unpack_level_kernel(const float4* __restrict__ in, float* dI3, float* ab, int n) {

@@ -16,7 +16,7 @@ struct UndistortCams { UndistortDev cam[SDV_MAX_CAMERAS]; };
 // every frame.  und: RAW input, each frame rectified with und->cam[PyrBatch::cam]
 void launch_pyramid_batch(const void* batch_dev, int nframes, bool src_u8, bool vec, int W, int H, int max_w, int max_h, int levels, cudaStream_t st, const UndistortCams* und = nullptr);
 void launch_pyramid_copy0(const void* batch_dev, int nframes, bool src_u8, int max_w, int max_h, cudaStream_t st, const UndistortCams* und = nullptr);
-void launch_grad_texels(const float* I, float4* out, int w, int h, cudaStream_t st);   // packed {I,dx,dy,|grad|^2} texels of one planar level
+void launch_grad_texels(const float* I, float4* out, int w, int h, const float* gw2, cudaStream_t st);   // packed {I,dx,dy,|grad|^2} texels of one planar level (gw2: gamma_w2)
 void launch_unpack_level(const float4* in, float* dI3, float* ab, int n, cudaStream_t st);
 
 cudaError_t kernels_init_device();        // per-device function attributes of the tracker kernels (called by sdv_create after cudaSetDevice)

@@ -31,9 +31,9 @@ bool sel_cam_bound(const sdv_ctx* c, int cam, int* slot) {
   for (size_t k = 0; k < s->cam.size(); k++) if (s->cam[k] == cam) { *slot = (int)k; return true; }
   return false;
 }
-static int sel_frame(sdv_ctx* c, int k, uint64_t id, int cam, sel::FrameImg& F, long long& need_seq, const char* who, bool texels = true) {
+static int sel_frame(sdv_ctx* c, int k, uint64_t id, int cam, sel::FrameImg& F, const float*& gw2, long long& need_seq, const char* who, bool texels = true) {
   FrameDev* f; { int rc = job_frame(c, who, k, id, cam, -1, &need_seq, &f); if (rc) return rc; }
-  F.I0 = f->I0; F.L1 = nullptr; F.L2 = nullptr;
+  F.I0 = f->I0; F.L1 = nullptr; F.L2 = nullptr; gw2 = cam_gw2(c, f->cam);           // the frame's camera weighed its texels: its table serves level 0 too
   if (texels) { int rc = ensure_texels(c, *f, 1); if (rc) return rc; F.L1 = f->lvl[1]; F.L2 = f->lvl[2]; }   // |grad|^2 of levels 1 and 2 (makeMaps / makeNewTraces read the packed texels)
   return SDV_OK;
 }
@@ -107,13 +107,13 @@ int sdv_selector_make_hists_cam(sdv_ctx* c, int cam, uint64_t frame, float* ths_
   if (!c) return SDV_ERR_ARG; SEL_STATE("selector_make_hists");
   { int rc = check_cams(c, 1, &cam, "selector_make_hists", nullptr); if (rc) return rc; }
   CK(cudaSetDevice(c->device));
-  sel::FrameImg F; long long need = 0; { int rc = sel_frame(c, 0, frame, cam, F, need, "selector_make_hists", false); if (rc) return rc; }
+  sel::FrameImg F; const float* gw2; long long need = 0; { int rc = sel_frame(c, 0, frame, cam, F, gw2, need, "selector_make_hists", false); if (rc) return rc; }
   { int rc = join_ingest_upto(c, need); if (rc) return rc; }
   const int w = c->cam_w[cam], h = c->cam_h[cam];
   const size_t tf = sel::SelEngine::ths_floats(w, h); if (c->scr.reserve(2*Scratch::need(tf, 4), c->st)) return ctx_fail(c, SDV_ERR_CUDA, "selector_make_hists: scratch");
   c->scr.reset(); float* a = c->scr.take<float>(tf); float* b = c->scr.take<float>(tf);
   CK(cudaMemsetAsync(a, 0, tf*4, c->st)); CK(cudaMemsetAsync(b, 0, tf*4, c->st));
-  sel::HistJob J{F.I0, a, b, w, h}; const long long l0 = s->eng.launches;
+  sel::HistJob J{F.I0, a, b, w, h, gw2}; const long long l0 = s->eng.launches;
   if (s->eng.make_hists(1, &J)) return sel_fail(c, s, -1, "selector_make_hists");
   c->launches += s->eng.launches - l0;
   const int n = (w/32)*(h/32);
@@ -136,7 +136,8 @@ int sdv_selector_make_maps_batch(sdv_ctx* c, int n, const int32_t* slots, const 
   CK(cudaSetDevice(c->device));
   long long need = 0; std::vector<int> jw(n), jh(n);                                   // job j works at its slot's camera size
   for (int j = 0; j < n; j++) { const int cam = s->cam[slots[j]]; jw[j] = c->cam_w[cam]; jh[j] = c->cam_h[cam]; }
-  std::vector<sel::FrameImg> F(n); for (int j = 0; j < n; j++) { int rc = sel_frame(c, j, frames[j], s->cam[slots[j]], F[j], need, "selector_make_maps"); if (rc) return rc; }
+  std::vector<sel::FrameImg> F(n); std::vector<const float*> G(n);
+  for (int j = 0; j < n; j++) { int rc = sel_frame(c, j, frames[j], s->cam[slots[j]], F[j], G[j], need, "selector_make_maps"); if (rc) return rc; }
   { int rc = join_ingest_upto(c, need); if (rc) return rc; }
   size_t bytes = 1024; for (int j = 0; j < n; j++) { const int m = lidar ? cloud_begin[j+1] - cloud_begin[j] : 0;
     bytes += 2*Scratch::need(sel::SelEngine::ths_floats(jw[j], jh[j]), 4) + Scratch::need(3*(size_t)m, 8) + Scratch::need(lidar ? (size_t)std::max(m, 1) : (size_t)jw[j]*jh[j], 1); }
@@ -147,9 +148,9 @@ int sdv_selector_make_maps_batch(sdv_ctx* c, int n, const int32_t* slots, const 
     double* cl = nullptr; if (lidar) { cl = c->scr.take<double>(3*(size_t)std::max(m, 1)); if (m) CK(cudaMemcpyAsync(cl, cloud3 + 3*(size_t)cloud_begin[j], 3*(size_t)m*sizeof(double), cudaMemcpyHostToDevice, c->st)); }
     sel::SelectorSlot& sl = s->slots[slots[j]];
     if (!lidar && !sl.mapD) { CK(cudaMalloc((void**)&sl.mapD, wh)); CK(cudaMemsetAsync(sl.mapD, 0, wh, c->st)); }
-    Hj[j] = sel::HistJob{F[j].I0, a, b, jw[j], jh[j]};
+    Hj[j] = sel::HistJob{F[j].I0, a, b, jw[j], jh[j], G[j]};
     M[j].img = F[j]; M[j].w = jw[j]; M[j].h = jh[j]; M[j].thsSm = b; M[j].cloud_dev = cl; M[j].n = m; M[j].map = lidar ? c->scr.take<unsigned char>(std::max(m, 1)) : sl.mapD; M[j].density = density[j];
-    M[j].recursionsLeft = recursions_left[j]; M[j].thFactor = th_factor[j]; M[j].currentPotential = &sl.currentPotential; M[j].numHaveSub = 0; M[j].passes = 0; }
+    M[j].recursionsLeft = recursions_left[j]; M[j].thFactor = th_factor[j]; M[j].currentPotential = &sl.currentPotential; M[j].numHaveSub = 0; M[j].passes = 0; M[j].gw2 = G[j]; }
   const long long l0 = s->eng.launches;
   if (s->eng.make_hists(n, Hj.data())) return sel_fail(c, s, -1, "selector_make_maps");
   if (s->eng.make_maps(M, lidar)) return sel_fail(c, s, -1, "selector_make_maps");
@@ -175,7 +176,7 @@ static int make_new_traces(sdv_ctx* c, int n, const int32_t* slots, const uint64
     if (!out) for (int k = 0; k < j; k++) if (frames[k] == frames[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces_store: frame %llu appears twice in one batch", (unsigned long long)frames[j]); }
   CK(cudaSetDevice(c->device));
   long long need = 0; std::vector<sel::SelEngine::NewTracesJob> J(n);
-  for (int j = 0; j < n; j++) { const int cam = s->cam[slots[j]]; int rc = sel_frame(c, j, frames[j], cam, J[j].img, need, "make_new_traces"); if (rc) return rc; J[j].w = c->cam_w[cam]; J[j].h = c->cam_h[cam];
+  for (int j = 0; j < n; j++) { const int cam = s->cam[slots[j]]; int rc = sel_frame(c, j, frames[j], cam, J[j].img, J[j].gw2, need, "make_new_traces"); if (rc) return rc; J[j].w = c->cam_w[cam]; J[j].h = c->cam_h[cam];
     J[j].cloud_host = cloud3 ? cloud3 + 3*(size_t)cloud_begin[j] : nullptr; J[j].cloud_dev = cloud_dev ? cloud_dev[j] : nullptr; J[j].n = cloud_begin[j+1] - cloud_begin[j]; J[j].slot = &s->slots[slots[j]]; J[j].densityLidar = density_lidar[j];
     J[j].densityDense = density_dense[j]; J[j].addFeaturePoint = add_feature_point[j]; J[j].out_host = out ? (sel::NewTrace*)out + (size_t)j*cap : nullptr;
     J[j].imm_host = (out && imm_out) ? (sel::ImmPt*)imm_out + (size_t)j*cap : nullptr; J[j].cap = cap; }
@@ -267,9 +268,10 @@ static int init_from_lidar(sdv_ctx* c, int n, const int32_t* slots, const uint64
     float* a = io.take<float>(tf); float* b = io.take<float>(tf); CK(cudaMemsetAsync(a, 0, tf*4, c->st)); CK(cudaMemsetAsync(b, 0, tf*4, c->st));
     const double* rows = cloud3 ? cl + 3*(size_t)cloud_begin[j] : cloud_dev[j];
     const int area = (lrud[4*j+1] - lrud[4*j])*(lrud[4*j+3] - lrud[4*j+2]);                      // lidarArea of the FullSystem box
-    Hj[j] = sel::HistJob{F[j]->I0, a, b, w, h};                                                  // a fresh PixelSelector: makeHists runs
+    const float* gw2 = cam_gw2(c, F[j]->cam);
+    Hj[j] = sel::HistJob{F[j]->I0, a, b, w, h, gw2};                                                  // a fresh PixelSelector: makeHists runs
     sel::MapsJobHost& q = M[j]; q.img = img[j]; q.w = w; q.h = h; q.thsSm = b; q.cloud_dev = rows; q.n = m; q.map = io.take<unsigned char>(mm);
-    q.density = 0.03f*area; q.recursionsLeft = 1; q.thFactor = 2; q.currentPotential = &pot[j]; q.numHaveSub = 0; q.passes = 0;   // makeMapsFromLidar(.., 0.03*lidarArea, 1, false, 2, ..)
+    q.density = 0.03f*area; q.recursionsLeft = 1; q.thFactor = 2; q.currentPotential = &pot[j]; q.numHaveSub = 0; q.passes = 0; q.gw2 = gw2;   // makeMapsFromLidar(.., 0.03*lidarArea, 1, false, 2, ..)
     InitPointsJob& P = J[j]; P.cloud = rows; P.map = q.map; P.draws = draws + (draw_begin[j] - draw_begin[0]); P.I0 = F[j]->I0; P.n = m; P.w = w; P.h = h; P.desired = desired[j];
     P.pts = io.take<sdv_immature_pt>(mm); P.meta = io.take<sdv_immature_meta>(mm); P.idepth = io.take<float>(mm); P.splat4 = io.take<float>(4*mm); P.round = io.take<int>(mm);
     P.mp = io.take<sdv_map_pt>(mm); P.counts = counts + 2*j; }

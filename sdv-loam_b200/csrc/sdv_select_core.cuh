@@ -39,6 +39,7 @@ struct SelJob {                          // one select pass of one frame
   unsigned char* map;                    // n bytes (LiDAR) or w*h bytes (dense): 0 / 1 / 2 / 4
   int* counters;                         // [0] n2 [1] n3 [2] n4 [3] sub-selected away
   int charTH;                            // random sub-selection threshold, -1 = none
+  const float* gw2 = nullptr;            // the frame camera's gamma weights of level 0 (gamma_w2; levels 1, 2 carry them in the texels); nullptr: no gamma set
 };
 
 SDV_DEVCONST float kSelDirs[16][2] = {{0,1.0000f},{0.3827f,0.9239f},{0.1951f,0.9808f},{0.9239f,0.3827f},{0.7071f,0.7071f},{0.3827f,-0.9239f},{0.8315f,0.5556f},{0.8315f,-0.5556f},
@@ -49,11 +50,12 @@ __device__ __forceinline__ int slot_of_cell(int cx, int cy, int nbx4) {         
   return (((cy>>2)*nbx4 + (cx>>2)) << 4) | (((cy>>1)&1) << 3) | (((cx>>1)&1) << 2) | ((cy&1) << 1) | (cx&1);
 }
 // the inputs of the three threshold tests for a candidate at float position (xf,yf) whose level-0 values are read at flat index idx
-__device__ __forceinline__ PtRec make_rec(const FrameImg& F, const float* __restrict__ thsSm, int w, int h, float xf, float yf, int idx, int out) {
+__device__ __forceinline__ PtRec make_rec(const FrameImg& F, const float* __restrict__ gw2, const float* __restrict__ thsSm, int w, int h, float xf, float yf, int idx, int out) {
   PtRec r; r.valid = 1; r.out = out;
   const int w32 = w/32, w1 = w>>1, w2 = w>>2;
   r.th0 = __ldg(thsSm + ((int)xf>>5) + ((int)yf>>5)*w32);
   planar_grad(F.I0, idx, w, h, r.dx, r.dy); r.ag0 = r.dx*r.dx + r.dy*r.dy;
+  if (gw2) r.ag0 *= gamma_w2(__ldg(F.I0 + idx), gw2);
   r.ag1 = __ldg(&F.L1[(int)(xf*0.5f+0.25f) + (int)(yf*0.5f+0.25f)*w1].w);
   r.ag2 = __ldg(&F.L2[(int)((double)(xf*0.25f)+0.125) + (int)((double)(yf*0.25f)+0.125)*w2].w);
   return r;
@@ -78,9 +80,11 @@ __device__ __forceinline__ void test_rec(const PtRec& r, float thF, float dw1, f
 }
 
 // ---------------------------------------------------------------------------------------------- makeHists
-struct HistJob { const float* I0; float* ths; float* thsSm; int w = 0, h = 0; };          // w, h: the frame's (its camera's) size; 0: the engine's
-__global__ void __launch_bounds__(128) sel_hist_kernel(const HistJob* __restrict__ jobs, SelSet S) {                    // CTA per 32x32 block of the largest job
-  const HistJob J = jobs[blockIdx.y]; const int w = J.w, h = J.h, w32 = w/32; if ((int)blockIdx.x >= w32*(h/32)) return;
+struct HistJob { const float* I0; float* ths; float* thsSm; int w = 0, h = 0;             // w, h: the frame's (its camera's) size; 0: the engine's
+                 const float* gw2 = nullptr; };                                          // the frame camera's gamma weights (gamma_w2); nullptr: no gamma set
+// G: some job of the launch has gamma weights (the host picks the instantiation, so a batch without them runs no gamma code)
+template <bool G> __global__ void __launch_bounds__(128) sel_hist_kernel(const HistJob* __restrict__ jobs, SelSet S) {      // CTA per 32x32 block of the largest job
+  const HistJob J = jobs[blockIdx.y]; const float* gw2 = G ? J.gw2 : nullptr; const int w = J.w, h = J.h, w32 = w/32; if ((int)blockIdx.x >= w32*(h/32)) return;
   const int bx = blockIdx.x % w32, by = blockIdx.x / w32;
   __shared__ int hist[64];
   if (threadIdx.x < 64) hist[threadIdx.x] = 0;
@@ -89,7 +93,8 @@ __global__ void __launch_bounds__(128) sel_hist_kernel(const HistJob* __restrict
     const int it = (k&31) + 32*bx, jt = (k>>5) + 32*by;
     if (it > w-2 || jt > h-2 || it < 1 || jt < 1) continue;
     float dx, dy; planar_grad(J.I0, it + jt*w, w, h, dx, dy);
-    int g = (int)sqrtf(dx*dx + dy*dy); if (g > 48) g = 48;
+    float ab = dx*dx + dy*dy; if (gw2) ab *= gamma_w2(__ldg(J.I0 + it + jt*w), gw2);
+    int g = (int)sqrtf(ab); if (g > 48) g = 48;
     atomicAdd(&hist[g+1], 1); atomicAdd(&hist[0], 1);
   }
   __syncthreads();
@@ -112,7 +117,7 @@ __global__ void __launch_bounds__(128) sel_smooth_kernel(const HistJob* __restri
 
 // ---------------------------------------------------------------------------------------------- one select pass
 // LiDAR pixels -> records + cell histogram (thread per cloud row)
-__global__ void __launch_bounds__(128) sel_point_kernel(const SelJob* __restrict__ jobs) {
+template <bool G> __global__ void __launch_bounds__(128) sel_point_kernel(const SelJob* __restrict__ jobs) {
   const SelJob J = jobs[blockIdx.y]; if (!J.active || !J.cloud) return;
   const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= J.n) return;
   const int w = J.w, h = J.h;
@@ -121,7 +126,7 @@ __global__ void __launch_bounds__(128) sel_point_kernel(const SelJob* __restrict
   int slot = -1;
   if (!(xf < 4 || xf >= w-5 || yf < 4 || yf > h-4) && cu == cu && cv == cv) {          // PixelSelector2.cpp:548 (also rejects NaN rows)
     const int idx = (int)(xf + (float)w*yf);                                             // sic: the float product of a fractional row with the width (:547)
-    r = make_rec(J.img, J.thsSm, w, h, xf, yf, idx, i);
+    r = make_rec(J.img, G ? J.gw2 : nullptr, J.thsSm, w, h, xf, yf, idx, i);
     slot = slot_of_cell((int)cu / J.pot, (int)cv / J.pot, J.nbx4);
     atomicAdd(&J.cnt[slot], 1);
   }
@@ -149,7 +154,7 @@ __global__ void __launch_bounds__(128) sel_scatter_kernel(const SelJob* __restri
   J.list[atomicAdd(&J.off[s], 1)] = i;                                                   // off[s] ends as the END of the cell's segment
 }
 // candidate k of a cell: LiDAR = k-th entry of its (index-sorted) list; dense = k-th pixel of the cell in raster order
-template <bool LIDAR> struct CellIter {
+template <bool LIDAR, bool G> struct CellIter {
   const SelJob& J; int w, h; int beg, cnt; int x0, y0, mx, my;
   __device__ CellIter(const SelJob& J_, int slot, int cx, int cy) : J(J_), w(J_.w), h(J_.h) {
     if (LIDAR) { cnt = J.cnt[slot]; beg = J.off[slot] - cnt; x0 = y0 = mx = my = 0; }
@@ -159,18 +164,18 @@ template <bool LIDAR> struct CellIter {
     if (LIDAR) { r = J.rec[J.list[beg + k]]; return true; }
     const int y1 = k / mx, x1 = k - y1*mx, xf = x0 + x1, yf = y0 + y1;
     if (xf < 4 || xf >= w-5 || yf < 4 || yf > h-4) return false;                          // PixelSelector2.cpp:276
-    r = make_rec(J.img, J.thsSm, w, h, (float)xf, (float)yf, xf + w*yf, xf + w*yf); return true;
+    r = make_rec(J.img, G ? J.gw2 : nullptr, J.thsSm, w, h, (float)xf, (float)yf, xf + w*yf, xf + w*yf); return true;
   }
 };
 // per cell: would it produce a level-2 pick, for each of the 16 directions (bit d)?  Exact: arg-max of |grad . dir_d| over the candidates above the level-0
 // threshold, first one wins ties, and the pick only counts when the winner's index is > 0 (PixelSelector2.cpp:319, :592)
-template <bool LIDAR> __global__ void __launch_bounds__(128) sel_cell_kernel(const SelJob* __restrict__ jobs, int dirDist) {
+template <bool LIDAR, bool G> __global__ void __launch_bounds__(128) sel_cell_kernel(const SelJob* __restrict__ jobs, int dirDist) {
   const SelJob J = jobs[blockIdx.y]; if (!J.active || (J.cloud != nullptr) != LIDAR) return;
   const int slot = blockIdx.x*blockDim.x + threadIdx.x; if (slot >= J.nslots) return;
   const int blk = slot >> 4, bx = blk % J.nbx4, by = blk / J.nbx4, cx = bx*4 + ((slot>>2)&1)*2 + (slot&1), cy = by*4 + ((slot>>3)&1)*2 + ((slot>>1)&1);
   int m = 0;
   if (cx < J.numPotW && cy < J.numPotH) {
-    CellIter<LIDAR> it(J, slot, cx, cy);
+    CellIter<LIDAR, G> it(J, slot, cx, cy);
     if (LIDAR && it.cnt > 1) {                                                           // atomics filled the segment in arbitrary order: restore cloud order
       int* L = J.list + it.beg;
       for (int a = 1; a < it.cnt; a++) { const int v = L[a]; int b = a-1; while (b >= 0 && L[b] > v) { L[b+1] = L[b]; b--; } L[b+1] = v; }
@@ -219,7 +224,7 @@ __global__ void __launch_bounds__(256) sel_n2_kernel(const SelJob* __restrict__ 
   if (threadIdx.x == 0) J.counters[0] = base;
 }
 // thread per 4x4-cell block: the three-level state machine of select / selectFromLidar with the directions now known
-template <bool LIDAR> __global__ void __launch_bounds__(128) sel_block_kernel(const SelJob* __restrict__ jobs, const unsigned char* __restrict__ rp, int dirDist, float dw1) {
+template <bool LIDAR, bool G> __global__ void __launch_bounds__(128) sel_block_kernel(const SelJob* __restrict__ jobs, const unsigned char* __restrict__ rp, int dirDist, float dw1) {
   const SelJob J = jobs[blockIdx.y]; if (!J.active || (J.cloud != nullptr) != LIDAR) return;
   const int blk = blockIdx.x*blockDim.x + threadIdx.x; if (blk >= J.nbx4*J.nby4) return;
   const int bx = blk % J.nbx4, by = blk / J.nbx4; const float dw2 = dw1*dw1;
@@ -234,7 +239,7 @@ template <bool LIDAR> __global__ void __launch_bounds__(128) sel_block_kernel(co
       const int slot = (blk << 4) | (sub << 2) | c;
       B.i2 = -1; B.v2 = 0;
       const float* dir2 = kSelDirs[rp[J.n2start[slot]] & 0xF];
-      CellIter<LIDAR> it(J, slot, cx, cy);
+      CellIter<LIDAR, G> it(J, slot, cx, cy);
       for (int k = 0; k < it.cnt; k++) { PtRec r; if (!it.get(k, r)) continue; test_rec(r, J.thFactor, dw1, dw2, dirDist, dir2, dir3, dir4, B); }
       if (B.i2 > 0) { J.map[B.i2] = 1; B.v3 = 1e10f; }
     }
@@ -248,7 +253,7 @@ template <bool LIDAR> __global__ void __launch_bounds__(128) sel_block_kernel(co
 // gathers the record of one pixel (threshold, level-0 gradient, the two coarser gradient magnitudes: the scattered loads, now 32 wide), then all lanes replay the
 // three-level state machine over the chunk from shared memory, redundantly and identically (no divergence; lane 0 writes).  A thread-per-block version walks 144 pixels per
 // thread with dependent loads.
-__global__ void __launch_bounds__(32) sel_block_dense_kernel(const SelJob* __restrict__ jobs, const unsigned char* __restrict__ rp, int dirDist, float dw1) {
+template <bool G> __global__ void __launch_bounds__(32) sel_block_dense_kernel(const SelJob* __restrict__ jobs, const unsigned char* __restrict__ rp, int dirDist, float dw1) {
   const SelJob J = jobs[blockIdx.y]; if (!J.active || J.cloud != nullptr) return;
   const int blk = blockIdx.x; if (blk >= J.nbx4*J.nby4) return;
   const int w = J.w, h = J.h;
@@ -260,7 +265,7 @@ __global__ void __launch_bounds__(32) sel_block_dense_kernel(const SelJob* __res
     { const int p = p0 + lane; PtRec r; r.valid = 0; r.out = 0; r.dx = r.dy = r.ag0 = r.ag1 = r.ag2 = r.th0 = 0;
       if (p < npx) { const int ci = p / pp, k = p - ci*pp, y1 = k / pot, x1 = k - y1*pot;
         const int cx = bx*4 + ((ci>>2)&1)*2 + (ci&1), cy = by*4 + (ci>>3)*2 + ((ci>>1)&1), xf = cx*pot + x1, yf = cy*pot + y1;
-        if (xf < w && yf < h && !(xf < 4 || xf >= w-5 || yf < 4 || yf > h-4)) r = make_rec(J.img, J.thsSm, w, h, (float)xf, (float)yf, xf + w*yf, xf + w*yf); }
+        if (xf < w && yf < h && !(xf < 4 || xf >= w-5 || yf < 4 || yf > h-4)) r = make_rec(J.img, G ? J.gw2 : nullptr, J.thsSm, w, h, (float)xf, (float)yf, xf + w*yf, xf + w*yf); }
       recs[lane] = r; }
     __syncthreads();
     const int cnt = imin_(32, npx - p0);
@@ -632,6 +637,7 @@ struct MapsJobHost {                     // one makeMaps / makeMapsFromLidar cal
   FrameImg img; int w = 0, h = 0; const float* thsSm; const double* cloud_dev; int n; unsigned char* map; float density; int recursionsLeft; float thFactor; int* currentPotential;
   int numHaveSub;                       // out
   int passes;                            // out: select passes run (1, or 2 after a recursion)
+  const float* gw2 = nullptr;            // the frame camera's gamma weights (SelJob::gw2)
 };
 
 struct SelEngine {
@@ -663,10 +669,11 @@ struct SelEngine {
     if (nj <= 0) return 0;
     if (scr2.reserve(Scratch::need(nj, sizeof(HistJob)), st)) { err = "scratch"; return -1; }
     scr2.reset(); HistJob* d = scr2.take<HistJob>(nj);
-    std::vector<HistJob> H(jobs_host, jobs_host + nj); int nb = 0;
-    for (auto& J : H) { size_or_engine(J); nb = std::max(nb, (J.w/32)*(J.h/32)); }
+    std::vector<HistJob> H(jobs_host, jobs_host + nj); int nb = 0; bool g = false;
+    for (auto& J : H) { size_or_engine(J); nb = std::max(nb, (J.w/32)*(J.h/32)); g |= J.gw2 != nullptr; }
     SEL_CK(cudaMemcpyAsync(d, H.data(), nj*sizeof(HistJob), cudaMemcpyHostToDevice, st));
-    SDV_LAUNCH_SYNC(sel_hist_kernel, dim3(nb, nj), dim3(128), st, d, S);
+    auto hist = g ? sel_hist_kernel<true> : sel_hist_kernel<false>;
+    SDV_LAUNCH_SYNC(hist, dim3(nb, nj), dim3(128), st, d, S);
     SDV_LAUNCH(sel_smooth_kernel, dim3((nb + 127)/128, nj), dim3(128), st, d);
     launches += 2; SEL_CK(cudaGetLastError());
     SEL_CK(cudaStreamSynchronize(st));                                                   // jobs_host / scr2 may be reused by the caller
@@ -688,13 +695,13 @@ struct SelEngine {
       if (scr.reserve(bytes, st)) { err = "scratch"; return -1; }
       scr.reset(); const int nc = j1 - j0; std::vector<SelJob> H(nc);
       SelJob* d = scr.take<SelJob>(nc); int* counters = scr.take<int>((size_t)nc*4);
-      int maxSlots = 0, maxN = 0, maxBlk = 0; const size_t zero_from = scr.used;
+      int maxSlots = 0, maxN = 0, maxBlk = 0; bool g = false; const size_t zero_from = scr.used;
       for (int k = 0; k < nc; k++) { MapsJobHost& M = *jobs[j0+k]; SelJob& J = H[k]; const int pot = *M.currentPotential, w = M.w, h = M.h;
         J.img = M.img; J.w = w; J.h = h; J.thsSm = M.thsSm; J.cloud = lidar ? M.cloud_dev : nullptr; J.n = lidar ? M.n : 0; J.pot = pot; J.thFactor = M.thFactor; J.active = 1; J.charTH = -1;
         J.numPotW = (w + pot-1)/pot; J.numPotH = (h + pot-1)/pot; J.nbx4 = (w + 4*pot-1)/(4*pot); J.nby4 = (h + 4*pot-1)/(4*pot); J.nslots = J.nbx4*J.nby4*16;
         J.mask = scr.take<int>(J.nslots); J.n2start = scr.take<int>(J.nslots); J.cnt = J.off = J.slot_of = J.list = nullptr; J.rec = nullptr;
         if (lidar) { J.cnt = scr.take<int>(J.nslots); J.off = scr.take<int>(J.nslots); J.slot_of = scr.take<int>(M.n); J.list = scr.take<int>(M.n); J.rec = scr.take<PtRec>(M.n); }
-        J.map = M.map; J.counters = counters + 4*k;
+        J.map = M.map; J.counters = counters + 4*k; J.gw2 = M.gw2; g |= M.gw2 != nullptr;
         maxSlots = std::max(maxSlots, J.nslots); maxN = std::max(maxN, J.n); maxBlk = std::max(maxBlk, J.nbx4*J.nby4);
         SEL_CK(cudaMemsetAsync(J.map, 0, lidar ? (size_t)std::max(M.n, 1) : (size_t)w*h, st)); }
       SEL_CK(cudaMemsetAsync(counters, 0, (size_t)nc*4*sizeof(int), st));
@@ -702,17 +709,22 @@ struct SelEngine {
       SEL_CK(cudaMemcpyAsync(d, H.data(), nc*sizeof(SelJob), cudaMemcpyHostToDevice, st));
       const int dd = S.selectDirectionDistribution;
       if (lidar) {
-        if (maxN > 0) SDV_LAUNCH(sel_point_kernel, dim3((maxN + 127)/128, nc), dim3(128), st, d);
+        auto point = g ? sel_point_kernel<true> : sel_point_kernel<false>;
+        auto cell = g ? sel_cell_kernel<true, true> : sel_cell_kernel<true, false>;
+        auto block = g ? sel_block_kernel<true, true> : sel_block_kernel<true, false>;
+        if (maxN > 0) SDV_LAUNCH(point, dim3((maxN + 127)/128, nc), dim3(128), st, d);
         SDV_LAUNCH_SYNC(sel_scan_kernel, dim3(nc), dim3(256), st, d);
         if (maxN > 0) SDV_LAUNCH(sel_scatter_kernel, dim3((maxN + 127)/128, nc), dim3(128), st, d);
-        SDV_LAUNCH(sel_cell_kernel<true>, dim3((maxSlots + 127)/128, nc), dim3(128), st, d, dd);
+        SDV_LAUNCH(cell, dim3((maxSlots + 127)/128, nc), dim3(128), st, d, dd);
         SDV_LAUNCH_SYNC(sel_n2_kernel, dim3(nc), dim3(256), st, d, rp);
-        SDV_LAUNCH(sel_block_kernel<true>, dim3((maxBlk + 127)/128, nc), dim3(128), st, d, rp, dd, S.gradDownweightPerLevel);
+        SDV_LAUNCH(block, dim3((maxBlk + 127)/128, nc), dim3(128), st, d, rp, dd, S.gradDownweightPerLevel);
         launches += 6;
       } else {
-        SDV_LAUNCH(sel_cell_kernel<false>, dim3((maxSlots + 127)/128, nc), dim3(128), st, d, dd);
+        auto cell = g ? sel_cell_kernel<false, true> : sel_cell_kernel<false, false>;
+        auto block = g ? sel_block_dense_kernel<true> : sel_block_dense_kernel<false>;
+        SDV_LAUNCH(cell, dim3((maxSlots + 127)/128, nc), dim3(128), st, d, dd);
         SDV_LAUNCH_SYNC(sel_n2_kernel, dim3(nc), dim3(256), st, d, rp);
-        SDV_LAUNCH_SYNC(sel_block_dense_kernel, dim3(maxBlk, nc), dim3(32), st, d, rp, dd, S.gradDownweightPerLevel);
+        SDV_LAUNCH_SYNC(block, dim3(maxBlk, nc), dim3(32), st, d, rp, dd, S.gradDownweightPerLevel);
         launches += 3;
       }
       SEL_CK(cudaGetLastError());
@@ -775,6 +787,7 @@ struct SelEngine {
     NewTrace* out_host; ImmPt* imm_host; int cap;                  // cap: room for the returned points (LiDAR + monocular)
     const double* cloud_dev = nullptr;                              // device-input path: the n rows are already on the device (cloud_host unused, nothing copied)
     int n_out, numPoints[2], passes[2];                             // out: points created, {numPointLidar, numPointMonocular}, select passes of the two makeMaps calls
+    const float* gw2 = nullptr;                                     // the frame camera's gamma weights (SelJob::gw2)
     const NewTrace* out_dev = nullptr; const ImmPt* imm_dev = nullptr;   // out: the n_out records on the device (engine scratch, valid until the next engine call);
                                                                     // out_host == nullptr: they stay there (device-output path)
   };
@@ -810,8 +823,8 @@ struct SelEngine {
       J.img = N.img; J.w = N.w; J.h = N.h; J.cloud = cl; J.n = N.n; J.mapL = mapL; J.mapD = N.slot->mapD; J.score = io.take<float>(N.n); J.flag = io.take<int>(N.n); J.pos = io.take<int>(N.n);
       J.occ = occ_all + o_occ[j]; J.state = io.take<unsigned char>(wh); J.cand = io.take<int>(N.cap); J.ncand_cap = N.cap;
       J.out = io.take<NewTrace>(N.cap); J.imm = io.take<ImmPt>(N.cap); J.cap = N.cap; J.counts = counts_all + 4*j;
-      Hj[j] = HistJob{N.img.I0, ths, thsSm, N.w, N.h};
-      MapsJobHost M; M.img = N.img; M.w = N.w; M.h = N.h; M.thsSm = thsSm; M.cloud_dev = cl; M.n = N.n; M.map = mapL; M.density = N.densityLidar; M.recursionsLeft = 1; M.thFactor = 1; M.currentPotential = &N.slot->currentPotential;
+      Hj[j] = HistJob{N.img.I0, ths, thsSm, N.w, N.h, N.gw2};
+      MapsJobHost M; M.img = N.img; M.w = N.w; M.h = N.h; M.thsSm = thsSm; M.cloud_dev = cl; M.n = N.n; M.map = mapL; M.density = N.densityLidar; M.recursionsLeft = 1; M.thFactor = 1; M.currentPotential = &N.slot->currentPotential; M.gw2 = N.gw2;
       M.numHaveSub = 0; M.passes = 0; ML.push_back(M);
     }
     if (make_hists(nj, Hj.data())) return -1;

@@ -20,6 +20,135 @@ def _f32_of_f64(x) -> np.float32:
     return np.float32(np.float64(x))
 
 
+def _parse_floats(line: str) -> list:
+    """std::istream_iterator<float> over one line: tokens read as float (strtof, correctly rounded) up to the first one that is not a number"""
+    out = []
+    for tok in line.split():
+        try:
+            d = float(tok)
+        except ValueError:
+            break
+        f = np.float32(d)
+        if np.float64(f) != d:                                                 # not exactly a float: round the decimal text once, as strtof does
+            f = np.float32(_strtof(tok.encode(), None))
+        out.append(f)
+    return out
+
+
+def _strtof(s, end):
+    import ctypes
+    fn = ctypes.CDLL(None).strtof; fn.restype = ctypes.c_float; fn.argtypes = [ctypes.c_char_p, ctypes.c_void_p]
+    return fn(s, end)
+
+
+class PhotometricUndistorter:
+    """Host mirror of the reference's PhotometricUndistorter constructor (util/Undistort.cpp:20-143) and of what processFrame (:177-214) applies.
+
+    gamma_text: the response file's text; its first line holds GDepth >= 256 values of the inverse response G, strictly increasing.  vignette: the
+    vignette image as a (h, w) uint16 (readImageBW_16U) or uint8 (readImageBW_8U) array of the raw size, or None.  photometric_calibration: the
+    reference's setting_photometricCalibration (2 by default; src/main.cpp modes 1 and 2 set 0).  Any failure leaves the object invalid: getG() is
+    None, and processFrame falls back to factor*v, as in the reference."""
+
+    def __init__(self, gamma_text: str | None, vignette, w: int, h: int, photometric_calibration: int = 2):
+        self.w, self.h = int(w), int(h); self.photometric_calibration = int(photometric_calibration)
+        self.valid = False; self.G = None; self.GDepth = 0; self.vignetteMap = None; self.vignetteMapInv = None
+        if gamma_text is None:                                                 # `if (!f.good()) return;`
+            return
+        lines = gamma_text.splitlines()
+        Gvec = _parse_floats(lines[0] if lines else "")
+        self.GDepth = GDepth = len(Gvec)
+        if GDepth < 256:
+            return
+        G = np.array(Gvec, np.float32)
+        if np.any(G[1:] <= G[:-1]):                                            # "G invalid! it has to be strictly increasing"
+            return
+        mn, mx = G[0], G[GDepth - 1]
+        G = (255.0 * (G - mn).astype(np.float64) / np.float64(mx - mn)).astype(np.float32)   # 255.0 * (G[i]-min) / (max-min): float difference, double rest
+        if self.photometric_calibration == 0:
+            G = (f32(255.0) * np.arange(GDepth, dtype=f32)) / f32(GDepth - 1)
+        self.G = G
+        if vignette is None:
+            return
+        v = np.asarray(vignette)
+        if v.dtype not in (np.uint16, np.uint8) or v.shape != (self.h, self.w):
+            return                                                             # "Invalid vignette image (size)"
+        vf = v.astype(f32); maxV = f32(0)
+        if v.size:
+            maxV = max(f32(0), vf.max())
+        self.vignetteMap = vf / maxV
+        self.vignetteMapInv = f32(1.0) / self.vignetteMap
+        self.valid = True
+
+    def getG(self):
+        """PhotometricUndistorter::getG(): the GDepth-entry G when valid, else None (FullSystem::setGammaFunction then keeps the identity)"""
+        return self.G if self.valid else None
+
+    @property
+    def ingest_G(self):
+        """the 256-entry response processFrame<unsigned char> applies to frames with exposure > 0, or None where it applies factor*v"""
+        return self.G[:256].copy() if self.valid and self.photometric_calibration != 0 else None
+
+    @property
+    def ingest_vignetteMapInv(self):
+        """the inverse vignette processFrame multiplies in (setting_photometricCalibration == 2 only), or None"""
+        return self.vignetteMapInv if self.ingest_G is not None and self.photometric_calibration == 2 else None
+
+    def processFrame(self, raw, exposure: float = 1.0, factor: float = 1.0):
+        """PhotometricUndistorter::processFrame<unsigned char> on a raw (h, w) mono8 image (test / data-preparation helper)"""
+        raw = np.asarray(raw, np.uint8); assert raw.shape == (self.h, self.w)
+        if self.ingest_G is None or not exposure > 0:
+            return f32(factor) * raw.astype(f32)
+        out = self.G[raw.astype(np.int64)]
+        if self.photometric_calibration == 2:
+            out = out * self.vignetteMapInv
+        return out.astype(f32)
+
+    @staticmethod
+    def from_files(gamma_path: str | None, vignette_path: str | None, w: int, h: int, photometric_calibration: int = 2) -> "PhotometricUndistorter":
+        """the constructor's file reads: the response text, and the vignette as a binary PGM (8 or 16 bit)"""
+        try:
+            with open(gamma_path) as f:
+                text = f.read()
+        except (OSError, TypeError):
+            text = None
+        try:
+            vig = read_pgm(vignette_path)
+        except (OSError, TypeError, ValueError):
+            vig = None
+        return PhotometricUndistorter(text, vig, w, h, photometric_calibration)
+
+
+def read_pgm(path: str):
+    """binary PGM (P5): uint8 for maxval < 256, big-endian 16-bit samples as uint16 otherwise"""
+    with open(path, "rb") as f:
+        data = f.read()
+    tok, pos = [], 0
+    while len(tok) < 4:
+        while data[pos:pos + 1].isspace():
+            pos += 1
+        if data[pos:pos + 1] == b"#":
+            pos = data.index(b"\n", pos) + 1; continue
+        e = pos
+        while not data[e:e + 1].isspace():
+            e += 1
+        tok.append(data[pos:e]); pos = e
+    if tok[0] != b"P5":
+        raise ValueError("not a binary PGM")
+    w, h, mx = int(tok[1]), int(tok[2]), int(tok[3]); pos += 1
+    dt = np.dtype(">u2") if mx > 255 else np.dtype(np.uint8)
+    return np.frombuffer(data, dt, w * h, pos).reshape(h, w).astype(np.uint16 if mx > 255 else np.uint8)
+
+
+def write_pgm(path: str, img):
+    img = np.asarray(img)
+    if img.dtype == np.uint16:
+        body, mx = img.astype(">u2").tobytes(), 65535
+    else:
+        body, mx = np.asarray(img, np.uint8).tobytes(), 255
+    with open(path, "wb") as f:
+        f.write(b"P5\n%d %d\n%d\n" % (img.shape[1], img.shape[0], mx) + body)
+
+
 class Undistort:
     """wOrg,hOrg: raw size; w,h: rectified size; K: 3x3 float64 (Undistort::getK()); remapX/remapY: (h,w) float32; passthrough: bool"""
 
@@ -98,6 +227,13 @@ class Undistort:
         k00 = (f32(w) - f32(1.0)) / (maxX - minX); k11 = (f32(h) - f32(1.0)) / (maxY - minY)
         self.K[0, 0] = np.float64(k00); self.K[1, 1] = np.float64(k11)
         self.K[0, 2] = np.float64(-minX) * self.K[0, 0]; self.K[1, 2] = np.float64(-minY) * self.K[1, 1]
+
+    def set_photometric(self, pu: PhotometricUndistorter) -> "Undistort":
+        """Undistort::loadPhotometricCalibration (:335-338): attach the PhotometricUndistorter of the raw size.  G / vignetteMapInv become what its
+        processFrame applies at ingest (Context.setUndistort reads them), and photometricUndist.getG() is what src/main.cpp hands to setGammaFunction."""
+        assert (pu.w, pu.h) == (self.wOrg, self.hOrg), "the photometric calibration has the raw image size"
+        self.photometricUndist = pu; self.G = pu.ingest_G; self.vignetteMapInv = pu.ingest_vignetteMapInv
+        return self
 
     @property
     def K4(self):
