@@ -25,9 +25,10 @@ void ba_destroy(sdv_ctx* c) {
 }
 }
 
+constexpr int kMaxWindows = (1<<20) + 1;                                     // window indices 0 .. 1<<20
 // the state of window `window` (sdv_ba_select numbering), created on first use
 static int ba_window(sdv_ctx* c, int window, BAState** out) {
-  if (window < 0 || window > 1<<20) return SDV_ERR_ARG;
+  if (window < 0 || window >= kMaxWindows) return SDV_ERR_ARG;
   if ((int)c->ba_windows.size() <= window) c->ba_windows.resize(window+1, nullptr);
   if (!c->ba_windows[window]) {
     BAState* b = new BAState(); memset(b, 0, sizeof(*b)); c->ba_windows[window] = b;
@@ -46,14 +47,9 @@ static int ba_get(sdv_ctx* c, BAState** out) {
   *out = c->ba; return SDV_OK;
 }
 static int32_t ba_index(const sdv_ctx* c, const BAState* b) { for (size_t i=0;i<c->ba_windows.size();i++) if (c->ba_windows[i] == b) return (int32_t)i; return -1; }
-// a batched entry's window list: n distinct indices in range; with `exist`, each names a window that has been set (*bs gets them)
-static int ba_list(sdv_ctx* c, const char* who, int n, const int32_t* windows, bool exist, std::vector<BAState*>* bs) {
-  std::vector<int32_t> s(windows, windows + n); std::sort(s.begin(), s.end());
-  for (int i=0;i<n;i++) {
-    if (s[i] < 0 || s[i] > 1<<20) return ctx_fail(c, SDV_ERR_ARG, "%s: window %d out of range", who, s[i]);
-    if (i > 0 && s[i] == s[i-1]) return ctx_fail(c, SDV_ERR_ARG, "%s: window %d listed twice", who, s[i]);
-  }
-  if (!exist) return SDV_OK;
+// a batched entry's window list: n distinct indices in range, each naming a window that has been set (*bs gets them)
+static int ba_list(sdv_ctx* c, const char* who, int n, const int32_t* windows, std::vector<BAState*>* bs) {
+  { int rc = check_ids(c, n, windows, kMaxWindows, who, "window"); if (rc) return rc; }
   bs->resize(n);
   for (int i=0;i<n;i++) {
     if (windows[i] >= (int)c->ba_windows.size() || !c->ba_windows[windows[i]]) return ctx_fail(c, SDV_ERR_ARG, "%s: BA window %d not set", who, windows[i]);
@@ -151,8 +147,8 @@ int sdv_ba_set_window_batch(sdv_ctx* c, int n, const int32_t* windows, const int
   if (!c || n < 1 || !windows || !f_begin || !frame_ids || !T_evalPT7 || !state10 || !state_zero10 || !calib_value_scaled) return SDV_ERR_ARG;
   SDV_GUARD_TRK(c);                                                           // frame table, pins, level-0 texel pool and the ingest join belong to the tracker domain
   CK(cudaSetDevice(c->device));
-  { int rc = ba_list(c, who, n, windows, false, nullptr); if (rc) return rc; }
-  if (f_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "%s: f_begin[0] = %d", who, f_begin[0]);
+  { int rc = check_ids(c, n, windows, kMaxWindows, who, "window"); if (rc) return rc; }
+  { int rc = check_offsets(c, n, f_begin, who, "f_begin"); if (rc) return rc; }
   for (int i=0;i<n;i++) { const int nF = f_begin[i+1] - f_begin[i];
     if (nF < 1 || nF > SDV_MAX_FRAMES_WINDOW) return ctx_fail(c, SDV_ERR_ARG, "%s: window %d has %d frames (1 .. %d)", who, windows[i], nF, SDV_MAX_FRAMES_WINDOW); }
   std::vector<FrameDev*> Fr(f_begin[n]); std::vector<int> cam0(n);
@@ -238,11 +234,12 @@ int sdv_ba_set_points_batch(sdv_ctx* c, int n, const int32_t* windows, const int
   const char* who = "sdv_ba_set_points_batch";
   if (!c || n < 1 || !windows || !p_begin || !r_begin || !res_begin) return SDV_ERR_ARG;
   CK(cudaSetDevice(c->device)); cudaStream_t st = c->st_ba;
-  std::vector<BAState*> bs; { int rc = ba_list(c, who, n, windows, true, &bs); if (rc) return rc; }
-  if (p_begin[0] != 0 || r_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "%s: p_begin[0] = %d, r_begin[0] = %d", who, p_begin[0], r_begin[0]);
+  std::vector<BAState*> bs; { int rc = ba_list(c, who, n, windows, &bs); if (rc) return rc; }
+  { int rc = check_offsets(c, n, p_begin, who, "p_begin"); if (rc) return rc; }
+  { int rc = check_offsets(c, n, r_begin, who, "r_begin"); if (rc) return rc; }
   int maxP = 1, maxR = 1;
   for (int i=0;i<n;i++) { const int nP = p_begin[i+1] - p_begin[i], nR = r_begin[i+1] - r_begin[i];
-    if (nP < 0 || nR < 0 || nP > kMaxPtsWin || nR > kMaxResWin) return ctx_fail(c, SDV_ERR_ARG, "%s: window %d: %d points, %d residuals", who, windows[i], nP, nR);
+    if (nP > kMaxPtsWin || nR > kMaxResWin) return ctx_fail(c, SDV_ERR_ARG, "%s: window %d: %d points, %d residuals", who, windows[i], nP, nR);
     if (nP == 0 && nR != 0) return ctx_fail(c, SDV_ERR_ARG, "%s: window %d: residuals without points", who, windows[i]);
     maxP = std::max(maxP, nP); maxR = std::max(maxR, nR); }
   const int totP = p_begin[n], totR = r_begin[n];
@@ -498,7 +495,7 @@ static int stage_windows(sdv_ctx* c, int n, BAState* const* bs, const BAWinDev**
   *Wd = W; *off_h = oh; *off_d = od; *maxP = mp; return SDV_OK;
 }
 static int ba_list_points(sdv_ctx* c, const char* who, int n, const int32_t* windows, std::vector<BAState*>& bs) {
-  { int rc = ba_list(c, who, n, windows, true, &bs); if (rc) return rc; }
+  { int rc = ba_list(c, who, n, windows, &bs); if (rc) return rc; }
   for (int i=0;i<n;i++) if (bs[i]->nP <= 0) return ctx_fail(c, SDV_ERR_STATE, "%s: window %d has no points (call sdv_ba_set_points)", who, windows[i]);
   return SDV_OK;
 }
@@ -554,11 +551,10 @@ int sdv_ba_marginalize_frames_batch(sdv_ctx* c, int n, const int32_t* windows, c
   const char* who = "sdv_ba_marginalize_frames_batch";
   if (!c || n < 1 || !windows || !k_begin) return SDV_ERR_ARG;
   CK(cudaSetDevice(c->device)); cudaStream_t st = c->st_ba;
-  std::vector<BAState*> bs; { int rc = ba_list(c, who, n, windows, true, &bs); if (rc) return rc; }
-  if (k_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "%s: k_begin[0] = %d", who, k_begin[0]);
+  std::vector<BAState*> bs; { int rc = ba_list(c, who, n, windows, &bs); if (rc) return rc; }
+  { int rc = check_offsets(c, n, k_begin, who, "k_begin"); if (rc) return rc; }
   int rounds = 0;
   for (int i=0;i<n;i++) { const int k = k_begin[i+1] - k_begin[i];
-    if (k < 0) return ctx_fail(c, SDV_ERR_ARG, "%s: k_begin not monotone at window %d", who, windows[i]);
     if (k > 0 && !idx) return SDV_ERR_ARG;
     int nF = bs[i]->nF;
     for (int j=k_begin[i]; j<k_begin[i+1]; j++, nF--)

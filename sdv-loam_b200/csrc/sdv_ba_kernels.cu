@@ -15,13 +15,12 @@
 // Accumulation kernels are "entry-parallel, item-sequential": one thread owns one accumulator cell and walks the items in the
 // reference's order with the reference's 1 / 1k / 1M float tiers, so every float sum is bit-identical to the CPU path's.
 #include "sdv_ba.cuh"
+#include "sdv_core_common.cuh"
 
 namespace sdv {
 
 #define BA_WIN(gate) const BAWinDev& Wn = wins[blockIdx.y]; BAHeader* __restrict__ H = Wn.hdr; \
   if (((gate) != 0) && ((H->flags & (gate)) != (gate))) return; BAPointsDev P = Wn.P; BAResDev R = Wn.R; const int nP = H->nP, nR = H->nR; (void)P; (void)R; (void)nP; (void)nR;
-
-__constant__ int c_pattern[8][2] = {{0,-2},{-1,-1},{1,-1},{-2,0},{0,0},{2,0},{-1,1},{0,2}};   // settings.cpp:250
 
 // ================================================================================================ frames / pairs
 __device__ void frame_set_state(BAFrameDev& f) {                          // HessianBlocks.h:141-153
@@ -207,7 +206,7 @@ __device__ __forceinline__ double lin_residual(BAHeader* __restrict__ H, BAPoint
     // (Tried in round 2: all 8 projections first, then the footprints of 4 pixels fetched together — 16 independent loads in flight per thread — and accumulated in
     // order.  Bit-identical, but 184 registers instead of 96 cut the resident warps by more than the extra memory parallelism gave: slower.)
     for (int idx = 0; idx < 8; idx++) {
-      float x = uv.x + c_pattern[idx][0], y = uv.y + c_pattern[idx][1];
+      float x = uv.x + staticPattern[idx][0], y = uv.y + staticPattern[idx][1];
       float q0 = ((pc.KRKi[0]*x + pc.KRKi[1]*y) + pc.KRKi[2]*1.0f) + pc.Kt[0]*ids;
       float q1 = ((pc.KRKi[3]*x + pc.KRKi[4]*y) + pc.KRKi[5]*1.0f) + pc.Kt[1]*ids;
       float q2 = ((pc.KRKi[6]*x + pc.KRKi[7]*y) + pc.KRKi[8]*1.0f) + pc.Kt[2]*ids;

@@ -363,6 +363,25 @@ int check_cams(sdv_ctx* c, int n, const int32_t* cams, const char* who, const ch
   }
   return SDV_OK;
 }
+int check_offsets(sdv_ctx* c, int n, const int32_t* off, const char* who, const char* what) {
+  if (off[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "%s: %s[0] = %d (must be 0)", who, what, off[0]);
+  for (int k=0;k<n;k++) if (off[k+1] < off[k]) return ctx_fail(c, SDV_ERR_ARG, "%s: %s decreases at entry %d", who, what, k);
+  return SDV_OK;
+}
+template <class T> static bool find_repeat(int n, const T* v, T* rep) {
+  std::vector<T> s(v, v + n); std::sort(s.begin(), s.end());
+  const auto it = std::adjacent_find(s.begin(), s.end()); if (it == s.end()) return false;
+  *rep = *it; return true;
+}
+int check_ids(sdv_ctx* c, int n, const int32_t* ids, int limit, const char* who, const char* what) {
+  for (int k=0;k<n;k++) if (ids[k] < 0 || ids[k] >= limit) return ctx_fail(c, SDV_ERR_ARG, "%s: entry %d names %s %d (valid: 0..%d)", who, k, what, ids[k], limit - 1);
+  int32_t r; if (find_repeat(n, ids, &r)) return ctx_fail(c, SDV_ERR_ARG, "%s: %s %d appears twice in one call", who, what, r);
+  return SDV_OK;
+}
+int check_distinct(sdv_ctx* c, int n, const uint64_t* ids, const char* who, const char* what) {
+  uint64_t r; if (find_repeat(n, ids, &r)) return ctx_fail(c, SDV_ERR_ARG, "%s: %s %llu appears twice in one call", who, what, (unsigned long long)r);
+  return SDV_OK;
+}
 }
 extern "C" {
 
@@ -505,14 +524,11 @@ int sdv_tracker_set_ref_batch(sdv_ctx* c, int n, const int32_t* slots, const uin
   const char* who = "sdv_tracker_set_ref_batch";
   if (!c || n < 0 || (n > 0 && (!slots || !ref_frames || !pt_begin))) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK;
-  if (pt_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "%s: pt_begin[0] must be 0", who);
-  for (int j = 0; j < n; j++) if (pt_begin[j+1] < pt_begin[j]) return ctx_fail(c, SDV_ERR_ARG, "%s: pt_begin decreases at job %d", who, j);
+  { int rc = check_offsets(c, n, pt_begin, who, "pt_begin"); if (rc) return rc; }
   if (pt_begin[n] > 0 && (!pts4 || !round_half)) return SDV_ERR_ARG;
-  const int ns = (int)c->slots.size(); std::vector<char> seen(ns, 0); std::vector<FrameDev*> F(n);
+  { int rc = check_ids(c, n, slots, (int)c->slots.size(), who, "slot"); if (rc) return rc; }
+  std::vector<FrameDev*> F(n);
   for (int j = 0; j < n; j++) {
-    if (slots[j] < 0 || slots[j] >= ns) return ctx_fail(c, SDV_ERR_ARG, "%s: job %d names slot %d of %d", who, j, slots[j], ns);
-    if (seen[slots[j]]) return ctx_fail(c, SDV_ERR_ARG, "%s: slot %d appears twice in one batch", who, slots[j]);
-    seen[slots[j]] = 1;
     { int rc = job_frame(c, who, j, ref_frames[j], -1, slots[j], nullptr, &F[j]); if (rc) return rc; }
     const int cam = c->slots[slots[j]].cam, w = c->cam_w[cam], h = c->cam_h[cam];        // makeCoarseDepthL0 at the slot's size
     for (int i = pt_begin[j]; i < pt_begin[j+1]; i++) {                                   // the reference would write out of bounds here; we refuse instead

@@ -1,5 +1,6 @@
 // sdv_core_common.cuh — what the self-contained device cores (sdv_select_core.cuh, sdv_lidar_core.cuh) share: launch macros (CUDA, or the host emulation of tests/emu),
-// a block-wide exclusive scan, a grow-only scratch allocator, makeImages' gradient of a planar plane.  Depends on nothing but the CUDA runtime.
+// a block-wide exclusive scan, a grow-only scratch allocator, makeImages' gradient of a planar plane, and the reference rules that more than one kernel restates:
+// staticPattern, getInterpolatedElement31 on a planar plane, the ImmaturePoint constructor and its status codes.  Depends on nothing but the CUDA runtime.
 #pragma once
 #include <stdint.h>
 #include <math.h>
@@ -45,6 +46,39 @@ __host__ __device__ __forceinline__ float gamma_w2(float I, const float* __restr
   int c = 5;
   if (t >= 6.0f && t < 2147483648.0f) c = t >= 250.0f ? 250 : (int)t;
   return gw2[c];
+}
+
+SDV_DEVCONST int staticPattern[8][2] = {{0,-2},{-1,-1},{1,-1},{-2,0},{0,0},{2,0},{-1,1},{0,2}};   // util/settings.cpp:250
+enum { IPS_GOOD = 0, IPS_OOB, IPS_OUTLIER, IPS_SKIPPED, IPS_BADCONDITION, IPS_UNINITIALIZED };      // ImmaturePointStatus (ImmaturePoint.h)
+
+// getInterpolatedElement31 (util/globalFuncs.h:102-116) on a planar plane of row stride w; the sum is ((a + b) + c) + d as in the reference
+__device__ __forceinline__ float interp31(const float* __restrict__ I, float x, float y, int w) {
+  const int ix = (int)x, iy = (int)y; const float dx = x - ix, dy = y - iy, dxdy = dx*dy; const float* bp = I + ix + iy*w;
+  return dxdy*__ldg(bp+1+w) + (dy-dxdy)*__ldg(bp+w) + (dx-dxdy)*__ldg(bp+1) + (1-dx-dy+dxdy)*__ldg(bp);
+}
+
+// ImmaturePoint::ImmaturePoint (ImmaturePoint.cpp:8-36) at integer pixel (u, v) of the level-0 plane I0 (row stride w); returns whether energyTH is finite.
+// Pt: sdv_immature_pt or its layout twin sel::ImmPt; Set: a settings struct with outlierTH, outlierTHSumComponent and overallEnergyTHWeight.
+template <class Pt, class Set>
+__device__ __forceinline__ bool imm_construct(const float* __restrict__ I0, int w, int u, int v, const Set& S, Pt& p) {
+  p.u = (float)u; p.v = (float)v; p.idepth_min = 0; p.idepth_max = NAN; p.lastTraceStatus = IPS_UNINITIALIZED;
+  for (int k = 0; k < 4; k++) p.gradH[k] = 0;
+  p.lastTraceUV[0] = p.lastTraceUV[1] = 0; p.quality = 10000; p.lastTracePixelInterval = 0; p.energyTH = NAN;
+  for (int k = 0; k < 8; k++) { p.color[k] = 0; p.weights[k] = 0; }
+  for (int idx = 0; idx < 8; idx++) {
+    const float x = p.u + staticPattern[idx][0], y = p.v + staticPattern[idx][1];
+    const int ix = (int)x, iy = (int)y; const float* bp = I0 + ix + iy*w;                         // getInterpolatedElement33BiLin, util/globalFuncs.h:142-164
+    const float tl = __ldg(bp), tr = __ldg(bp+1), bl = __ldg(bp+w), br = __ldg(bp+w+1);
+    const float dx = x - ix, dy = y - iy;
+    const float topInt = dx*tr + (1-dx)*tl, botInt = dx*br + (1-dx)*bl, leftInt = dy*bl + (1-dy)*tl, rightInt = dy*br + (1-dy)*tr;
+    const float c0 = dx*rightInt + (1-dx)*leftInt, gx = rightInt-leftInt, gy = botInt-topInt;
+    p.color[idx] = c0;
+    if (!isfinite(c0)) return false;
+    p.gradH[0] += gx*gx; p.gradH[1] += gx*gy; p.gradH[2] += gy*gx; p.gradH[3] += gy*gy;
+    p.weights[idx] = sqrtf(S.outlierTHSumComponent / (S.outlierTHSumComponent + (gx*gx + gy*gy)));
+  }
+  p.energyTH = 8*S.outlierTH; p.energyTH *= S.overallEnergyTHWeight*S.overallEnergyTHWeight;
+  return true;
 }
 
 namespace sel {

@@ -152,6 +152,11 @@ inline FrameDev* find_frame(sdv_ctx* c, uint64_t id) { auto it = c->frame_index.
 int  job_frame(sdv_ctx* c, const char* who, int k, uint64_t id, int cam, int slot, long long* need_seq, FrameDev** out);
 // SDV_ERR_ARG (with a message) unless every cams[k] of the n is a camera; cams == NULL: every entry is camera 0
 int  check_cams(sdv_ctx* c, int n, const int32_t* cams, const char* who, const char* what);
+// the argument checks of the batched entries, each SDV_ERR_ARG (with a message) when it fails: the CSR offsets off[0..n] (named `what`) start at 0 and never
+// decrease; each of the n ids (slots or windows) is in [0, limit) and none repeats; none of the n frame / host handles repeats
+int  check_offsets(sdv_ctx* c, int n, const int32_t* off, const char* who, const char* what);
+int  check_ids(sdv_ctx* c, int n, const int32_t* ids, int limit, const char* who, const char* what);
+int  check_distinct(sdv_ctx* c, int n, const uint64_t* ids, const char* who, const char* what);
 bool sel_cam_bound(const sdv_ctx* c, int cam, int* slot);                          // a selector slot (*slot) is bound to camera cam (sdv_selector_set_slot_cams)
 bool rp_slot_set(const sdv_ctx* c, int slot);                                     // map slot `slot` holds a resident map (sdv_map_set, not cleared)
 }

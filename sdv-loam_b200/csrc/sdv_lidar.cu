@@ -6,7 +6,6 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <vector>
-#include <unordered_set>
 #include "sdv_ctx.cuh"
 #include "sdv_pool.cuh"
 #include "sdv_lidar_core.cuh"
@@ -67,9 +66,8 @@ int sdv_lidar_handler_batch_cams(sdv_ctx* c, int n, const int32_t* sweep_begin, 
   if (!c || n < 0 || (n && (!sweep_begin || !Rlc9 || !tlc3 || !K4 || !lrud_io || !cloud3_out || !n_out || cap < 1))) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK;
   LidarState* s = (LidarState*)c->lidar; if (!s) return ctx_fail(c, SDV_ERR_STATE, "lidar_handler: sdv_lidar_init has not been called");
-  if (sweep_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler: sweep_begin[0] must be 0");
-  for (int j = 0; j < n; j++) { if (sweep_begin[j+1] < sweep_begin[j]) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler: sweep_begin is not ascending at sweep %d", j);
-    if (sweep_begin[j+1] > sweep_begin[j] && !xyzi) return SDV_ERR_ARG; }
+  { int rc = check_offsets(c, n, sweep_begin, "lidar_handler", "sweep_begin"); if (rc) return rc; }
+  if (sweep_begin[n] > 0 && !xyzi) return SDV_ERR_ARG;
   { int rc = check_cams(c, n, cams, "lidar_handler", "sweep"); if (rc) return rc; }
   CK(cudaSetDevice(c->device));
   std::vector<lidar::LidarEngine::Sweep> S(n);
@@ -98,13 +96,11 @@ int sdv_lidar_handler_rows_batch(sdv_ctx* c, int n, const int32_t* slots, const 
   LidarState* s = (LidarState*)c->lidar; if (!s) return ctx_fail(c, SDV_ERR_STATE, "lidar_handler_rows: sdv_lidar_init has not been called");
   const int ns = sel_n_slots(c); if (ns < 0) return ctx_fail(c, SDV_ERR_STATE, "lidar_handler_rows: sdv_selector_init has not been called (the pixel box lives with the selector slot)");
   if (cap < 1) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler_rows: cap %d (>= 1)", cap);
-  if (sweep_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler_rows: sweep_begin[0] must be 0");
-  std::vector<char> slot_seen(ns, 0); std::unordered_set<uint64_t> frame_seen; frame_seen.reserve(2*n);
-  for (int j = 0; j < n; j++) { if (sweep_begin[j+1] < sweep_begin[j]) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler_rows: sweep_begin is not ascending at sweep %d", j);
-    if (sweep_begin[j+1] > sweep_begin[j] && !xyzi) return SDV_ERR_ARG;
-    if (slots[j] < 0 || slots[j] >= ns) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler_rows: sweep %d names selector slot %d of %d", j, slots[j], ns);
-    if (slot_seen[slots[j]]++) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler_rows: slot %d appears twice in one call (the order of its box updates would be ambiguous)", slots[j]);
-    if (!frame_seen.insert(frames[j]).second) return ctx_fail(c, SDV_ERR_ARG, "lidar_handler_rows: frame %llu appears twice in one call", (unsigned long long)frames[j]); }
+  { int rc = check_offsets(c, n, sweep_begin, "lidar_handler_rows", "sweep_begin"); if (rc) return rc; }
+  if (sweep_begin[n] > 0 && !xyzi) return SDV_ERR_ARG;
+  // a slot named twice would leave the order of its box updates ambiguous
+  { int rc = check_ids(c, n, slots, ns, "lidar_handler_rows", "selector slot"); if (rc) return rc; }
+  { int rc = check_distinct(c, n, frames, "lidar_handler_rows", "frame"); if (rc) return rc; }
   CK(cudaSetDevice(c->device));
   RowStore* R = rows_store(c); std::vector<int> room(n, cap); std::vector<RowStore::Plan> P;
   { int rc = R->plan(c, n, frames, room.data(), P, "lidar row sets", "rows"); if (rc) return rc; }

@@ -213,11 +213,13 @@ int sdv_tracker_struct_pose_batch_slots(sdv_ctx* c, int n_jobs, const int32_t* s
                                         const double* host_T7, double* curToWorld_io, float* res_out, int32_t* iterations, int32_t* accepts) { SDV_GUARD_TRK(c);
   if (!c || n_jobs <= 0 || !pt_begin || !host_begin || !host_T7 || !curToWorld_io) return SDV_ERR_ARG;
   if (slots) for (int k=0;k<n_jobs;k++) if (slots[k] < 0 || slots[k] >= (int)c->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "struct_pose job %d: slot %d of %d", k, slots[k], (int)c->slots.size());
+  { int rc = check_offsets(c, n_jobs, pt_begin, "struct_pose", "pt_begin"); if (rc) return rc; }
+  { int rc = check_offsets(c, n_jobs, host_begin, "struct_pose", "host_begin"); if (rc) return rc; }
   const int nP = pt_begin[n_jobs], nH = host_begin[n_jobs];
-  if (pt_begin[0] != 0 || host_begin[0] != 0 || nP < 0 || nH <= 0 || (nP > 0 && !pts)) return SDV_ERR_ARG;   // both CSRs start at 0: nothing is indexed below it
+  if (nH <= 0 || (nP > 0 && !pts)) return SDV_ERR_ARG;
   for (int k=0;k<n_jobs;k++) {
     int hs = host_begin[k+1]-host_begin[k];
-    if (pt_begin[k+1] < pt_begin[k] || hs < 0 || hs > kRefMaxHosts) return ctx_fail(c, SDV_ERR_ARG, "struct_pose job %d: bad ranges (hosts %d, max %d)", k, hs, kRefMaxHosts);
+    if (hs > kRefMaxHosts) return ctx_fail(c, SDV_ERR_ARG, "struct_pose job %d: bad ranges (hosts %d, max %d)", k, hs, kRefMaxHosts);
     for (int i=pt_begin[k]; i<pt_begin[k+1]; i++) if (pts[i].host < 0 || pts[i].host >= hs) return ctx_fail(c, SDV_ERR_ARG, "struct_pose job %d: point %d names host %d of %d", k, i, pts[i].host, hs);
   }
   CK(cudaSetDevice(c->device));

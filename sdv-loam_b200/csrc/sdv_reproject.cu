@@ -64,12 +64,6 @@ __device__ __forceinline__ bool in_frame(int w, int h, double x, double y, int b
   const int ox = (int)x, oy = (int)y;
   return ox >= boundary && ox < w-boundary && oy >= boundary && oy < h-boundary;
 }
-__device__ __forceinline__ float interp_plane(const float* __restrict__ I, float x, float y, int width) {                       // getInterpolatedElement33()[0]
-  const int ix = (int)x, iy = (int)y; const float dx = x-ix, dy = y-iy, dxdy = dx*dy;
-  const float* bp = I + ix + iy*width;
-  return ((dxdy*__ldg(bp+1+width) + (dy-dxdy)*__ldg(bp+width)) + (dx-dxdy)*__ldg(bp+1)) + (1-dx-dy+dxdy)*__ldg(bp);
-}
-
 template <bool OWN_K>                                                          // OWN_K: as in find_match_direct
 __device__ __forceinline__ void project_point(const RpJob& jb, const RpConst& C, const MapDev* __restrict__ m, const sdv_map_pt& p, double* px) {
   double pw[3], c[3]; point_world(OWN_K ? jb.Ki : C.Ki, m, p, pw);
@@ -173,7 +167,7 @@ __device__ bool find_match_direct(const RpJob& jb, const RpConst& C, const sdv_m
         float p0 = (float)(x-5), p1 = (float)(y-5); p0 *= (1<<level); p1 *= (1<<level);
         const float qx = (a00*p0 + a01*p1) + prx, qy = (a10*p0 + a11*p1) + pry;
         float v = 0.f;
-        if (!(qx < 0 || qy < 0 || qx >= w0-1 || qy >= h0-1)) v = (float)(unsigned char)(interp_plane(I, qx, qy, w0));
+        if (!(qx < 0 || qy < 0 || qx >= w0-1 || qy >= h0-1)) v = (float)(unsigned char)(interp31(I, qx, qy, w0));
         sm.pwb[q] = v; } }
     __syncwarp(); }
   double pxs[2] = {px_io.x/(1<<level), px_io.y/(1<<level)};
@@ -353,7 +347,6 @@ int sdv_map_set_batch(sdv_ctx* c, int n, const int32_t* slots, const int32_t* ho
                       const double* host_ab, const int32_t* pt_begin, const sdv_map_pt* pts) { SDV_GUARD_TRK(c);
   if (!c || n < 0 || (n > 0 && (!slots || !host_begin || !pt_begin))) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK;
-  if (host_begin[0] != 0 || pt_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "sdv_map_set_batch: host_begin[0] and pt_begin[0] must be 0");
   return map_set_impl(c, n, slots, host_begin, host_frames, host_T7, host_ab, pt_begin, pts, cudaMemcpyHostToDevice);
 }
 }  // extern "C"
@@ -368,16 +361,15 @@ __global__ void map_copy_kernel(const MapCopySeg* __restrict__ seg, int nseg) {
 int sdv::map_set_impl(sdv_ctx* c, int n, const int32_t* slots, const int32_t* host_begin, const uint64_t* host_frames, const double* host_T7, const double* host_ab,
                       const int32_t* pt_begin, const sdv_map_pt* pts, cudaMemcpyKind kind) {
   if (!c) return SDV_ERR_ARG;
-  CK(cudaSetDevice(c->device)); RpState* st = rp_state(c);
   // every check of every job before any slot, pin or buffer changes
-  for (int j = 0; j < n; j++) if (host_begin[j+1] <= host_begin[j] || pt_begin[j+1] < pt_begin[j]) return SDV_ERR_ARG;
-  std::vector<char> seen(st->maps.size(), 0); std::vector<FrameDev*> F((size_t)host_begin[n]); long long need_seq = 0; size_t maxP = 0, totP = 0;
+  { int rc = check_offsets(c, n, host_begin, "sdv_map_set_batch", "host_begin"); if (rc) return rc; }
+  { int rc = check_offsets(c, n, pt_begin, "sdv_map_set_batch", "pt_begin"); if (rc) return rc; }
+  CK(cudaSetDevice(c->device)); RpState* st = rp_state(c);
+  { int rc = check_ids(c, n, slots, (int)st->maps.size(), "sdv_map_set_batch", "slot"); if (rc) return rc; }
+  std::vector<FrameDev*> F((size_t)host_begin[n]); long long need_seq = 0; size_t maxP = 0, totP = 0;
   for (int j = 0; j < n; j++) {
     const int nH = host_begin[j+1] - host_begin[j], nP = pt_begin[j+1] - pt_begin[j];
-    if (nH < 1 || nH > kRpMaxHosts || !host_frames || !host_T7 || nP < 0 || nP >= (1 << 27) || (nP > 0 && !pts)) return SDV_ERR_ARG;   // point index packs into 27 bits of the sort key
-    if (slots[j] < 0 || slots[j] >= (int)st->maps.size()) return SDV_ERR_ARG;
-    if (seen[slots[j]]) return ctx_fail(c, SDV_ERR_ARG, "sdv_map_set_batch: slot %d appears twice in one batch", slots[j]);
-    seen[slots[j]] = 1;
+    if (nH < 1 || nH > kRpMaxHosts || !host_frames || !host_T7 || nP >= (1 << 27) || (nP > 0 && !pts)) return SDV_ERR_ARG;   // point index packs into 27 bits of the sort key
     for (int k = host_begin[j]; k < host_begin[j+1]; k++) { int rcs = job_frame(c, "sdv_map_set", k - host_begin[j], host_frames[k], -1, slots[j], &need_seq, &F[k]); if (rcs) return rcs; }
     maxP = std::max(maxP, (size_t)nP); totP += nP;
   }

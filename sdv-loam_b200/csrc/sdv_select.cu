@@ -129,10 +129,8 @@ int sdv_selector_make_maps_batch(sdv_ctx* c, int n, const int32_t* slots, const 
   if (!c || n < 0 || (n && (!slots || !frames || !density || !recursions_left || !th_factor || !maps_out))) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK; SEL_STATE("selector_make_maps");
   const bool lidar = cloud_begin != nullptr; if (lidar && !cloud3) return SDV_ERR_ARG;
-  if (lidar) { if (cloud_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "selector_make_maps: cloud_begin[0] must be 0");
-    for (int j = 0; j < n; j++) if (cloud_begin[j+1] < cloud_begin[j]) return ctx_fail(c, SDV_ERR_ARG, "selector_make_maps: cloud_begin is not ascending at job %d", j); }
-  for (int j = 0; j < n; j++) { if (slots[j] < 0 || slots[j] >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "selector_make_maps: slot %d of %d", slots[j], (int)s->slots.size());
-    for (int k = 0; k < j; k++) if (slots[k] == slots[j]) return ctx_fail(c, SDV_ERR_ARG, "selector_make_maps: slot %d appears twice in one batch", slots[j]); }
+  if (lidar) { int rc = check_offsets(c, n, cloud_begin, "selector_make_maps", "cloud_begin"); if (rc) return rc; }
+  { int rc = check_ids(c, n, slots, (int)s->slots.size(), "selector_make_maps", "slot"); if (rc) return rc; }
   CK(cudaSetDevice(c->device));
   long long need = 0; std::vector<int> jw(n), jh(n);                                   // job j works at its slot's camera size
   for (int j = 0; j < n; j++) { const int cam = s->cam[slots[j]]; jw[j] = c->cam_w[cam]; jh[j] = c->cam_h[cam]; }
@@ -168,12 +166,10 @@ static int make_new_traces(sdv_ctx* c, int n, const int32_t* slots, const uint64
                            const float* density_dense, const int32_t* add_feature_point, int cap, sdv_new_trace* out, sdv_immature_pt* imm_out, int32_t* n_out, int32_t* num_points2,
                            const double* const* cloud_dev = nullptr /* job j's rows on the device (row sets), instead of cloud3 */) {
   if (n == 0) return SDV_OK; SEL_STATE("make_new_traces");
-  if (cloud_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: cloud_begin[0] must be 0");
-  for (int j = 0; j < n; j++) { if (cloud_begin[j+1] < cloud_begin[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: cloud_begin is not ascending at job %d", j);
-    if (cloud_begin[j+1] > cloud_begin[j] && !cloud3 && !cloud_dev) return SDV_ERR_ARG;
-    if (slots[j] < 0 || slots[j] >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: slot %d of %d", slots[j], (int)s->slots.size());
-    for (int k = 0; k < j; k++) if (slots[k] == slots[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces: slot %d appears twice in one batch", slots[j]);
-    if (!out) for (int k = 0; k < j; k++) if (frames[k] == frames[j]) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces_store: frame %llu appears twice in one batch", (unsigned long long)frames[j]); }
+  { int rc = check_offsets(c, n, cloud_begin, "make_new_traces", "cloud_begin"); if (rc) return rc; }
+  if (cloud_begin[n] > 0 && !cloud3 && !cloud_dev) return SDV_ERR_ARG;
+  { int rc = check_ids(c, n, slots, (int)s->slots.size(), "make_new_traces", "slot"); if (rc) return rc; }
+  if (!out) { int rc = check_distinct(c, n, frames, "make_new_traces_store", "frame"); if (rc) return rc; }
   CK(cudaSetDevice(c->device));
   long long need = 0; std::vector<sel::SelEngine::NewTracesJob> J(n);
   for (int j = 0; j < n; j++) { const int cam = s->cam[slots[j]]; int rc = sel_frame(c, j, frames[j], cam, J[j].img, J[j].gw2, need, "make_new_traces"); if (rc) return rc; J[j].w = c->cam_w[cam]; J[j].h = c->cam_h[cam];
@@ -210,7 +206,7 @@ int sdv_make_new_traces_rows_store_batch(sdv_ctx* c, int n, const int32_t* slots
                                          int32_t* num_points2) { SDV_GUARD_TRK(c);
   if (!c || n < 0 || (n && (!slots || !frames || !desired_density || !n_out || cap < 1))) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK; SEL_STATE("make_new_traces_rows");
-  for (int j = 0; j < n; j++) if (slots[j] < 0 || slots[j] >= (int)s->slots.size()) return ctx_fail(c, SDV_ERR_ARG, "make_new_traces_rows: slot %d of %d", slots[j], (int)s->slots.size());
+  { int rc = check_ids(c, n, slots, (int)s->slots.size(), "make_new_traces_rows", "slot"); if (rc) return rc; }
   CK(cudaSetDevice(c->device));
   std::vector<const double*> rows(n); std::vector<LidarRowsInfo> I(n);                   // all headers in one copy: the row counts size the engine's scratch and grids
   { int rc = lidar_rows_fetch(c, n, frames, rows.data(), I.data(), "make_new_traces_rows"); if (rc) return rc; }
@@ -232,15 +228,13 @@ static int init_from_lidar(sdv_ctx* c, int n, const int32_t* slots, const uint64
                            sdv_immature_pt* pts_out, sdv_immature_meta* meta_out, float* idepth_out) {
   const char* who = "init_from_lidar";
   if (n == 0) return SDV_OK; SEL_STATE("init_from_lidar");
-  const int ns = (int)c->slots.size();
-  if (cloud_begin[0] != 0 || draw_begin[0] < 0) return ctx_fail(c, SDV_ERR_ARG, "%s: cloud_begin[0] must be 0 and draw_begin[0] >= 0", who);
+  { int rc = check_offsets(c, n, cloud_begin, who, "cloud_begin"); if (rc) return rc; }
+  if (draw_begin[0] < 0) return ctx_fail(c, SDV_ERR_ARG, "%s: draw_begin[0] = %d (must be >= 0)", who, draw_begin[0]);
+  if (cloud_begin[n] > 0 && !cloud3 && !cloud_dev) return SDV_ERR_ARG;
   for (int j = 0; j < n; j++) { const int m = cloud_begin[j+1] - cloud_begin[j];
-    if (m < 0) return ctx_fail(c, SDV_ERR_ARG, "%s: cloud_begin is not ascending at job %d", who, j);
-    if (m > 0 && !cloud3 && !cloud_dev) return SDV_ERR_ARG;
-    if (draw_begin[j+1] - draw_begin[j] < m) return ctx_fail(c, SDV_ERR_ARG, "%s: job %d has %d rows and %d rand() draws", who, j, m, draw_begin[j+1] - draw_begin[j]);
-    if (slots[j] < 0 || slots[j] >= ns) return ctx_fail(c, SDV_ERR_ARG, "%s: slot %d of %d", who, slots[j], ns);
-    for (int k = 0; k < j; k++) { if (slots[k] == slots[j]) return ctx_fail(c, SDV_ERR_ARG, "%s: slot %d appears twice in one batch", who, slots[j]);
-      if (frames[k] == frames[j]) return ctx_fail(c, SDV_ERR_ARG, "%s: frame %llu appears twice in one batch", who, (unsigned long long)frames[j]); } }
+    if (draw_begin[j+1] - draw_begin[j] < m) return ctx_fail(c, SDV_ERR_ARG, "%s: job %d has %d rows and %d rand() draws", who, j, m, draw_begin[j+1] - draw_begin[j]); }
+  { int rc = check_ids(c, n, slots, (int)c->slots.size(), who, "slot"); if (rc) return rc; }
+  { int rc = check_distinct(c, n, frames, who, "frame"); if (rc) return rc; }
   CK(cudaSetDevice(c->device));
   long long need = 0; std::vector<FrameDev*> F(n); std::vector<int> cam(n);
   for (int j = 0; j < n; j++) { cam[j] = c->slots[slots[j]].cam;
@@ -332,13 +326,14 @@ int sel_activate_select(sdv_ctx* c, int n, const int32_t* host_begin, const int3
                         const float* min_act_dist, const int32_t* cams, int32_t* decision_out, float* dist_map_out) {
   if (!c || n < 0 || (n && (!host_begin || !pt_begin || !cand_host_begin || !cand_begin || !min_act_dist))) return SDV_ERR_ARG;
   if (n == 0) return SDV_OK; SEL_STATE("activate_select");
-  if (host_begin[0] != 0 || cand_host_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "activate_select: host_begin[0] and cand_host_begin[0] must be 0");
+  { int rc = check_offsets(c, n, host_begin, "activate_select", "host_begin"); if (rc) return rc; }
+  { int rc = check_offsets(c, n, cand_host_begin, "activate_select", "cand_host_begin"); if (rc) return rc; }
   { int rc = check_cams(c, n, cams, "activate_select", "sequence"); if (rc) return rc; }
   // the engine wants, per sequence, CSR offsets that start at 0: rebase the global ones
   std::vector<std::vector<int>> pb(n), cb(n); std::vector<sel::SelEngine::ActJob> J(n); size_t map_off = 0;     // distance maps back to back, each at its camera's level-1 size
   for (int j = 0; j < n; j++) {
     const int h0 = host_begin[j], h1 = host_begin[j+1], g0 = cand_host_begin[j], g1 = cand_host_begin[j+1];
-    if (h1 < h0 || g1 < g0 || h1 - h0 > 16 || g1 - g0 > 16) return ctx_fail(c, SDV_ERR_ARG, "activate_select: sequence %d has %d source / %d candidate keyframes (0..16)", j, h1 - h0, g1 - g0);
+    if (h1 - h0 > 16 || g1 - g0 > 16) return ctx_fail(c, SDV_ERR_ARG, "activate_select: sequence %d has %d source / %d candidate keyframes (0..16)", j, h1 - h0, g1 - g0);
     for (int k = h0; k <= h1; k++) { if (k > h0 && pt_begin[k] < pt_begin[k-1]) return ctx_fail(c, SDV_ERR_ARG, "activate_select: pt_begin is not ascending"); pb[j].push_back(pt_begin[k] - pt_begin[h0]); }
     for (int k = g0; k <= g1; k++) { if (k > g0 && cand_begin[k] < cand_begin[k-1]) return ctx_fail(c, SDV_ERR_ARG, "activate_select: cand_begin is not ascending"); cb[j].push_back(cand_begin[k] - cand_begin[g0]); }
     const int np = pb[j].back(), nc = cb[j].back();

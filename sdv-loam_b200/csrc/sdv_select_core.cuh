@@ -44,7 +44,6 @@ struct SelJob {                          // one select pass of one frame
 
 SDV_DEVCONST float kSelDirs[16][2] = {{0,1.0000f},{0.3827f,0.9239f},{0.1951f,0.9808f},{0.9239f,0.3827f},{0.7071f,0.7071f},{0.3827f,-0.9239f},{0.8315f,0.5556f},{0.8315f,-0.5556f},
                                       {0.5556f,-0.8315f},{0.9808f,0.1951f},{0.9239f,-0.3827f},{0.7071f,-0.7071f},{0.5556f,0.8315f},{0.9808f,-0.1951f},{1.0000f,0.0000f},{0.1951f,-0.9808f}};
-SDV_DEVCONST int kSelPat[8][2] = {{0,-2},{-1,-1},{1,-1},{-2,0},{0,0},{2,0},{-1,1},{0,2}};
 
 __device__ __forceinline__ int slot_of_cell(int cx, int cy, int nbx4) {                 // position of cell (cx,cy) in the reference's visiting order (4x4 block, 2x2 sub-block, cell)
   return (((cy>>2)*nbx4 + (cx>>2)) << 4) | (((cy>>1)&1) << 3) | (((cx>>1)&1) << 2) | ((cy&1) << 1) | (cx&1);
@@ -332,27 +331,6 @@ __device__ float shi_tomasi(const float* __restrict__ I, int w, int h, int u, in
   const float l1 = (float)(0.5*(dXX + dYY - disc)), l2 = (float)(0.5*(dXX + dYY + disc));
   const float k = 0.04f;
   return (l1*l2 - k*(l1+l2)*(l1+l2));
-}
-// ImmaturePoint::ImmaturePoint (ImmaturePoint.cpp:8-36), same arithmetic as imm_init_kernel (sdv_trace.cu); returns whether energyTH is finite
-__device__ bool imm_construct(const float* __restrict__ I0, int w, int u, int v, const SelSet& S, ImmPt& p) {
-  p.u = (float)u; p.v = (float)v; p.idepth_min = 0; p.idepth_max = NAN; p.lastTraceStatus = 5 /* IPS_UNINITIALIZED */;
-  for (int k = 0; k < 4; k++) p.gradH[k] = 0;
-  p.lastTraceUV[0] = p.lastTraceUV[1] = 0; p.quality = 10000; p.lastTracePixelInterval = 0; p.energyTH = NAN;
-  for (int k = 0; k < 8; k++) { p.color[k] = 0; p.weights[k] = 0; }
-  for (int idx = 0; idx < 8; idx++) {
-    const float x = p.u + kSelPat[idx][0], y = p.v + kSelPat[idx][1];
-    const int ix = (int)x, iy = (int)y; const float* bp = I0 + ix + iy*w;
-    const float tl = __ldg(bp), tr = __ldg(bp+1), bl = __ldg(bp+w), br = __ldg(bp+w+1);
-    const float dx = x - ix, dy = y - iy;
-    const float topInt = dx*tr + (1-dx)*tl, botInt = dx*br + (1-dx)*bl, leftInt = dy*bl + (1-dy)*tl, rightInt = dy*br + (1-dy)*tr;
-    const float c0 = dx*rightInt + (1-dx)*leftInt, gx = rightInt-leftInt, gy = botInt-topInt;
-    p.color[idx] = c0;
-    if (!isfinite(c0)) return false;
-    p.gradH[0] += gx*gx; p.gradH[1] += gx*gy; p.gradH[2] += gy*gx; p.gradH[3] += gy*gy;
-    p.weights[idx] = sqrtf(S.outlierTHSumComponent / (S.outlierTHSumComponent + (gx*gx + gy*gy)));
-  }
-  p.energyTH = 8*S.outlierTH; p.energyTH *= S.overallEnergyTHWeight*S.overallEnergyTHWeight;
-  return true;
 }
 __device__ __forceinline__ void paint_mask(unsigned char* occ, int w, int h, int Ku, int Kv, int pot) {        // FullSystem::setMask :1261-1271
   for (int i = Ku-pot; i <= Ku+pot; i++) for (int j = Kv-1; j <= Kv+1; j++) if (j < h && j >= 0 && i < w && i >= 0) occ[j*w + i] = 1;

@@ -23,8 +23,6 @@ using namespace sdv;
 
 namespace sdv {
 
-__constant__ int kTracePat[8][2] = {{0,-2},{-1,-1},{1,-1},{-2,0},{0,0},{2,0},{-1,1},{0,2}};   // staticPattern[8], util/settings.cpp:250
-enum { IPS_GOOD = 0, IPS_OOB, IPS_OUTLIER, IPS_SKIPPED, IPS_BADCONDITION, IPS_UNINITIALIZED };
 
 struct TraceGroupDev { const float* I0; float KRKi[9], Kt[3], aff[2]; int pt_begin, pt_end; int w, h; };   // one (host keyframe, traced frame) pair; w, h: its camera's size
 struct TraceSet { float outlierTH, outlierTHSumComponent, overallEnergyTHWeight, huberTH, maxPixSearch; int minTraceTestRadius; float stepsize; int GNIterations;
@@ -33,10 +31,6 @@ struct TraceSet { float outlierTH, outlierTHSumComponent, overallEnergyTHWeight,
 // dIp[0][idx] = {I, dx, dy} from the planar level-0 plane
 __device__ __forceinline__ void texel0(const float* __restrict__ I, int idx, int w, int h, float& c, float& dx, float& dy) {
   c = __ldg(I + idx); planar_grad(I, idx, w, h, dx, dy);
-}
-__device__ __forceinline__ float interp31(const float* __restrict__ I, float x, float y, int w) {   // getInterpolatedElement31, util/globalFuncs.h:102-116
-  const int ix = (int)x, iy = (int)y; const float dx = x - ix, dy = y - iy, dxdy = dx*dy; const float* bp = I + ix + iy*w;
-  return dxdy*__ldg(bp+1+w) + (dy-dxdy)*__ldg(bp+w) + (dx-dxdy)*__ldg(bp+1) + (1-dx-dy+dxdy)*__ldg(bp);
 }
 __device__ __forceinline__ void interp33(const float* __restrict__ I, float x, float y, int w, int h, float out[3]) {   // getInterpolatedElement33, :51-65
   const int ix = (int)x, iy = (int)y; const float dx = x - ix, dy = y - iy, dxdy = dx*dy; const int b = ix + iy*w;
@@ -47,31 +41,10 @@ __device__ __forceinline__ void interp33(const float* __restrict__ I, float x, f
   for (int k = 0; k < 3; k++) out[k] = w11*c11[k] + w01*c01[k] + w10*c10[k] + w00*c00[k];
 }
 
-// ---- ImmaturePoint::ImmaturePoint (ImmaturePoint.cpp:8-36) at integer pixel (u, v) of the level-0 plane I0 (row stride w)
-__device__ __forceinline__ void imm_construct(const float* __restrict__ I0, int w, int u, int v, sdv_immature_pt& p, const TraceSet& S) {
-  p.u = (float)u; p.v = (float)v; p.idepth_min = 0; p.idepth_max = NAN; p.lastTraceStatus = IPS_UNINITIALIZED;
-  for (int k = 0; k < 4; k++) p.gradH[k] = 0;
-  p.lastTraceUV[0] = p.lastTraceUV[1] = 0; p.quality = 10000; p.lastTracePixelInterval = 0; p.energyTH = NAN;
-  for (int k = 0; k < 8; k++) { p.color[k] = 0; p.weights[k] = 0; }
-  bool finite = true;
-  for (int idx = 0; idx < 8 && finite; idx++) {
-    const float x = p.u + kTracePat[idx][0], y = p.v + kTracePat[idx][1];
-    const int ix = (int)x, iy = (int)y; const float* bp = I0 + ix + iy*w;                       // getInterpolatedElement33BiLin, util/globalFuncs.h:142-164
-    const float tl = __ldg(bp), tr = __ldg(bp+1), bl = __ldg(bp+w), br = __ldg(bp+w+1);
-    const float dx = x - ix, dy = y - iy;
-    const float topInt = dx*tr + (1-dx)*tl, botInt = dx*br + (1-dx)*bl, leftInt = dy*bl + (1-dy)*tl, rightInt = dy*br + (1-dy)*tr;
-    const float c0 = dx*rightInt + (1-dx)*leftInt, gx = rightInt-leftInt, gy = botInt-topInt;
-    p.color[idx] = c0;
-    if (!isfinite(c0)) { finite = false; break; }
-    p.gradH[0] += gx*gx; p.gradH[1] += gx*gy; p.gradH[2] += gy*gx; p.gradH[3] += gy*gy;
-    p.weights[idx] = sqrtf(S.outlierTHSumComponent / (S.outlierTHSumComponent + (gx*gx + gy*gy)));
-  }
-  if (finite) { p.energyTH = 8*S.outlierTH; p.energyTH *= S.overallEnergyTHWeight*S.overallEnergyTHWeight; }
-}
 // one thread per candidate
 __global__ void __launch_bounds__(128) imm_init_kernel(const float* __restrict__ I0, int w, int h, int n, const int* __restrict__ uv, sdv_immature_pt* __restrict__ out, TraceSet S) {
   const int i = blockIdx.x*blockDim.x + threadIdx.x; if (i >= n) return;
-  sdv_immature_pt p; imm_construct(I0, w, uv[2*i], uv[2*i+1], p, S);
+  sdv_immature_pt p; imm_construct(I0, w, uv[2*i], uv[2*i+1], S, p);
   out[i] = p;
 }
 
@@ -130,7 +103,7 @@ __device__ int trace_on(sdv_immature_pt& p, const float* __restrict__ I, int wG0
   float ptx = uMin-randShift*dx, pty = vMin-randShift*dy;
   float rpx[8], rpy[8];
 #pragma unroll
-  for (int idx = 0; idx < 8; idx++) { const float px = (float)kTracePat[idx][0], py = (float)kTracePat[idx][1]; rpx[idx] = R00*px + R01*py; rpy[idx] = R10*px + R11*py; }
+  for (int idx = 0; idx < 8; idx++) { const float px = (float)staticPattern[idx][0], py = (float)staticPattern[idx][1]; rpx[idx] = R00*px + R01*py; rpy[idx] = R10*px + R11*py; }
   if (!isfinite(dx) || !isfinite(dy)) { p.lastTracePixelInterval = 0; p.lastTraceUV[0] = -1; p.lastTraceUV[1] = -1; return p.lastTraceStatus = IPS_OOB; }
   float errors[100]; float bestU = 0, bestV = 0, bestEnergy = 1e10f; int bestIdx = -1;
   if (numSteps >= 100) numSteps = 99;
@@ -225,7 +198,7 @@ __device__ double linearize_residual(const sdv_immature_pt& p, const OptTargetDe
   if (r.state_state == RS_OOB) { r.state_NewState = RS_OOB; return r.state_energy; }
   float energyLeft = 0; const float wM3G = (float)(wG0-3), hM3G = (float)(hG0-3);
   for (int idx = 0; idx < 8; idx++) {
-    const int dx = kTracePat[idx][0], dy = kTracePat[idx][1];
+    const int dx = staticPattern[idx][0], dy = staticPattern[idx][1];
     const float K0 = (p.u+dx-C.cxl)*C.fxli, K1 = (p.v+dy-C.cyl)*C.fyli, K2 = 1;
     float ptp[3];
 #pragma unroll
@@ -460,7 +433,7 @@ __global__ void __launch_bounds__(256) init_points_kernel(const InitPointsJob* _
     if (sel && !((float)J.draws[k] / (float)2147483647 > keepPercentage)) {                      // glibc RAND_MAX
       pu = (int)((float)J.cloud[3*i] + 0.5f); pv = (int)((float)J.cloud[3*i+1] + 0.5f);
       keep = pu >= 0 && pu < w && pv >= 0 && pv < h && pu + (pv-2)*w >= 0 && pu + 1 + (pv+3)*w < w*h;
-      if (keep) { imm_construct(J.I0, w, pu, pv, p, S); keep = isfinite(p.energyTH); }
+      if (keep) { imm_construct(J.I0, w, pu, pv, S, p); keep = isfinite(p.energyTH); }
     }
     const int o = obase + block_excl_scan(keep, wt, tot); obase += tot;
     if (keep) {
@@ -508,8 +481,7 @@ int sdv_immature_trace_batch_cams(sdv_ctx* c, int n_groups, const uint64_t* fram
   if (!c || n_groups < 0 || (n_groups && (!frames || !pt_begin || !KRKi9 || !Kt3 || !aff2))) return SDV_ERR_ARG;
   if (n_groups == 0) return SDV_OK;
   { int rc = check_cams(c, n_groups, cams, "immature_trace", "group"); if (rc) return rc; }
-  if (pt_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "immature_trace: pt_begin[0] must be 0");
-  for (int g = 0; g < n_groups; g++) if (pt_begin[g+1] < pt_begin[g]) return ctx_fail(c, SDV_ERR_ARG, "immature_trace: pt_begin is not ascending at group %d", g);
+  { int rc = check_offsets(c, n_groups, pt_begin, "immature_trace", "pt_begin"); if (rc) return rc; }
   const int n = pt_begin[n_groups];
   if (n == 0) return SDV_OK;
   if (!pts_io) return SDV_ERR_ARG;
@@ -547,9 +519,9 @@ int sdv_immature_optimize_batch_cams(sdv_ctx* c, int n_groups, const int32_t* pt
   if (!c || n_groups < 0 || (n_groups && (!pt_begin || !tgt_begin || !target_frames || !pre14 || !calib6))) return SDV_ERR_ARG;
   if (n_groups == 0) return SDV_OK;
   { int rc = check_cams(c, n_groups, cams, "immature_optimize", "group"); if (rc) return rc; }
-  if (pt_begin[0] != 0 || tgt_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "immature_optimize: pt_begin[0] and tgt_begin[0] must be 0");
-  for (int g = 0; g < n_groups; g++) { if (pt_begin[g+1] < pt_begin[g] || tgt_begin[g+1] < tgt_begin[g]) return ctx_fail(c, SDV_ERR_ARG, "immature_optimize: offsets not ascending at group %d", g);
-    const int nres = tgt_begin[g+1] - tgt_begin[g]; if (nres > kOptMaxRes || nres > res_stride) return ctx_fail(c, SDV_ERR_ARG, "immature_optimize: group %d has %d targets (max %d, res_stride %d)", g, nres, kOptMaxRes, res_stride); }
+  { int rc = check_offsets(c, n_groups, pt_begin, "immature_optimize", "pt_begin"); if (rc) return rc; }
+  { int rc = check_offsets(c, n_groups, tgt_begin, "immature_optimize", "tgt_begin"); if (rc) return rc; }
+  for (int g = 0; g < n_groups; g++) { const int nres = tgt_begin[g+1] - tgt_begin[g]; if (nres > kOptMaxRes || nres > res_stride) return ctx_fail(c, SDV_ERR_ARG, "immature_optimize: group %d has %d targets (max %d, res_stride %d)", g, nres, kOptMaxRes, res_stride); }
   const int n = pt_begin[n_groups], nt = tgt_begin[n_groups];
   if (n == 0) return SDV_OK;
   if (!pts || !status_out || !idepth_out || !res_state_out || res_stride < 1) return SDV_ERR_ARG;
@@ -643,13 +615,12 @@ int sdv_immature_trace_store_batch(sdv_ctx* c, int n_groups, const uint64_t* hos
   if (!c || n_groups < 0 || (n_groups && (!hosts || !frames || !KRKi9 || !Kt3 || !aff2))) return SDV_ERR_ARG;
   if (n_groups == 0) return SDV_OK;
   { int rc = check_cams(c, n_groups, cams, "immature_trace_store", "group"); if (rc) return rc; }
+  { int rc = check_distinct(c, n_groups, hosts, "immature_trace_store", "host"); if (rc) return rc; }
   const ImmStore* S = (const ImmStore*)c->imm_store;
   std::vector<TraceStoreGroupDev> G(n_groups); std::vector<int> gbeg(n_groups + 1, 0); std::vector<FrameDev*> F(n_groups); long long need_seq = 0;
-  std::unordered_map<uint64_t, int> seen; seen.reserve(2*n_groups);
   for (int g = 0; g < n_groups; g++) {
     auto bt = S ? S->blocks.find(hosts[g]) : decltype(S->blocks.end())();
     if (!S || bt == S->blocks.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "immature_trace_store: host %llu has no block (group %d)", (unsigned long long)hosts[g], g);
-    if (!seen.emplace(hosts[g], g).second) return ctx_fail(c, SDV_ERR_ARG, "immature_trace_store: host %llu in groups %d and %d", (unsigned long long)hosts[g], seen[hosts[g]], g);
     const int cam = cams ? cams[g] : 0; { int rc = job_frame(c, "immature_trace_store", g, frames[g], cam, -1, &need_seq, &F[g]); if (rc) return rc; }
     const ImmBlock& blk = bt->second; TraceStoreGroupDev& D = G[g];
     D.I0 = F[g]->I0; D.w = c->cam_w[cam]; D.h = c->cam_h[cam]; D.ro = blk.ro; D.rw = blk.rw;
@@ -694,17 +665,16 @@ int sdv_activate_points_store_batch(sdv_ctx* c, int n, const int32_t* host_begin
   if (cap > 0 && (!act_host || !act_idx || !act_pts || !act_meta || !act_idepth || !act_res_state)) return SDV_ERR_ARG;
   if (!c->sel) return ctx_fail(c, SDV_ERR_STATE, "activate_points_store: sdv_selector_init has not been called");
   { int rc = check_cams(c, n, cams, "activate_points_store", "sequence"); if (rc) return rc; }
-  if (host_begin[0] != 0) return ctx_fail(c, SDV_ERR_ARG, "activate_points_store: host_begin[0] must be 0");
+  { int rc = check_offsets(c, n, host_begin, "activate_points_store", "host_begin"); if (rc) return rc; }
   for (int j = 0; j < n; j++) { const int nH = host_begin[j+1] - host_begin[j];
     if (nH < 1 || nH > 16 || nH - 1 > SDV_MAX_FRAMES_WINDOW) return ctx_fail(c, SDV_ERR_ARG, "activate_points_store: sequence %d has %d keyframes (1..16, at most %d targets)", j, nH, SDV_MAX_FRAMES_WINDOW); }
   const int NH = host_begin[n]; const ImmStore* S = (const ImmStore*)c->imm_store;
+  { int rc = check_distinct(c, NH, hosts, "activate_points_store", "host"); if (rc) return rc; }
   std::vector<int> seq_of(NH), gbeg(NH + 1, 0), pre_begin(n + 1, 0); std::vector<FrameDev*> F(NH); std::vector<ActHostDev> HD(NH); long long need_seq = 0;
-  std::unordered_map<uint64_t, int> seen; seen.reserve(2*NH);
   for (int j = 0; j < n; j++) { const int nH = host_begin[j+1] - host_begin[j]; pre_begin[j+1] = pre_begin[j] + nH*(nH - 1);
     for (int g = host_begin[j]; g < host_begin[j+1]; g++) { seq_of[g] = j;
       auto bt = S ? S->blocks.find(hosts[g]) : decltype(S->blocks.end())();
       if (!S || bt == S->blocks.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "activate_points_store: host %llu has no block", (unsigned long long)hosts[g]);
-      if (!seen.emplace(hosts[g], g).second) return ctx_fail(c, SDV_ERR_ARG, "activate_points_store: host %llu appears twice", (unsigned long long)hosts[g]);
       { int rc = job_frame(c, "activate_points_store", g, hosts[g], cams ? cams[j] : 0, -1, &need_seq, &F[g]); if (rc) return rc; }
       const ImmBlock& blk = bt->second; HD[g] = ActHostDev{blk.ro, blk.rw, blk.meta, g == host_begin[j+1] - 1 ? 1 : 0, flagged[g] ? 1 : 0}; gbeg[g+1] = gbeg[g] + blk.n; } }
   const int N = gbeg[NH];
