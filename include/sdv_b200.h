@@ -128,9 +128,11 @@ int  sdv_frame_build_batch_dev(sdv_ctx* c, int n, const uint64_t* frames, const 
  * valid and unmodified until sdv_frame_release / the handle is re-uploaded — for producers that already write into device memory). */
 /* Cameras of different rectified sizes in one context (KITTI 1200x360 next to KITTI-360 1400x360).  Camera 0 always has the context size (sdv_create's
  * w, h); cameras 1..SDV_MAX_CAMERAS-1 start at it.  sdv_set_camera_size gives camera `cam` another rectified size w x h: w <= the context's w, h <= its
- * h (frame storage is allocated at the context size: create the context at the largest size), and the context's pyramid depth valid at that size (even
- * w, h when levels > 1, every level non-empty).  Camera 0, a camera index out of range or a size outside these rules return SDV_ERR_ARG; resizing a
- * camera that has Undistort tables, a resident frame or a bound tracker or selector slot (sdv_set_calib_slots_cams, sdv_selector_set_slot_cams) returns SDV_ERR_STATE.  A refused call changes nothing.
+ * h (the reprojection grid, tracker-slot clouds and keyframe-rate scratch have the context size: create the context at the largest size), and the
+ * context's pyramid depth valid at that size (even w, h when levels > 1, every level non-empty).  Frames are stored in the context's pool at the context
+ * size unless the camera has a pool of its own at its size (sdv_set_camera_storage).  Camera 0, a camera index out of range or a size outside these rules
+ * return SDV_ERR_ARG; resizing a camera that has Undistort tables, a resident frame, a bound tracker or selector slot (sdv_set_calib_slots_cams,
+ * sdv_selector_set_slot_cams) or a frame pool of its own returns SDV_ERR_STATE.  A refused call changes nothing.
  * sdv_set_undistort_cam then takes remap tables of that camera's size.  A frame has the size of the camera it was ingested for:
  * sdv_frame_upload_batch_cams takes host float (fmt 0) or mono8 (fmt 1) images, and sdv_frame_build_batch_dev_cams device images with the fmt values of
  * sdv_frame_build_batch_dev (fmt 2 adopts a buffer of w_cam*h_cam floats), each at its camera's size.  cams == NULL is camera 0 (the entries without
@@ -141,6 +143,21 @@ int  sdv_frame_build_batch_dev(sdv_ctx* c, int n, const uint64_t* frames, const 
  * (selector, makeNewTraces, activation, immature points, LiDAR front-end) names a camera per job (the _cam / _cams entries, sdv_selector_set_slot_cams)
  * and works at that camera's size; a frame of another size returns SDV_ERR_ARG and changes no state.  The entries without _cam(s) are camera 0. */
 int  sdv_set_camera_size(sdv_ctx* c, int cam, int w, int h);
+/* Frame storage per camera.  sdv_create allocates the context pool: max_frames frames and max_kf_images keyframe level-0 images at the context size, for
+ * every camera.  sdv_set_camera_storage gives camera `cam` (1..SDV_MAX_CAMERAS-1) a pool of its own at its rectified size (sdv_set_camera_size):
+ * max_frames frames and max_kf_images keyframe level-0 images (0: the default of sdv_settings::max_kf_images; at most max_frames).  The storage depth stays
+ * the context's `levels`.  From then on every frame of the camera is claimed from that pool and its keyframe images too, with no fallback to the context
+ * pool: a full pool returns SDV_ERR_CAPACITY.  A handle resident in another pool than its new camera's moves when it is uploaded again: every image of
+ * the upload is given its frame first, and a full pool (SDV_ERR_CAPACITY) or a pinned handle (SDV_ERR_STATE) refuses the whole upload with every handle
+ * left as it was; then each moved handle's old frame is released as sdv_frame_release would.  Adopted level-0 buffers (fmt 2) work as before: only the levels >= 1 and the texel caches come from the pool.  max_frames == 0 drops the
+ * camera's pool: its frames come from the context pool again.  Camera 0, a camera out of range or a negative count return SDV_ERR_ARG; replacing or
+ * dropping a pool while one of its frames is resident or one of its keyframe images is taken returns SDV_ERR_STATE.  All-or-nothing: the new pool is
+ * allocated before the old one is freed, and a failed allocation returns SDV_ERR_CUDA with the old pool in place.  Waits for the context's streams.
+ * sdv_camera_storage_bytes: the device bytes of one frame and of one keyframe level-0 image of camera `cam` (0..SDV_MAX_CAMERAS-1) as they are stored now
+ * (its own pool, or the context size); either pointer may be NULL.  A frame is 4 w h + 20 P bytes with P = sum over levels l >= 1 of (w>>l)(h>>l), a
+ * keyframe image 16 w h. */
+int  sdv_set_camera_storage(sdv_ctx* c, int cam, int max_frames, int max_kf_images);
+int  sdv_camera_storage_bytes(sdv_ctx* c, int cam, uint64_t* frame_bytes, uint64_t* kf_image_bytes);
 /* Cameras of different pyramid depths in one context (pyrLevelsUsed, util/globalCalib.cpp:22-30: KITTI-CARLA's 1392x1024 has 5 levels, KITTI's 1200x360 4).
  * sdv_create's `levels` is the STORAGE depth: every frame is built to it, whatever its camera.  A camera's depth is what its tracker / map slots and jobs
  * use, as the reference's pyrLevelsUsed: sdv_tracker_set_ref builds clouds for that many levels, trackNewestCoarse starts at depth - 1 by default

@@ -123,6 +123,13 @@ int shim_camera_depths(int n_cams, const int* w, const int* h) {
   for (int cam = 0; cam < n_cams; cam++) rc |= sdv_set_camera_levels(gpu, cam, sdv_pyr_levels(w[cam], h[cam]));
   return rc;
 }
+// §4 frame storage per camera: each camera's pool at its own size (before its first frame), and the bytes one frame and one keyframe image take there
+int shim_camera_storage(int n_cams, const int* max_frames, const int* max_kf_images, uint64_t* frame_bytes, uint64_t* kf_bytes) {
+  int rc = 0;
+  for (int cam = 1; cam < n_cams; cam++) rc |= sdv_set_camera_storage(gpu, cam, max_frames[cam], max_kf_images[cam]);
+  for (int cam = 0; cam < n_cams; cam++) rc |= sdv_camera_storage_bytes(gpu, cam, &frame_bytes[cam], &kf_bytes[cam]);
+  return rc;
+}
 int shim_track_own_depths(int n, const int32_t* slots, const uint64_t* frames, double* T, double* ab, double* lastRes, double* flow, int32_t* good) {
   return sdv_tracker_track_batch_levels(gpu, n, slots, frames, T, ab, /*each job at its camera's depth - 1*/nullptr, nullptr, lastRes, flow, good, nullptr);
 }

@@ -59,6 +59,8 @@ def _load():
     L.sdv_set_calib_slots_cams.argtypes = [_vp, C.c_int, _i32p, _vp, _vp]
     L.sdv_set_camera_size.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.sdv_set_camera_levels.argtypes = [_vp, C.c_int, C.c_int]
+    L.sdv_set_camera_storage.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
+    L.sdv_camera_storage_bytes.argtypes = [_vp, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.sdv_frame_upload_batch_cams.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _vp, C.c_int, _f32p]
     L.sdv_frame_build_batch_dev_cams.argtypes = [_vp, C.c_int, _u64p, C.POINTER(_vp), _vp, C.c_int, _f32p]
     L.sdv_frame_upload.argtypes = [_vp, C.c_uint64, _vp, C.c_float]
@@ -192,6 +194,17 @@ class Context:
     def setCameraSize(self, cam: int, w: int, h: int):
         """give camera `cam` (1..SDV_MAX_CAMERAS-1) the rectified size w x h <= the context size, at the context's pyramid depth (see sdv_b200.h)"""
         self._ck(LIB.sdv_set_camera_size(self.p, int(cam), int(w), int(h))); self.cam_wh[int(cam)] = (int(w), int(h))
+
+    def setCameraStorage(self, cam: int, max_frames: int, max_kf_images: int = 0):
+        """give camera `cam` (1..SDV_MAX_CAMERAS-1) its own pool of max_frames frames and max_kf_images keyframe level-0 images (0: the default) at its
+        size; max_frames == 0 drops it (its frames come from the context pool again).  See sdv_b200.h"""
+        self._ck(LIB.sdv_set_camera_storage(self.p, int(cam), int(max_frames), int(max_kf_images)))
+
+    def cameraStorageBytes(self, cam: int = 0):
+        """(frame_bytes, kf_image_bytes): device bytes of one frame and one keyframe level-0 image of camera `cam` as they are stored now"""
+        fb, kb = C.c_uint64(), C.c_uint64()
+        self._ck(LIB.sdv_camera_storage_bytes(self.p, int(cam), C.byref(fb), C.byref(kb)))
+        return int(fb.value), int(kb.value)
 
     def camLevels(self, cam: int = 0) -> int:
         """pyramid depth (pyrLevelsUsed) of camera `cam`: what its tracker / map slots and jobs use"""

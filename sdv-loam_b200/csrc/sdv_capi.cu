@@ -96,7 +96,8 @@ int sdv_set_calib_slots_cams(sdv_ctx* c, int n, const int32_t* slots, const sdv_
 }
 int sdv_set_calib_slots(sdv_ctx* c, int n, const int32_t* slots, const sdv_calib* K) { return sdv_set_calib_slots_cams(c, n, slots, K, nullptr); }
 
-// A camera's rectified size: at most the context size (frame storage), with the context's pyramid depth.  Refused while anything depends on the old size.
+// A camera's rectified size: at most the context size, with the context's pyramid depth.  Refused while anything depends on the old size, its own
+// frame pool included (sized for the old size).
 int sdv_set_camera_size(sdv_ctx* c, int cam, int w, int h) { SDV_GUARD_TRK(c);
   if (!c) return SDV_ERR_ARG;
   if (cam == 0) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_camera_size: camera 0 always has the context size %dx%d", c->w, c->h);
@@ -106,6 +107,7 @@ int sdv_set_camera_size(sdv_ctx* c, int cam, int w, int h) { SDV_GUARD_TRK(c);
   if ((w >> (c->levels - 1)) < 1 || (h >> (c->levels - 1)) < 1) return ctx_fail(c, SDV_ERR_ARG, "sdv_set_camera_size: %dx%d has an empty level at the context's %d levels", w, h, c->levels);
   if (w == c->cam_w[cam] && h == c->cam_h[cam]) return SDV_OK;
   if (c->und.cam[cam].remapX) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_size: camera %d has Undistort tables of its current size", cam);
+  if (c->pools[cam].n_frames > 0) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_size: camera %d has a frame pool of its current size (sdv_set_camera_storage)", cam);
   for (const FrameDev& f : c->frames) if (f.used && f.cam == cam) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_size: camera %d has resident frame %llu", cam, (unsigned long long)f.id);
   for (size_t s=0;s<c->slots.size();s++) if (c->slots[s].cam == cam) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_size: slot %d is bound to camera %d", (int)s, cam);
   { int s; if (sel_cam_bound(c, cam, &s)) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_size: selector slot %d is bound to camera %d", s, cam); }
@@ -125,6 +127,79 @@ int sdv_set_camera_levels(sdv_ctx* c, int cam, int levels) { SDV_GUARD_TRK(c);
                     c->slots[s].ref_frame != ~0ull ? "tracker reference" : "map", c->cam_levels[cam]);
   { int s; if (levels < 3 && sel_cam_bound(c, cam, &s)) return ctx_fail(c, SDV_ERR_STATE, "sdv_set_camera_levels: selector slot %d is bound to camera %d and reads levels 0..2", s, cam); }
   c->cam_levels[cam] = levels;
+  return SDV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ frame storage
+// One frame of a pool of w x h: planar intensity of every level (level 0, plus one allocation for levels >= 1) and the storage of the packed-texel cache
+// of levels >= 1, both at the offsets of the frame's own size (frame_layout); packed level-0 texels come from the pool's keyframe level-0 images.
+static size_t pyr_texels(int w, int h, int levels) { size_t n = 0; for (int l=1;l<levels;l++) n += (size_t)(w>>l)*(h>>l); return n; }
+static uint64_t frame_bytes(int w, int h, int levels) { return (uint64_t)w*h*sizeof(float) + pyr_texels(w, h, levels)*(sizeof(float) + sizeof(float4)); }
+static uint64_t kf_image_bytes(int w, int h) { return (uint64_t)w*h*sizeof(float4); }
+static int kf_count(int max_kf_images, int max_frames) { const int n = max_kf_images > 0 ? max_kf_images : SDV_MAX_FRAMES_WINDOW + 4; return n > max_frames ? max_frames : n; }
+// every field set before the first allocation, so frame_free is safe on a frame whose allocation failed half way
+static cudaError_t frame_alloc(FrameDev& f, int pool, int w, int h, int levels) {
+  f = FrameDev{}; f.lvl0_slot = -1; f.pool = pool;
+  const size_t texels = pyr_texels(w, h, levels);
+  cudaError_t e = cudaMalloc(&f.I0_own, (size_t)w*h*sizeof(float)); f.I0 = f.I0_own; f.img[0] = f.I0;
+  if (e == cudaSuccess && texels) e = cudaMalloc(&f.pyr, texels*sizeof(float));
+  if (e == cudaSuccess && texels) e = cudaMalloc(&f.base, texels*sizeof(float4));
+  return e;
+}
+static void frame_free(FrameDev& f) { cudaFree(f.base); cudaFree(f.pyr); cudaFree(f.I0_own); f.base = nullptr; f.pyr = nullptr; f.I0_own = nullptr; }
+static cudaError_t kf_alloc(FramePool& P, int n, int w, int h) {
+  P.lvl0.assign(n, nullptr); P.lvl0_free.clear();
+  for (int i=0;i<n;i++) { cudaError_t e = cudaMalloc(&P.lvl0[i], kf_image_bytes(w, h)); if (e != cudaSuccess) return e; P.lvl0_free.push_back(n-1-i); }
+  return cudaSuccess;
+}
+static void kf_free(FramePool& P) { for (float4* p : P.lvl0) cudaFree(p); P.lvl0.clear(); P.lvl0_free.clear(); }
+// where the levels >= 1 of a frame of camera f.cam sit in its storage: level l at the sum of the sizes of levels 1..l-1 of the camera's own size, in every
+// pool (pyr_fused_kernel writes them there); set whenever the frame is claimed for a camera
+static void frame_layout(const sdv_ctx* c, FrameDev& f) {
+  const int w = c->cam_w[f.cam], h = c->cam_h[f.cam]; size_t off = 0;
+  for (int l=1;l<c->levels;l++) { f.img[l] = f.pyr + off; f.lvl[l] = f.base + off; off += (size_t)(w>>l)*(h>>l); }
+}
+
+// Camera cam's own frame pool: max_frames frames and max_kf_images keyframe level-0 images (0: the default, at most max_frames) at its rectified size, or,
+// with max_frames == 0, none (its frames come from the context pool again).  Refused while a frame of the pool is resident or one of its keyframe images is
+// taken.  All-or-nothing: the new pool is allocated before the old one is freed.
+int sdv_set_camera_storage(sdv_ctx* c, int cam, int max_frames, int max_kf_images) { SDV_GUARD_TRK(c);
+  const char* who = "sdv_set_camera_storage";
+  if (!c) return SDV_ERR_ARG;
+  if (cam < 1 || cam >= SDV_MAX_CAMERAS) return ctx_fail(c, SDV_ERR_ARG, "%s: camera %d outside 1..%d (camera 0 uses the context pool)", who, cam, SDV_MAX_CAMERAS - 1);
+  if (max_frames < 0 || max_kf_images < 0) return ctx_fail(c, SDV_ERR_ARG, "%s: negative count (max_frames %d, max_kf_images %d)", who, max_frames, max_kf_images);
+  FramePool& P = c->pools[cam];
+  for (const FrameDev& f : c->frames) if (f.used && f.pool == cam)
+    return ctx_fail(c, SDV_ERR_STATE, "%s: frame %llu of camera %d's pool is resident: release it first", who, (unsigned long long)f.id, cam);
+  if (P.lvl0_free.size() != P.lvl0.size()) return ctx_fail(c, SDV_ERR_STATE, "%s: a keyframe image of camera %d's pool is taken", who, cam);
+  if (max_frames == 0 && P.n_frames == 0) return SDV_OK;
+  CK(cudaSetDevice(c->device));
+  CK(cudaStreamSynchronize(c->st_cp)); CK(cudaStreamSynchronize(c->st_in)); CK(cudaStreamSynchronize(c->st)); CK(cudaStreamSynchronize(c->st_ba));   // work enqueued before may still read the old pool's released frames
+  const int w = c->cam_w[cam], h = c->cam_h[cam];
+  std::vector<FrameDev> nf(max_frames); FramePool np; np.w = w; np.h = h; np.n_frames = max_frames;
+  cudaError_t e = cudaSuccess;
+  for (auto& f : nf) if ((e = frame_alloc(f, cam, w, h, c->levels)) != cudaSuccess) break;
+  if (e == cudaSuccess && max_frames > 0) e = kf_alloc(np, kf_count(max_kf_images, max_frames), w, h);
+  if (e != cudaSuccess) {
+    cudaGetLastError(); for (auto& f : nf) frame_free(f); kf_free(np);
+    return ctx_fail(c, SDV_ERR_CUDA, "%s: camera %d: %d frames and their keyframe images of %dx%d -> %s (the old pool is kept)", who, cam, max_frames, w, h, cudaGetErrorString(e));
+  }
+  std::vector<FrameDev> keep; keep.reserve(c->frames.size() + nf.size());
+  for (FrameDev& f : c->frames) { if (f.pool == cam) frame_free(f); else keep.push_back(f); }
+  kf_free(P);
+  for (const FrameDev& f : nf) keep.push_back(f);
+  c->frames.swap(keep); P = np;
+  c->frame_index.clear();                                                // indices moved: every resident handle is found again
+  for (size_t i=0;i<c->frames.size();i++) if (c->frames[i].used) c->frame_index[c->frames[i].id] = (int)i;
+  return SDV_OK;
+}
+// device bytes of one frame and one keyframe level-0 image of camera cam as its frames are stored now: in its own pool, or at the context size
+int sdv_camera_storage_bytes(sdv_ctx* c, int cam, uint64_t* frame_bytes_out, uint64_t* kf_image_bytes_out) { SDV_GUARD_TRK(c);
+  if (!c) return SDV_ERR_ARG;
+  { int rc = check_cams(c, 1, &cam, "sdv_camera_storage_bytes", nullptr); if (rc) return rc; }
+  const FramePool& P = c->pools[frame_pool_of(c, cam)];
+  if (frame_bytes_out) *frame_bytes_out = frame_bytes(P.w, P.h, c->levels);
+  if (kf_image_bytes_out) *kf_image_bytes_out = kf_image_bytes(P.w, P.h);
   return SDV_OK;
 }
 
@@ -164,19 +239,11 @@ static int create_impl(sdv_ctx* c, const sdv_calib* K, int w, int h, int levels,
   make_geom(c, K, 0, 0);
   CK(cudaMalloc(&c->geom_dev, c->geom.size()*sizeof(GeomRow)));
   CK(cudaMemcpy(c->geom_dev, c->geom.data(), c->geom.size()*sizeof(GeomRow), cudaMemcpyHostToDevice));
-  // frame pool: planar intensity of every level per frame (level 0 + one allocation for levels >= 1), plus the storage of the packed-texel cache of
-  // levels >= 1; packed level-0 texels come from a small keyframe pool
-  size_t texels = 0; c->lvl_off[0] = 0; for (int l=1;l<levels;l++) { c->lvl_off[l] = texels; texels += (size_t)(w>>l)*(h>>l); }
-  c->frame_texels = texels;
+  // the context's frame pool: max_frames frames and the keyframe level-0 images, at the context size
   c->frames.resize(s.max_frames);
-  for (auto& f : c->frames) {
-    f.used = false; f.adopted = false; f.trk_async = false; f.lvl0_slot = -1; f.hi_tex = false; f.pyr = nullptr; f.base = nullptr; f.ingest_seq = 0; f.cam = 0;
-    CK(cudaMalloc(&f.I0_own, (size_t)w*h*sizeof(float))); f.I0 = f.I0_own; f.img[0] = f.I0;
-    if (texels) { CK(cudaMalloc(&f.pyr, texels*sizeof(float))); CK(cudaMalloc(&f.base, texels*sizeof(float4))); }
-    f.lvl[0] = nullptr; for (int l=1;l<levels;l++) { f.img[l] = f.pyr + c->lvl_off[l]; f.lvl[l] = f.base + c->lvl_off[l]; }
-  }
-  { int nkf = s.max_kf_images > 0 ? s.max_kf_images : SDV_MAX_FRAMES_WINDOW + 4; if (nkf > s.max_frames) nkf = s.max_frames;
-    c->lvl0_pool.resize(nkf); for (int i=0;i<nkf;i++) { CK(cudaMalloc(&c->lvl0_pool[i], (size_t)w*h*sizeof(float4))); c->lvl0_free.push_back(nkf-1-i); } }
+  for (auto& f : c->frames) CK(frame_alloc(f, 0, w, h, levels));
+  c->pools[0].w = w; c->pools[0].h = h; c->pools[0].n_frames = s.max_frames;
+  CK(kf_alloc(c->pools[0], kf_count(s.max_kf_images, s.max_frames), w, h));
   // tracker slots
   c->slots.resize(s.n_tracker_slots);
   for (auto& t : c->slots) {
@@ -199,8 +266,8 @@ void sdv_destroy(sdv_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
   if (c->st_cp) cudaStreamSynchronize(c->st_cp); if (c->st_in) cudaStreamSynchronize(c->st_in); if (c->st) cudaStreamSynchronize(c->st);
-  for (auto& f : c->frames) { cudaFree(f.base); cudaFree(f.pyr); cudaFree(f.I0_own); }
-  for (auto p : c->lvl0_pool) cudaFree(p);
+  for (auto& f : c->frames) frame_free(f);
+  for (auto& P : c->pools) kf_free(P);
   for (auto& t : c->slots) for (int l=0;l<c->levels;l++) cudaFree(t.pts[l]);
   for (int i=0;i<2;i++) { c->ing_dev[i].release(); c->ing_host[i].release(); } cudaFree(c->partials); cudaFree(c->ticket); cudaFree(c->totals_dev); cudaFreeHost(c->totals_host);
   cudaFree(c->tc_dev); cudaFree(c->geom_dev); c->scr.release(); c->scr_host.release();
@@ -227,12 +294,20 @@ int sdv_debug_gs_entry_rc(int k) { int r, c; if (k < 0 || k >= kNH) return -1; g
 float sdv_last_kernel_ms(sdv_ctx* c) { return c ? c->last_ms : 0.f; }
 
 // ------------------------------------------------------------------------------------------------ frames
-static void frame_drop_texels(sdv_ctx* c, FrameDev& f) { if (f.lvl0_slot >= 0) { c->lvl0_free.push_back(f.lvl0_slot); f.lvl0_slot = -1; } f.lvl[0] = nullptr; f.hi_tex = false; }
+static void frame_drop_texels(sdv_ctx* c, FrameDev& f) { if (f.lvl0_slot >= 0) { c->pools[f.pool].lvl0_free.push_back(f.lvl0_slot); f.lvl0_slot = -1; } f.lvl[0] = nullptr; f.hi_tex = false; }
+// hands frame entry idx back to its pool (sdv_frame_release): the caller may reuse an adopted buffer at once, its keyframe image goes back to the pool
+static int frame_release_idx(sdv_ctx* c, int idx) {
+  FrameDev& f = c->frames[idx];
+  { int rcf = frame_fence(c, f, nullptr, nullptr, f.adopted); if (rcf) return rcf; }
+  f.used = false; frame_drop_texels(c, f); f.adopted = false; f.I0 = f.I0_own; f.img[0] = f.I0; c->frame_index.erase(f.id);
+  return SDV_OK;
+}
 
 // kind bit0: mono8 input, bit1: input already in device memory, bit2: adopt the (device, float) buffer as the frame's level-0 plane,
 // bit3: RAW mono8 input of the camera's native size, rectified through the tables of sdv_set_undistort_cam inside the level-0 kernel.
 // Image k is camera cams[k] (cams == NULL: camera 0) and becomes a frame of that camera's rectified size, so the byte size, the staging offset and the
-// coalesced copies are per frame.
+// coalesced copies are per frame.  Its storage comes from the camera's pool (frame_pool_of); a handle resident in another pool moves: every image's frame
+// is claimed first (a pinned handle or a full pool refuses the batch and leaves every handle as it was), then the moved handles' old frames are released.
 // Everything is enqueued on the ingest stream; the compute stream picks it up through ev_in at the next tracker / BA call, so an
 // upload overlaps the tracking of the previous batch.  Every level is a planar intensity image: a pinned-host float upload lands directly in
 // frame storage, levels >= 1 are built by one fused launch, and the consumers form gradients on the fly.
@@ -258,17 +333,34 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
   sd.reset(); sh.reset(); PyrBatchHost* desc_dev = sd.take<PyrBatchHost>(n); PyrBatchHost* desc = sh.take<PyrBatchHost>(n); unsigned char* stage_u8 = sd.take<unsigned char>(stage);
   c->cp_dst.clear(); c->cp_src.clear(); c->cp_sz.clear();
   if (c->levels > 1 && ((c->w | c->h) & 1)) return ctx_fail(c, SDV_ERR_ARG, "pyramid needs even image sizes");
+  // every image's frame is planned before any frame changes: a refused batch (a pinned handle, a full pool) leaves every handle as it was
+  std::vector<int> idx_of(n), old_of(n, -1); std::vector<char> taken(c->frames.size(), 0); std::unordered_map<uint64_t, int> planned;
+  for (int k=0;k<n;k++) {
+    const int p = frame_pool_of(c, cam_of(k));
+    auto pl = planned.find(frames[k]);
+    if (pl != planned.end()) {                                            // the same handle twice in one batch: one frame for both, as before
+      if (c->frames[idx_of[pl->second]].pool != p)
+        return ctx_fail(c, SDV_ERR_ARG, "frame %llu appears twice in one upload with cameras of different frame pools", (unsigned long long)frames[k]);
+      idx_of[k] = idx_of[pl->second]; continue;
+    }
+    planned[frames[k]] = k; int idx = -1;
+    auto it = c->frame_index.find(frames[k]);
+    if (it != c->frame_index.end()) {
+      if (frame_pinned(c, frames[k])) return ctx_fail(c, SDV_ERR_STATE, "frame %llu is referenced by a resident BA window / map slot and cannot be re-uploaded", (unsigned long long)frames[k]);
+      if (c->frames[it->second].pool == p) idx = it->second; else old_of[k] = it->second;   // storage in another pool: the handle moves to pool p
+    }
+    if (idx < 0) for (size_t i=0;i<c->frames.size();i++) if (!c->frames[i].used && !taken[i] && c->frames[i].pool == p) { idx = (int)i; break; }
+    if (idx < 0) return p == 0 ? ctx_fail(c, SDV_ERR_CAPACITY, "frame pool exhausted (max_frames=%d)", c->pools[0].n_frames)
+                               : ctx_fail(c, SDV_ERR_CAPACITY, "frame pool of camera %d exhausted (max_frames=%d)", p, c->pools[p].n_frames);
+    taken[idx] = 1; idx_of[k] = idx;
+  }
   bool vec = true; size_t stage_off = 0; int max_w = 0, max_h = 0;
   for (int k=0;k<n;k++) {
-    int idx = -1;
-    auto it = c->frame_index.find(frames[k]);
-    if (it != c->frame_index.end()) { idx = it->second;
-      if (frame_pinned(c, frames[k])) return ctx_fail(c, SDV_ERR_STATE, "frame %llu is referenced by a resident BA window / map slot and cannot be re-uploaded", (unsigned long long)frames[k]); }
-    else { for (size_t i=0;i<c->frames.size();i++) if (!c->frames[i].used) { idx = (int)i; break; } }
-    if (idx < 0) return ctx_fail(c, SDV_ERR_CAPACITY, "frame pool exhausted (max_frames=%d)", (int)c->frames.size());
+    const int idx = idx_of[k];
+    if (old_of[k] >= 0) { int rco = frame_release_idx(c, old_of[k]); if (rco) return rco; }   // the moved handle's old frame, once its new one is certain
     { int rcf = frame_fence(c, c->frames[idx], c->st_cp, c->st_in, c->frames[idx].adopted); if (rcf) return rcf; }   // an earlier trace may still read its storage
     FrameDev& f = c->frames[idx]; f.used = true; f.id = frames[k]; f.exposure = exposures ? exposures[k] : 1.0f; c->frame_index[frames[k]] = idx;
-    frame_drop_texels(c, f); f.ingest_seq = seq; f.cam = cam_of(k);
+    frame_drop_texels(c, f); f.ingest_seq = seq; f.cam = cam_of(k); frame_layout(c, f);
     f.adopted = adopt; f.I0 = adopt ? const_cast<float*>(reinterpret_cast<const float*>(imgs[k])) : f.I0_own; f.img[0] = f.I0;
     PyrBatchHost& b = desc[k];
     b.pyr = f.pyr; b.I0 = f.I0; b.flags = (f.exposure > 0.f) ? 1 : 0; b.cam = f.cam; b.w = c->cam_w[f.cam]; b.h = c->cam_h[f.cam];
@@ -296,7 +388,7 @@ static int frame_ingest(sdv_ctx* c, int n, const uint64_t* frames, const void* c
   launch_h2d_words(desc_dev, desc, (size_t)n*sizeof(PyrBatchHost), c->st_in);   // kernel copy: a cudaMemcpyAsync here becomes ready only after this batch's bulk copy and
   c->launches += 1;                                                                              // would queue behind the NEXT batch's bulk copy on the H2D engine
   const UndistortCams* und = raw ? &c->und : nullptr;
-  if (c->levels > 1) { launch_pyramid_batch(desc_dev, n, u8, vec, c->w, c->h, max_w, max_h, c->levels, c->st_in, und); c->launches += 1; }
+  if (c->levels > 1) { launch_pyramid_batch(desc_dev, n, u8, vec, max_w, max_h, c->levels, c->st_in, und); c->launches += 1; }
   else if (u8 || (dev && !adopt)) { launch_pyramid_copy0(desc_dev, n, u8, max_w, max_h, c->st_in, und); c->launches += 1; }
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev_ing[seq % sdv_ctx::kIngRing], c->st_in)); c->ingest_seq = seq; c->ingest_pending = true;
@@ -322,9 +414,11 @@ int join_ingest_upto(sdv_ctx* c, long long seq) {  // the compute stream waits f
 int join_ingest(sdv_ctx* c) { c->ingest_pending = false; return join_ingest_upto(c, c->ingest_seq); }
 int ensure_lvl0(sdv_ctx* c, FrameDev& f) {        // FrameHessian::dI of a keyframe: packed level-0 texels, built once on demand
   if (f.lvl[0]) return SDV_OK;
-  if (c->lvl0_free.empty()) return ctx_fail(c, SDV_ERR_CAPACITY, "keyframe level-0 image pool exhausted (max_kf_images=%d)", (int)c->lvl0_pool.size());
+  FramePool& P = c->pools[f.pool];                                       // the pool of the frame's storage: no fallback to another pool
+  if (P.lvl0_free.empty()) return f.pool == 0 ? ctx_fail(c, SDV_ERR_CAPACITY, "keyframe level-0 image pool exhausted (max_kf_images=%d)", (int)P.lvl0.size())
+                                              : ctx_fail(c, SDV_ERR_CAPACITY, "keyframe level-0 image pool of camera %d exhausted (max_kf_images=%d)", f.pool, (int)P.lvl0.size());
   int rc = join_ingest(c); if (rc) return rc;
-  f.lvl0_slot = c->lvl0_free.back(); c->lvl0_free.pop_back(); f.lvl[0] = c->lvl0_pool[f.lvl0_slot];
+  f.lvl0_slot = P.lvl0_free.back(); P.lvl0_free.pop_back(); f.lvl[0] = P.lvl0[f.lvl0_slot];
   launch_grad_texels(f.I0, f.lvl[0], c->cam_w[f.cam], c->cam_h[f.cam], cam_gw2(c, f.cam), c->st); c->launches += 1;
   CK(cudaGetLastError());
   return SDV_OK;
@@ -466,8 +560,7 @@ int sdv_frame_release(sdv_ctx* c, uint64_t frame) { SDV_GUARD_TRK(c);
   if (!c) return SDV_ERR_ARG;
   auto it = c->frame_index.find(frame); if (it == c->frame_index.end()) return ctx_fail(c, SDV_ERR_NOFRAME, "unknown frame %llu", (unsigned long long)frame);
   if (frame_pinned(c, frame)) return ctx_fail(c, SDV_ERR_STATE, "frame %llu is referenced by a resident BA window / map slot: replace or clear that window / map first", (unsigned long long)frame);
-  { int rcf = frame_fence(c, c->frames[it->second], nullptr, nullptr, c->frames[it->second].adopted); if (rcf) return rcf; }   // the caller may reuse an adopted buffer at once
-  FrameDev& f = c->frames[it->second]; f.used = false; frame_drop_texels(c, f); f.adopted = false; f.I0 = f.I0_own; f.img[0] = f.I0; c->frame_index.erase(it); return SDV_OK;
+  return frame_release_idx(c, it->second);
 }
 int sdv_frame_download(sdv_ctx* c, uint64_t frame, int lvl, float* dI3_out, float* abs_out) { SDV_GUARD_TRK(c);
   if (!c || lvl < 0 || lvl >= c->levels) return SDV_ERR_ARG;

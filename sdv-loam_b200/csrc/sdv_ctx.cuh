@@ -17,15 +17,22 @@ using PinnedScratch = ScratchOf<PinnedMem>;
 struct FrameDev {                         // one FrameHessian's images on the device
   uint64_t id; float exposure; bool used;
   float* I0; float* I0_own; bool adopted;  // level-0 intensity plane (own storage, or an adopted caller buffer)
-  float* pyr;                             // planar intensity of levels >= 1 (level l at sdv_ctx::lvl_off[l])
-  const float* img[kLevels];              // planar intensity of every level: img[0] = I0, img[l] = pyr + lvl_off[l]
+  float* pyr;                             // planar intensity of levels >= 1, level l at the offsets of the frame's own size (frame_layout)
+  const float* img[kLevels];              // planar intensity of every level: img[0] = I0, img[l] = pyr + offset of level l
   // packed {I,dx,dy,|grad|^2} texels: a cache built on demand from the planes (ensure_texels) for the keyframe-rate consumers, dropped by a re-ingest.
-  // lvl[0] is a slot of the keyframe level-0 pool (lvl0_slot, -1 if not built); levels >= 1 live in `base` at lvl_off[l] and are valid while hi_tex is set.
+  // lvl[0] is an image of its pool's keyframe level-0 images (lvl0_slot, -1 if not built); levels >= 1 live in `base` at the offsets of img[l] and are
+  // valid while hi_tex is set.
   float4* base; float4* lvl[kLevels]; int lvl0_slot; bool hi_tex;
   long long ingest_seq;                   // ingest call that (re)built this frame's pyramid
-  int cam;                                // camera it was ingested for: its size is sdv_ctx::cam_w/cam_h[cam] (storage stays at the context size and lvl_off)
+  int cam;                                // camera it was ingested for: its size is sdv_ctx::cam_w/cam_h[cam]
+  int pool;                               // the FramePool its storage belongs to: 0 (the context's) or a camera with its own (sdv_set_camera_storage)
   bool trk_async;                         // read by tracker-stream work that may still be pending (sdv_ctx::ev_trk_async marks its end)
 };
+
+// Storage of frames and keyframe level-0 images of one size.  pools[0] is the context's (sdv_create: max_frames frames and max_kf_images images at the
+// context size); pools[k], k >= 1, is camera k's own (sdv_set_camera_storage, at its rectified size), active while n_frames > 0.  The frames themselves
+// sit in sdv_ctx::frames, each naming its pool; a frame of a camera with a pool is always claimed from that pool, every other frame from pools[0].
+struct FramePool { int w = 0, h = 0, n_frames = 0; std::vector<float4*> lvl0; std::vector<int> lvl0_free; };
 
 struct TrackerSlot {                      // one CoarseTracker instance (reference keeps two: FullSystem.h coarseTracker / coarseTracker_forNewKF)
   float4* pts[kLevels]; int npts[kLevels]; int cap[kLevels];
@@ -52,11 +59,11 @@ struct sdv_ctx {
   int w, h, levels; sdv_settings set;
   int cam_w[SDV_MAX_CAMERAS], cam_h[SDV_MAX_CAMERAS];                  // rectified size per camera (sdv_set_camera_size); camera 0 is always w x h
   int cam_levels[SDV_MAX_CAMERAS];                                     // pyramid depth per camera (sdv_set_camera_levels), 1..levels: what its slots and jobs use; frames are stored at `levels`
+  sdv::FramePool pools[SDV_MAX_CAMERAS];                               // frame storage: the context's (0) and the cameras' own (sdv_set_camera_storage)
   sdv::TrackConst tc; sdv::TrackConst* tc_dev;
   // geometry table (CoarseTracker::makeK per K): row 0 = the context calibration (sdv_set_calib), row 1 + s = tracker slot s's own K (sdv_set_calib_slots).
   // Host mirror + device copy; every consumer indexes it with TrackerSlot::geom_row, none derives the geometry from K itself.
   std::vector<sdv::GeomRow> geom; sdv::GeomRow* geom_dev;
-  size_t lvl_off[sdv::kLevels]; size_t frame_texels;
   std::vector<sdv::FrameDev> frames; std::unordered_map<uint64_t,int> frame_index;
   // frames whose device images are referenced by a resident BA window (BAHeader::frames[].img0) or map slot (MapDev::hostI0): refcount per handle.
   // A pinned frame can be neither released nor re-uploaded (SDV_ERR_STATE) — its pool storage would be handed to another frame under the reader.
@@ -68,7 +75,6 @@ struct sdv_ctx {
   // sdv_set_gamma_cam: per camera, the 256 factors gamma_w2 reads (FullSystem::setGammaFunction's B as makeImages weighs |grad|^2 with it), in one allocation
   // of SDV_MAX_CAMERAS rows; a camera without gamma (B[i] = i) passes nullptr to the kernels
   float* gw2_dev = nullptr; bool gamma_set[SDV_MAX_CAMERAS] = {};
-  std::vector<float4*> lvl0_pool; std::vector<int> lvl0_free;
   std::vector<void*> cp_dst, cp_src; std::vector<size_t> cp_sz; bool no_batch_copy = false;
   std::vector<sdv::TrackerSlot> slots;
   double* partials; unsigned int* ticket; double* totals_dev; double* totals_host;
@@ -138,6 +144,8 @@ inline bool frame_pinned(const sdv_ctx* c, uint64_t id) { return c->pins.find(id
 int  join_ingest(sdv_ctx* c);                  // compute stream waits for every ingest enqueued so far
 int  join_ingest_upto(sdv_ctx* c, long long seq);   // ... for ingest calls <= seq only (frames carry their ingest_seq)
 inline const GeomRow& slot_geom(const sdv_ctx* c, int slot) { return c->geom[c->slots[slot].geom_row]; }   // the K a tracker / map slot uses, at every level
+// the pool a frame of camera cam is claimed from: the camera's own, or the context's
+inline int frame_pool_of(const sdv_ctx* c, int cam) { return cam > 0 && c->pools[cam].n_frames > 0 ? cam : 0; }
 // frames are depth-agnostic (stored at the context's depth): a frame fits a camera of the same size.  A tracker / map slot holds clouds built at its camera's
 // depth as well: it may only keep them on a camera of the same size and depth.
 inline const float* cam_gw2(const sdv_ctx* c, int cam) { return c->gamma_set[cam] ? c->gw2_dev + 256*(size_t)cam : nullptr; }   // gamma weights of camera cam, or nullptr

@@ -28,7 +28,8 @@ static int num_sms() {
 }
 
 // ================================================================================================ pyramid
-// Every level of a frame is a planar float intensity plane (level 0: the frame's I0; levels >= 1: the frame's `pyr` allocation at lvl_off[l]).
+// Every level of a frame is a planar float intensity plane (level 0: the frame's I0; levels >= 1: the frame's `pyr` allocation, level l after levels
+// 1..l-1 of the frame's own size).
 // Packed {I,dx,dy,|grad|^2} texels are a derived cache that only keyframe-rate consumers build (grad_texel_kernel).
 struct PyrBatch { const void* src; float* I0; float* pyr; int flags; int cam; int w, h; };   // per frame: level-0 input (float/u8; may equal I0), level-0 plane, planes of levels >= 1; flags bit0: photometric response applies (exposure > 0); cam: Undistort camera of a RAW input; w x h: the frame's (its camera's) size
 static_assert(sizeof(PyrBatch) == sizeof(PyrBatchHost), "PyrBatch mirrors PyrBatchHost");
@@ -88,11 +89,12 @@ __global__ void __launch_bounds__(256) pyr_remap0_kernel(const PyrBatch* __restr
 // simply has fewer (or no) rows there.  Level 0 comes from a float plane (resident or adopted), mono8, or RAW mono8 through its camera's Undistort tables (RAW),
 // and is written to the frame's I0 plane whenever the input is not that plane already.
 // Each frame has its own size b.w x b.h (its camera's); the grid covers the bands of the tallest frame, and the CTAs past a frame's last band exit.  Level l
-// is written at the context's lvl_off[l] (computed from the context size W x H), so every frame fits the frame storage allocated at the context size.
+// is written after levels 1..l-1 of that size, so a frame fits storage of its own size (a camera's pool) as well as the context's.
 // P = level-1 pixels per work item: 2 reads each parent row as one 16-byte (float) / 4-byte (mono8) vector, 1 reads scalars (unaligned input or w % 4 != 0).
+// The second bound keeps the register count of the offsets of the frame's own size at the parent layout's: 32 (8 CTAs per SM) for the plane inputs, 40 for RAW.
 constexpr int kPyrThreads = 256;
 template <typename T, bool RAW, int P>
-__global__ void __launch_bounds__(kPyrThreads) pyr_fused_kernel(const PyrBatch* __restrict__ batch, const __grid_constant__ UndistortCams cams, int W, int H, int levels) {
+__global__ void __launch_bounds__(kPyrThreads, RAW ? 6 : 8) pyr_fused_kernel(const PyrBatch* __restrict__ batch, const __grid_constant__ UndistortCams cams, int levels) {
   extern __shared__ float pyr_band[];                       // levels 1..levels-2 of the band: [R1][w1] [R1/2][w2] ...
   const PyrBatch b = batch[blockIdx.y];
   const int w = b.w, R1 = 1 << (levels - 2);                // R1: level-1 rows per band
@@ -140,7 +142,7 @@ __global__ void __launch_bounds__(kPyrThreads) pyr_fused_kernel(const PyrBatch* 
     }
   }
   const float* prev = pyr_band; float* cur = pyr_band + (size_t)R1*w1;
-  int wp = w1, hp = h1; size_t off = (size_t)(W >> 1)*(H >> 1);   // off: the context's lvl_off[l]
+  int wp = w1, hp = h1; size_t off = (size_t)w1*h1;          // off: level l's offset in the frame's pyr
   for (int l = 2; l < levels; l++) {
     __syncthreads();
     const int wl = wp >> 1, hl = hp >> 1, Rl = R1 >> (l - 1), yl = blockIdx.x*Rl, nl = min(Rl, hl - yl);
@@ -153,7 +155,7 @@ __global__ void __launch_bounds__(kPyrThreads) pyr_fused_kernel(const PyrBatch* 
       out[(size_t)(yl + rr)*wl + x] = v;
       if (keep_l) cur[rr*wl + x] = v;
     }
-    prev = cur; cur += (size_t)Rl*wl; off += (size_t)(W >> l)*(H >> l); wp = wl; hp = hl;
+    prev = cur; cur += (size_t)Rl*wl; off += (size_t)wl*hl; wp = wl; hp = hl;
   }
 }
 static size_t pyr_band_bytes(int w, int levels) {
@@ -162,24 +164,24 @@ static size_t pyr_band_bytes(int w, int levels) {
   return n*sizeof(float);
 }
 template <typename T, bool RAW, int P>
-static void launch_pyr_fused(const PyrBatch* batch_dev, int nframes, int W, int H, int max_w, int max_h, int levels, const UndistortCams& U, cudaStream_t st) {
+static void launch_pyr_fused(const PyrBatch* batch_dev, int nframes, int max_w, int max_h, int levels, const UndistortCams& U, cudaStream_t st) {
   const size_t smem = pyr_band_bytes(max_w, levels);
   if (smem > 48*1024) cudaFuncSetAttribute(pyr_fused_kernel<T, RAW, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);   // very wide images; a refusal surfaces as the launch error
   const int R1 = 1 << (levels - 2);
   dim3 g(((max_h >> 1) + R1 - 1)/R1, nframes);
-  pyr_fused_kernel<T, RAW, P><<<g, kPyrThreads, smem, st>>>(batch_dev, U, W, H, levels);
+  pyr_fused_kernel<T, RAW, P><<<g, kPyrThreads, smem, st>>>(batch_dev, U, levels);
 }
 
 // batch_dev: nframes PyrBatch descriptors in device memory.  src_u8: level-0 input is mono8 (sensor_msgs/Image wire format) instead of float.
 // vec: every level-0 input (and I0 plane written) of the batch is 16-byte aligned and every frame's w % 4 == 0 (the 4-pixel vector path).
 // Requires even w,h whenever levels > 1 (pyrLevelsUsed only halves even sizes, globalCalib.cpp:24).
-void launch_pyramid_batch(const void* batch_dev_v, int nframes, bool src_u8, bool vec, int W, int H, int max_w, int max_h, int levels, cudaStream_t st, const UndistortCams* und) {
+void launch_pyramid_batch(const void* batch_dev_v, int nframes, bool src_u8, bool vec, int max_w, int max_h, int levels, cudaStream_t st, const UndistortCams* und) {
   const PyrBatch* batch_dev = reinterpret_cast<const PyrBatch*>(batch_dev_v);
   if (nframes <= 0 || levels < 2) return;
   const UndistortCams U = und ? *und : UndistortCams{};
-  if (und) launch_pyr_fused<unsigned char, true, 1>(batch_dev, nframes, W, H, max_w, max_h, levels, U, st);
-  else if (src_u8) { if (vec) launch_pyr_fused<unsigned char, false, 2>(batch_dev, nframes, W, H, max_w, max_h, levels, U, st); else launch_pyr_fused<unsigned char, false, 1>(batch_dev, nframes, W, H, max_w, max_h, levels, U, st); }
-  else             { if (vec) launch_pyr_fused<float, false, 2>(batch_dev, nframes, W, H, max_w, max_h, levels, U, st);         else launch_pyr_fused<float, false, 1>(batch_dev, nframes, W, H, max_w, max_h, levels, U, st); }
+  if (und) launch_pyr_fused<unsigned char, true, 1>(batch_dev, nframes, max_w, max_h, levels, U, st);
+  else if (src_u8) { if (vec) launch_pyr_fused<unsigned char, false, 2>(batch_dev, nframes, max_w, max_h, levels, U, st); else launch_pyr_fused<unsigned char, false, 1>(batch_dev, nframes, max_w, max_h, levels, U, st); }
+  else             { if (vec) launch_pyr_fused<float, false, 2>(batch_dev, nframes, max_w, max_h, levels, U, st);         else launch_pyr_fused<float, false, 1>(batch_dev, nframes, max_w, max_h, levels, U, st); }
 }
 // levels == 1: the level-0 plane still has to be materialised from a foreign / mono8 source
 template <typename T> __global__ void pyr_copy0_kernel(const PyrBatch* __restrict__ batch) {

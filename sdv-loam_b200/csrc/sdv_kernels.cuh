@@ -11,10 +11,10 @@ struct PyrBatchHost { const void* src; float* I0; float* pyr; int flags; int cam
 struct UndistortDev { const float* remapX; const float* remapY; const float* G; const float* vignette; int wOrg, hOrg; float factor; };
 // the cameras of a context (sdv_set_undistort_cam), passed by value to the RAW kernels; an unset camera has remapX == nullptr
 struct UndistortCams { UndistortDev cam[SDV_MAX_CAMERAS]; };
-// all planes of levels >= 1 in one launch (levels > 1; `pyr` of a frame holds level l at lvl_off[l], the offsets of the context W x H); each frame has its own
-// size PyrBatch::w x h <= W x H; max_w x max_h: the largest frame of the batch (grid and shared memory); vec: 16-byte aligned inputs / I0 and w % 4 == 0 for
-// every frame.  und: RAW input, each frame rectified with und->cam[PyrBatch::cam]
-void launch_pyramid_batch(const void* batch_dev, int nframes, bool src_u8, bool vec, int W, int H, int max_w, int max_h, int levels, cudaStream_t st, const UndistortCams* und = nullptr);
+// all planes of levels >= 1 in one launch (levels > 1); each frame has its own size PyrBatch::w x h, and its `pyr` holds level l after levels 1..l-1 of
+// that size; max_w x max_h: the largest frame of the batch (grid and shared memory); vec: 16-byte aligned inputs / I0 and w % 4 == 0 for every frame.
+// und: RAW input, each frame rectified with und->cam[PyrBatch::cam]
+void launch_pyramid_batch(const void* batch_dev, int nframes, bool src_u8, bool vec, int max_w, int max_h, int levels, cudaStream_t st, const UndistortCams* und = nullptr);
 void launch_pyramid_copy0(const void* batch_dev, int nframes, bool src_u8, int max_w, int max_h, cudaStream_t st, const UndistortCams* und = nullptr);
 void launch_grad_texels(const float* I, float4* out, int w, int h, const float* gw2, cudaStream_t st);   // packed {I,dx,dy,|grad|^2} texels of one planar level (gw2: gamma_w2)
 void launch_unpack_level(const float4* in, float* dI3, float* ab, int n, cudaStream_t st);
